@@ -38,23 +38,23 @@ WORKLOADS = {
     # config 3: the same video with a faster camera so that the 0.20 overlap filter actually removes long-range pairs
     "config3_300f_384x224_grid16x12_sep10_maskratio0.20": dict(frames=300, w=384, h=224, gx=16, gy=12, sep=10, mask_ratio=0.20,
                                                                scene=dict(rot_deg=1.2, motion=0.04)),
-    # config 4: Huber robustifier (an extension: the reference only has Cauchy, SURVEY fact 1)
-    "config4_1000f_640x384_grid32x24_sep10": dict(frames=1000, w=640, h=384, gx=32, gy=24, sep=10),
-    "config4_1000f_640x384_grid32x24_sep10_huber": dict(frames=1000, w=640, h=384, gx=32, gy=24, sep=10, cfg=dict(robust_type=abi.ROBUST_HUBER, robustness=0.05)),
+    # config 4: Huber robustifier (an extension: the reference only has Cauchy, SURVEY fact 1).  600 frames: the factor of the
+    # 32x24 grid (npad 784, 4.9 MB per block) takes ~0.1 GB per frame, so this is about the longest video one 80 GB H100 holds
+    "config4_600f_640x384_grid32x24_sep10": dict(frames=600, w=640, h=384, gx=32, gy=24, sep=10),
+    "config4_600f_640x384_grid32x24_sep10_huber": dict(frames=600, w=640, h=384, gx=32, gy=24, sep=10, cfg=dict(robust_type=abi.ROBUST_HUBER, robustness=0.05)),
     # config 5: dynamic-mask holes (29 % of every frame => ~50 % of the pixels of a pair keep both ends visible) and a dolly-in
     # (divergent flow field)
     "config5_300f_384x224_grid16x12_sep10_holes50_dolly": dict(frames=300, w=384, h=224, gx=16, gy=12, sep=10, scene=dict(hole_fraction=0.29, dolly=0.008)),
 }
 METRIC = "flow_residual_constraints_per_sec_per_gn_iteration"
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the two roofline kernels, from the `ncu --set full` captures of THIS
-    round's kernels (profiles/r2_ncu_traffic.json, written by tools/round_profiles_post.sh together with the kernel names and the capture
-    command); null when the file is missing or was captured for other kernels."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")))
-        return {"update": t["k_update_tma"]["dram_bytes_per_launch"], "accumulate": t["k_accumulate_runs"]["dram_bytes_per_launch"], "source": t["source"]}
-    except Exception:
-        return {"update": None, "accumulate": None, "source": None}
+H100_HBM_GBS = 3350.0      # H100 SXM data sheet (HBM3); used when MEASURED_PEAKS.json gives no measured figure
+
+
+def dump_outputs(out_dir, it):
+    """Writes what the last timed step computed as DIR/<name>.npy (float64), so that two builds can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in it.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.atleast_1d(np.asarray(v, np.float64)))
 
 
 def build_case(wl, frames=None, sep=None, seed=2, valid_fraction=1.0):
@@ -235,6 +235,8 @@ def run_ours(args):
     wall = time.perf_counter() - t0
     launches = P.launch_count() - l0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, P.last_iteration())      # before any other call overwrites the step's buffers
     ms = tm["iter_ms"]
     if world > 1:
         tt = torch.tensor([ms], dtype=torch.float64, device="cuda")
@@ -264,7 +266,8 @@ def run_ours(args):
             parity["multi_gpu"] = {"ranks": world, "max_rel_diff_cost_gradnorm_gradl1_vs_rank0_full_evaluation": float(max(np.max(np.abs(a.cpu().numpy() - ref) / np.abs(ref)) for a in allchk)),
                                    "max_abs_grad_diff_rank0": float(np.abs(g_sh - g_full).max()), "grad_max": float(np.abs(g_full).max())}
     lin_prof = P.profile_linear(reps=3)            # per-kernel-class device time, serialised (CUDA events around every launch)
-    peak64 = solver.fp64_tensor_peak(local)        # live DMMA peak (TFLOP/s) of this GPU
+    peaks64 = solver.fp64_tensor_peaks(local)      # live DMMA peak (TFLOP/s) of this GPU per mma.sync shape
+    peak64 = max(peaks64.values())
     # ---- e2e: C ABI with host buffers, copies inside the timed region ----
     e2e_iters = args.e2e_iters
     opt = abi.default_solve_options(max_iterations=e2e_iters)
@@ -291,7 +294,7 @@ def run_ours(args):
         return s, P.get_state()
     e2e = None
     if world == 1:
-        P.close()          # the e2e calls create their own handle; two resident copies of a large problem (config 4: ~107 GB) do not fit
+        P.close()          # the e2e calls create their own handle; two resident copies of a large problem (config 4) do not fit in 80 GB
     if not args.skip_e2e:
         call = e2e_once if world == 1 else e2e_once_multi
         call()
@@ -318,31 +321,28 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
-    traffic = ncu_traffic()
+    hbm_peak = peaks.get("hbm_gbs", H100_HBM_GBS)
     # algorithmic bytes of the residual/Jacobian/accumulate pass (SURVEY 8d): 24 B per constraint + per pair
     # ids + 2 parameter vectors + the outputs (gradient + H blocks of the original structure)
     nf, npad = info["stride"], info["npad"]
     alg_bytes = 24.0 * C_total + len(pairs) * (8 + 16 * nf) + 8.0 * cfg.num_frames * nf + 8.0 * info["h_blocks"] * nf * nf
     roof_acc = {"bound": "hbm", "kernel": "gn_accumulate (memset of H + k_accumulate_runs + k_regularisers + cost reduction)", "achieved": alg_bytes / (acc_ms * 1e-3) / 1e9,
                 "peak": hbm_peak, "unit": "GB/s", "frac": alg_bytes / (acc_ms * 1e-3) / 1e9 / hbm_peak,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst)" if peaks else "fallback 6650 GB/s",
-                "traffic": traffic["accumulate"], "traffic_source": traffic["source"], "ms": acc_ms,
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst)" if "hbm_gbs" in peaks else "H100 SXM data sheet 3350 GB/s (not measured)", "ms": acc_ms,
                 "note": "latency / fp64-issue bound at matchSeparation 10 (22 MB of records, L2 resident), not HBM bound: see DESIGN.md section 4"}
-    traffic_note = None
     # dominant kernel of the step: k_update_tma, the fp64 tensor-core block updates of the sparse Cholesky
     n_g = max(lin_prof["gemm_launches"], 1.0)
     g_tf = lin_prof["gemm_flops"] / max(lin_prof["gemm_ms"] * 1e-3, 1e-12) / 1e12
     roof = {"bound": "tensor", "kernel": "k_update_tma (TMA-fed fp64 DMMA Schur updates of the block Cholesky)" if not args.legacy_update else "k_gemm_nt (round-1 cp.async kernel)", "achieved": g_tf, "peak": peak64, "unit": "TFLOP/s",
-            "frac": g_tf / peak64, "peak_source": "fp64 DMMA.8x8x4 register loop measured live (rcvd_debug_fp64_tensor_peak); MEASURED_PEAKS.json has no fp64 figure",
-            "traffic": traffic["update"], "traffic_source": traffic["source"], "launches_per_step": int(n_g), "avg_launch_us": lin_prof["gemm_ms"] * 1e3 / n_g,
+            "frac": g_tf / peak64, "peak_source": "fastest fp64 mma.sync shape in a register loop, measured live (rcvd_debug_fp64_tensor_peak)", "peak_by_shape": peaks64,
+            "launches_per_step": int(n_g), "avg_launch_us": lin_prof["gemm_ms"] * 1e3 / n_g,
             "flops_per_launch": lin_prof["gemm_flops"] / n_g, "share_of_step_serialised": lin_prof["gemm_ms"] / max(sum(lin_prof[k] for k in ("load_ms", "potrf_ms", "trinv_ms", "trsm_ms", "gemm_ms", "solve_ms")) + acc_ms, 1e-9)}
     line = {"metric": METRIC, "value": C_total / (ms * 1e-3), "unit": "constraints/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": args.workload if not args.frames else f"{args.workload}[frames={args.frames}]", "frames": spec["frames"], "image": [spec["w"], spec["h"]],
                        "depth_grid": [spec["gx"], spec["gy"]], "match_separation": spec["sep"], "pairs": int(len(pairs)), "constraints": C_total,
                        "unknowns": int(cfg.num_frames * nf), "parallelism": (f"pair-sharded x{world}; " + ("H reduced to block owners, wide elimination levels factored by frame owners (one fused NCCL broadcast of the new factor blocks per level), narrow tail + substitution replicated" if dinfo["distributed"] else "H all-reduced, factorisation replicated")) if world > 1 else "single GPU",
-                       "distribution": dinfo, "l2_note": "H/L working set >> L2 (126 MB)",
+                       "distribution": dinfo, "l2_note": "H/L working set >> L2 (50 MB on the H100)",
                        "structure": info},
             "breakdown_ms": {"accumulate": tm["accumulate_ms"], "factor_solve": tm["linear_ms"], "candidate_cost": tm["cost_ms"], "accumulate_isolated": acc_ms},
             "linear_kernels_ms_serialised": {k: lin_prof[k] for k in ("load_ms", "potrf_ms", "trinv_ms", "trsm_ms", "gemm_ms", "solve_ms")},
@@ -392,7 +392,11 @@ def main():
     ap.add_argument("--legacy-update", action="store_true", help="A/B: round-1 cp.async update GEMM instead of the TMA-fed persistent kernel")
     ap.add_argument("--side-ipc", type=int, default=0, help="A/B: items-per-CTA cap of the overlapped (side-stream) update launches")
     ap.add_argument("--skip-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the gradient, candidate state and costs of the last timed step to DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

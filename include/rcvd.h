@@ -1,5 +1,5 @@
 /*
- * rcvd.h -- C ABI of the B200-native temporal-consistency optimizer.
+ * rcvd.h -- C ABI of the H100-native temporal-consistency optimizer.
  *
  * This is the drop-in boundary beneath the reference's `lib_python` module
  * (reference: lib/PythonBindings.cpp:170-555).  Everything the reference does

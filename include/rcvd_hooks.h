@@ -24,14 +24,19 @@ int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* 
  * assembled H), |S g|, cost, |g|_2, |y|_2, non-positive-pivot flag}: the parity evidence bench.py prints at the size it times */
 int32_t rcvd_debug_linear_residual(rcvd_problem* p, double radius, double out[6]);
 
+/* what the last rcvd_time_iteration step computed, in the caller's frame order: g = gradient at the state, xc = candidate state
+ * of the damped LM step (N*stride doubles each); out = {cost, candidate cost}.  Read it before any other call on the handle. */
+int32_t rcvd_debug_last_iteration(rcvd_problem* p, double* g, double* xc, double out[2]);
+
 /* per-kernel-class device time of one factorisation + solve: out_ms[0..5] = load, potrf, trinv, trsm, update GEMM,
  * substitution; [6] = update-GEMM launches, [7] = their algorithmic flops.  reps > 0: serialised on one stream;
  * reps < 0: two-stream overlap kept, main-stream view. */
 int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double out_ms[8]);
 /* per-level view of the last rcvd_debug_profile_linear call: out[level][6] ms of {load, potrf, trinv, trsm, update, substitution} */
 int32_t rcvd_debug_level_profile(rcvd_problem* p, double* out, int32_t max_levels);
-/* fp64 tensor-core (DMMA) peak of the device in TFLOP/s, measured live */
-int32_t rcvd_debug_fp64_tensor_peak(int32_t device, double* tflops);
+/* fp64 tensor-core (DMMA) peak of the device in TFLOP/s for one mma.sync shape (0 m8n8k4, 1 m16n8k4, 2 m16n8k8, 3 m16n8k16),
+ * measured live */
+int32_t rcvd_debug_fp64_tensor_peak(int32_t device, int32_t shape, double* tflops);
 
 /* A/B switches (defaults in parentheses) */
 int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on);        /* (1) specialised accumulate kernel */

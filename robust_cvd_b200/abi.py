@@ -1,4 +1,4 @@
-"""ctypes mirror of include/rcvd.h (the C ABI of the B200 solver).
+"""ctypes mirror of include/rcvd.h (the C ABI of the H100 solver).
 
 Struct layouts must match include/rcvd.h exactly; `tests/test_abi.py` checks
 sizes against the compiled library (`rcvd_abi_version`, `rcvd_frame_stride`).

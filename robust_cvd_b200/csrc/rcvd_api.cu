@@ -1,4 +1,4 @@
-// rcvd_api.cu -- host driver + C ABI (include/rcvd.h) of the B200 temporal-consistency solver.
+// rcvd_api.cu -- host driver + C ABI (include/rcvd.h) of the H100 temporal-consistency solver.
 //
 // Replaces ceres::Solve as called from DepthVideoPoseOptimizer::poseOptimizationStep
 // (reference lib/PoseOptimizer.cpp:954-962) and ::normalizeDepth (:1117-1125): Levenberg-
@@ -247,7 +247,7 @@ struct rcvd_problem {
   std::vector<int> uperm, iperm, fa_off, fa_cnt, fb_off, fb_cnt, tseg, bseg, hseg;   // *_off/_cnt: per-owner frame ranges (phase A / B); segs: (first, count) pairs
   int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr; int n_own_l = 0, n_own_h = 0;
   // TMA-fed persistent update kernel (rcvd_update.cuh)
-  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int upd_rb = 0, upd_neff = 0, num_sms = 148, upd_ipc = 0, upd_dbg = 0, upd_team_items = 1, upd_reserve = 0;   // upd_reserve: SMs kept free by the overlapped updates of narrow levels; upd_team_items: launches of <= that many items per SM take the two-team shape
+  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int upd_rb = 0, upd_neff = 0, num_sms = 132, upd_ipc = 0, upd_dbg = 0, upd_team_items = 1, upd_reserve = 0;   // upd_reserve: SMs kept free by the overlapped updates of narrow levels; upd_team_items: launches of <= that many items per SM take the two-team shape
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
   double upd_flops = 0.0;   // algorithmic flops of the update GEMMs of one factorisation (2 nf^3 per product, nf^2 (nf+1) on symmetric targets)
   rcvd_problem() {}
@@ -1448,6 +1448,16 @@ RCVD_API int32_t rcvd_time_iteration(rcvd_problem* p, int32_t iters, double radi
   *ms_iter = tt / iters; if (ms_acc) *ms_acc = ta / iters; if (ms_lin) *ms_lin = tl / iters; if (ms_cost) *ms_cost = tc / iters;
   return RCVD_OK;
 }
+// Bench hook: the outputs of the last rcvd_time_iteration step (gradient, candidate state, cost, candidate cost), caller's frame order.
+RCVD_API int32_t rcvd_debug_last_iteration(rcvd_problem* p, double* g, double* xc, double out[2]) {
+  if (!p || !g || !xc || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (!p->structure_ready) return set_err(RCVD_ERR_INVALID, "no iteration has run on this handle");
+  SET_DEVICE(p->device);
+  int rc = read_scalars(p); if (rc) return rc;
+  out[0] = p->h_scal[SC_COST]; out[1] = p->h_scal[SC_CAND];
+  if ((rc = download_frames(p, g, p->d_g, p->L.nf, p->L.npad, p->L.nf))) return rc;
+  return download_frames(p, xc, p->d_xc, p->L.nf, p->L.nf, p->L.nf);
+}
 // Bench hook: one factorisation + solve, un-captured on a single stream with one CUDA event per launch; returns the
 // summed device time per kernel class: out_ms[0..5] = load, potrf, trinv, trsm, update GEMM (k_gemm_nt), substitution;
 // out_ms[6] = number of k_gemm_nt update launches, out_ms[7] = algorithmic flops of those GEMMs.
@@ -1485,36 +1495,54 @@ RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double
   out_ms[7] = p->upd_flops;
   return rc;
 }
-// Bench hook: fp64 tensor-core (DMMA m8n8k4) peak of this device, measured live with a register-only loop on all SMs.
-// MEASURED_PEAKS.json carries HBM and bf16 figures only; this is the denominator of the update-GEMM roofline.
+// Bench hook: fp64 tensor-core (DMMA) peak of this device for one mma.sync shape, measured live with a register-only loop on all SMs:
+// shape 0 = m8n8k4, 1 = m16n8k4, 2 = m16n8k8, 3 = m16n8k16.  The fastest shape is the denominator of the update-GEMM roofline.
+template <int SHAPE>
 __global__ void k_dmma_peak(double* out, int iters) {
-  double c[8][2];
+  double c[8][4];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { c[i][0] = 0; c[i][1] = 0; }
+  for (int i = 0; i < 8; ++i) { c[i][0] = 0; c[i][1] = 0; c[i][2] = 0; c[i][3] = 0; }
   const double a = threadIdx.x * 1e-3, b = 1.0 + threadIdx.x * 1e-6;
   for (int it = 0; it < iters; ++it) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) dmma_8x8x4(c[i][0], c[i][1], a, b);
+    for (int i = 0; i < 8; ++i) {
+      if (SHAPE == 0) dmma_8x8x4(c[i][0], c[i][1], a, b);
+      if (SHAPE == 1) dmma_16x8x4(c[i][0], c[i][1], c[i][2], c[i][3], a, a, b);
+      if (SHAPE == 2)
+        asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%4,%4,%4}, {%5,%5}, {%0,%1,%2,%3};"
+                     : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(b));
+      if (SHAPE == 3)
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%4,%4,%4,%4,%4,%4,%4}, {%5,%5,%5,%5}, {%0,%1,%2,%3};"
+                     : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(b));
+    }
   }
   double s = 0;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1];
+  for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
   out[(size_t)blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-RCVD_API int32_t rcvd_debug_fp64_tensor_peak(int32_t device, double* tflops) {
-  if (!tflops) return set_err(RCVD_ERR_INVALID, "null argument");
+RCVD_API int32_t rcvd_debug_fp64_tensor_peak(int32_t device, int32_t shape, double* tflops) {
+  if (!tflops || shape < 0 || shape > 3) return set_err(RCVD_ERR_INVALID, "bad argument");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return set_err(RCVD_ERR_NO_DEVICE, "no usable CUDA device");
   SET_DEVICE(device);
   cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, device));
-  const int threads = 512, blocks = prop.multiProcessorCount * 4, iters = 20000;
+  const int threads = 512, blocks = prop.multiProcessorCount * 4, iters = 20000 >> shape;
+  const double flops_per_mma = 512.0 * (1 << shape);      // 2*m*n*k: 512, 1024, 2048, 4096
   double* out = nullptr; CK(cudaMalloc((void**)&out, (size_t)blocks * threads * sizeof(double)));
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   double best = 0;
   for (int rep = 0; rep < 4; ++rep) {
-    cudaEventRecord(e0); k_dmma_peak<<<blocks, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
+    cudaEventRecord(e0);
+    switch (shape) {
+      case 0: k_dmma_peak<0><<<blocks, threads>>>(out, iters); break;
+      case 1: k_dmma_peak<1><<<blocks, threads>>>(out, iters); break;
+      case 2: k_dmma_peak<2><<<blocks, threads>>>(out, iters); break;
+      default: k_dmma_peak<3><<<blocks, threads>>>(out, iters); break;
+    }
+    cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
-    const double tf = 2.0 * 256 * 8 * iters * (double)blocks * (threads / 32) / (ms * 1e-3) / 1e12;
+    const double tf = flops_per_mma * 8 * iters * (double)blocks * (threads / 32) / (ms * 1e-3) / 1e12;
     if (rep > 0 && tf > best) best = tf;
   }
   cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(out);

@@ -1,4 +1,4 @@
-// rcvd_device.cuh -- device-side math of the temporal-consistency optimizer (sm_100a).
+// rcvd_device.cuh -- device-side math of the temporal-consistency optimizer (sm_90a).
 //
 // What each function computes is fixed by the reference (file:line cited per
 // function); how it is computed is ours: analytic Jacobians in "local"

@@ -2,8 +2,8 @@
 // TMA-fed fp64 tensor-core kernel (the dominant kernel of an LM iteration at BASELINE config 2).
 //
 // The reference leaves this arithmetic to Ceres' SPARSE_NORMAL_CHOLESKY (lib/PoseOptimizer.cpp:956); here it is
-// the supernodal update step of our own factorisation (rcvd_linalg.cuh).  fp64 has no tcgen05 kind, so the MMA is
-// mma.sync.m8n8k4.f64 (DMMA); what is Blackwell-native is the data movement:
+// the supernodal update step of our own factorisation (rcvd_linalg.cuh).  wgmma has no fp64 kind, so the MMA is
+// mma.sync.m16n8k4.f64 (DMMA; two 8-row units of the warp tile per instruction); what is Hopper-native is the data movement:
 //   * operands are fetched by the TMA (cp.async.bulk.tensor.2d, one elected producer thread) straight from the
 //     row-major factor blocks into a 5-deep shared-memory ring, completion signalled on mbarriers (no cp.async
 //     groups, no __syncthreads in the K loop);
@@ -17,8 +17,8 @@
 //   * persistent CTAs (one per SM) walk a cost-sorted list of (target tile, source-pair list) work items, so the producer
 //     prefetches the next item's first stages while the DMMA warps are in the epilogue of the previous one, and a
 //     launch never has a tail of under-filled waves;
-//   * a warp issues at most one DMMA per 16 clk, so a lone 4-warp tile is latency-bound (1300 DMMAs per warp and K = 200: ~11 us,
-//     measured on the narrow-level launches of the factorisation): TWO teams of four DMMA warps take alternate K stages of the same
+//   * a single warp issues DMMAs far below the SM's rate, so a lone 4-warp tile is latency-bound (1300 DMMAs per warp at
+//     K = 200 on the narrow-level launches of the factorisation): TWO teams of four DMMA warps take alternate K stages of the same
 //     tile, team 1 hands its partial accumulators to team 0 through shared memory (named barriers, no __syncthreads) and goes on
 //     to the next item while team 0 does the read-modify-write of the target;
 //   * tiles are 80 x 80 (5 x 5 m8n8 units for each of the 2 x 2 warps: balanced), the remainder of the block last:
@@ -41,7 +41,7 @@ struct UpdItem {
 // Two shapes of the same kernel (template TEAMS):
 //   TEAMS = 1: 4 DMMA warps + producer, 5-stage ring, two CTAs per SM            -- launches with more items than the machine holds
 //   TEAMS = 2: two teams of 4 DMMA warps + producer, 8-stage ring, one CTA per SM -- launches of a few items (the narrow levels of the
-//              factorisation), where a lone 4-warp tile is bound by the one-DMMA-per-16-clk issue rate of a warp
+//              factorisation), where a lone 4-warp tile is bound by the DMMA issue rate of a single warp
 constexpr int kUpdMaxTile = 80;       // rows / columns of a CTA tile (<= 5 m8n8 units per warp and dimension)
 constexpr int kUpdPartial = 4 * 25 * 32 * 2;   // doubles: team 1's accumulators on their way to team 0
 template <int TEAMS> struct UpdShape { static constexpr int stages = TEAMS == 2 ? 8 : 5, threads = TEAMS * 128 + 32, ctas = TEAMS == 2 ? 1 : 2; };
@@ -72,6 +72,19 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
                ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
+// One k4 step of the warp tile: pairs of 8-row units as m16n8k4 (one instruction per pair and column unit), an odd last unit as m8n8k4.
+template <int NI, int NJ>
+__device__ __forceinline__ void upd_mma(const double (&af)[NI], const double (&bf)[NJ], double (&acc)[5][5][2]) {
+#pragma unroll
+  for (int i = 0; i + 1 < NI; i += 2)
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) dmma_16x8x4(acc[i][j][0], acc[i][j][1], acc[i + 1][j][0], acc[i + 1][j][1], af[i], af[i + 1], bf[j]);
+  if (NI & 1) {
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) dmma_8x8x4(acc[NI - 1][j][0], acc[NI - 1][j][1], af[NI - 1], bf[j]);
+  }
+}
+
 // One K stage (16 deep, k4n <= 4 steps of 4) of a warp's (NI*8) x (NJ*8) tile.  As/Bs: byte pointers to this lane's row inside
 // the swizzled [rb][128 B] tiles; kc[k4] = byte offset of this lane's (k4, t) element inside its row (swizzle applied).
 template <int NI, int NJ>
@@ -84,10 +97,7 @@ __device__ __forceinline__ void upd_stage(const unsigned char* __restrict__ As, 
       for (int i = 0; i < NI; ++i) af[i] = *reinterpret_cast<const double*>(As + kc[k4] + i * 1024);
 #pragma unroll
       for (int j = 0; j < NJ; ++j) bf[j] = *reinterpret_cast<const double*>(Bs + kc[k4] + j * 1024);
-#pragma unroll
-      for (int i = 0; i < NI; ++i)
-#pragma unroll
-        for (int j = 0; j < NJ; ++j) dmma_8x8x4(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+      upd_mma<NI, NJ>(af, bf, acc);
     }
   } else {
 #pragma unroll
@@ -98,10 +108,7 @@ __device__ __forceinline__ void upd_stage(const unsigned char* __restrict__ As, 
         for (int i = 0; i < NI; ++i) af[i] = *reinterpret_cast<const double*>(As + kc[k4] + i * 1024);
 #pragma unroll
         for (int j = 0; j < NJ; ++j) bf[j] = *reinterpret_cast<const double*>(Bs + kc[k4] + j * 1024);
-#pragma unroll
-        for (int i = 0; i < NI; ++i)
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) dmma_8x8x4(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+        upd_mma<NI, NJ>(af, bf, acc);
       }
     }
   }

@@ -31,7 +31,7 @@ static py::object imageToNp(const Image* img) {
 }
 
 PYBIND11_MODULE(lib_python, m) {
-  m.doc() = "B200-native drop-in for robust_cvd's lib_python (pose / depth-deformation optimizer on CUDA).";
+  m.doc() = "H100-native drop-in for robust_cvd's lib_python (pose / depth-deformation optimizer on CUDA).";
   m.def("initLib", []() {});
   m.def("logToStdout", []() { setLogToStdout(true); });
 

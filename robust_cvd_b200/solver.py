@@ -1,4 +1,4 @@
-"""Python binding (ctypes) of the C ABI in include/rcvd.h -- the B200 solver.
+"""Python binding (ctypes) of the C ABI in include/rcvd.h -- the H100 solver.
 
 `Problem` is the array-level equivalent of the reference's
 DepthVideoPoseOptimizer::poseOptimizationStep / normalizeDepth
@@ -151,6 +151,12 @@ class Problem:
         a, b, c, d = C.c_double(), C.c_double(), C.c_double(), C.c_double()
         _check(self.L.rcvd_time_iteration(self.h, C.c_int32(iters), C.c_double(radius), C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return {"iter_ms": a.value, "accumulate_ms": b.value, "linear_ms": c.value, "cost_ms": d.value}
+
+    def last_iteration(self):
+        """Bench hook: what the last time_iteration step computed -- gradient, candidate state (both [N, stride]), cost, candidate cost."""
+        g, xc, out = np.empty(self.U, np.float64), np.empty(self.U, np.float64), (C.c_double * 2)()
+        _check(self.L.rcvd_debug_last_iteration(self.h, _p(g, C.c_double), _p(xc, C.c_double), out))
+        return {"gradient": g.reshape(self.N, self.stride), "candidate_state": xc.reshape(self.N, self.stride), "cost": out[0], "candidate_cost": out[1]}
 
     def structure_info(self):
         out = (C.c_int32 * 8)()
@@ -318,8 +324,14 @@ def static_flags(masks, distance, pair_frames=None, pair_offsets=None, pair_locs
     return ps, ts, dist
 
 
-def fp64_tensor_peak(device=0):
-    """Bench hook: live-measured fp64 tensor-core (DMMA) peak of `device` in TFLOP/s."""
-    v = C.c_double()
-    _check(lib().rcvd_debug_fp64_tensor_peak(C.c_int32(device), C.byref(v)))
-    return v.value
+FP64_MMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
+
+
+def fp64_tensor_peaks(device=0):
+    """Bench hook: live-measured fp64 tensor-core (DMMA) peak of `device` in TFLOP/s for every mma.sync f64 shape."""
+    out = {}
+    for i, name in enumerate(FP64_MMA_SHAPES):
+        v = C.c_double()
+        _check(lib().rcvd_debug_fp64_tensor_peak(C.c_int32(device), C.c_int32(i), C.byref(v)))
+        out[name] = v.value
+    return out

@@ -58,3 +58,16 @@ def setup_problem(P, cfg, pairs, offs, rec, med, x, adaptive=None):
     P.set_constraints(pairs, offs, rec)
     P.set_state(x)
     return P
+
+
+def write_masked_scene(root):
+    """8-frame 128x96 synthetic scene directory with one dynamic blob per frame (0 = dynamic, 255 = static) so that the static flag
+    matters; the scene of tests/test_host.py and of the recorded pose_optimization.py trace (tests/golden/make_golden.py)."""
+    from robust_cvd_b200 import synthetic, synthetic_files
+    sc = synthetic.Scene(8, 128, 96, seed=3)
+    rng = np.random.default_rng(5)
+    masks = []
+    for i in range(sc.N):
+        m = np.full((96, 128), 255, np.uint8); cx, cy = rng.integers(30, 100), rng.integers(30, 70); m[cy - 8:cy + 8, cx - 10:cx + 10] = 0; masks.append(m)
+    pairs = synthetic_files.write_scene(sc, root, dynamic_masks=masks)
+    return sc, pairs, masks

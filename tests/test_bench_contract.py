@@ -19,8 +19,8 @@ def test_workloads_follow_baseline_configs():
     spec2 = wl["config2_300f_384x224_grid16x12_sep10"]
     assert (spec2["frames"], spec2["w"], spec2["h"], spec2["gx"], spec2["gy"], spec2["sep"]) == (300, 384, 224, 16, 12, 10)      # configs[1]
     assert wl["config3_300f_384x224_grid16x12_sep10_maskratio0.20"]["mask_ratio"] == 0.20                                       # configs[2]
-    s4 = wl["config4_1000f_640x384_grid32x24_sep10_huber"]
-    assert (s4["frames"], s4["w"], s4["h"], s4["gx"], s4["gy"]) == (1000, 640, 384, 32, 24) and s4["cfg"]["robust_type"] == bench.abi.ROBUST_HUBER   # configs[3]
+    s4 = wl["config4_600f_640x384_grid32x24_sep10_huber"]
+    assert (s4["frames"], s4["w"], s4["h"], s4["gx"], s4["gy"]) == (600, 640, 384, 32, 24) and s4["cfg"]["robust_type"] == bench.abi.ROBUST_HUBER   # configs[3]
     assert wl["config5_300f_384x224_grid16x12_sep10_holes50_dolly"]["scene"]["hole_fraction"] > 0                                # configs[4]
     # config 1 builds in a blink: records, pair list and medians have consistent shapes; the overlap filter and the holes act
     spec, sc, cfg, pairs, offs, rec, med = bench.build_case("config1_8f_128x96_grid4x4_sep10")

@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle on identical inputs.
-Run on the B200 box with `pytest -m gpu`."""
+Run on an H100 with `pytest -m gpu`."""
 import numpy as np
 import pytest
 
@@ -295,3 +295,22 @@ def test_cuda_residuals_vanish_on_reference_python_correspondences():
         cost = cost[0] if isinstance(cost, tuple) else cost
         assert 0.0 <= cost < 2 * n * 3 * (5e-6) ** 2, (loss, cost)
         G.close()
+
+
+def test_last_iteration_returns_what_the_timed_step_computed():
+    """rcvd_debug_last_iteration (bench.py --dump-outputs): gradient and cost of the last timed LM step equal an evaluation at the same
+    state (npad -> stride packing, caller's frame order); the candidate state is that state plus a finite, non-zero step."""
+    from robust_cvd_b200 import solver
+    sc, cfg, pairs, offs, rec, med = helpers.make_case(num_frames=8, depth_type=abi.DEPTH_GRID, depth_grid_x=4, depth_grid_y=4)
+    off_d, nd = helpers.layout_numbers(cfg)
+    G = solver.Problem(cfg)
+    x = helpers.initial_state(sc, cfg, G.stride, off_d, nd)
+    helpers.setup_problem(G, cfg, pairs, offs, rec, med, x)
+    G.time_iteration(iters=1)
+    it = G.last_iteration()
+    c, g = G.evaluate(True)
+    assert it["gradient"].shape == it["candidate_state"].shape == (cfg.num_frames, G.stride)
+    assert abs(it["cost"] - c) <= 1e-12 * abs(c)
+    np.testing.assert_allclose(it["gradient"].ravel(), g, rtol=0, atol=1e-9 * np.abs(g).max())
+    step = it["candidate_state"] - G.get_state()
+    assert np.isfinite(step).all() and np.abs(step).max() > 0 and np.isfinite(it["candidate_cost"])

@@ -79,5 +79,5 @@ def test_config2_300_frames_matches_oracle():
 
 
 def test_large_block_path_40_frames_grid32x24_matches_oracle():
-    info = _check_case("config4_1000f_640x384_grid32x24_sep10", 40, lm_iters=3)
+    info = _check_case("config4_600f_640x384_grid32x24_sep10", 40, lm_iters=3)
     assert info["npad"] > 224

@@ -15,6 +15,7 @@ sys.path.insert(0, os.path.join(ROOT, "robust_cvd_b200", "host"))
 lp = pytest.importorskip("lib_python")
 from robust_cvd_b200 import abi, synthetic, synthetic_files  # noqa: E402
 from oracle import host_ref  # noqa: E402
+from tests.helpers import write_masked_scene  # noqa: E402
 
 CV_32FC3, CV_8UC1 = 21, 0
 
@@ -29,12 +30,7 @@ def _host_constraint_builder(monkeypatch):
 @pytest.fixture(scope="module")
 def scene_dir(tmp_path_factory):
     root = str(tmp_path_factory.mktemp("scene8"))
-    sc = synthetic.Scene(8, 128, 96, seed=3)
-    rng = np.random.default_rng(5)
-    masks = []
-    for i in range(sc.N):           # a dynamic blob (0 = dynamic, 255 = static) so that the static flag matters
-        m = np.full((96, 128), 255, np.uint8); cx, cy = rng.integers(30, 100), rng.integers(30, 70); m[cy - 8:cy + 8, cx - 10:cx + 10] = 0; masks.append(m)
-    pairs = synthetic_files.write_scene(sc, root, dynamic_masks=masks)
+    sc, pairs, masks = write_masked_scene(root)
     return sc, root, pairs, masks
 
 
@@ -356,35 +352,54 @@ def test_grid_split_resamples_bilinearly(scene_dir):
     assert abs(f.intrinsics.hFov - 2 * np.arctan(np.float32(0.3461538376301239))) < 1e-6
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/pose_optimization.py"), reason="reference checkout only exists in the build container")
 def test_reference_pose_optimization_py_runs_unchanged_up_to_the_solve(scene_dir):
-    """The reference's own pose_optimization.py, unmodified, against our lib_python: everything up to the
-    device solve runs here; the solve itself must refuse to run without a GPU (no CPU fallback)."""
-    import importlib, types
+    """The reference's own pose_optimization.py against our lib_python, as recorded in tests/golden/pose_optimization_calls.json (every
+    name it looks up, every field it writes -- convert_opt_params sets all 31 DepthVideoPoseOptimizer.Params fields -- and every call,
+    in order): PoseOptimizer(...) writes video.dat and flow_constraints.dat; optimize_poses() reaches its first solve, which must refuse
+    to run without a GPU (no CPU fallback)."""
+    import json
     sc, root, pairs, masks = scene_dir
-    for f in ("flow_constraints.dat",):
-        if os.path.exists(f"{root}/{f}"): os.remove(f"{root}/{f}")
-    sys.path.insert(0, "/root/reference")
-    try:
-        po = importlib.import_module("pose_optimization")
-        from utils.helpers import Nestedspace
-        dflt = lp.DepthVideoPoseOptimizer.Params()
-        o = Nestedspace()
-        for k, v in dict(max_iterations=50, num_threads=12, num_steps=4, robustness=0.5, static_loss_type="ReproDisparity", static_spatial_weight=1.0,
-                         static_depth_weight=1.0, smooth_loss_type="ReproDisparityLaplacian", smooth_static_weight=0.0, smooth_dynamic_weight=0.0,
-                         position_regularization=0.0, scale_regularization=1.0, scale_regularization_grid_size=10, deformation_regularization_initial=1.0,
-                         deformation_regularization_final=0.1, adaptive_deformation_cost=0.0, spatial_deformation_regularization=1.0,
-                         graduate_deformation_regularization=False, focal_regularization=1.0, coarse_to_fine=True, ctf_long=dflt.ctfLong, ctf_short=dflt.ctfShort,
-                         deferred_spatial_opt=False, dso_long=4, dso_short=3, focal_long=dflt.focalLong, intr_opt="PerFrame", fix_poses=False,
-                         fix_depth_transforms=False, fix_spatial_transforms=False, use_global_scale=False, dynamic_constraints="Mask").items():
-            setattr(o, k, v)
-        opt = po.PoseOptimizer(root, "midas2", list(range(8)), o)
-        assert os.path.exists(f"{root}/flow_constraints.dat") and os.path.exists(f"{root}/video.dat")
-        import torch
-        if not torch.cuda.is_available():
-            with pytest.raises(RuntimeError, match="no CPU fallback|no usable CUDA device"):
-                opt.optimize_poses()
-    finally:
-        sys.path.remove("/root/reference")
-        for m in [k for k in sys.modules if k == "pose_optimization" or k.startswith("utils")]:
-            sys.modules.pop(m, None)
+    if os.path.exists(f"{root}/flow_constraints.dat"):
+        os.remove(f"{root}/flow_constraints.dat")
+    events = json.load(open(os.path.join(ROOT, "tests", "golden", "pose_optimization_calls.json")))["events"]
+    objs = [lp]
+
+    def val(e):
+        if "ref" in e:
+            return objs[e["ref"]]
+        if "path" in e:
+            return root + e["path"]
+        if "list" in e:
+            return [val(x) for x in e["list"]]
+        return e["lit"]
+
+    def keep(out, r):
+        if "ref" in out:
+            assert out["ref"] == len(objs)
+            objs.append(r)
+        elif isinstance(out["lit"], float):
+            assert r == pytest.approx(out["lit"], rel=1e-6)
+        else:
+            assert r == out["lit"], (out, r)
+
+    for ev in events:
+        o = objs[ev["obj"]]
+        if ev["op"] == "get":
+            keep(ev["out"], getattr(o, ev["name"]))
+        elif ev["op"] == "set":
+            setattr(o, ev["name"], val(ev["value"]))
+            if "lit" in ev["value"]:
+                keep(ev["value"], getattr(o, ev["name"]))
+        elif "raises" in ev:
+            import torch
+            if torch.cuda.is_available():
+                o(*[val(a) for a in ev["args"]])
+            else:
+                with pytest.raises(RuntimeError, match="no CPU fallback|no usable CUDA device"):
+                    o(*[val(a) for a in ev["args"]])
+            break
+        else:
+            keep(ev["out"], o(*[val(a) for a in ev["args"]]))
+    else:
+        pytest.fail("the recorded sequence ends without reaching the solve")
+    assert os.path.exists(f"{root}/flow_constraints.dat") and os.path.exists(f"{root}/video.dat")

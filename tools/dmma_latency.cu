@@ -1,6 +1,6 @@
-// DMMA (mma.sync m8n8k4 f64) issue behaviour of a single warp / few warps per SM sub-core on sm_100a:
+// DMMA (mma.sync m8n8k4 f64) issue behaviour of a single warp / few warps per SM sub-core on sm_90a:
 // cycles per DMMA for W warps per CTA (one CTA per SM) with ACC independent accumulators each, and DFMA for comparison.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/dmma_latency.bin tools/dmma_latency.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/dmma_latency.bin tools/dmma_latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 template <int ACC> __global__ void k(double* out, long long* cyc, int iters) {
@@ -40,16 +40,17 @@ template <int ACC> __global__ void kf(double* out, long long* cyc, int iters) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
   if (threadIdx.x == 0 && blockIdx.x == 0) *cyc = t1 - t0;
 }
-template <int ACC> void run(int warps, double* out, long long* dc) {
+template <int ACC> void run(int sms, int warps, double* out, long long* dc) {
   const int iters = 2000; long long c = 0;
-  k<ACC><<<148, warps * 32>>>(out, dc, iters); cudaDeviceSynchronize(); cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
+  k<ACC><<<sms, warps * 32>>>(out, dc, iters); cudaDeviceSynchronize(); cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
   printf("DMMA  warps/CTA=%2d acc=%2d: %.1f cycles per DMMA per warp\n", warps, ACC, (double)c / (iters * ACC));
-  kf<ACC><<<148, warps * 32>>>(out, dc, iters); cudaDeviceSynchronize(); cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
+  kf<ACC><<<sms, warps * 32>>>(out, dc, iters); cudaDeviceSynchronize(); cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
   printf("DFMA  warps/CTA=%2d acc=%2d: %.1f cycles per DFMA per warp\n", warps, ACC, (double)c / (iters * ACC));
 }
 int main() {
-  double* out; long long* dc; cudaMalloc(&out, 148 * 1024 * 8); cudaMalloc(&dc, 8);
-  for (int w : {1, 4, 8, 16, 32}) { run<1>(w, out, dc); run<4>(w, out, dc); run<16>(w, out, dc); }
+  int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  double* out; long long* dc; cudaMalloc(&out, (size_t)sms * 1024 * 8); cudaMalloc(&dc, 8);
+  for (int w : {1, 4, 8, 16, 32}) { run<1>(sms, w, out, dc); run<4>(sms, w, out, dc); run<16>(sms, w, out, dc); }
   printf("%s\n", cudaGetErrorString(cudaGetLastError()));
   return 0;
 }

@@ -1,7 +1,7 @@
 // fp64 tensor-core (DMMA m8n8k4) throughput on register / shared-memory operand patterns that a real GEMM inner loop has.
 // The round-1 peak probe (rcvd_debug_fp64_tensor_peak) multiplies the SAME a, b registers into 8 accumulators; a GEMM warp tile of
 // NI x NJ units feeds NI + NJ distinct fragments into NI * NJ accumulators and reloads them from shared memory every 4 k.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/dmma_patterns.bin tools/dmma_patterns.cu && tools/dmma_patterns.bin
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/dmma_patterns.bin tools/dmma_patterns.cu && tools/dmma_patterns.bin
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {

@@ -1,5 +1,5 @@
 // fp64 peak microbenchmark for the roofline denominators (SURVEY.md section 8d): DFMA (SIMT) and
-// DMMA m8n8k4 (tensor) throughput on all SMs.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_peak fp64_peak.cu
+// DMMA m8n8k4 (tensor) throughput on all SMs.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peak fp64_peak.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k_dfma(double* out, int iters) {
@@ -23,11 +23,12 @@ __global__ void k_dmma(double* out, int iters) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 int main() {
-  double* out; cudaMalloc(&out, 148 * 8 * 1024 * sizeof(double));
+  int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  double* out; cudaMalloc(&out, (size_t)sms * 8 * 1024 * sizeof(double));
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   const int iters = 20000;
   for (int threads : {256, 512, 1024}) {
-    const int blocks = 148 * (2048 / threads);
+    const int blocks = sms * (2048 / threads);
     for (int rep = 0; rep < 2; ++rep) {
       cudaEventRecord(e0); k_dfma<<<blocks, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
       float ms; cudaEventElapsedTime(&ms, e0, e1);

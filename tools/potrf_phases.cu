@@ -1,5 +1,5 @@
 // Cycle breakdown of k_potrf_smem (one CTA, npad = 208) from thread 0's point of view.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -DRCVD_POTRF_PHASES -I include -I robust_cvd_b200/csrc -o /tmp/potrf_phases tools/potrf_phases.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -DRCVD_POTRF_PHASES -I include -I robust_cvd_b200/csrc -o tools/potrf_phases.bin tools/potrf_phases.cu
 #include <cstdio>
 #include <vector>
 #include <cmath>
