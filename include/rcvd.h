@@ -255,6 +255,34 @@ int32_t rcvd_flow_guided_filter(const rcvd_filter_params* prm, int32_t device, c
                                 const float* fwd_flow, const uint8_t* fwd_mask, const float* bwd_flow, const uint8_t* bwd_mask,
                                 const int32_t* far_pairs, const float* far_flow, const uint8_t* far_mask, float* out);
 
+/* ---- joint depth / colour bilateral depth filter (DESIGN.md section 1 row 8f-5) ----
+ * Replaces DepthVideoProcessor::bilateralFilter (lib/Processor.cpp:183-313) for any set of output frames in one call.
+ * Arrays are indexed by a local frame index 0..num_frames-1 where index 0 is the absolute frame
+ * max(0, min(range) - frame_radius) and the last is min(numFrames - 1, max(range) + frame_radius): clamping a temporal window to
+ * this stack is then the reference's clamping to the video.
+ *   depth        [num_frames][height][width] f32   transformed depth of depth stream 0 (DepthFrame::depth())
+ *   color_bgr    [num_frames][height][width][3] f32 "down" colour stream (BGR); read only when color_sigma > 0, may be NULL otherwise
+ *   out_frames   [num_out] i32  ascending local indices of the frames to filter
+ *   xform_cfg    dense depth-transform configuration of stream 0 (num_frames = 1, as for rcvd_depth_apply) and
+ *   xform_params [num_frames][k] f64 each frame's depth-transform parameters: read only when in_place and frame_radius > 0
+ *   out          [num_out][height][width] f32  filtered depth (the raw image the reference passes to setDepth)
+ * in_place: the output goes back into stream 0 (Params::depthStream == 0).  The reference then reads, for a frame g after an output
+ * frame f, xform_f(filtered_f) instead of f's original depth; this call reproduces that by filtering the output frames one after the
+ * other and rewriting each filtered frame's slot of the stack with its transform.  Otherwise all frames are filtered in one launch.
+ * median: at most 4096 samples per pixel (min(2r+1, width) * min(2r+1, height) * min(2 frame_radius + 1, num_frames));
+ * larger windows fail with RCVD_ERR_INVALID.  The mean has no limit. */
+typedef struct rcvd_bilateral_params {
+  int32_t num_frames, width, height, num_out;
+  int32_t frame_radius;   /* Params::frameRadius (lib/Processor.h:68) */
+  int32_t spatial_radius; /* Params::spatialRadius */
+  int32_t median;         /* Params::median: 0 weighted mean, 1 weighted median */
+  float depth_sigma;      /* Params::depthSigma: depth range term when > 0 */
+  float color_sigma;      /* Params::colorSigma: colour range term when > 0 */
+  int32_t in_place;       /* Params::depthStream == 0 */
+} rcvd_bilateral_params;
+int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t device, const float* depth, const float* color_bgr,
+                              const int32_t* out_frames, const rcvd_config* xform_cfg, const double* xform_params, float* out);
+
 /* ---- GPU flow-constraint builder (SURVEY.md section 8f-2) ----
  * Replaces FlowConstraintsCollection::compute (lib/FlowConstraints.cpp:401-550: admission tests, cv::cornerMinEigenVal
  * priorities) and sampleConstraints (:352-397: greedy disc sampler) for a batch of frame pairs and frame triplets.

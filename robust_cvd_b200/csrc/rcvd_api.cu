@@ -23,6 +23,7 @@
 #include "rcvd_update.cuh"
 #include "rcvd_dense.cuh"
 #include "rcvd_filter.cuh"
+#include "rcvd_bilateral.cuh"
 #include "rcvd_builder.cuh"
 static int64_t g_filter_launches = 0;
 
@@ -1811,6 +1812,114 @@ RCVD_API int32_t rcvd_flow_guided_filter(const rcvd_filter_params* prm, int32_t 
   return rc;
 }
 RCVD_API int64_t rcvd_filter_launch_count() { return g_filter_launches; }
+
+// ---------------------------------------------------------------------------
+// Joint depth / colour bilateral filter (rcvd_bilateral.cuh)
+// ---------------------------------------------------------------------------
+RCVD_API int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t device, const float* depth, const float* color_bgr,
+                                       const int32_t* out_frames, const rcvd_config* xform_cfg, const double* xform_params, float* out) {
+  if (!prm || !depth || !out_frames || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_bilateral_params& q = *prm;
+  const int F = q.num_frames;
+  if (F <= 0 || q.width <= 0 || q.height <= 0 || q.num_out <= 0 || q.frame_radius < 0 || q.spatial_radius < 0 || (q.median != 0 && q.median != 1))
+    return set_err(RCVD_ERR_INVALID, "bad bilateral filter parameters");
+  for (int i = 0; i < q.num_out; ++i)
+    if (out_frames[i] < 0 || out_frames[i] >= F || (i > 0 && out_frames[i] <= out_frames[i - 1]))
+      return set_err(RCVD_ERR_INVALID, "output frames must be ascending local indices in [0, num_frames)");
+  const bool color = q.color_sigma > 0.f;
+  if (color && !color_bgr) return set_err(RCVD_ERR_INVALID, "color_sigma > 0 needs the colour stack");
+  // in place, a later output frame reads xform(filtered) of the frames before it (the reference writes into the stream it reads)
+  const bool recur = q.in_place != 0 && q.frame_radius > 0;
+  Layout L{};
+  if (recur) {
+    if (!xform_cfg || !make_layout(*xform_cfg, L)) return set_err(RCVD_ERR_INVALID, "in-place filtering needs a supported depth-transform configuration");
+    if (L.nd > 0 && !xform_params) return set_err(RCVD_ERR_INVALID, "in-place filtering needs the per-frame depth-transform parameters");
+  }
+  const long long r = q.spatial_radius, fr = q.frame_radius;
+  const long long max_samples = std::min<long long>(2 * r + 1, q.width) * std::min<long long>(2 * r + 1, q.height) * std::min<long long>(2 * fr + 1, F);
+  if (q.median && max_samples > kBilateralMaxSamples)
+    return set_err(RCVD_ERR_INVALID, "the weighted median supports at most %d samples per pixel; this window has %lld", kBilateralMaxSamples, max_samples);
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
+    return set_err(RCVD_ERR_NO_DEVICE, "no usable CUDA device (%s); this library has no CPU fallback", e != cudaSuccess ? cudaGetErrorString(e) : "device ordinal out of range");
+  SET_DEVICE(device);
+  const size_t plane = (size_t)q.width * q.height;
+  // launch geometry and shared memory
+  BilateralArgs a{};
+  a.F = F; a.w = q.width; a.h = q.height; a.frame_radius = q.frame_radius; a.radius = q.spatial_radius;
+  a.use_depth = q.depth_sigma > 0.f; a.depth_sigma = q.depth_sigma; a.color_sigma = q.color_sigma;
+  size_t smem = 0; bool staged = false;
+  if (q.median) {
+    a.P = 32; while (a.P < max_samples) a.P <<= 1;
+    smem = (size_t)kBfMedianWarps * a.P * sizeof(unsigned long long);
+  } else {
+    a.sw = kBfTx + 2 * q.spatial_radius; a.sh = kBfTy + 2 * q.spatial_radius;
+    const size_t bytes = 2 * (size_t)a.sw * a.sh * (color ? 4 : 1) * sizeof(float);   // two frame buffers
+    staged = bytes <= 200 * 1024;
+    smem = staged ? bytes : 0;
+  }
+  auto launch_filter = [&](cudaStream_t s, int base, int n) {
+    a.out_base = base;
+    if (q.median) {
+      const dim3 grid((unsigned)((plane + kBfMedianWarps - 1) / kBfMedianWarps), 1, n);
+      if (color) k_bilateral_median<true><<<grid, 32 * kBfMedianWarps, smem, s>>>(a); else k_bilateral_median<false><<<grid, 32 * kBfMedianWarps, smem, s>>>(a);
+    } else {
+      const dim3 grid((q.width + kBfTx - 1) / kBfTx, (q.height + kBfTy - 1) / kBfTy, n);
+      if (color) { if (staged) k_bilateral_mean<true, true><<<grid, kBfTx * kBfTy, smem, s>>>(a); else k_bilateral_mean<true, false><<<grid, kBfTx * kBfTy, 0, s>>>(a); }
+      else { if (staged) k_bilateral_mean<false, true><<<grid, kBfTx * kBfTy, smem, s>>>(a); else k_bilateral_mean<false, false><<<grid, kBfTx * kBfTy, 0, s>>>(a); }
+    }
+    g_filter_launches++;
+  };
+  if (smem > 48 * 1024) {
+    const void* fn = q.median ? (color ? (const void*)k_bilateral_median<true> : (const void*)k_bilateral_median<false>)
+                              : (color ? (const void*)k_bilateral_mean<true, true> : (const void*)k_bilateral_mean<false, true>);
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  // per-frame transform vectors in the dense kernel's frame layout (depth parameters at offD)
+  std::vector<double> pv;
+  if (recur) {
+    pv.assign((size_t)F * L.nf, 0.0);
+    for (int f = 0; f < F; ++f) for (int i = 0; i < L.nd; ++i) pv[(size_t)f * L.nf + L.offD + i] = xform_params[(size_t)f * L.nd + i];
+  }
+  cudaStream_t st; CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  std::vector<void*> bufs; bool ok = true;
+  // every allocation is checked before the first launch (an illegal address is a sticky context error, and PyTorch shares this context)
+  auto dev = [&](size_t bytes) -> void* { void* ptr = nullptr; if (cudaMallocAsync(&ptr, std::max<size_t>(bytes, 16), st) != cudaSuccess) { ok = false; cudaGetLastError(); return nullptr; } bufs.push_back(ptr); return ptr; };
+  auto up = [&](const void* src, size_t bytes) -> void* { void* d = dev(bytes); if (d && src && bytes) cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, st); return d; };
+  float* d_depth = (float*)up(depth, (size_t)F * plane * 4);
+  a.depth = d_depth;
+  a.color = color ? (const float*)up(color_bgr, (size_t)F * plane * 12) : nullptr;
+  a.out_frames = (const int*)up(out_frames, (size_t)q.num_out * 4);
+  a.out = (float*)dev((size_t)q.num_out * plane * 4);
+  const double* d_pv = recur ? (const double*)up(pv.data(), pv.size() * 8) : nullptr;
+  int rc = RCVD_OK;
+  if (!ok) rc = set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_bilateral_filter");
+  else {
+    float* const out_dev = a.out;
+    if (recur) {
+      // frame-sequential: filter output o, then rewrite its slot of the depth stack with xform_o(filtered) for the frames after it
+      for (int o = 0; o < q.num_out; ++o) {
+        a.out = out_dev + (size_t)o * plane;
+        launch_filter(st, o, 1);
+        const int f = out_frames[o];
+        k_dense<0><<<nblk(plane), 256, 0, st>>>(*xform_cfg, L, d_pv + (size_t)f * L.nf, a.out, d_depth + (size_t)f * plane, q.height, q.width);
+      }
+    } else {
+      for (int o = 0; o < q.num_out; o += 65535) {   // grid.z limit
+        a.out = out_dev + (size_t)o * plane;
+        launch_filter(st, o, std::min(65535, q.num_out - o));
+      }
+    }
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, out_dev, (size_t)q.num_out * plane * 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) rc = set_err(RCVD_ERR_CUDA, "bilateral filter failed: %s", cudaGetErrorString(e));
+  }
+  for (void* b : bufs) cudaFreeAsync(b, st);
+  cudaStreamSynchronize(st); cudaStreamDestroy(st);
+  return rc;
+}
 
 // ---------------------------------------------------------------------------
 // GPU flow-constraint builder (rcvd_builder.cuh)

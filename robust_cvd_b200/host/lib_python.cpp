@@ -228,7 +228,8 @@ PYBIND11_MODULE(lib_python, m) {
       .value("ResetNormalizeOptimize", Op::ResetNormalizeOptimize);
   dvp.def(py::init<DepthVideo*>(), py::keep_alive<1, 2>())
       .def("process", &DepthVideoProcessor::process).def("gridXformSplit", &DepthVideoProcessor::gridXformSplit)
-      .def("reset", &DepthVideoProcessor::reset).def("copy", &DepthVideoProcessor::copy).def("flowGuidedFilter", &DepthVideoProcessor::flowGuidedFilter)
+      .def("reset", &DepthVideoProcessor::reset).def("copy", &DepthVideoProcessor::copy).def("bilateralFilter", &DepthVideoProcessor::bilateralFilter)
+      .def("flowGuidedFilter", &DepthVideoProcessor::flowGuidedFilter)
       .def("resetPoses", &DepthVideoProcessor::resetPoses).def("resetDepthXforms", &DepthVideoProcessor::resetDepthXforms)
       .def("resetSpatialXforms", &DepthVideoProcessor::resetSpatialXforms)
       .def("normalizeDepth", &DepthVideoProcessor::normalizeDepth).def("optimizePoses", &DepthVideoProcessor::optimizePoses);

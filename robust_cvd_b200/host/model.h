@@ -146,6 +146,7 @@ class Xform {
 };
 void fillDepthConfig(const XformDescriptor& d, rcvd_config& cfg);
 void fillSpatialConfig(const XformDescriptor& d, rcvd_config& cfg);
+void denseConfig(const XformDescriptor& d, rcvd_config& cfg);   // one-frame configuration of the dense kernels (Xform::apply etc.)
 
 // --- DepthPhoto::Intrinsics / Extrinsics (lib/DepthPhoto.{h,cpp}) ---
 struct Extrinsics {
@@ -381,6 +382,7 @@ class DepthVideoProcessor {
   void process(const Params& params);
   void reset(const Params& params);               // lib/Processor.cpp:146-150
   void copy(const Params& params);                // :152-180
+  void bilateralFilter(const Params& params);     // :183-313, on the GPU (rcvd_bilateral_filter)
   void flowGuidedFilter(const Params& params);    // :315-590, on the GPU (rcvd_flow_guided_filter)
   void gridXformSplit(const Params& params);      // lib/Processor.cpp:888-985
   void resetPoses(const Params& params);          // :987-1003

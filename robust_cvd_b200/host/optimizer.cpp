@@ -310,8 +310,7 @@ void DepthVideoProcessor::process(const Params& params) {   // lib/Processor.cpp
     case Op::Reset: reset(params); break;
     case Op::Copy: copy(params); break;
     case Op::FlowGuidedFilter: flowGuidedFilter(params); break;
-    case Op::BilateralFilter:
-      throw std::runtime_error("The bilateral depth filter is outside the pose-optimization path and is not implemented in this build.");
+    case Op::BilateralFilter: bilateralFilter(params); break;
     default: throw std::runtime_error("Unsupported operation selected.");
   }
 }
@@ -329,6 +328,76 @@ void DepthVideoProcessor::copy(const Params& params) {   // :152-180
     if (!depth) throw std::runtime_error("Source depth frame " + std::to_string(frame) + " has no depth image.");
     dst.setDepth(*depth);
     dst.intrinsics = src.intrinsics; dst.extrinsics = src.extrinsics;
+  }
+}
+// Joint depth / colour bilateral filter (:183-313).  The reference filters frame by frame on the CPU, reading its guides from depth
+// stream 0 and the "down" colour stream; here the host gathers the frames the temporal windows of the range reach once and one call
+// (rcvd_bilateral_filter, csrc/rcvd_bilateral.cuh) filters every frame of the range.  Everything that can be wrong with the inputs is
+// checked on the host images before the first device call.
+void DepthVideoProcessor::bilateralFilter(const Params& params) {
+  struct Trim { ~Trim() { rcvd_trim_device_memory(currentDevice()); } } trimAtExit;
+  logInfo("Applying bilateral filter...");
+  if (params.depthStream < 0 || params.depthStream >= video_->numDepthStreams()) throw std::runtime_error("Depth stream out of range.");
+  ColorStream& cs = video_->colorStream("down");
+  const int N = video_->numFrames();
+  FrameRange range = params.frameRange; range.resolve(N);   // an empty range is every frame
+  const int first = range.firstFrame(), last = range.lastFrame();
+  if (params.frameRadius < 0 || params.spatialRadius < 0) throw std::runtime_error("Filter radii must not be negative.");
+  DepthStream& ds = video_->depthStream(0);
+  // the stack: every frame a temporal window of the range reaches (clamping to it is the reference's clamping to the video)
+  const int base = std::max(0, first - params.frameRadius), F = std::min(N - 1, last + params.frameRadius) - base + 1;
+  const bool useColor = params.colorSigma > 0.f;
+  if (useColor && cs.type() != cvMakeType(CV_32F, 3)) throw std::runtime_error("The bilateral filter needs the 'down' color stream as CV_32FC3.");
+  int w = -1, h = -1;
+  for (int i = 0; i < F; ++i) {
+    const Image* s = ds.frame(base + i).sourceDepth();   // depth() exists exactly when the source depth does, with its size
+    if (!s) throw std::runtime_error("Depth frame " + std::to_string(base + i) + " of depth stream 0 has no depth image.");
+    if (w < 0) { w = s->cols; h = s->rows; }
+    if (s->cols != w || s->rows != h) throw std::runtime_error("Depth frame has inconsistent dimensions.");
+    if (useColor) {
+      const Image* c = cs.frame(base + i).image();
+      if (!c) throw std::runtime_error("Color frame " + std::to_string(base + i) + " of stream 'down' is missing.");
+      if (c->type != cvMakeType(CV_32F, 3)) throw std::runtime_error("The bilateral filter needs the 'down' color stream as CV_32FC3.");
+      if (c->cols != w || c->rows != h) throw std::runtime_error("Color frame " + std::to_string(base + i) + " and depth frame differ in size.");
+    }
+  }
+  // in place with a temporal window, later frames see xform(filtered) of earlier ones: the kernel re-applies each frame's transform
+  const bool inPlace = params.depthStream == 0, recur = inPlace && params.frameRadius > 0;
+  rcvd_config cfg{}; std::vector<double> xp;
+  if (recur) {
+    const XformDescriptor& desc = ds.frame(base).depthXform().desc();
+    denseConfig(desc, cfg);
+    if (rcvd_frame_stride(&cfg) < 0) throw std::runtime_error("Unsupported depth transform for the in-place bilateral filter.");
+    const int nd = rcvd_spatial_param_offset(&cfg) - rcvd_depth_param_offset(&cfg);
+    xp.resize(size_t(F) * nd);
+    for (int i = 0; i < F; ++i) {
+      const Xform& x = ds.frame(base + i).depthXform();
+      if (x.desc() != desc || x.numParams() != nd) throw std::runtime_error("The frames' depth transforms differ in type.");
+      std::copy(x.params().begin(), x.params().end(), xp.begin() + size_t(i) * nd);
+    }
+  }
+  std::vector<float> depth(size_t(F) * w * h), color(useColor ? size_t(F) * w * h * 3 : 0);
+  for (int i = 0; i < F; ++i) {
+    const Image* d = ds.frame(base + i).depth();
+    std::memcpy(depth.data() + size_t(i) * w * h, d->ptr<float>(), size_t(w) * h * sizeof(float));
+    if (useColor) std::memcpy(color.data() + size_t(i) * w * h * 3, cs.frame(base + i).image()->ptr<float>(), size_t(w) * h * 3 * sizeof(float));
+  }
+  std::vector<int32_t> outFrames;
+  for (int f : range.frames) outFrames.push_back(f - base);
+  rcvd_bilateral_params prm{};
+  prm.num_frames = F; prm.width = w; prm.height = h; prm.num_out = int(outFrames.size());
+  prm.frame_radius = params.frameRadius; prm.spatial_radius = params.spatialRadius; prm.median = params.median ? 1 : 0;
+  prm.depth_sigma = params.depthSigma; prm.color_sigma = params.colorSigma; prm.in_place = inPlace ? 1 : 0;
+  const size_t plane = size_t(w) * h;
+  std::vector<float> out(size_t(prm.num_out) * plane);
+  const int rc = rcvd_bilateral_filter(&prm, currentDevice(), depth.data(), useColor ? color.data() : nullptr, outFrames.data(),
+                                       recur ? &cfg : nullptr, recur ? xp.data() : nullptr, out.data());
+  if (rc != RCVD_OK) throw std::runtime_error(std::string("bilateral filter failed: ") + rcvd_last_error());
+  DepthStream& dstDs = video_->depthStream(params.depthStream);
+  for (int i = 0; i < prm.num_out; ++i) {
+    Image img; img.create(h, w, cvMakeType(CV_32F, 1));
+    std::memcpy(img.ptr<float>(), out.data() + size_t(i) * plane, plane * sizeof(float));
+    dstDs.frame(base + outFrames[i]).setDepth(img);
   }
 }
 // Flow-guided temporal filter (:315-590).  The reference walks frame by frame and pixel by pixel on the CPU; here the host

@@ -275,7 +275,28 @@ def flow_guided_filter(depth, cams, fwd_flow, fwd_mask, bwd_flow, bwd_mask, firs
     return out
 
 
-def build_constraints(color_bgr, pair_frames, pair_flow, pair_mask, match_separation, inv_aspect, dyn_dist=None, min_dynamic_distance=-1.0,
+def bilateral_filter(depth, out_frames, color_bgr=None, frame_radius=2, spatial_radius=0, depth_sigma=0.3, color_sigma=0.0, median=False,
+                     in_place=False, xform_cfg=None, xform_params=None, device=0):
+    """rcvd_bilateral_filter (DepthVideoProcessor::bilateralFilter, reference lib/Processor.cpp:183-313) on the GPU.
+    depth [F,h,w] f32, out_frames ascending local indices, color_bgr [F,h,w,3] f32 (needed when color_sigma > 0) -> [num_out,h,w] f32.
+    in_place with frame_radius > 0 feeds each filtered frame, through its depth transform (xform_cfg, xform_params [F,k] f64), to the
+    windows of the frames after it, as the reference does when it filters stream 0 into itself."""
+    depth = np.ascontiguousarray(depth, np.float32)
+    F, h, w = depth.shape
+    of = np.ascontiguousarray(out_frames, np.int32).reshape(-1)
+    col = None if color_bgr is None else np.ascontiguousarray(color_bgr, np.float32)
+    if col is not None and col.shape != (F, h, w, 3):
+        raise ValueError(f"colour stack has shape {col.shape}, expected {(F, h, w, 3)}")
+    xp = None if xform_params is None else np.ascontiguousarray(xform_params, np.float64)
+    prm = abi.BilateralParams(num_frames=F, width=w, height=h, num_out=len(of), frame_radius=frame_radius, spatial_radius=spatial_radius,
+                              median=1 if median else 0, depth_sigma=depth_sigma, color_sigma=color_sigma, in_place=1 if in_place else 0)
+    out = np.zeros((len(of), h, w), np.float32)
+    _check(lib().rcvd_bilateral_filter(C.byref(prm), C.c_int32(device), _p(depth, C.c_float), _p(col, C.c_float), _p(of, C.c_int32),
+                                       None if xform_cfg is None else C.byref(xform_cfg), _p(xp, C.c_double), _p(out, C.c_float)))
+    return out
+
+
+def build_constraints(color_bgr, pair_frames,pair_flow, pair_mask, match_separation, inv_aspect, dyn_dist=None, min_dynamic_distance=-1.0,
                       trip_frames=None, trip_flow=None, trip_mask=None, device=0):
     """rcvd_build_constraints (FlowConstraintsCollection::compute + sampleConstraints, reference lib/FlowConstraints.cpp:352-550) on the GPU.
     Returns (pair_offsets, pair_constraints [n,4], trip_offsets, trip_constraints [m,6])."""
