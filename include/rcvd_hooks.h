@@ -39,18 +39,13 @@ int32_t rcvd_debug_level_profile(rcvd_problem* p, double* out, int32_t max_level
 int32_t rcvd_debug_fp64_tensor_peak(int32_t device, int32_t shape, double* tflops);
 
 /* A/B switches (defaults in parentheses) */
-int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on);        /* (1) specialised accumulate kernel */
+int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on);        /* (1) specialised accumulate kernels; 0 = generic kernel */
 int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on);          /* (1) two-stream factorisation graph */
-int32_t rcvd_debug_set_trsm_ll(rcvd_problem* p, int32_t on);          /* (1) left-looking tensor-core TRSM */
 int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack);   /* (4) multiple-elimination degree slack; -1 greedy */
-int32_t rcvd_debug_set_trim_gemm(rcvd_problem* p, int32_t on);        /* (1) update GEMMs skip the zero padding beyond ceil8(unknowns) */
-int32_t rcvd_debug_set_potrf_chain_warp(rcvd_problem* p, int32_t on); /* (1) warp 0 of k_potrf_smem is dedicated to the pivot chain; bit 1 set: round-1 shuffle Cholesky of the 16x16 pivot tile */
-int32_t rcvd_debug_set_fused_substitution(rcvd_problem* p, int32_t on); /* (1) forward + backward substitution of the narrow levels as one persistent dataflow kernel; 0 = level-scheduled GEMV launches; n > 1: levels of <= n tasks per phase */
 int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on);        /* (0) cost / gradient evaluations only: no matrix storage (the whole-problem check of a multi-GPU bench) */
 int32_t rcvd_debug_set_distributed(rcvd_problem* p, int32_t on);      /* (1) nranks > 1: distributed factorisation; 0 = all-reduce H + replicated factorisation */
 int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]);       /* {distributed, first replicated level, levels, frames owned by this rank} */
-int32_t rcvd_debug_set_side_slice(rcvd_problem* p, int32_t ctas);     /* (0) grid cap of one overlapped update launch */
-int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta); /* (1, 0) persistent TMA-fed update kernel / round-1 cp.async kernel; items-per-CTA cap of overlapped launches */
+int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta); /* (1, 0) persistent TMA-fed update kernel / cp.async kernel; items-per-CTA cap of the one-team launches (0: none) */
 
 #ifdef __cplusplus
 }

@@ -120,30 +120,6 @@ __device__ __forceinline__ double project_lb(const rcvd_config& c, const Layout&
   if (c.depth_lower_bound && l >= L.offD && l < L.offS && ((l - L.offD) % L.k) == 0 && in_range[f]) return fmax(v, 0.0);
   return v;
 }
-// xc = Plus(x, alpha * (-y*S)) with bounds projection; accumulates |x - xc|^2 over active params,
-// g . delta and max|delta| (for the line search).  y, S, g have npad stride; x, xc nf stride.
-__global__ void __launch_bounds__(256) k_candidate(rcvd_config cfg, Layout L, const uint8_t* __restrict__ in_range, const uint8_t* __restrict__ active,
-                                                    const double* __restrict__ x, const double* __restrict__ y, const double* __restrict__ S,
-                                                    const double* __restrict__ g, double alpha, double* __restrict__ xc, double* __restrict__ scal, int N) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  double d2 = 0.0, gd = 0.0, dm = 0.0;
-  if (i < N * L.nf) {
-    const int f = i / L.nf, l = i % L.nf;
-    const size_t v = (size_t)f * L.npad + l;
-    const double delta = -y[v] * S[v];
-    const double xn = project_lb(cfg, L, in_range, f, l, x[i] + alpha * delta);
-    xc[i] = xn;
-    if (active[v]) { const double d = x[i] - xn; d2 = d * d; }
-    gd = g[v] * delta; dm = fabs(delta);
-  }
-  d2 = warp_sum(d2); gd = warp_sum(gd);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) dm = fmax(dm, __shfl_xor_sync(0xffffffffu, dm, o));
-  if ((threadIdx.x & 31) == 0) {
-    red_add(scal + SC_STEP2, d2); red_add(scal + SC_GDOTD, gd);
-    atomicMax((unsigned long long*)(scal + SC_DMAX), (unsigned long long)__double_as_longlong(dm));   // dm >= 0: bit pattern is monotone
-  }
-}
 // |x|^2 over active params and max-norm of the projected gradient step x - Plus(x, -g)
 __global__ void __launch_bounds__(256) k_state_norms(rcvd_config cfg, Layout L, const uint8_t* __restrict__ in_range, const uint8_t* __restrict__ active,
                                                       const double* __restrict__ x, const double* __restrict__ g, double* __restrict__ scal, int N) {
@@ -227,14 +203,14 @@ struct rcvd_problem {
   std::vector<HBlock> hblocks;
   // schedule
   std::vector<Level> levels; int *d_lvl_frames = nullptr; GemmTask *d_trsm_tasks = nullptr, *d_upd_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
-  SubTask* d_sub_tasks = nullptr; int n_sub_tasks = 0; int* d_sub_counters = nullptr; int* d_sub_need = nullptr; int fused_subst = 1, sub_first_level = 0;   // k_substitution: levels >= sub_first_level (fused_subst: 0 off, 1 default width limit, > 1 that many tasks per level phase)
-  SolveTask *d_fwd_tasks = nullptr, *d_col_tasks = nullptr; int* d_col_ptr = nullptr; TrsmTask* d_trsm_ll = nullptr; bool use_trsm_ll = false, trsm_deep = true;
+  SubTask* d_sub_tasks = nullptr; int n_sub_tasks = 0; int* d_sub_counters = nullptr; int* d_sub_need = nullptr; int sub_first_level = 0;   // k_substitution: levels >= sub_first_level
+  SolveTask *d_fwd_tasks = nullptr, *d_col_tasks = nullptr; int* d_col_ptr = nullptr; TrsmTask* d_trsm_ll = nullptr; bool use_trsm_ll = false;
   cudaGraphExec_t solve_graph = nullptr;
   bool structure_ready = false, constraints_set = false, frames_set = false;
   // multi GPU
   int nranks = 1, rank = 0; nccl::Comm comm = nullptr;
   int64_t launches = 0, graph_launches = 0;
-  std::vector<double> h_state; bool state_dirty = false; bool use_fast = true; bool overlap = true; bool trim_gemm = true; bool potrf_chain_warp = true; bool potrf_blocked = true; int side_slice = 0; bool allow_trsm_ll = true; bool sub_solves = false; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
+  std::vector<double> h_state; bool state_dirty = false; bool use_fast = true; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
   cudaStream_t side_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   double *d_g2 = nullptr, *d_delta = nullptr; int* h_fail = nullptr;
   cudaEvent_t ev[8] = {nullptr};
@@ -243,12 +219,12 @@ struct rcvd_problem {
   std::vector<std::pair<int, cudaEvent_t>>* prof = nullptr;
   // distributed factorisation (nranks > 1): ownership, internal frame numbering, broadcast / reduce segments
   bool eval_only = false;   // test / bench hook: only rcvd_evaluate is used (no H, no factor storage)
-  bool use_runs = true, records_sorted = false;   // run path of the accumulate kernel (bilinear depth grid): records sorted by cell pair
+  bool records_sorted = false;   // run path of the accumulate kernel (bilinear depth grid): records sorted by cell pair
   bool dist_enabled = true, dist = false, identity_perm = true, graph_warm = false, force_full_H = false; int LB = 0;
   std::vector<int> uperm, iperm, fa_off, fa_cnt, fb_off, fb_cnt, tseg, bseg, hseg;   // *_off/_cnt: per-owner frame ranges (phase A / B); segs: (first, count) pairs
   int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr; int n_own_l = 0, n_own_h = 0;
   // TMA-fed persistent update kernel (rcvd_update.cuh)
-  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int upd_rb = 0, upd_neff = 0, num_sms = 132, upd_ipc = 0, upd_dbg = 0, upd_team_items = 1, upd_reserve = 0;   // upd_reserve: SMs kept free by the overlapped updates of narrow levels; upd_team_items: launches of <= that many items per SM take the two-team shape
+  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int upd_rb = 0, upd_neff = 0, num_sms = 132, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
   double upd_flops = 0.0;   // algorithmic flops of the update GEMMs of one factorisation (2 nf^3 per product, nf^2 (nf+1) on symmetric targets)
   rcvd_problem() {}
@@ -511,7 +487,7 @@ static int build_structure(rcvd_problem* p) {
     // The wide levels at the bottom of the tree stay level-scheduled launches (thousands of independent GEMVs: a launch spreads them
     // over the machine at once, a persistent CTA works through them one memory latency at a time); the narrow levels above them -- a
     // latency chain of four tiny launches per level -- run as ONE dataflow kernel: forward narrow, backward narrow in a single launch.
-    const int limit = p->fused_subst <= 0 ? -1 : (p->fused_subst == 1 ? 4 * p->num_sms : p->fused_subst);
+    const int limit = 4 * p->num_sms;
     int LS = (int)p->levels.size();
     while (LS > 0 && (p->levels[LS - 1].nframes + p->levels[LS - 1].nfwd) * nch <= limit) --LS;
     p->sub_first_level = LS;
@@ -550,7 +526,7 @@ static int build_structure(rcvd_problem* p) {
     UP(p->d_pair_frames, pf_int); UP(p->d_records, p->records_h);
   }
   p->records_sorted = false;
-  if (p->use_runs && run_path_ok_host(p->cfg, L) && p->C > 0 && p->C < (int64_t)0x7fffffff) {
+  if (run_path_ok_host(p->cfg, L) && p->C > 0 && p->C < (int64_t)0x7fffffff) {
     // run path of the accumulate kernel: the records of every pair sorted by (source cell, target cell) -- device segmented sort by pair
     const long long n = p->C;
     unsigned *d_k0 = nullptr, *d_k1 = nullptr; int *d_i0 = nullptr, *d_i1 = nullptr; float* d_sorted = nullptr; int64_t* d_off = nullptr; void* d_tmp = nullptr;
@@ -660,7 +636,7 @@ static int build_structure(rcvd_problem* p) {
   CK(cudaFuncSetAttribute(k_trinv, cudaFuncAttributeMaxDynamicSharedMemorySize, (npad * 16 + 16 * (npad + 1)) * (int)sizeof(double)));
   CK(cudaFuncSetAttribute(k_accumulate_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmem));
   CK(cudaFuncSetAttribute(k_accumulate_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, kRunSmem));
-  p->use_trsm_ll = p->allow_trsm_ll && trsm_ll_smem_bytes(npad) <= 220 * 1024;
+  p->use_trsm_ll = trsm_ll_smem_bytes(npad) <= 220 * 1024;
   if (p->use_trsm_ll) { CK(cudaFuncSetAttribute(k_trsm_ll<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2))); if (trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) CK(cudaFuncSetAttribute(k_trsm_ll<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4))); }
   if (potrf_smem_bytes(npad) <= 220 * 1024) CK(cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_smem_bytes(npad)));
   CK(cudaStreamSynchronize(p->stream));
@@ -703,9 +679,9 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     if (!p->prof) return;
     cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); p->prof->push_back({cls < 0 ? cls : (cls | (prof_level << 8)), e});
   };
-  const int neff = p->trim_gemm ? std::min(npad, (L.nf + 7) / 8 * 8) : npad;
+  const int neff = std::min(npad, (L.nf + 7) / 8 * 8);
   auto gemm = [&](cudaStream_t cs, int ntasks, double* dstp, const double* A, const double* B, const GemmTask* tasks, const int2* prs, double alpha, double beta) {
-    // trimming applies to the update products only (beta != 0): the legacy inverse-times-block TRSM must write every padded row of T
+    // trimming applies to the update products only (beta != 0): the inverse-times-block TRSM of large blocks must write every padded row of T
     k_gemm_nt<<<dim3(tiles, tiles, ntasks), 128, 0, cs>>>(dstp, A, B, tasks, prs, npad, beta != 0.0 ? neff : npad, alpha, beta);
   };
   mark(-1);
@@ -733,7 +709,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     const int* lframes = p->d_lvl_own + lv.own_off; const int nfr = lv.nown;      // the frames this rank factors at this level
     if (nfr > 0) {
     if (potrf_smem_bytes(npad) <= 220 * 1024)
-      k_potrf_smem<<<nfr, kPotrfSmemThreads, potrf_smem_bytes(npad), st>>>(p->d_Lb, p->d_invT, lframes, npad, p->d_fail, (p->potrf_chain_warp ? 1 : 0) | (p->potrf_blocked ? 2 : 0));
+      k_potrf_smem<<<nfr, kPotrfSmemThreads, potrf_smem_bytes(npad), st>>>(p->d_Lb, p->d_invT, lframes, npad, p->d_fail);
     else {
       // large blocks: 16-wide panels, panel factor on one CTA per frame, trailing update on the whole machine
       const int nt16 = npad / 16;
@@ -754,7 +730,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       p->launches += 1; mark(P_TRINV);
       if (lv.ntrsm > 0) {
         const int strips = (npad + kTrsmStrip - 1) / kTrsmStrip;
-        if (p->trsm_deep && strips * lv.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024)   // a single wave: deep panel prefetch, one CTA per SM
+        if (strips * lv.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024)   // a single wave: deep panel prefetch, one CTA per SM
           k_trsm_ll<4><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 4), st>>>(p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad);
         else
           k_trsm_ll<2><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 2), st>>>(p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad);
@@ -776,51 +752,37 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0));
     }
     if (side_pending) { CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }   // U2(l-1) before U1(l)
-    auto update = [&](cudaStream_t cs, int off, int n, bool side_launch) {   // persistent TMA-fed update kernel
-      if (side_launch && p->upd_reserve > 0 && lv.nframes <= p->upd_reserve) {
-        // overlapped updates of a narrow level: one CTA per SM and `upd_reserve` SMs left free, so that the next level's potrf CTAs
-        // (a whole SM each) start at once instead of waiting for a persistent CTA of this launch to retire
-        k_update_tma<2><<<std::max(1, std::min(n, p->num_sms - p->upd_reserve)), UpdShape<2>::threads, upd_smem_bytes(p->upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, p->upd_dbg);
-        return;
-      }
-      if (n <= p->num_sms * p->upd_team_items) {   // few items: two DMMA teams per tile, one CTA per SM
-        k_update_tma<2><<<std::min(n, p->num_sms), UpdShape<2>::threads, upd_smem_bytes(p->upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, p->upd_dbg);
+    auto update = [&](cudaStream_t cs, int off, int n) {   // persistent TMA-fed update kernel
+      if (n <= p->num_sms) {   // few items: two DMMA teams per tile, one CTA per SM
+        k_update_tma<2><<<n, UpdShape<2>::threads, upd_smem_bytes(p->upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, 0);
       } else {
         int grid = std::min(n, 2 * p->num_sms);
         if (p->upd_ipc > 0) grid = std::max(grid, (n + p->upd_ipc - 1) / p->upd_ipc);
-        k_update_tma<1><<<grid, UpdShape<1>::threads, upd_smem_bytes(p->upd_rb, 1), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, p->upd_dbg);
+        k_update_tma<1><<<grid, UpdShape<1>::threads, upd_smem_bytes(p->upd_rb, 1), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, 0);
       }
     };
     if (p->gemm_tma) {
-      if (lv.nit > 0) { update(st, lv.it_off, lv.nit, false); p->launches++; mark(P_GEMM); }
+      if (lv.nit > 0) { update(st, lv.it_off, lv.nit); p->launches++; mark(P_GEMM); }
       if (lv.nit2 > 0) {
-        update(p->overlap ? side : st, lv.it2_off, lv.nit2, p->overlap); p->launches++; mark(P_GEMM);
+        update(p->overlap ? side : st, lv.it2_off, lv.nit2); p->launches++; mark(P_GEMM);
         if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
       }
       continue;
     }
     if (lv.nupd > 0) { gemm(st, lv.nupd, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; mark(P_GEMM); }
     if (lv.nupd2 > 0) {
-      cudaStream_t us = p->overlap ? side : st;
-      // sliced so that the grid of one launch is about `side_slice` CTAs: a potrf / trsm CTA of the chain needs most of an SM's
-      // shared memory and can only start on an SM that has drained, which a long low-priority grid never lets happen
-      const int per = (p->overlap && p->side_slice > 0) ? std::max(1, p->side_slice / (tiles * tiles)) : lv.nupd2;
-      for (int o = 0; o < lv.nupd2; o += per) {
-        gemm(us, std::min(per, lv.nupd2 - o), p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off + o, p->d_upd_pairs, -1.0, 1.0); p->launches++; mark(P_GEMM);
-      }
+      gemm(p->overlap ? side : st, lv.nupd2, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; mark(P_GEMM);
       if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
     }
   }
   if (p->dist && p->LB >= (int)p->levels.size()) { int rc = phase_boundary(); if (rc) return rc; }
   if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); }
   CK(cudaMemcpyAsync(p->d_rhs, p->d_gs, (size_t)N * npad * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  const bool sub = p->use_trsm_ll && p->sub_solves;
   const int nlv = (int)p->levels.size();
-  const int LS = sub ? nlv : p->sub_first_level;       // levels >= LS: the persistent dataflow kernel (rcvd_linalg.cuh, k_substitution)
+  const int LS = p->sub_first_level;       // levels >= LS: the persistent dataflow kernel (rcvd_linalg.cuh, k_substitution)
   for (int l = 0; l < LS; ++l) {
     const Level& lv = p->levels[l];
-    if (sub) k_fwd_diag_sub<<<lv.nframes, 256, (npad + 16) * sizeof(double), st>>>(p->d_Lb, p->d_invT, p->d_rhs, p->d_ytmp, p->d_lvl_frames + lv.frame_off, npad);
-    else k_fwd_diag<<<dim3((npad + 7) / 8, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_rhs, p->d_ytmp, p->d_lvl_frames + lv.frame_off, npad);
+    k_fwd_diag<<<dim3((npad + 7) / 8, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_rhs, p->d_ytmp, p->d_lvl_frames + lv.frame_off, npad);
     p->launches++;
     if (lv.nfwd > 0) { k_fwd_update<<<dim3((npad + 7) / 8, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_ytmp, p->d_rhs, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; }
   }
@@ -834,8 +796,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   for (int l = LS - 1; l >= 0; --l) {
     const Level& lv = p->levels[l];
     if (lv.nfwd > 0) { k_bwd_update<<<dim3((npad + 31) / 32, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_y, p->d_ytmp, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; }
-    if (sub) k_bwd_diag_sub<<<lv.nframes, 256, (npad + 16) * sizeof(double), st>>>(p->d_Lb, p->d_invT, p->d_ytmp, p->d_y, p->d_lvl_frames + lv.frame_off, npad);
-    else k_bwd_diag<<<dim3((npad + 31) / 32, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_ytmp, p->d_y, p->d_lvl_frames + lv.frame_off, npad);
+    k_bwd_diag<<<dim3((npad + 31) / 32, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_ytmp, p->d_y, p->d_lvl_frames + lv.frame_off, npad);
     p->launches += 1;
   }
   mark(P_SOLVE);
@@ -1060,9 +1021,11 @@ static int enqueue_model_terms(rcvd_problem* p) {
   return RCVD_OK;
 }
 
-__global__ void __launch_bounds__(256) k_candidate2(rcvd_config cfg, Layout L, const uint8_t* __restrict__ in_range, const uint8_t* __restrict__ active,
-                                                     const double* __restrict__ x, const double* __restrict__ delta, const double* __restrict__ g,
-                                                     double alpha, double* __restrict__ xc, double* __restrict__ scal, int N) {
+// xc = Plus(x, alpha * delta) with bounds projection, delta = -y*S (k_make_delta); accumulates |x - xc|^2 over active params,
+// g . delta and max|delta| (for the line search).  delta, g have npad stride; x, xc nf stride.
+__global__ void __launch_bounds__(256) k_candidate(rcvd_config cfg, Layout L, const uint8_t* __restrict__ in_range, const uint8_t* __restrict__ active,
+                                                    const double* __restrict__ x, const double* __restrict__ delta, const double* __restrict__ g,
+                                                    double alpha, double* __restrict__ xc, double* __restrict__ scal, int N) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double d2 = 0.0, gd = 0.0, dm = 0.0;
   if (i < N * L.nf) {
@@ -1079,13 +1042,13 @@ __global__ void __launch_bounds__(256) k_candidate2(rcvd_config cfg, Layout L, c
   for (int o = 16; o > 0; o >>= 1) dm = fmax(dm, __shfl_xor_sync(0xffffffffu, dm, o));
   if ((threadIdx.x & 31) == 0) {
     red_add(scal + SC_STEP2, d2); red_add(scal + SC_GDOTD, gd);
-    atomicMax((unsigned long long*)(scal + SC_DMAX), (unsigned long long)__double_as_longlong(dm));
+    atomicMax((unsigned long long*)(scal + SC_DMAX), (unsigned long long)__double_as_longlong(dm));   // dm >= 0: bit pattern is monotone
   }
 }
 
 static int enqueue_candidate(rcvd_problem* p, double alpha, const double* g) {
   const size_t U = (size_t)p->N * p->L.nf;
-  k_candidate2<<<nblk(U), 256, 0, p->stream>>>(p->cfg, p->L, p->d_in_range, p->d_active, p->d_x, p->d_delta, g, alpha, p->d_xc, p->d_scal, p->N);
+  k_candidate<<<nblk(U), 256, 0, p->stream>>>(p->cfg, p->L, p->d_in_range, p->d_active, p->d_x, p->d_delta, g, alpha, p->d_xc, p->d_scal, p->N);
   p->launches++;
   return RCVD_OK;
 }
@@ -1594,30 +1557,20 @@ RCVD_API int32_t rcvd_debug_level_profile(rcvd_problem* p, double* out, int32_t 
   return n;
 }
 RCVD_API int64_t rcvd_launch_count(rcvd_problem* p) { return p ? p->launches : 0; }
-// Test hook: 0 forces the generic accumulate kernel, 1 (default) allows the specialised one.
 // Test / bench hook: elimination-order variant (-1 greedy minimum degree, >= 0 multiple elimination with that degree slack).
 RCVD_API int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack) { if (!p) return RCVD_ERR_INVALID; p->order_slack = slack; p->structure_ready = false; return RCVD_OK; }
-// Test / bench hook: 1 (default) = the substitutions of the narrow levels as one persistent dataflow kernel, 0 = level-scheduled GEMV launches throughout.
-RCVD_API int32_t rcvd_debug_set_fused_substitution(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->fused_subst = on; p->structure_ready = false; return RCVD_OK; }   // > 1: levels of at most that many tasks per phase go to the dataflow kernel
 // Test / bench hook: 0 = single-stream factorisation graph, 1 (default) = overlap non-critical updates on a second stream.
 RCVD_API int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->overlap = on != 0; if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; } return RCVD_OK; }
-// Test / bench hook: 0 = explicit inverse + GEMM for the off-diagonal solves, 1 (default) = left-looking tensor-core TRSM.
-RCVD_API int32_t rcvd_debug_set_trsm_ll(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->allow_trsm_ll = (on & 1) != 0; p->trsm_deep = !(on & 2); p->structure_ready = false; return RCVD_OK; }   // bit 0: left-looking TRSM; bit 1: no deep panel prefetch on single-wave launches
-// Test / bench hook: grid-size cap (CTAs) of one overlapped update launch on the side stream; 0 = unsliced.
-RCVD_API int32_t rcvd_debug_set_side_slice(rcvd_problem* p, int32_t ctas) { if (!p) return RCVD_ERR_INVALID; p->side_slice = ctas; if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; } return RCVD_OK; }
-// Test / bench hook: 0 = update GEMMs over the padded size, 1 (default) = trimmed to the unknowns rounded to 8.
-RCVD_API int32_t rcvd_debug_set_trim_gemm(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->trim_gemm = on != 0; if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; } return RCVD_OK; }
-// Test / bench hook: 1 (default) = warp 0 of k_potrf_smem only runs the pivot-tile chain, 0 = it also takes trailing tiles.
-RCVD_API int32_t rcvd_debug_set_potrf_chain_warp(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->potrf_chain_warp = (on & 1) != 0; p->potrf_blocked = !(on & 2);   /* bit 1: round-1 shuffle Cholesky of the 16x16 pivot tile */ if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; } return RCVD_OK; }
-// Test / bench hook: 1 (default) = persistent TMA-fed update kernel (k_update_tma), 0 = round-1 cp.async kernel (k_gemm_nt).
+// Test / bench hook: 1 (default) = persistent TMA-fed update kernel (k_update_tma), 0 = cp.async tile kernel (k_gemm_nt).
+// side_items_per_cta > 0 caps the items per CTA of the one-team update launches (a larger grid); 0 (default) = no cap.
 RCVD_API int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta) {
   if (!p) return RCVD_ERR_INVALID;
-  p->gemm_tma = (tma & 1) != 0; p->upd_dbg = (tma >> 8) & 0xff; p->upd_team_items = (tma >> 16) ? (tma >> 16) - 1 : 1; p->upd_ipc = side_items_per_cta & 0xffff; p->upd_reserve = side_items_per_cta >> 16;   // second argument: items-per-CTA cap | reserved SMs << 16; bits 16+ of the first: (items per SM up to which the two-team shape is used) + 1   // bits 8+: timing experiments of k_update_tma (results invalid)
+  p->gemm_tma = tma != 0; p->upd_ipc = side_items_per_cta;
   if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; }
   if (p->gemm_tma && !p->tmap_ok) p->structure_ready = false;
   return RCVD_OK;
 }
-// Test / bench hook (nranks > 1): 1 (default) = distributed factorisation (owner-computes phase A, reduce-to-owner of H), 0 = round-1 scheme
+// Test / bench hook (nranks > 1): 1 (default) = distributed factorisation (owner-computes phase A, reduce-to-owner of H), 0 = replicated scheme
 // (all-reduce of H, factorisation replicated on every rank).  out (optional): {distributed active, first replicated level, levels}.
 // Test / bench hook: 1 = the handle will only evaluate cost / gradient (rcvd_evaluate): no normal matrix, no factor storage is allocated
 RCVD_API int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->eval_only = on != 0; p->structure_ready = false; return RCVD_OK; }
@@ -1629,14 +1582,8 @@ RCVD_API int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]) {
   out[0] = p->dist ? 1 : 0; out[1] = p->LB; out[2] = (int)p->levels.size(); out[3] = p->dist ? p->fa_cnt[p->rank] + p->fb_cnt[p->rank] : p->N;
   return RCVD_OK;
 }
-// 0: generic kernel, 1 (default): specialised kernels (run path on a bilinear depth grid), 2: specialised kernel without the run path (round 1)
-RCVD_API int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on) {
-  if (!p) return RCVD_ERR_INVALID;
-  p->use_fast = on != 0;
-  const bool runs = on != 2;
-  if (runs != p->use_runs) { p->use_runs = runs; if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; } p->structure_ready = false; }
-  return RCVD_OK;
-}
+// Test hook: 0 = generic accumulate kernel (the tests' reference), 1 (default) = specialised kernels (run path on a bilinear depth grid).
+RCVD_API int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->use_fast = on != 0; return RCVD_OK; }
 RCVD_API int32_t rcvd_solve(rcvd_problem* p, const rcvd_solve_options* opt, rcvd_solve_summary* summary) {
   if (!p || !summary) return set_err(RCVD_ERR_INVALID, "null argument");
   SET_DEVICE(p->device);

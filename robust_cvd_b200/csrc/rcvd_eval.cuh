@@ -346,7 +346,7 @@ __global__ void __launch_bounds__(kTile) k_accumulate_fast(DevProblem p, const d
 }
 
 // ---------------------------------------------------------------------------
-// K1 (run path, round 2): bilinear depth grid, the reference's default once coarse-to-fine has left the Global transform.
+// K1 (run path): bilinear depth grid, the reference's default once coarse-to-fine has left the Global transform.
 // The records of a pair are sorted by (source cell, target cell) when the problem is set up (rcvd_api.cu, device segmented sort), so
 // consecutive constraints share their eight spline nodes.  A run = the constraints of one warp with the same cell pair.  Per run the
 // node rows of the normal equations,

@@ -128,40 +128,6 @@ __device__ __forceinline__ void tile_mma_nt(const double* __restrict__ At, const
   }
 }
 
-// Register-resident right-looking Cholesky of one 16x16 tile by a single warp (lane i mod 16 owns row i).
-// Writes L back to the swizzled tile and the reciprocal pivots 1/l_jj to pinv[0..15].
-// (Measured dead ends, tools/potrf_phases.cu: a branch-free variant with an fp32-seeded Newton rsqrt: 7.5 k cycles per tile
-// against 5.6 k -- the F2F conversions cost more than the library's MUFU.RSQ64H path; a rotated-row loop form that is not
-// unrolled over j: 17 k cycles.)
-__device__ __forceinline__ void warp_chol16(double* __restrict__ D, double* __restrict__ pinv, int lane, int* __restrict__ fail) {
-  // (round 2: a "pivot-first" ordering -- column j+1 and the next rsqrt issued before the other column updates of step j -- measured
-  // SLOWER, potrf 3.44 -> 3.78 ms per factorisation: the dependent chain shfl, rsqrt, mul, shfl, fma per pivot is the same either way)
-  const int i = lane & 15;
-  double a[16];
-#pragma unroll
-  for (int c = 0; c < 16; ++c) a[c] = (c <= i) ? D[swz(i, c)] : 0.0;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    double d = __shfl_sync(0xffffffffu, a[j], j);
-    if (!(d > 0.0) || !isfinite(d)) { if (lane == 0) *fail = 1; d = 1.0; }
-    const double pi = rsqrt(d);
-    const double lij = (i == j) ? d * pi : a[j] * pi;
-    if (i >= j) a[j] = lij;
-    if (lane == 0) pinv[j] = pi;
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-      if (c > j) {   // constant trip count so that a[] stays in registers
-        const double lcj = __shfl_sync(0xffffffffu, a[j], c);
-        if (i >= c) a[c] -= lij * lcj;
-      }
-    }
-  }
-  if (lane < 16) {
-#pragma unroll
-    for (int c = 0; c < 16; ++c) D[swz(i, c)] = a[c];
-  }
-}
-
 #ifdef RCVD_POTRF_PHASES   // tools/potrf_phases.cu: cycle counts per phase of CTA 0 (thread 0's view)
 __device__ long long g_potrf_phase[16];
 #define POTRF_PHASE(n) do { if (threadIdx.x == 0 && blockIdx.x == 0) { const long long now_ = clock64(); g_potrf_phase[n] += now_ - last_; last_ = now_; } } while (0)
@@ -171,12 +137,12 @@ __device__ long long g_potrf_phase[16];
 #define POTRF_PHASE(n) do { } while (0)
 #endif
 
-// Round 2: 4x4-blocked Cholesky of one 16x16 tile by a single warp.  The pivot chain of warp_chol16 is 16 x (shuffle, rsqrt, mul,
-// 15 shuffle+FMA column updates) ~ 5.6 k cycles, most of it the shuffle traffic of the rank-1 updates.  Here the tile lives in the
-// DMMA accumulator fragments (three 8x8 units of the lower triangle); per block of four columns every lane factors the 4x4 diagonal block
-// redundantly from ten broadcast shared-memory loads (no communication inside the four-pivot chain), the lanes of the rows below solve
-// their 4-wide panel row, and the rank-4 trailing update is three DMMA.8x8x4 with K = 4.  Same outputs as warp_chol16: L in the
-// swizzled tile (lower triangle), reciprocal pivots in pinv.
+// 4x4-blocked Cholesky of one 16x16 tile by a single warp.  Column by column with one row per lane, the pivot chain is 16 x (shuffle,
+// rsqrt, mul, 15 shuffle+FMA column updates) ~ 5.6 k cycles, most of it the shuffle traffic of the rank-1 updates.  Here the tile lives in
+// the DMMA accumulator fragments (three 8x8 units of the lower triangle); per block of four columns every lane factors the 4x4 diagonal
+// block redundantly from ten broadcast shared-memory loads (no communication inside the four-pivot chain), the lanes of the rows below
+// solve their 4-wide panel row, and the rank-4 trailing update is three DMMA.8x8x4 with K = 4.  Writes L back to the swizzled tile
+// (lower triangle) and the reciprocal pivots 1/l_jj to pinv[0..15].
 __device__ __forceinline__ void warp_chol16_blocked(double* __restrict__ D, double* __restrict__ pinv, int lane, int* __restrict__ fail) {
   const int g = lane >> 2, t = lane & 3;
   double c[3][2];                                  // units (0,0), (1,0), (1,1): rows 8*ui + g, columns 8*uj + 2t, + 1
@@ -259,7 +225,7 @@ __device__ __forceinline__ void warp_chol16_blocked(double* __restrict__ D, doub
 
 
 __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __restrict__ Lb, double* __restrict__ invT,
-                                                                   const int* __restrict__ frames, int npad, int* __restrict__ fail, int chain_warp) {
+                                                                   const int* __restrict__ frames, int npad, int* __restrict__ fail) {
   extern __shared__ __align__(16) double tiles[];
   const int frame = frames[blockIdx.x];
   double* A = Lb + (size_t)frame * npad * npad;
@@ -284,28 +250,26 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   POTRF_PHASE(0);
-  if (warp == 0) { if (chain_warp & 2) warp_chol16_blocked(tiles, pinv, lane, fail); else warp_chol16(tiles, pinv, lane, fail); }
+  if (warp == 0) warp_chol16_blocked(tiles, pinv, lane, fail);
   __syncthreads();
   POTRF_PHASE(1);
   for (int jb = 0; jb < nt; ++jb) {
     const double* D = tiles + (size_t)(jb * (jb + 1) / 2 + jb) * kTileSz;
     const double* pv = pinv + jb * 16;
     // ---- panel by forward substitution (one thread per row below the tile); warp nw-1 computes the tile inverse ----
-    // Chain mode (default): warp 0 solves only the rows of tile (jb+1, jb) -- all its lookahead needs -- updates tile (jb+1, jb+1),
+    // Warp 0, the chain warp, solves only the rows of tile (jb+1, jb) -- all its lookahead needs -- updates tile (jb+1, jb+1),
     // ARRIVES on named barrier 2 and factors the tile; the other warps SYNC on barrier 2 before they start their panel rows, so the
     // chain warp has the shared-memory pipe and the fp64 pipe to itself for its short serial part, and the others' panel + trailing
-    // tiles run beside the next pivot tile's Cholesky.  (tools/potrf_phases.cu, thread 0's view of one step with every warp entering
-    // the panel and the DMMA section together: panel 1.45 k -- 152 broadcast LDS per row thread, LSU-bound -- + barrier 0.2 k + own
-    // tile update 1.4 k cycles, next to 5.3 k of Cholesky.)
+    // tiles run beside the next pivot tile's Cholesky.  (tools/potrf_phases.cu, thread 0's view of one step when every warp entered
+    // the panel and the DMMA section together and the pivot tile was a shuffle chain: panel 1.45 k -- 152 broadcast LDS per row
+    // thread, LSU-bound -- + barrier 0.2 k + own tile update 1.4 k cycles, next to 5.3 k of Cholesky.)
     const int rows = (nt - jb - 1) * 16;
-    const bool chain = (chain_warp & 1) != 0;
     int prow = -1;                                   // this thread's panel row (index below the pivot tile), -1: none
     // (keeping the warps that share the chain warp's scheduler idle made the pivot tile faster, 4.3 k -> 3.9 k cycles, and the other
     // warps' trailing update slower by more: 2.77 against 2.68 ms per factorisation)
     const int nwork = nw - 1, widx = warp - 1;       // worker warps beside the chain warp
-    if (chain) { if (warp == 0) { if (lane < 16 && rows > 0) prow = lane; } else if (widx * 32 + lane < rows - 16) prow = 16 + widx * 32 + lane; }
-    else if (tid < rows) prow = tid;
-    if (chain && warp != 0) asm volatile("bar.sync 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
+    if (warp == 0) { if (lane < 16 && rows > 0) prow = lane; } else if (widx * 32 + lane < rows - 16) prow = 16 + widx * 32 + lane;
+    if (warp != 0) asm volatile("bar.sync 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
     if (prow >= 0) {
       const int ti = jb + 1 + (prow >> 4), r = prow & 15;
       double* Tt = tiles + (size_t)(ti * (ti + 1) / 2 + jb) * kTileSz;
@@ -345,8 +309,7 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
       for (int r = 0; r < 16; ++r) iT[(size_t)jb * 256 + r * 16 + cidx] = xcol[r];
     }
     POTRF_PHASE(2);
-    if (!chain) __syncthreads();
-    else if (warp != 0) asm volatile("bar.sync 3, %0;" ::"n"(kPotrfSmemThreads - 32) : "memory");
+    if (warp != 0) asm volatile("bar.sync 3, %0;" ::"n"(kPotrfSmemThreads - 32) : "memory");
     POTRF_PHASE(3);
     // ---- trailing update (DMMA) with lookahead: warp 0 updates tile (jb+1, jb+1) first and factors it at once ----
     const int m = nt - jb - 1, ntr = m * (m + 1) / 2;
@@ -371,26 +334,18 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
       while (ti * (ti + 1) / 2 > tl) --ti;
       gi = jb + 1 + ti; gj = jb + 1 + (tl - ti * (ti + 1) / 2);
     };
-    if (chain) {
-      // warp 0 owns the chain (measured: 88.7 -> 83.0 us per 208x208 block in tools/potrf_phases.cu): its panel rows, tile (jb+1, jb+1)
-      // and the next pivot tile, with the SM to itself until it arrives on barrier 2
-      if (warp == 0) {
-        double* Ct = nullptr;
-        if (ntr > 0) { __syncwarp(); Ct = upd_tile(jb + 1, jb + 1); }
-        __threadfence_block();
-        asm volatile("bar.arrive 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
-        POTRF_PHASE(4);
-        if (ntr > 0) { __syncwarp(); if (chain_warp & 2) warp_chol16_blocked(Ct, pinv + (jb + 1) * 16, lane, fail); else warp_chol16(Ct, pinv + (jb + 1) * 16, lane, fail); }
-        POTRF_PHASE(5);
-      } else {
-        for (int tl = 1 + widx; tl < ntr; tl += nwork) { int gi, gj; tile_of(tl, gi, gj); upd_tile(gi, gj); }
-      }
+    // warp 0 owns the chain (measured: 88.7 -> 83.0 us per 208x208 block in tools/potrf_phases.cu, against every warp taking
+    // trailing tiles): its panel rows, tile (jb+1, jb+1) and the next pivot tile, with the SM to itself until it arrives on barrier 2
+    if (warp == 0) {
+      double* Ct = nullptr;
+      if (ntr > 0) { __syncwarp(); Ct = upd_tile(jb + 1, jb + 1); }
+      __threadfence_block();
+      asm volatile("bar.arrive 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
+      POTRF_PHASE(4);
+      if (ntr > 0) { __syncwarp(); warp_chol16_blocked(Ct, pinv + (jb + 1) * 16, lane, fail); }
+      POTRF_PHASE(5);
     } else {
-      for (int tl = warp; tl < ntr; tl += nw) {
-        int gi, gj; tile_of(tl, gi, gj);
-        double* Ct = upd_tile(gi, gj);
-        if (tl == 0) { __syncwarp(); if (chain_warp & 2) warp_chol16_blocked(Ct, pinv + (jb + 1) * 16, lane, fail); else warp_chol16(Ct, pinv + (jb + 1) * 16, lane, fail); }
-      }
+      for (int tl = 1 + widx; tl < ntr; tl += nwork) { int gi, gj; tile_of(tl, gi, gj); upd_tile(gi, gj); }
     }
     POTRF_PHASE(6);
     __syncthreads();
@@ -645,7 +600,7 @@ constexpr int kTrsmRW = 8;
 constexpr int kTrsmStrip = 4 * kTrsmRW;
 // The L row panels are prefetched AHEAD steps ahead through a ring.  AHEAD = 2 (108 KB at npad 208, two CTAs per SM) for launches that
 // fill the machine; AHEAD = 4 (169 KB, one CTA per SM) for the narrow levels, where a launch is a single wave and every step of the
-// chain otherwise waits for its panel to come back from L2 (measured in round 2: all launches at AHEAD = 4 made the wide levels slower,
+// chain otherwise waits for its panel to come back from L2 (measured: all launches at AHEAD = 4 made the wide levels slower,
 // trsm 2.03 -> 2.72 ms per factorisation, because occupancy halves where throughput counts).
 __host__ __device__ inline size_t trsm_ll_smem_bytes(int npad, int ahead = 2) { return ((size_t)kTrsmStrip * (npad + 4) + ahead * 16 * (size_t)(npad + 4) + ahead * 16 * 20) * sizeof(double); }
 
@@ -768,69 +723,6 @@ __global__ void __launch_bounds__(128) k_trsm_ll(double* __restrict__ T, const d
   }
 }
 
-// Triangular solves with L_kk by 16-row tile substitution using the diagonal-tile inverses (no explicit inverse):
-//   forward  y_jt = Di_jt (b_jt - sum_{pt<jt} L[jt,pt] y_pt),   backward  x_jt = Di_jt^T (y_jt - sum_{pt>jt} L[pt,jt]^T x_pt)
-// one CTA (256 threads) per frame of the level; vectors are staged in shared memory.
-__global__ void __launch_bounds__(256) k_fwd_diag_sub(const double* __restrict__ Lb, const double* __restrict__ invT, const double* __restrict__ rhs,
-                                                       double* __restrict__ y, const int* __restrict__ frames, int npad) {
-  extern __shared__ double vs[];      // [npad] solution so far, [16] temp
-  double* tmp = vs + npad;
-  const int frame = frames[blockIdx.x];
-  const double* A = Lb + (size_t)frame * npad * npad; const double* iT = invT + (size_t)frame * npad * 16;
-  const double* b = rhs + (size_t)frame * npad;
-  const int tid = threadIdx.x, r = tid >> 4, c = tid & 15, nt = npad / 16;
-  for (int jt = 0; jt < nt; ++jt) {
-    // partial dot of row (jt*16 + r) over columns k = c, c+16, ... < jt*16
-    double s = 0.0;
-    const double* row = A + (size_t)(jt * 16 + r) * npad;
-    for (int k = c; k < jt * 16; k += 16) s += row[k] * vs[k];
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);   // 16 lanes of a row are contiguous within the warp
-    if (c == 0) tmp[r] = b[jt * 16 + r] - s;
-    __syncthreads();
-    if (tid < 16) {
-      double acc = 0.0;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) acc += iT[(size_t)jt * 256 + tid * 16 + q] * tmp[q];
-      vs[jt * 16 + tid] = acc;
-      y[(size_t)frame * npad + jt * 16 + tid] = acc;
-    }
-    __syncthreads();
-  }
-}
-__global__ void __launch_bounds__(256) k_bwd_diag_sub(const double* __restrict__ Lb, const double* __restrict__ invT, const double* __restrict__ yin,
-                                                       double* __restrict__ x, const int* __restrict__ frames, int npad) {
-  extern __shared__ double vs[];
-  double* tmp = vs + npad;
-  const int frame = frames[blockIdx.x];
-  const double* A = Lb + (size_t)frame * npad * npad; const double* iT = invT + (size_t)frame * npad * 16;
-  const double* b = yin + (size_t)frame * npad;
-  const int tid = threadIdx.x, r = tid >> 4, c = tid & 15, nt = npad / 16;
-  for (int jt = nt - 1; jt >= 0; --jt) {
-    // column (jt*16 + c) of L below the tile, rows k = (jt+1)*16 + r, + 16, ...: sum_k L[k][jt*16+c] x_k
-    double s = 0.0;
-    for (int k = (jt + 1) * 16 + r; k < npad; k += 16) s += A[(size_t)k * npad + jt * 16 + c] * vs[k];
-    // reduce over r (stride 16 in tid): via shared memory
-    __shared__ double red[256];
-    red[tid] = s;
-    __syncthreads();
-    if (tid < 16) {
-      double acc = 0.0;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) acc += red[q * 16 + tid];
-      tmp[tid] = b[jt * 16 + tid] - acc;
-    }
-    __syncthreads();
-    if (tid < 16) {
-      double acc = 0.0;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) acc += iT[(size_t)jt * 256 + q * 16 + tid] * tmp[q];    // Di^T
-      vs[jt * 16 + tid] = acc;
-      x[(size_t)frame * npad + jt * 16 + tid] = acc;
-    }
-    __syncthreads();
-  }
-}
 
 // ---------------------------------------------------------------------------
 // Triangular solves as GEMVs with inv(L_kk); vectors have npad stride per frame.
@@ -913,7 +805,7 @@ __global__ void __launch_bounds__(256) k_bwd_diag(const double* __restrict__ inv
 }
 
 // ---------------------------------------------------------------------------
-// Round 2: the whole forward + backward substitution as ONE persistent dataflow kernel.  The level-scheduled version above is
+// The forward + backward substitution of the narrow levels as ONE persistent dataflow kernel.  The level-scheduled version above is
 // 4 launches per level (172 at config 2), each a single short wave: 1.35 ms of launch latency for ~0.3 ms of memory traffic.  Here the
 // same GEMVs are tasks of a list in topological order (level-major; forward levels ascending, then backward levels descending), cut
 // into kSubChunk-row (forward) / -column (backward) chunks.  A CTA takes the next task with an atomic ticket, waits on the counters its

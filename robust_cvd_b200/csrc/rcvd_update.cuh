@@ -8,8 +8,8 @@
 //     row-major factor blocks into a 5-deep shared-memory ring, completion signalled on mbarriers (no cp.async
 //     groups, no __syncthreads in the K loop);
 //   * the TMA box is [rows][16 doubles] = 128-byte rows with the 128-byte swizzle (16-byte chunk index XOR row & 7).  A first
-//     version used [rows][4 doubles] boxes (32-byte rows, conflict-free by construction): same speed as the round-1 cp.async
-//     kernel, the DMMA warps starved on the full barriers -- the TMA is bound by row requests, not bytes.  With 128-byte
+//     version used [rows][4 doubles] boxes (32-byte rows, conflict-free by construction): same speed as the cp.async
+//     kernel k_gemm_nt, the DMMA warps starved on the full barriers -- the TMA is bound by row requests, not bytes.  With 128-byte
 //     rows the fragment loads stay conflict-free by feeding the m8n8k4 fragment row g with tile row pi(g) = 2 (g & 3) + (g >> 2):
 //     the 16 lanes of a half-warp then touch 16 distinct 8-byte slots of the 128-byte bank window.  The same permutation on
 //     the B side permutes the accumulator columns; one shuffle per accumulator pair restores adjacent column pairs for
@@ -152,6 +152,9 @@ __device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("
 
 // dst[it.dst] (tile) -= sum_p T[pairs[p].x] (rows m0..) * T[pairs[p].y] (rows n0..)^T over k < neff.
 // tmap: 2-D view of the T buffer, inner dimension = k (npad doubles per row), outer = block * npad + row; box = [rb][16], 128-B swizzle.
+// dbg: timing experiments (results invalid); the solver passes 0.  The argument and its branches stay because without them ptxas
+// allocates the K loop differently and spills its counters (CUDA 12.9): the update GEMMs measured 5-7 % slower at configs 2 and 4
+// (H100 80GB HBM3, 700 W power limit).
 template <int TEAMS>
 __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::ctas) k_update_tma(const __grid_constant__ CUtensorMap tmap, double* __restrict__ dst,
                                                                const UpdItem* __restrict__ items, int nitems, const int2* __restrict__ pairs,

@@ -179,11 +179,12 @@ class Problem:
         return dict(zip(keys, list(out)))
 
     def set_fast_path(self, on=True):
-        """Test hook: False / 0 forces the generic accumulate kernel, 2 the round-1 specialised kernel without the run path."""
+        """Test hook: False forces the generic accumulate kernel (the tests' reference); True (default) allows the specialised ones."""
         _check(self.L.rcvd_debug_set_fast_path(self.h, C.c_int32(int(on))))
 
     def set_update_kernel(self, tma=True, side_items_per_cta=0):
-        """Test / bench hook: persistent TMA-fed update kernel (default) or the round-1 cp.async kernel."""
+        """Test / bench hook: persistent TMA-fed update kernel (default) or the cp.async kernel; side_items_per_cta > 0 caps the
+        work items per CTA of the one-team update launches."""
         _check(self.L.rcvd_debug_set_update_kernel(self.h, C.c_int32(1 if tma else 0), C.c_int32(side_items_per_cta)))
 
     def set_eval_only(self, on=True):
@@ -191,25 +192,13 @@ class Problem:
         _check(self.L.rcvd_debug_set_eval_only(self.h, C.c_int32(1 if on else 0)))
 
     def set_distributed(self, on=True):
-        """Test / bench hook (nranks > 1): distributed factorisation (default) or the round-1 replicated scheme."""
+        """Test / bench hook (nranks > 1): distributed factorisation (default) or the replicated scheme."""
         _check(self.L.rcvd_debug_set_distributed(self.h, C.c_int32(1 if on else 0)))
 
     def distribution_info(self):
         out = (C.c_int32 * 4)()
         _check(self.L.rcvd_distribution_info(self.h, out))
         return dict(zip(["distributed", "first_replicated_level", "levels", "frames_owned"], list(out)))
-
-    def set_side_slice(self, ctas):
-        _check(self.L.rcvd_debug_set_side_slice(self.h, C.c_int32(ctas)))
-
-    def set_trim_gemm(self, on=True):
-        _check(self.L.rcvd_debug_set_trim_gemm(self.h, C.c_int32(1 if on else 0)))
-
-    def set_fused_substitution(self, on=True):
-        _check(self.L.rcvd_debug_set_fused_substitution(self.h, C.c_int32(int(on))))
-
-    def set_trsm_ll(self, on=True):
-        _check(self.L.rcvd_debug_set_trsm_ll(self.h, C.c_int32(1 if on else 0)))
 
     def set_order_slack(self, slack):
         _check(self.L.rcvd_debug_set_order_slack(self.h, C.c_int32(slack)))

@@ -13,15 +13,14 @@ int main() {
   int zero = 0; cudaMemcpy(dF, &zero, 4, cudaMemcpyHostToDevice); cudaMemset(dfail, 0, 4);
   cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_smem_bytes(n));
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-  for (int rep = 0; rep < 4; ++rep) {
-    const int mode = rep < 2 ? 3 : 1;   // bit 0 chain warp, bit 1 blocked pivot tile (default 3); 1: round-1 shuffle version
+  for (int rep = 0; rep < 4; ++rep) {   // rep 0 warms up
     cudaMemcpy(dA, A.data(), A.size() * 8, cudaMemcpyHostToDevice);
     long long z[16] = {0}; cudaMemcpyToSymbol(g_potrf_phase, z, sizeof(z));
-    cudaEventRecord(e0); k_potrf_smem<<<1, kPotrfSmemThreads, potrf_smem_bytes(n)>>>(dA, dT, dF, n, dfail, mode); cudaEventRecord(e1); cudaEventSynchronize(e1);
+    cudaEventRecord(e0); k_potrf_smem<<<1, kPotrfSmemThreads, potrf_smem_bytes(n)>>>(dA, dT, dF, n, dfail); cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
     long long ph[16]; cudaMemcpyFromSymbol(ph, g_potrf_phase, sizeof(ph));
-    printf("rep %d mode %d: %.1f us; cycles: load %lld, first chol %lld, panel(thread0) %lld, wait-panel %lld, update-to-lookahead %lld, lookahead chol %lld, rest of update %lld, wait-update %lld  (%s)\n",
-           rep, mode, ms * 1e3, ph[0], ph[1], ph[2], ph[3], ph[4], ph[5], ph[6], ph[7], cudaGetErrorString(cudaGetLastError()));
+    printf("rep %d: %.1f us; cycles: load %lld, first chol %lld, panel(thread0) %lld, wait-panel %lld, update-to-lookahead %lld, lookahead chol %lld, rest of update %lld, wait-update %lld  (%s)\n",
+           rep, ms * 1e3, ph[0], ph[1], ph[2], ph[3], ph[4], ph[5], ph[6], ph[7], cudaGetErrorString(cudaGetLastError()));
     printf("        blocked chol16 (14 tiles x 4 block steps): store+sync+block loads %lld, pivot chain %lld, row solves+sync %lld, diag rows+DMMA %lld\n", ph[8], ph[9], ph[10], ph[11]);
   }
   // correctness: compare with a plain host Cholesky

@@ -13,16 +13,12 @@ ap.add_argument("--iters", type=int, default=1)
 ap.add_argument("--accumulate-only", action="store_true")
 ap.add_argument("--slack", type=int, default=None)
 ap.add_argument("--no-overlap", action="store_true")
-ap.add_argument("--side-slice", type=int, default=None)
-ap.add_argument("--trim-gemm", type=int, default=None)
 ap.add_argument("--classes", action="store_true", help="also print the serialised per-kernel-class times")
 a = ap.parse_args()
 spec, sc, cfg, pairs, offs, rec, med = bench.build_case(a.workload, frames=a.frames, sep=a.sep)
 P = solver.Problem(cfg)
 if a.slack is not None: P.set_order_slack(a.slack)
 if a.no_overlap: P.set_overlap(False)
-if a.side_slice is not None: P.set_side_slice(a.side_slice)
-if a.trim_gemm is not None: P.set_trim_gemm(bool(a.trim_gemm))
 P.set_frames(np.ones(cfg.num_frames, np.uint8), med); P.set_constraints(pairs, offs, rec); P.set_state(bench.initial_state(sc, cfg, P.stride))
 if a.accumulate_only:
     print("accumulate ms", P.time_accumulate(iters=a.iters))
