@@ -20,6 +20,21 @@ int32_t rcvd_structure_info(rcvd_problem* p, int32_t out[8]);
 /* y = (S H S + diag(D2))^-1 b with the current H (exercises factorisation + substitution alone) */
 int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y);
 
+/* y = (H + diag(D2))^-1 b for a dense symmetric U x U matrix H (U = N * stride, caller's frame order) through the production
+ * factorisation graph, S = 1: H is scattered into the H blocks of the frame graph set by rcvd_problem_set_structure /
+ * rcvd_problem_set_constraints (no evaluation).  A non-zero entry in a frame pair the graph does not couple: RCVD_ERR_INVALID;
+ * a non-positive pivot: RCVD_ERR_NUMERIC. */
+int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y);
+/* what the last factorisation left on the device: order[N] = caller's frame index of each eliminated frame, in elimination order;
+ * L = dense U x U lower-triangular factor of P A P^T in that order (padding stripped, strict upper triangle zero); Linv (may be null)
+ * = the N * stride * stride explicit inverses of the diagonal blocks (k_trinv), same order.  RCVD_ERR_INVALID before any factorisation. */
+int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, double* Linv);
+/* launches of each factorisation / solve kernel path since the handle was created: {k_potrf_smem, k_potrf_panel, k_trsm_ll<4>,
+ * k_trsm_ll<2>, TRSM by explicit inverse (k_gemm_nt), k_update_tma<1>, k_update_tma<2>, update by k_gemm_nt, level-launched
+ * substitution (k_fwd_* / k_bwd_*), k_substitution, k_trinv, the rest (k_load_factor, k_potrf_trail), k_update_tma<1> launches with
+ * fewer CTAs than items (CTAs that walk several items)} */
+int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]);
+
 /* one damped LM step at the current state with trust-region `radius`; out = {|(S H S + D2) y - S g| / |S g| (device SpMV over the
  * assembled H), |S g|, cost, |g|_2, |y|_2, non-positive-pivot flag}: the parity evidence bench.py prints at the size it times */
 int32_t rcvd_debug_linear_residual(rcvd_problem* p, double radius, double out[6]);

@@ -173,6 +173,10 @@ __global__ void k_h_to_dense(const double* __restrict__ H, const HBlock* __restr
   out[((size_t)uc * nf + j) * U + (size_t)ur * nf + i] = v;
 }
 
+// launch counters of enqueue_factor_solve by kernel path (rcvd_debug_linear_paths; include/rcvd_hooks.h lists the same order)
+enum { LP_POTRF_SMEM = 0, LP_POTRF_PANEL, LP_TRSM_LL4, LP_TRSM_LL2, LP_TRSM_GEMM, LP_UPD_TMA1, LP_UPD_TMA2, LP_UPD_GEMM, LP_SUB_LEVEL, LP_SUB_FUSED,
+       LP_TRINV, LP_OTHER, LP_UPD_TMA1_MULTI, LP_N };   // LP_UPD_TMA1_MULTI: k_update_tma<1> launches with fewer CTAs than items
+
 // ---------------------------------------------------------------------------
 struct Level { int frame_off, nframes; int trsm_off, ntrsm; int upd_off, nupd; int upd2_off, nupd2; int fwd_off, nfwd; int it_off, nit, it2_off, nit2; int own_off, nown; };   // frame_off: every frame of the level (substitution); own_off: the frames this rank factors   // upd: targets consumed by the next level; upd2: the rest
 
@@ -227,6 +231,10 @@ struct rcvd_problem {
   UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int upd_rb = 0, upd_neff = 0, num_sms = 132, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
   double upd_flops = 0.0;   // algorithmic flops of the update GEMMs of one factorisation (2 nf^3 per product, nf^2 (nf+1) on symmetric targets)
+  // test hooks (rcvd_debug_factor_dense, rcvd_debug_linear_paths): elimination order (internal frame ids), every factor block's
+  // (row frame, column frame), per-kernel-path launch counters (enqueue_factor_solve counts, graph replays add graph_paths)
+  std::vector<int> elim_order; std::vector<HBlock> lblocks_h; bool factored = false;
+  int64_t paths[LP_N] = {0}, graph_paths[LP_N] = {0};
   rcvd_problem() {}
 };
 
@@ -252,7 +260,7 @@ static void free_all(rcvd_problem* p) {
   p->allocs.clear();
   if (p->stream) cudaStreamSynchronize(p->stream);
   if (p->h_scal) { cudaFreeHost(p->h_scal); p->h_scal = nullptr; }
-  p->structure_ready = false;
+  p->structure_ready = false; p->factored = false;
 }
 
 static DevProblem dev_problem(const rcvd_problem* p) {
@@ -403,6 +411,7 @@ static int build_structure(rcvd_problem* p) {
   for (int f = 0; f < N; ++f) lblocks[f] = {f, f, f};
   for (auto& kv : lid) lblocks[kv.second] = {-1, kv.first.first, kv.first.second};
   for (int h = N; h < p->nHblocks; ++h) lblocks[p->hblocks[h].lblk].lblk = h;
+  p->elim_order = order; p->lblocks_h = lblocks;
   // blocks this rank owns: what it loads into the factor and what it multiplies in the model term (all of them without distribution)
   std::vector<int> own_lblocks, own_hblocks;
   for (int b = 0; b < N + nLoff; ++b) { const int c = b < N ? b : lcol[b - N]; if (!dist || own[c] == p->rank) own_lblocks.push_back(b); }
@@ -686,7 +695,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   };
   mark(-1);
   k_load_factor<<<dim3((npad * npad + 255) / 256, p->dist ? p->n_own_l : nL), 256, 0, st>>>(p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, L.nf, p->dist ? p->d_own_lblocks : nullptr);
-  p->launches += 1; mark(P_LOAD);
+  p->launches += 1; p->paths[LP_OTHER]++; mark(P_LOAD);
   // Two-stream schedule (fork/join inside the captured graph): the non-critical update GEMMs of level l run on `side`
   // concurrently with potrf / inverse / trsm of level l+1 on `st`.
   cudaStream_t side = p->side_stream;
@@ -708,16 +717,17 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     if (p->dist && (int)li == p->LB) { int rc = phase_boundary(); if (rc) return rc; }
     const int* lframes = p->d_lvl_own + lv.own_off; const int nfr = lv.nown;      // the frames this rank factors at this level
     if (nfr > 0) {
-    if (potrf_smem_bytes(npad) <= 220 * 1024)
+    if (potrf_smem_bytes(npad) <= 220 * 1024) {
       k_potrf_smem<<<nfr, kPotrfSmemThreads, potrf_smem_bytes(npad), st>>>(p->d_Lb, p->d_invT, lframes, npad, p->d_fail);
-    else {
+      p->paths[LP_POTRF_SMEM]++;
+    } else {
       // large blocks: 16-wide panels, panel factor on one CTA per frame, trailing update on the whole machine
       const int nt16 = npad / 16;
       for (int jb = 0; jb < nt16; ++jb) {
         k_potrf_panel<<<nfr, kPotrfThreads, 0, st>>>(p->d_Lb, p->d_invT, lframes, npad, jb, p->d_fail);
-        p->launches += 1;
+        p->launches += 1; p->paths[LP_POTRF_PANEL]++;
         const int m = npad - (jb + 1) * 16;
-        if (m > 0) { const int n64 = (m + 63) / 64; k_potrf_trail<<<dim3(n64 * (n64 + 1) / 2, nfr), 128, 0, st>>>(p->d_Lb, lframes, npad, jb); p->launches += 1; }
+        if (m > 0) { const int n64 = (m + 63) / 64; k_potrf_trail<<<dim3(n64 * (n64 + 1) / 2, nfr), 128, 0, st>>>(p->d_Lb, lframes, npad, jb); p->launches += 1; p->paths[LP_OTHER]++; }
       }
       p->launches -= 1;   // (the common increment below)
     }
@@ -727,19 +737,22 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       cudaStream_t is = st;
       if (p->overlap) { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0)); is = side; side_used = true; }
       k_trinv<<<dim3(npad / 16, nfr), 256, (npad * 16 + 16 * (npad + 1)) * sizeof(double), is>>>(p->d_Lb, p->d_invT, p->d_invL, lframes, npad);
-      p->launches += 1; mark(P_TRINV);
+      p->launches += 1; p->paths[LP_TRINV]++; mark(P_TRINV);
       if (lv.ntrsm > 0) {
         const int strips = (npad + kTrsmStrip - 1) / kTrsmStrip;
-        if (strips * lv.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024)   // a single wave: deep panel prefetch, one CTA per SM
+        if (strips * lv.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) {   // a single wave: deep panel prefetch, one CTA per SM
           k_trsm_ll<4><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 4), st>>>(p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad);
-        else
+          p->paths[LP_TRSM_LL4]++;
+        } else {
           k_trsm_ll<2><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 2), st>>>(p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad);
+          p->paths[LP_TRSM_LL2]++;
+        }
         p->launches++; mark(P_TRSM);
       }
     } else {
       k_trinv<<<dim3(npad / 16, nfr), 256, (npad * 16 + 16 * (npad + 1)) * sizeof(double), st>>>(p->d_Lb, p->d_invT, p->d_invL, lframes, npad);
-      p->launches += 1; mark(P_TRINV);
-      if (lv.ntrsm > 0) { gemm(st, lv.ntrsm, p->d_T, p->d_Lb, p->d_invL, p->d_trsm_tasks + lv.trsm_off, p->d_trsm_pairs, 1.0, 0.0); p->launches++; mark(P_TRSM); }
+      p->launches += 1; p->paths[LP_TRINV]++; mark(P_TRINV);
+      if (lv.ntrsm > 0) { gemm(st, lv.ntrsm, p->d_T, p->d_Lb, p->d_invL, p->d_trsm_tasks + lv.trsm_off, p->d_trsm_pairs, 1.0, 0.0); p->launches++; p->paths[LP_TRSM_GEMM]++; mark(P_TRSM); }
     }
     }
     if (p->dist && (int)li < p->LB) {
@@ -755,10 +768,12 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     auto update = [&](cudaStream_t cs, int off, int n) {   // persistent TMA-fed update kernel
       if (n <= p->num_sms) {   // few items: two DMMA teams per tile, one CTA per SM
         k_update_tma<2><<<n, UpdShape<2>::threads, upd_smem_bytes(p->upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, 0);
+        p->paths[LP_UPD_TMA2]++;
       } else {
         int grid = std::min(n, 2 * p->num_sms);
         if (p->upd_ipc > 0) grid = std::max(grid, (n + p->upd_ipc - 1) / p->upd_ipc);
         k_update_tma<1><<<grid, UpdShape<1>::threads, upd_smem_bytes(p->upd_rb, 1), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, 0);
+        p->paths[LP_UPD_TMA1]++; if (grid < n) p->paths[LP_UPD_TMA1_MULTI]++;
       }
     };
     if (p->gemm_tma) {
@@ -769,9 +784,9 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       }
       continue;
     }
-    if (lv.nupd > 0) { gemm(st, lv.nupd, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; mark(P_GEMM); }
+    if (lv.nupd > 0) { gemm(st, lv.nupd, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM); }
     if (lv.nupd2 > 0) {
-      gemm(p->overlap ? side : st, lv.nupd2, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; mark(P_GEMM);
+      gemm(p->overlap ? side : st, lv.nupd2, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM);
       if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
     }
   }
@@ -783,21 +798,21 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   for (int l = 0; l < LS; ++l) {
     const Level& lv = p->levels[l];
     k_fwd_diag<<<dim3((npad + 7) / 8, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_rhs, p->d_ytmp, p->d_lvl_frames + lv.frame_off, npad);
-    p->launches++;
-    if (lv.nfwd > 0) { k_fwd_update<<<dim3((npad + 7) / 8, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_ytmp, p->d_rhs, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; }
+    p->launches++; p->paths[LP_SUB_LEVEL]++;
+    if (lv.nfwd > 0) { k_fwd_update<<<dim3((npad + 7) / 8, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_ytmp, p->d_rhs, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; p->paths[LP_SUB_LEVEL]++; }
   }
   if (LS < nlv && p->n_sub_tasks > 0) {
     CK(cudaMemsetAsync(p->d_sub_counters, 0, ((size_t)4 * N + 4) * sizeof(int), st));
     SubCounters cn; cn.ticket = p->d_sub_counters; cn.fin = p->d_sub_counters + 4; cn.fdone = cn.fin + N; cn.bin = cn.fdone + N; cn.bdone = cn.bin + N;
     cn.fin_need = p->d_sub_need; cn.bin_need = p->d_sub_need + N;
     k_substitution<<<std::min(p->n_sub_tasks, p->num_sms), kSubThreads, substitution_smem_bytes(npad), st>>>(p->d_invL, p->d_T, p->d_rhs, p->d_ytmp, p->d_y, p->d_sub_tasks, p->n_sub_tasks, cn, npad);
-    p->launches++;
+    p->launches++; p->paths[LP_SUB_FUSED]++;
   }
   for (int l = LS - 1; l >= 0; --l) {
     const Level& lv = p->levels[l];
-    if (lv.nfwd > 0) { k_bwd_update<<<dim3((npad + 31) / 32, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_y, p->d_ytmp, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; }
+    if (lv.nfwd > 0) { k_bwd_update<<<dim3((npad + 31) / 32, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_y, p->d_ytmp, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; p->paths[LP_SUB_LEVEL]++; }
     k_bwd_diag<<<dim3((npad + 31) / 32, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_ytmp, p->d_y, p->d_lvl_frames + lv.frame_off, npad);
-    p->launches += 1;
+    p->launches += 1; p->paths[LP_SUB_LEVEL]++;
   }
   mark(P_SOLVE);
   CK(cudaGetLastError());
@@ -807,15 +822,17 @@ static int enqueue_factor_solve(rcvd_problem* p) {
 // factor+solve through a CUDA graph (the level schedule is ~5 launches per level)
 static int factor_solve(rcvd_problem* p) {
   if (p->nranks > 1 && !p->graph_warm) {   // NCCL establishes its connections lazily on first use: not inside a stream capture
-    p->graph_warm = true;
+    p->graph_warm = true; p->factored = true;
     return enqueue_factor_solve(p);
   }
   if (!p->solve_graph) {
     cudaGraph_t graph;
     const int64_t l0 = p->launches;
+    int64_t paths0[LP_N]; std::copy(p->paths, p->paths + LP_N, paths0);
     CK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
     int rc = enqueue_factor_solve(p);
     cudaError_t e = cudaStreamEndCapture(p->stream, &graph);
+    for (int i = 0; i < LP_N; ++i) { p->graph_paths[i] = p->paths[i] - paths0[i]; p->paths[i] = paths0[i]; }
     if (rc) return rc;
     if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
     CK(cudaGraphInstantiate(&p->solve_graph, graph, 0));
@@ -825,6 +842,8 @@ static int factor_solve(rcvd_problem* p) {
   }
   CK(cudaGraphLaunch(p->solve_graph, p->stream));
   p->launches += p->graph_launches;
+  for (int i = 0; i < LP_N; ++i) p->paths[i] += p->graph_paths[i];
+  p->factored = true;
   return RCVD_OK;
 }
 
@@ -1349,6 +1368,23 @@ RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
   if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "copy failed: %s", cudaGetErrorString(e));
   return RCVD_OK;
 }
+// factorisation + solve of (S H S + diag(D2)) y = b with the H blocks already on the device; S == nullptr: S = 1
+static int solve_loaded(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y) {
+  const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t Upad = (size_t)N * npad;
+  std::vector<double> hs(Upad, 1.0), hd(Upad, 1.0), hb(Upad, 0.0);
+  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) { const size_t u = (size_t)p->uperm[f] * nf + l; hs[(size_t)f * npad + l] = S ? S[u] : 1.0; hd[(size_t)f * npad + l] = D2[u]; hb[(size_t)f * npad + l] = b[u]; }
+  CK(cudaMemcpyAsync(p->d_S, hs.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
+  CK(cudaMemcpyAsync(p->d_D2, hd.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
+  CK(cudaMemcpyAsync(p->d_gs, hb.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
+  CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), p->stream));
+  int rc = factor_solve(p); if (rc) return rc;
+  std::vector<double> hy(Upad);
+  CK(cudaMemcpyAsync(hy.data(), p->d_y, Upad * 8, cudaMemcpyDeviceToHost, p->stream));
+  rc = read_scalars(p); if (rc) return rc;
+  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) y[(size_t)p->uperm[f] * nf + l] = hy[(size_t)f * npad + l];
+  if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, "factorisation hit a non-positive pivot");
+  return RCVD_OK;
+}
 // Debug/test: solve (S H S + diag(D2)) y = b with H = J^T J at the current state.
 // S, D2, b, y: N*stride host doubles.
 RCVD_API int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y) {
@@ -1356,19 +1392,67 @@ RCVD_API int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
   rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST); if (rc) return rc;
-  const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t Upad = (size_t)N * npad;
-  std::vector<double> hs(Upad, 1.0), hd(Upad, 1.0), hb(Upad, 0.0);
-  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) { const size_t u = (size_t)p->uperm[f] * nf + l; hs[(size_t)f * npad + l] = S[u]; hd[(size_t)f * npad + l] = D2[u]; hb[(size_t)f * npad + l] = b[u]; }
-  CK(cudaMemcpyAsync(p->d_S, hs.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
-  CK(cudaMemcpyAsync(p->d_D2, hd.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
-  CK(cudaMemcpyAsync(p->d_gs, hb.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
-  CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), p->stream));
-  rc = factor_solve(p); if (rc) return rc;
-  std::vector<double> hy(Upad);
-  CK(cudaMemcpyAsync(hy.data(), p->d_y, Upad * 8, cudaMemcpyDeviceToHost, p->stream));
-  rc = read_scalars(p); if (rc) return rc;
-  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) y[(size_t)p->uperm[f] * nf + l] = hy[(size_t)f * npad + l];
-  if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, "factorisation hit a non-positive pivot");
+  return solve_loaded(p, S, D2, b, y);
+}
+// Test hook: (H + diag(D2)) y = b for a caller-supplied dense symmetric H (U x U, U = N * stride, caller's frame order) through the
+// production factorisation graph with S = 1.  H is scattered into the H blocks of the problem's frame graph (no evaluation); an entry
+// in a frame pair the graph does not couple is an error.
+RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
+  if (!p || !H || !D2 || !b || !y) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (p->nranks > 1) return set_err(RCVD_ERR_INVALID, "rcvd_debug_solve_matrix works on single-GPU handles only");
+  if (p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no factor storage");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
+  std::vector<uint8_t> coupled((size_t)N * N, 0);
+  for (const HBlock& hb : p->hblocks) { const int a = p->uperm[hb.r], c = p->uperm[hb.c]; coupled[(size_t)a * N + c] = coupled[(size_t)c * N + a] = 1; }
+  for (int a = 0; a < N; ++a) for (int c = 0; c < N; ++c) {
+    if (coupled[(size_t)a * N + c]) continue;
+    for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j)
+      if (H[((size_t)a * nf + i) * U + (size_t)c * nf + j] != 0.0)
+        return set_err(RCVD_ERR_INVALID, "H couples frames %d and %d, which the problem's frame graph does not couple", a, c);
+  }
+  std::vector<double> hH((size_t)p->nHblocks * bs, 0.0);
+  for (int h = 0; h < p->nHblocks; ++h) {        // block h holds rows of frame r, columns of frame c (internal ids)
+    const int a = p->uperm[p->hblocks[h].r], c = p->uperm[p->hblocks[h].c];
+    for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) hH[h * bs + (size_t)i * npad + j] = H[((size_t)a * nf + i) * U + (size_t)c * nf + j];
+  }
+  CK(cudaMemcpyAsync(p->d_H, hH.data(), hH.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+  return solve_loaded(p, nullptr, D2, b, y);
+}
+// Test hook: the factor the last factorisation left on the device (see include/rcvd_hooks.h).
+RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, double* Linv) {
+  if (!p || !order || !L) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (!p->structure_ready || !p->factored) return set_err(RCVD_ERR_INVALID, "no factorisation has run on this handle");
+  if (p->dist) return set_err(RCVD_ERR_INVALID, "the distributed factorisation keeps its blocks on their owners");
+  SET_DEVICE(p->device);
+  CK(cudaStreamSynchronize(p->side_stream)); CK(cudaStreamSynchronize(p->stream));
+  const int N = p->N, nf = p->L.nf, npad = p->L.npad, nT = p->nLoff; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
+  std::vector<double> hL((size_t)N * bs), hT((size_t)nT * bs);
+  CK(cudaMemcpy(hL.data(), p->d_Lb, hL.size() * sizeof(double), cudaMemcpyDeviceToHost));   // the first N blocks: diagonal blocks L_kk
+  if (nT > 0) CK(cudaMemcpy(hT.data(), p->d_T, hT.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  std::vector<size_t> off(N);
+  for (int q = 0; q < N; ++q) { off[p->elim_order[q]] = (size_t)q * nf; order[q] = p->uperm[p->elim_order[q]]; }
+  std::fill(L, L + U * U, 0.0);
+  for (int f = 0; f < N; ++f)                      // lower triangle only: the update epilogue may leave values above the diagonal
+    for (int i = 0; i < nf; ++i) for (int j = 0; j <= i; ++j) L[(off[f] + i) * U + off[f] + j] = hL[f * bs + (size_t)i * npad + j];
+  for (int t = 0; t < nT; ++t) {
+    const HBlock& b = p->lblocks_h[N + t];
+    for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) L[(off[b.r] + i) * U + off[b.c] + j] = hT[t * bs + (size_t)i * npad + j];
+  }
+  if (Linv) {
+    CK(cudaMemcpy(hL.data(), p->d_invL, hL.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (int f = 0; f < N; ++f) {
+      double* out = Linv + off[f] * nf;
+      for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) out[(size_t)i * nf + j] = j <= i ? hL[f * bs + (size_t)i * npad + j] : 0.0;
+    }
+  }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]) {
+  if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  static_assert(LP_N == 13, "include/rcvd_hooks.h documents thirteen counters");
+  std::copy(p->paths, p->paths + LP_N, out);
   return RCVD_OK;
 }
 RCVD_API int32_t rcvd_time_accumulate(rcvd_problem* p, int32_t iters, double* ms) {
@@ -1440,7 +1524,7 @@ RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double
     CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), p->stream));
     evs.clear(); p->prof = &evs;
     rc = enqueue_factor_solve(p);
-    p->prof = nullptr;
+    p->prof = nullptr; p->factored = true;
     cudaStreamSynchronize(p->stream); cudaStreamSynchronize(p->side_stream);
     double ngemm = 0;
     for (size_t i = 1; i < evs.size(); ++i) {

@@ -136,6 +136,32 @@ class Problem:
         _check(self.L.rcvd_debug_linear_solve(self.h, _p(S, C.c_double), _p(D2, C.c_double), _p(b, C.c_double), _p(y, C.c_double)))
         return y
 
+    def solve_matrix(self, H, D2, b):
+        """Test hook: y = (H + diag(D2))^-1 b through the production factorisation graph (S = 1) for a dense symmetric H [U, U] in the
+        caller's frame order, restricted to the frame graph set by set_structure / set_constraints."""
+        H = np.ascontiguousarray(H, np.float64); D2 = np.ascontiguousarray(D2, np.float64); b = np.ascontiguousarray(b, np.float64)
+        assert H.shape == (self.U, self.U) and D2.size == self.U and b.size == self.U
+        y = np.zeros(self.U, np.float64)
+        _check(self.L.rcvd_debug_solve_matrix(self.h, _p(H, C.c_double), _p(D2, C.c_double), _p(b, C.c_double), _p(y, C.c_double)))
+        return y
+
+    def factor_dense(self, inverses=False):
+        """Test hook: (order, L, Linv) of the last factorisation -- caller's frame index of each eliminated frame, the dense lower factor
+        of P A P^T in that order, and (inverses=True) the explicit inverses of its diagonal blocks [N, stride, stride], else None."""
+        order = np.zeros(self.N, np.int32); Lf = np.zeros((self.U, self.U), np.float64)
+        Li = np.zeros((self.N, self.stride, self.stride), np.float64) if inverses else None
+        _check(self.L.rcvd_debug_factor_dense(self.h, _p(order, C.c_int32), _p(Lf, C.c_double), _p(Li, C.c_double)))
+        return order, Lf, Li
+
+    LINEAR_PATHS = ("potrf_smem", "potrf_panel", "trsm_ll4", "trsm_ll2", "trsm_gemm", "update_tma1", "update_tma2", "update_gemm",
+                    "substitution_levels", "substitution_fused", "trinv", "other", "update_tma1_multi_item")
+
+    def linear_paths(self):
+        """Test hook: launches of each factorisation / solve kernel path since the handle was created (LINEAR_PATHS)."""
+        out = (C.c_int64 * len(self.LINEAR_PATHS))()
+        _check(self.L.rcvd_debug_linear_paths(self.h, out))
+        return dict(zip(self.LINEAR_PATHS, list(out)))
+
     def solve(self, options=None):
         opt = options or abi.default_solve_options()
         s = abi.SolveSummary()
