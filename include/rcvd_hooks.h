@@ -17,6 +17,16 @@ int64_t rcvd_builder_last_rounds(void);          /* selection rounds of the last
 /* {frames, off-diagonal factor blocks, levels, H blocks, npad, stride, tiles, update tasks} */
 int32_t rcvd_structure_info(rcvd_problem* p, int32_t out[8]);
 
+/* the block-Cholesky plan (robust_cvd_b200/csrc/rcvd_plan.h) of the frame graph of np pairs and nt triplet centres under cfg (shared
+ * intrinsics, position regulariser, stride), as rank `rank` of `nranks` with the distributed factorisation enabled, on a device of
+ * num_sms SMs.  Host only: no handle, no device.  Per frame, in the caller's frame ids: order[N] = elimination order, level[N] = level,
+ * owner[N] = owning rank, perm[N] = caller's frame of each internal frame id.  out = {levels, off-diagonal factor blocks, H blocks,
+ * update targets, k_update_tma items, k_substitution tasks, distributed, first replicated level, first k_substitution level,
+ * this rank's L blocks, H blocks, frames}.  An out-of-range pair or triplet centre: RCVD_ERR_INVALID. */
+int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                               int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
+                               int32_t* order, int32_t* level, int32_t* owner, int32_t* perm, int32_t out[12]);
+
 /* y = (S H S + diag(D2))^-1 b with the current H (exercises factorisation + substitution alone) */
 int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y);
 

@@ -12,8 +12,6 @@
 #include <cstring>
 #include <dlfcn.h>
 #include <limits>
-#include <map>
-#include <set>
 #include <string>
 #include <vector>
 
@@ -21,6 +19,7 @@
 #include "rcvd_eval.cuh"
 #include "rcvd_linalg.cuh"
 #include "rcvd_update.cuh"
+#include "rcvd_plan.h"
 #include "rcvd_dense.cuh"
 #include "rcvd_filter.cuh"
 #include "rcvd_bilateral.cuh"
@@ -178,8 +177,6 @@ enum { LP_POTRF_SMEM = 0, LP_POTRF_PANEL, LP_TRSM_LL4, LP_TRSM_LL2, LP_TRSM_GEMM
        LP_TRINV, LP_OTHER, LP_UPD_TMA1_MULTI, LP_N };   // LP_UPD_TMA1_MULTI: k_update_tma<1> launches with fewer CTAs than items
 
 // ---------------------------------------------------------------------------
-struct Level { int frame_off, nframes; int trsm_off, ntrsm; int upd_off, nupd; int upd2_off, nupd2; int fwd_off, nfwd; int it_off, nit, it2_off, nit2; int own_off, nown; };   // frame_off: every frame of the level (substitution); own_off: the frames this rank factors   // upd: targets consumed by the next level; upd2: the rest
-
 struct rcvd_problem {
   rcvd_config cfg; Layout L; int N = 0; int device = 0;
   cudaStream_t stream = nullptr;
@@ -203,12 +200,12 @@ struct rcvd_problem {
   int npartial = 0;
   // matrices
   double *d_H = nullptr, *d_Lb = nullptr, *d_T = nullptr, *d_invL = nullptr, *d_invT = nullptr;
-  int nHblocks = 0, nLoff = 0; HBlock *d_hblocks = nullptr, *d_lblocks = nullptr; int* d_fail = nullptr;
-  std::vector<HBlock> hblocks;
-  // schedule
-  std::vector<Level> levels; int *d_lvl_frames = nullptr; GemmTask *d_trsm_tasks = nullptr, *d_upd_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
-  SubTask* d_sub_tasks = nullptr; int n_sub_tasks = 0; int* d_sub_counters = nullptr; int* d_sub_need = nullptr; int sub_first_level = 0;   // k_substitution: levels >= sub_first_level
-  SolveTask *d_fwd_tasks = nullptr, *d_col_tasks = nullptr; int* d_col_ptr = nullptr; TrsmTask* d_trsm_ll = nullptr; bool use_trsm_ll = false;
+  HBlock *d_hblocks = nullptr, *d_lblocks = nullptr; int* d_fail = nullptr;
+  // the block-Cholesky plan (rcvd_plan.h) and its device copies
+  FactorPlan plan;
+  int *d_lvl_frames = nullptr; GemmTask *d_trsm_tasks = nullptr, *d_upd_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
+  SubTask* d_sub_tasks = nullptr; int* d_sub_counters = nullptr; int* d_sub_need = nullptr;
+  SolveTask* d_fwd_tasks = nullptr; TrsmTask* d_trsm_ll = nullptr; bool use_trsm_ll = false;
   cudaGraphExec_t solve_graph = nullptr;
   bool structure_ready = false, constraints_set = false, frames_set = false;
   // multi GPU
@@ -221,19 +218,17 @@ struct rcvd_problem {
   std::vector<void*> allocs;
   // kernel-class profiling (rcvd_debug_profile_linear): when set, enqueue_factor_solve records one event per launch
   std::vector<std::pair<int, cudaEvent_t>>* prof = nullptr;
-  // distributed factorisation (nranks > 1): ownership, internal frame numbering, broadcast / reduce segments
   bool eval_only = false;   // test / bench hook: only rcvd_evaluate is used (no H, no factor storage)
   bool records_sorted = false;   // run path of the accumulate kernel (bilinear depth grid): records sorted by cell pair
-  bool dist_enabled = true, dist = false, identity_perm = true, graph_warm = false, force_full_H = false; int LB = 0;
-  std::vector<int> uperm, iperm, fa_off, fa_cnt, fb_off, fb_cnt, tseg, bseg, hseg;   // *_off/_cnt: per-owner frame ranges (phase A / B); segs: (first, count) pairs
-  int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr; int n_own_l = 0, n_own_h = 0;
+  bool dist_enabled = true, graph_warm = false, force_full_H = false;
+  // distributed factorisation (nranks > 1): the frames this rank factors per level, the blocks it owns, internal -> caller's frame ids
+  int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr;
   // TMA-fed persistent update kernel (rcvd_update.cuh)
-  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int upd_rb = 0, upd_neff = 0, num_sms = 132, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
+  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int num_sms = 0, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
-  double upd_flops = 0.0;   // algorithmic flops of the update GEMMs of one factorisation (2 nf^3 per product, nf^2 (nf+1) on symmetric targets)
-  // test hooks (rcvd_debug_factor_dense, rcvd_debug_linear_paths): elimination order (internal frame ids), every factor block's
-  // (row frame, column frame), per-kernel-path launch counters (enqueue_factor_solve counts, graph replays add graph_paths)
-  std::vector<int> elim_order; std::vector<HBlock> lblocks_h; bool factored = false;
+  // test hooks (rcvd_debug_factor_dense, rcvd_debug_linear_paths): whether a factorisation has run, per-kernel-path launch counters
+  // (enqueue_factor_solve counts, graph replays add graph_paths)
+  bool factored = false;
   int64_t paths[LP_N] = {0}, graph_paths[LP_N] = {0};
   rcvd_problem() {}
 };
@@ -273,255 +268,22 @@ static DevProblem dev_problem(const rcvd_problem* p) {
   return d;
 }
 
-// ---- structure: block layout, elimination order, level schedule ----
-static int build_structure(rcvd_problem* p) {
-  free_all(p);
-  const int N = p->N; const Layout& L = p->L; const int npad = L.npad; const size_t bs = (size_t)npad * npad;
-  CK(cudaSetDevice(p->device));
-  // frame graph
-  std::vector<std::set<int>> adj(N);
-  auto addEdge = [&](int a, int b) { if (a != b) { adj[a].insert(b); adj[b].insert(a); } };
-  const std::vector<int32_t>& sp = p->struct_pairs.empty() ? p->pair_frames : p->struct_pairs;
-  for (size_t i = 0; i + 1 < sp.size(); i += 2) {
-    const int a = sp[i], b = sp[i + 1];
-    if (a < 0 || a >= N || b < 0 || b >= N) return set_err(RCVD_ERR_INVALID, "pair frame index out of range");
-    addEdge(a, b);
-    if (p->cfg.intr_opt == RCVD_INTR_SHARED) { addEdge(a, 0); addEdge(b, 0); }
-  }
-  if (p->cfg.position_reg > 0.0) for (int f = 0; f + 2 < N; ++f) { addEdge(f, f + 1); addEdge(f, f + 2); addEdge(f + 1, f + 2); }
-  for (size_t t = 0; t < p->trip_centers.size(); ++t) {
-    const int f = p->trip_centers[t];
-    if (f < 1 || f + 1 >= N) return set_err(RCVD_ERR_INVALID, "triplet centre frame out of range");
-    addEdge(f - 1, f); addEdge(f - 1, f + 1); addEdge(f, f + 1);
-    if (p->cfg.intr_opt == RCVD_INTR_SHARED) { addEdge(f - 1, 0); addEdge(f, 0); addEdge(f + 1, 0); }
-  }
-  std::vector<std::set<int>> orig = adj;
-  // Multiple minimum-degree elimination: each round eliminates a maximal independent set of frames whose current degree is
-  // within `slack` of the minimum (ties -> lowest frame id).  slack = 0 is plain greedy minimum degree one frame at a time
-  // semantics-wise; a small slack trades a few % more fill for a shallower elimination tree (fewer sequential levels).
-  std::vector<int> order, pos(N, -1); std::vector<std::vector<int>> cs(N);
-  {
-    std::vector<uint8_t> done(N, 0);
-    const int slack = p->order_slack;
-    while ((int)order.size() < N) {
-      size_t md = (size_t)-1;
-      for (int f = 0; f < N; ++f) if (!done[f]) md = std::min(md, adj[f].size());
-      std::vector<int> cand;
-      const size_t lim = md + (size_t)(slack > 0 ? slack : 0);
-      for (int f = 0; f < N; ++f) if (!done[f] && adj[f].size() <= lim) cand.push_back(f);
-      std::stable_sort(cand.begin(), cand.end(), [&](int a, int b) { return adj[a].size() < adj[b].size(); });
-      std::vector<uint8_t> blocked(N, 0); std::vector<int> chosen;
-      for (int f : cand) { if (blocked[f]) continue; chosen.push_back(f); blocked[f] = 1; for (int a : adj[f]) blocked[a] = 1; if (slack < 0) break; }
-      for (int best : chosen) {
-        done[best] = 1; pos[best] = (int)order.size(); order.push_back(best);
-        std::vector<int> nb(adj[best].begin(), adj[best].end());
-        cs[best] = nb;
-        for (int a : nb) adj[a].erase(best);
-        for (size_t i = 0; i < nb.size(); ++i) for (size_t j = i + 1; j < nb.size(); ++j) { adj[nb[i]].insert(nb[j]); adj[nb[j]].insert(nb[i]); }
-      }
-    }
-    for (int f = 0; f < N; ++f) std::sort(cs[f].begin(), cs[f].end(), [&](int a, int b) { return pos[a] < pos[b]; });
-  }
-  // levels
-  std::vector<int> lvl(N, 0); int nl = 0;
-  for (int k : order) { for (int a : cs[k]) lvl[a] = std::max(lvl[a], lvl[k] + 1); nl = std::max(nl, lvl[k] + 1); }
-  std::vector<std::vector<int>> lf(nl);
-  for (int k : order) lf[lvl[k]].push_back(k);
-
-  // ---- multi-GPU distribution of the factorisation (DESIGN.md section 5) ----
-  // Phase A = the wide early levels (throughput-bound: thousands of block products): every frame (= block column of the factor) has an
-  // owner rank that factors it (potrf, trsm) and computes every update INTO its column; after the trsm of a level the new off-diagonal
-  // factor blocks X_rk are broadcast from their owners (they are the operands of everybody's updates and of the replicated
-  // substitution).  Phase B = the tail of narrow levels (< 3 frames per level: a latency chain that does not shard) is replicated:
-  // at the boundary every owner broadcasts its trailing blocks.  H is reduced to the owners only (no all-reduce of the matrix).
-  const int R = p->nranks;
-  bool dist = R > 1 && p->dist_enabled && p->cfg.intr_opt != RCVD_INTR_SHARED && !(p->cfg.position_reg > 0.0) && p->trip_centers.empty();
-  int LB = 0;
-  if (dist) { LB = nl; while (LB > 0 && (int)lf[LB - 1].size() < 3) --LB; if (LB == 0) dist = false; }
-  p->dist = dist; p->LB = LB;
-  std::vector<int> own(N, 0);
-  if (dist) {
-    // incoming update work of every column over the phase-A levels (block products; symmetric targets count half)
-    std::vector<double> tot_in(N, 0.0);
-    for (int l = 0; l < LB; ++l) for (int k : lf[l]) { const auto& m = cs[k]; for (size_t a = 0; a < m.size(); ++a) for (size_t b = 0; b <= a; ++b) tot_in[m[b]] += (a == b) ? 0.5 : 1.0; }
-    std::vector<double> load(R, 0.0);
-    for (int l = 0; l < nl; ++l) {
-      std::vector<int> fr = lf[l];
-      auto w = [&](int k) { return tot_in[k] + (l < LB ? 0.6 * cs[k].size() + 0.3 : 0.0); };   // + its own trsm / potrf
-      std::stable_sort(fr.begin(), fr.end(), [&](int a, int b) { return w(a) > w(b); });
-      for (int k : fr) { int q = 0; for (int t = 1; t < R; ++t) if (load[t] < load[q]) q = t; own[k] = q; load[q] += w(k); }
-    }
-  }
-  // internal frame numbering: owner-major, phase-A frames first -- every per-frame array an owner broadcasts / reduces is one contiguous range
-  std::vector<int> uperm, iperm(N, -1);
-  p->fa_off.assign(R, 0); p->fa_cnt.assign(R, 0); p->fb_off.assign(R, 0); p->fb_cnt.assign(R, 0);
-  for (int q = 0; q < R; ++q) for (int ph = 0; ph < 2; ++ph) {
-    (ph ? p->fb_off : p->fa_off)[q] = (int)uperm.size();
-    for (int f = 0; f < N; ++f) if (own[f] == q && ((lvl[f] >= LB) == (ph == 1))) uperm.push_back(f);
-    (ph ? p->fb_cnt : p->fa_cnt)[q] = (int)uperm.size() - (ph ? p->fb_off : p->fa_off)[q];
-  }
-  for (int i = 0; i < N; ++i) iperm[uperm[i]] = i;
-  p->identity_perm = true; for (int i = 0; i < N; ++i) if (uperm[i] != i) p->identity_perm = false;
-  p->uperm = uperm; p->iperm = iperm;
-  if (!p->identity_perm) {
-    auto I = [&](int f) { return iperm[f]; };
-    std::vector<int> order2(N), pos2(N), lvl2(N), own2(N); std::vector<std::vector<int>> cs2(N); std::vector<std::set<int>> orig2(N);
-    for (int i = 0; i < N; ++i) order2[i] = I(order[i]);
-    for (int f = 0; f < N; ++f) { pos2[I(f)] = pos[f]; lvl2[I(f)] = lvl[f]; own2[I(f)] = own[f]; for (int a : cs[f]) cs2[I(f)].push_back(I(a)); for (int a : orig[f]) orig2[I(f)].insert(I(a)); }
-    for (auto& v : lf) for (int& k : v) k = I(k);
-    order.swap(order2); pos.swap(pos2); lvl.swap(lvl2); own.swap(own2); cs.swap(cs2); orig.swap(orig2);
-  }
-  // L off-diagonal blocks (r later than c).  Phase A: level-major, owner-major inside a level (what a rank produces in one level is one
-  // contiguous range of T); phase B: owner-major (what a rank owns of the trailing matrix is one contiguous range of L).
-  std::map<std::pair<int, int>, int> lid; int nLoff = 0;
-  std::vector<int> lcol;   // column (earlier-eliminated) frame of each off-diagonal factor block
-  auto number_col = [&](int k) { for (int r : cs[k]) { lid[{r, k}] = N + nLoff++; lcol.push_back(k); } };
-  p->tseg.assign((size_t)std::max(LB, 0) * R * 2, 0); p->bseg.assign((size_t)R * 2, 0);
-  for (int l = 0; l < LB; ++l) for (int q = 0; q < R; ++q) {
-    const int first = nLoff;
-    for (int k : lf[l]) if (own[k] == q) number_col(k);
-    p->tseg[((size_t)l * R + q) * 2] = first; p->tseg[((size_t)l * R + q) * 2 + 1] = nLoff - first;
-  }
-  for (int q = 0; q < R; ++q) {
-    const int first = nLoff;
-    for (int l = LB; l < nl; ++l) for (int k : lf[l]) if (own[k] == q) number_col(k);
-    p->bseg[(size_t)q * 2] = first; p->bseg[(size_t)q * 2 + 1] = nLoff - first;
-  }
-  p->nLoff = nLoff;
-  // H blocks: diagonal first (internal frame order = owner-major), then original off-diagonals oriented (later, earlier), owner-major
-  p->hblocks.clear();
-  std::vector<int32_t> blk_of((size_t)N * N, -1);
-  for (int f = 0; f < N; ++f) p->hblocks.push_back({f, f, f});
-  p->hseg.assign((size_t)R * 2, 0);
-  for (int q = 0; q < R; ++q) {
-    p->hseg[(size_t)q * 2] = (int)p->hblocks.size();
-    for (int a = 0; a < N; ++a) for (int b : orig[a]) if (a < b) {
-      const int r = pos[a] > pos[b] ? a : b, c = pos[a] > pos[b] ? b : a;
-      if (own[c] != q) continue;
-      const int hid = (int)p->hblocks.size();
-      p->hblocks.push_back({lid[{r, c}], r, c});
-      blk_of[(size_t)r * N + c] = hid * 2 + 1;   // (fa = r) is the row side
-      blk_of[(size_t)c * N + r] = hid * 2 + 0;
-    }
-    p->hseg[(size_t)q * 2 + 1] = (int)p->hblocks.size() - p->hseg[(size_t)q * 2];
-  }
-  p->nHblocks = (int)p->hblocks.size();
-  // all L blocks with their H source (or -1)
-  std::vector<HBlock> lblocks(N + nLoff);
-  for (int f = 0; f < N; ++f) lblocks[f] = {f, f, f};
-  for (auto& kv : lid) lblocks[kv.second] = {-1, kv.first.first, kv.first.second};
-  for (int h = N; h < p->nHblocks; ++h) lblocks[p->hblocks[h].lblk].lblk = h;
-  p->elim_order = order; p->lblocks_h = lblocks;
-  // blocks this rank owns: what it loads into the factor and what it multiplies in the model term (all of them without distribution)
-  std::vector<int> own_lblocks, own_hblocks;
-  for (int b = 0; b < N + nLoff; ++b) { const int c = b < N ? b : lcol[b - N]; if (!dist || own[c] == p->rank) own_lblocks.push_back(b); }
-  for (int h = 0; h < p->nHblocks; ++h) if (!dist || own[p->hblocks[h].c] == p->rank) own_hblocks.push_back(h);
-  p->n_own_l = (int)own_lblocks.size(); p->n_own_h = (int)own_hblocks.size();
-  double upd_flops = 0.0;
-  std::vector<int> lvl_frames, lvl_own; std::vector<GemmTask> trsm_tasks, upd_tasks; std::vector<int2> trsm_pairs, upd_pairs;
-  std::vector<SolveTask> fwd_tasks, col_tasks; std::vector<int> col_ptr(N + 1, 0); std::vector<TrsmTask> trsm_ll;
-  std::vector<UpdItem> upd_items;
-  // tile cut of the update targets: kUpdMaxTile-row tiles over the unknowns (rounded to 8)
-  const int upd_neff = std::min(npad, (L.nf + 7) / 8 * 8);
-  const int upd_nt = (upd_neff + kUpdMaxTile - 1) / kUpdMaxTile;
-  const int upd_tile = std::min(kUpdMaxTile, upd_neff);          // 80-row tiles (balanced 5 x 5 units per warp), the remainder last
-  p->upd_rb = upd_tile; p->upd_neff = upd_neff;
-  p->levels.clear();
-  for (int l = 0; l < nl; ++l) {
-    Level lv; lv.frame_off = (int)lvl_frames.size(); lv.nframes = (int)lf[l].size(); lv.own_off = (int)lvl_own.size();
-    lv.trsm_off = (int)trsm_tasks.size(); lv.upd_off = (int)upd_tasks.size(); lv.fwd_off = (int)fwd_tasks.size();
-    std::map<int, std::vector<int2>> upd;   // target L block id -> source pairs
-    const bool shared_level = !dist || l >= LB;   // replicated work: every rank does all of it
-    for (int k : lf[l]) {
-      lvl_frames.push_back(k);
-      const bool mine = shared_level || own[k] == p->rank;
-      if (mine) lvl_own.push_back(k);
-      for (int r : cs[k]) {
-        const int id = lid[{r, k}];
-        if (mine) {
-          trsm_tasks.push_back({id - N, (int)trsm_pairs.size(), 1, 2});
-          trsm_pairs.push_back(make_int2(id, k));
-          trsm_ll.push_back({id - N, id, k});
-        }
-        fwd_tasks.push_back({id - N, r, k});
-      }
-      for (size_t a = 0; a < cs[k].size(); ++a) for (size_t b = 0; b <= a; ++b) {
-        const int r = cs[k][a], c = cs[k][b];                     // c is eliminated before r: the target lives in column c
-        if (!shared_level && own[c] != p->rank) continue;
-        const int target = (r == c) ? r : lid[{r, c}];
-        upd[target].push_back(make_int2(lid[{r, k}] - N, lid[{c, k}] - N));
-      }
-    }
-    lv.nown = (int)lvl_own.size() - lv.own_off;
-    // targets whose column frame is eliminated in the very next level must be complete before that level starts (critical);
-    // all other updates may overlap the next level's potrf / inverse / trsm on a second stream.
-    for (int pass = 0; pass < 2; ++pass) {
-      if (pass == 1) lv.upd2_off = (int)upd_tasks.size();
-      for (auto& kv : upd) {
-        const int cframe = kv.first < N ? kv.first : lcol[kv.first - N];
-        const bool critical = (lvl[cframe] == l + 1);
-        if (critical != (pass == 0)) continue;
-        upd_tasks.push_back({kv.first, (int)upd_pairs.size(), (int)kv.second.size(), kv.first < N ? 1 : 0});
-        { const double n = (double)L.nf; upd_flops += (double)kv.second.size() * (kv.first < N ? n * n * (n + 1.0) : 2.0 * n * n * n); }
-        upd_pairs.insert(upd_pairs.end(), kv.second.begin(), kv.second.end());
-      }
-    }
-    lv.ntrsm = (int)trsm_tasks.size() - lv.trsm_off; lv.nupd = lv.upd2_off - lv.upd_off; lv.nupd2 = (int)upd_tasks.size() - lv.upd2_off; lv.nfwd = (int)fwd_tasks.size() - lv.fwd_off;
-    // work items of the persistent update kernel: one per (target tile, source-pair list), heaviest first
-    for (int pass = 0; pass < 2; ++pass) {
-      const int t0 = pass ? lv.upd2_off : lv.upd_off, tn = pass ? lv.nupd2 : lv.nupd;
-      const size_t i0 = upd_items.size();
-      for (int q = t0; q < t0 + tn; ++q) {
-        const GemmTask& tk = upd_tasks[q];
-        for (int ti = 0; ti < upd_nt; ++ti) for (int tj = 0; tj < ((tk.lower_only & 1) ? ti + 1 : upd_nt); ++tj) {
-          UpdItem it; it.dst = tk.dst; it.first = tk.first; it.count = tk.count; it.m0 = (short)(ti * upd_tile); it.n0 = (short)(tj * upd_tile);
-          it.mrows = (short)std::min(upd_tile, upd_neff - ti * upd_tile); it.ncols = (short)std::min(upd_tile, upd_neff - tj * upd_tile);
-          it.flags = ((tk.lower_only & 1) && ti == tj) ? 1 : 0;
-          upd_items.push_back(it);
-        }
-      }
-      auto cost = [](const UpdItem& a) { return (long)a.count * (a.mrows / 8) * (a.ncols / 8) * ((a.flags & 1) ? 3 : 4); };
-      std::stable_sort(upd_items.begin() + i0, upd_items.end(), [&](const UpdItem& a, const UpdItem& b) { return cost(a) > cost(b); });
-      if (pass) { lv.it2_off = (int)i0; lv.nit2 = (int)(upd_items.size() - i0); } else { lv.it_off = (int)i0; lv.nit = (int)(upd_items.size() - i0); }
-    }
-    p->levels.push_back(lv);
-  }
-  for (int k = 0; k < N; ++k) { col_ptr[k] = (int)col_tasks.size(); for (int r : cs[k]) col_tasks.push_back({lid[{r, k}] - N, r, k}); }
-  col_ptr[N] = (int)col_tasks.size();
-  // task list of the fused substitution kernel (k_substitution): forward levels ascending, backward levels descending, every GEMV cut
-  // into kSubChunk-row / -column chunks; a task depends only on tasks before it
-  std::vector<SubTask> sub_tasks; std::vector<int> sub_need(2 * (size_t)N, 0);
-  {
-    const int nch = (npad + kSubChunk - 1) / kSubChunk;
-    // The wide levels at the bottom of the tree stay level-scheduled launches (thousands of independent GEMVs: a launch spreads them
-    // over the machine at once, a persistent CTA works through them one memory latency at a time); the narrow levels above them -- a
-    // latency chain of four tiny launches per level -- run as ONE dataflow kernel: forward narrow, backward narrow in a single launch.
-    const int limit = 4 * p->num_sms;
-    int LS = (int)p->levels.size();
-    while (LS > 0 && (p->levels[LS - 1].nframes + p->levels[LS - 1].nfwd) * nch <= limit) --LS;
-    p->sub_first_level = LS;
-    for (size_t l = LS; l < p->levels.size(); ++l) {
-      const Level& lv = p->levels[l];
-      for (int i = 0; i < lv.nframes; ++i) for (int c = 0; c < nch; ++c) sub_tasks.push_back({0, -1, -1, lvl_frames[lv.frame_off + i], c});
-      for (int q = 0; q < lv.nfwd; ++q) { const SolveTask& t = fwd_tasks[lv.fwd_off + q]; for (int c = 0; c < nch; ++c) sub_tasks.push_back({1, t.blk, t.r, t.k, c}); sub_need[t.r] += nch; sub_need[N + t.k] += nch; }
-    }
-    for (int l = (int)p->levels.size() - 1; l >= LS; --l) {
-      const Level& lv = p->levels[l];
-      for (int q = 0; q < lv.nfwd; ++q) { const SolveTask& t = fwd_tasks[lv.fwd_off + q]; for (int c = 0; c < nch; ++c) sub_tasks.push_back({2, t.blk, t.r, t.k, c}); }
-      for (int i = 0; i < lv.nframes; ++i) for (int c = 0; c < nch; ++c) sub_tasks.push_back({3, -1, -1, lvl_frames[lv.frame_off + i], c});
-    }
-    p->n_sub_tasks = (int)sub_tasks.size();
-  }
-
-  // ---- device allocations ----
-  int rc;
+// ---- structure: the plan on the device, the problem data, the storage ----
 #define UP(ptr, vec) if ((rc = upload(p, &(ptr), vec))) return rc
-  p->upd_flops = upd_flops;
-  UP(p->d_blk_of, blk_of); UP(p->d_hblocks, p->hblocks); UP(p->d_lblocks, lblocks); UP(p->d_lvl_frames, lvl_frames); UP(p->d_lvl_own, lvl_own);
-  UP(p->d_own_lblocks, own_lblocks); UP(p->d_own_hblocks, own_hblocks); UP(p->d_uperm, p->uperm);
-  UP(p->d_trsm_tasks, trsm_tasks); UP(p->d_upd_tasks, upd_tasks); UP(p->d_trsm_pairs, trsm_pairs); UP(p->d_upd_pairs, upd_pairs);
-  UP(p->d_sub_tasks, sub_tasks); UP(p->d_sub_need, sub_need); if ((rc = dalloc(p, &p->d_sub_counters, (size_t)4 * N + 4))) return rc;
-  UP(p->d_fwd_tasks, fwd_tasks); UP(p->d_col_tasks, col_tasks); UP(p->d_col_ptr, col_ptr); UP(p->d_trsm_ll, trsm_ll); UP(p->d_upd_items, upd_items);
+#define DA(ptr, n) if ((rc = dalloc(p, &(ptr), (n)))) return rc
+static int upload_plan(rcvd_problem* p) {
+  const FactorPlan& pl = p->plan; int rc;
+  UP(p->d_blk_of, pl.blk_of); UP(p->d_hblocks, pl.hblocks); UP(p->d_lblocks, pl.lblocks); UP(p->d_lvl_frames, pl.lvl_frames); UP(p->d_lvl_own, pl.lvl_own);
+  UP(p->d_own_lblocks, pl.own_lblocks); UP(p->d_own_hblocks, pl.own_hblocks); UP(p->d_uperm, pl.uperm);
+  UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_upd_tasks, pl.upd_tasks); UP(p->d_trsm_pairs, pl.trsm_pairs); UP(p->d_upd_pairs, pl.upd_pairs);
+  UP(p->d_sub_tasks, pl.sub_tasks); UP(p->d_sub_need, pl.sub_need); DA(p->d_sub_counters, (size_t)4 * p->N + 4);
+  UP(p->d_fwd_tasks, pl.fwd_tasks); UP(p->d_trsm_ll, pl.trsm_ll); UP(p->d_upd_items, pl.upd_items);
+  return RCVD_OK;
+}
+
+// constraint and triplet tiles, the record sort of the run path, the per-frame inputs in internal frame order, the scale lattice
+static int set_up_problem_data(rcvd_problem* p) {
+  const int N = p->N; const Layout& L = p->L; const std::vector<int>& uperm = p->plan.uperm; int rc;
   // tiles
   const int np = (int)(p->pair_frames.size() / 2);
   std::vector<int32_t> tile_pair, tile_count; std::vector<int64_t> tile_begin;
@@ -531,7 +293,7 @@ static int build_structure(rcvd_problem* p) {
   UP(p->d_tile_pair, tile_pair); UP(p->d_tile_begin, tile_begin); UP(p->d_tile_count, tile_count);
   {
     std::vector<int32_t> pf_int(p->pair_frames.size());
-    for (size_t i = 0; i < pf_int.size(); ++i) pf_int[i] = p->iperm[p->pair_frames[i]];
+    for (size_t i = 0; i < pf_int.size(); ++i) pf_int[i] = p->plan.iperm[p->pair_frames[i]];
     UP(p->d_pair_frames, pf_int); UP(p->d_records, p->records_h);
   }
   p->records_sorted = false;
@@ -561,11 +323,11 @@ static int build_structure(rcvd_problem* p) {
   }
   {
     std::vector<uint8_t> ir(N); std::vector<double> md(N), ad;
-    for (int i = 0; i < N; ++i) { ir[i] = p->in_range[p->uperm[i]]; md[i] = p->median[p->uperm[i]]; }
+    for (int i = 0; i < N; ++i) { ir[i] = p->in_range[uperm[i]]; md[i] = p->median[uperm[i]]; }
     UP(p->d_in_range, ir); UP(p->d_median, md);
     if (!p->adaptive.empty()) {
       const size_t G = p->adaptive.size() / N; ad.resize(p->adaptive.size());
-      for (int i = 0; i < N; ++i) std::copy(p->adaptive.begin() + (size_t)p->uperm[i] * G, p->adaptive.begin() + (size_t)(p->uperm[i] + 1) * G, ad.begin() + (size_t)i * G);
+      for (int i = 0; i < N; ++i) std::copy(p->adaptive.begin() + (size_t)uperm[i] * G, p->adaptive.begin() + (size_t)(uperm[i] + 1) * G, ad.begin() + (size_t)i * G);
       UP(p->d_adaptive, ad);
     }
   }
@@ -581,11 +343,16 @@ static int build_structure(rcvd_problem* p) {
     p->nscale = (int)(locs.size() / 2);
     UP(p->d_scale_locs, locs);
   }
-#undef UP
   p->first_frame = 0; p->last_frame = -1;
   { bool any = false; for (int f = 0; f < N; ++f) if (p->in_range[f]) { if (!any) { p->first_frame = f; any = true; } p->last_frame = f; } }
+  return RCVD_OK;
+}
+#undef UP
+
+// state, vectors and matrices, the TMA map of the factor blocks, the active-parameter mask, the kernels' shared-memory limits
+static int allocate_storage(rcvd_problem* p) {
+  const int N = p->N; const Layout& L = p->L; const int npad = L.npad, nLoff = p->plan.nLoff; const size_t bs = (size_t)npad * npad; int rc;
   const size_t Upad = (size_t)N * npad, U = (size_t)N * L.nf;
-#define DA(ptr, n) if ((rc = dalloc(p, &(ptr), (n)))) return rc
   DA(p->d_x, U); DA(p->d_xc, U); DA(p->d_xsave, U);
   DA(p->d_g, 2 * Upad + 8); p->d_diagH = p->d_g + Upad + 8;   // [gradient | 8 scalars | diag H]: one packed all-reduce at N > 1
   DA(p->d_S, Upad); DA(p->d_lmdiag, Upad); DA(p->d_D2, Upad); DA(p->d_gs, Upad); DA(p->d_rhs, Upad);
@@ -596,28 +363,27 @@ static int build_structure(rcvd_problem* p) {
   DA(p->d_partial, (size_t)p->npartial);
   if (p->eval_only) { DA(p->d_H, 1); DA(p->d_Lb, 1); DA(p->d_T, 1); DA(p->d_invL, 1); DA(p->d_invT, 1); }   // cost / gradient evaluations only: no matrices
   else {
-    DA(p->d_H, (size_t)p->nHblocks * bs); DA(p->d_Lb, (size_t)(N + nLoff) * bs); DA(p->d_T, (size_t)std::max(nLoff, 1) * bs);
+    DA(p->d_H, p->plan.hblocks.size() * bs); DA(p->d_Lb, (size_t)(N + nLoff) * bs); DA(p->d_T, (size_t)std::max(nLoff, 1) * bs);
     DA(p->d_invL, (size_t)N * bs); DA(p->d_invT, (size_t)N * npad * 16);
   }
 #undef DA
   {
     // 2-D TMA view of the T buffer (off-diagonal factor blocks X_rk, row-major): inner = k, outer = block * npad + row, box [rb][16], 128-B swizzle
     p->tmap_ok = false;
-    cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, p->device);
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
     void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && fn && qres == cudaDriverEntryPointSuccess) {
       const cuuint64_t gdim[2] = {(cuuint64_t)npad, (cuuint64_t)std::max(nLoff, 1) * npad};
       const cuuint64_t gstr[1] = {(cuuint64_t)npad * sizeof(double)};
-      const cuuint32_t box[2] = {16u, (cuuint32_t)p->upd_rb};
+      const cuuint32_t box[2] = {16u, (cuuint32_t)p->plan.upd_rb};
       const cuuint32_t estr[2] = {1u, 1u};
       const CUresult r = ((EncodeFn)fn)(&p->tmapT, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, p->d_T, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       p->tmap_ok = (r == CUDA_SUCCESS);
     }
     cudaGetLastError();
-    if (p->tmap_ok) { CK(cudaFuncSetAttribute(k_update_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->upd_rb, 1))); CK(cudaFuncSetAttribute(k_update_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->upd_rb, 2))); }
+    if (p->tmap_ok) { CK(cudaFuncSetAttribute(k_update_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->plan.upd_rb, 1))); CK(cudaFuncSetAttribute(k_update_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->plan.upd_rb, 2))); }
     else if (p->gemm_tma) return set_err(RCVD_ERR_CUDA, "cuTensorMapEncodeTiled unavailable or failed: the TMA update kernel cannot run");
   }
   CK(cudaMallocHost((void**)&p->h_scal, (SC_N + 2) * sizeof(double)));
@@ -648,6 +414,17 @@ static int build_structure(rcvd_problem* p) {
   p->use_trsm_ll = trsm_ll_smem_bytes(npad) <= 220 * 1024;
   if (p->use_trsm_ll) { CK(cudaFuncSetAttribute(k_trsm_ll<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2))); if (trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) CK(cudaFuncSetAttribute(k_trsm_ll<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4))); }
   if (potrf_smem_bytes(npad) <= 220 * 1024) CK(cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_smem_bytes(npad)));
+  return RCVD_OK;
+}
+
+static int build_structure(rcvd_problem* p) {
+  free_all(p);
+  CK(cudaSetDevice(p->device));
+  if (const char* e = make_factor_plan(p->plan, p->cfg, p->struct_pairs.empty() ? p->pair_frames : p->struct_pairs, p->trip_centers, p->order_slack,
+                                       p->nranks, p->rank, p->dist_enabled, p->num_sms))
+    return set_err(RCVD_ERR_INVALID, "%s", e);
+  int rc;
+  if ((rc = upload_plan(p)) || (rc = set_up_problem_data(p)) || (rc = allocate_storage(p))) return rc;
   CK(cudaStreamSynchronize(p->stream));
   p->structure_ready = true;
   return RCVD_OK;
@@ -680,7 +457,7 @@ static int grouped(rcvd_problem* p, double* base, size_t unit, const std::vector
 // Enqueues factorisation of (S H S + D2) and the solve y = A^{-1} gs on p->stream.
 static int enqueue_factor_solve(rcvd_problem* p) {
   const Layout& L = p->L; const int N = p->N, npad = L.npad; cudaStream_t st = p->stream;
-  const int nL = N + p->nLoff;
+  const int nL = N + p->plan.nLoff;
   const int tiles = (npad + 63) / 64;
   enum { P_LOAD = 0, P_POTRF, P_TRINV, P_TRSM, P_GEMM, P_SOLVE };
   int prof_level = 0;
@@ -694,7 +471,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     k_gemm_nt<<<dim3(tiles, tiles, ntasks), 128, 0, cs>>>(dstp, A, B, tasks, prs, npad, beta != 0.0 ? neff : npad, alpha, beta);
   };
   mark(-1);
-  k_load_factor<<<dim3((npad * npad + 255) / 256, p->dist ? p->n_own_l : nL), 256, 0, st>>>(p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, L.nf, p->dist ? p->d_own_lblocks : nullptr);
+  k_load_factor<<<dim3((npad * npad + 255) / 256, p->plan.dist ? (int)p->plan.own_lblocks.size() : nL), 256, 0, st>>>(p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, L.nf, p->plan.dist ? p->d_own_lblocks : nullptr);
   p->launches += 1; p->paths[LP_OTHER]++; mark(P_LOAD);
   // Two-stream schedule (fork/join inside the captured graph): the non-critical update GEMMs of level l run on `side`
   // concurrently with potrf / inverse / trsm of level l+1 on `st`.
@@ -706,15 +483,15 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   auto phase_boundary = [&]() -> int {
     if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }
     std::vector<Seg> inv, tr;
-    for (int q = 0; q < p->nranks; ++q) inv.push_back({(size_t)p->fa_off[q], (size_t)p->fa_cnt[q]});
-    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)p->fb_off[q], (size_t)p->fb_cnt[q]});
-    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)N + (size_t)p->bseg[2 * q], (size_t)p->bseg[2 * q + 1]});
+    for (int q = 0; q < p->nranks; ++q) inv.push_back({(size_t)p->plan.fa_off[q], (size_t)p->plan.fa_cnt[q]});
+    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)p->plan.fb_off[q], (size_t)p->plan.fb_cnt[q]});
+    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)N + (size_t)p->plan.bseg[2 * q], (size_t)p->plan.bseg[2 * q + 1]});
     int rc = grouped(p, p->d_invL, bsz, inv, true); if (rc) return rc;
     return grouped(p, p->d_Lb, bsz, tr, true);
   };
-  for (size_t li = 0; li < p->levels.size(); ++li) {
-    const Level& lv = p->levels[li]; prof_level = (int)li;
-    if (p->dist && (int)li == p->LB) { int rc = phase_boundary(); if (rc) return rc; }
+  for (size_t li = 0; li < p->plan.levels.size(); ++li) {
+    const Level& lv = p->plan.levels[li]; prof_level = (int)li;
+    if (p->plan.dist && (int)li == p->plan.LB) { int rc = phase_boundary(); if (rc) return rc; }
     const int* lframes = p->d_lvl_own + lv.own_off; const int nfr = lv.nown;      // the frames this rank factors at this level
     if (nfr > 0) {
     if (potrf_smem_bytes(npad) <= 220 * 1024) {
@@ -755,10 +532,10 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       if (lv.ntrsm > 0) { gemm(st, lv.ntrsm, p->d_T, p->d_Lb, p->d_invL, p->d_trsm_tasks + lv.trsm_off, p->d_trsm_pairs, 1.0, 0.0); p->launches++; p->paths[LP_TRSM_GEMM]++; mark(P_TRSM); }
     }
     }
-    if (p->dist && (int)li < p->LB) {
+    if (p->plan.dist && (int)li < p->plan.LB) {
       // the off-diagonal factor blocks of this level, from their owners to everybody (one fused NCCL launch)
       std::vector<Seg> segs;
-      for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->tseg[(li * p->nranks + q) * 2], (size_t)p->tseg[(li * p->nranks + q) * 2 + 1]});
+      for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->plan.tseg[(li * p->nranks + q) * 2], (size_t)p->plan.tseg[(li * p->nranks + q) * 2 + 1]});
       int rc = grouped(p, p->d_T, bsz, segs, true); if (rc) return rc;
     }
     if (lv.nupd2 > 0 && p->overlap) {
@@ -767,12 +544,12 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     if (side_pending) { CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }   // U2(l-1) before U1(l)
     auto update = [&](cudaStream_t cs, int off, int n) {   // persistent TMA-fed update kernel
       if (n <= p->num_sms) {   // few items: two DMMA teams per tile, one CTA per SM
-        k_update_tma<2><<<n, UpdShape<2>::threads, upd_smem_bytes(p->upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, 0);
+        k_update_tma<2><<<n, UpdShape<2>::threads, upd_smem_bytes(p->plan.upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->plan.upd_neff, p->plan.upd_rb, 0);
         p->paths[LP_UPD_TMA2]++;
       } else {
         int grid = std::min(n, 2 * p->num_sms);
         if (p->upd_ipc > 0) grid = std::max(grid, (n + p->upd_ipc - 1) / p->upd_ipc);
-        k_update_tma<1><<<grid, UpdShape<1>::threads, upd_smem_bytes(p->upd_rb, 1), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->upd_neff, p->upd_rb, 0);
+        k_update_tma<1><<<grid, UpdShape<1>::threads, upd_smem_bytes(p->plan.upd_rb, 1), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->plan.upd_neff, p->plan.upd_rb, 0);
         p->paths[LP_UPD_TMA1]++; if (grid < n) p->paths[LP_UPD_TMA1_MULTI]++;
       }
     };
@@ -790,26 +567,26 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
     }
   }
-  if (p->dist && p->LB >= (int)p->levels.size()) { int rc = phase_boundary(); if (rc) return rc; }
+  if (p->plan.dist && p->plan.LB >= (int)p->plan.levels.size()) { int rc = phase_boundary(); if (rc) return rc; }
   if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); }
   CK(cudaMemcpyAsync(p->d_rhs, p->d_gs, (size_t)N * npad * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  const int nlv = (int)p->levels.size();
-  const int LS = p->sub_first_level;       // levels >= LS: the persistent dataflow kernel (rcvd_linalg.cuh, k_substitution)
+  const int nlv = (int)p->plan.levels.size();
+  const int LS = p->plan.sub_first_level;       // levels >= LS: the persistent dataflow kernel (rcvd_linalg.cuh, k_substitution)
   for (int l = 0; l < LS; ++l) {
-    const Level& lv = p->levels[l];
+    const Level& lv = p->plan.levels[l];
     k_fwd_diag<<<dim3((npad + 7) / 8, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_rhs, p->d_ytmp, p->d_lvl_frames + lv.frame_off, npad);
     p->launches++; p->paths[LP_SUB_LEVEL]++;
     if (lv.nfwd > 0) { k_fwd_update<<<dim3((npad + 7) / 8, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_ytmp, p->d_rhs, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; p->paths[LP_SUB_LEVEL]++; }
   }
-  if (LS < nlv && p->n_sub_tasks > 0) {
+  if (LS < nlv && !p->plan.sub_tasks.empty()) {
     CK(cudaMemsetAsync(p->d_sub_counters, 0, ((size_t)4 * N + 4) * sizeof(int), st));
     SubCounters cn; cn.ticket = p->d_sub_counters; cn.fin = p->d_sub_counters + 4; cn.fdone = cn.fin + N; cn.bin = cn.fdone + N; cn.bdone = cn.bin + N;
     cn.fin_need = p->d_sub_need; cn.bin_need = p->d_sub_need + N;
-    k_substitution<<<std::min(p->n_sub_tasks, p->num_sms), kSubThreads, substitution_smem_bytes(npad), st>>>(p->d_invL, p->d_T, p->d_rhs, p->d_ytmp, p->d_y, p->d_sub_tasks, p->n_sub_tasks, cn, npad);
+    k_substitution<<<std::min((int)p->plan.sub_tasks.size(), p->num_sms), kSubThreads, substitution_smem_bytes(npad), st>>>(p->d_invL, p->d_T, p->d_rhs, p->d_ytmp, p->d_y, p->d_sub_tasks, (int)p->plan.sub_tasks.size(), cn, npad);
     p->launches++; p->paths[LP_SUB_FUSED]++;
   }
   for (int l = LS - 1; l >= 0; --l) {
-    const Level& lv = p->levels[l];
+    const Level& lv = p->plan.levels[l];
     if (lv.nfwd > 0) { k_bwd_update<<<dim3((npad + 31) / 32, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_y, p->d_ytmp, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; p->paths[LP_SUB_LEVEL]++; }
     k_bwd_diag<<<dim3((npad + 31) / 32, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_ytmp, p->d_y, p->d_lvl_frames + lv.frame_off, npad);
     p->launches += 1; p->paths[LP_SUB_LEVEL]++;
@@ -859,7 +636,7 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
   DevProblem d = dev_problem(p);
   const RegCounts rcn = reg_counts(p->cfg, L, N, p->nscale);
   const int regblocks = (rcn.total + 127) / 128;
-  if (wantH) CK(cudaMemsetAsync(p->d_H, 0, (size_t)p->nHblocks * bs * sizeof(double), st));
+  if (wantH) CK(cudaMemsetAsync(p->d_H, 0, p->plan.hblocks.size() * bs * sizeof(double), st));
   if (wantG) CK(cudaMemsetAsync(gout, 0, (Upad + 8) * sizeof(double), st));
   if (p->num_tiles > 0) {
     if (wantH && p->use_fast && p->records_sorted) k_accumulate_runs<<<p->num_tiles, kTile, kRunSmem, st>>>(d, x, p->d_H, gout, p->d_partial);
@@ -897,13 +674,13 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
       CK(cudaMemcpyAsync(p->d_scal + slot, gout + Upad, sizeof(double), cudaMemcpyDeviceToDevice, st));
     } else if ((rc = allreduce(p, p->d_scal + slot, 1))) return rc;
     if (wantH) {
-      if (p->dist && !p->force_full_H) {
+      if (p->plan.dist && !p->force_full_H) {
         // the normal matrix is summed onto the OWNER of every block only (its frames' diagonal blocks, the off-diagonal blocks of its columns)
         std::vector<Seg> segs;
-        for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->fa_off[q], (size_t)(p->fa_cnt[q] + p->fb_cnt[q])});
-        for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->hseg[2 * q], (size_t)p->hseg[2 * q + 1]});
+        for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->plan.fa_off[q], (size_t)(p->plan.fa_cnt[q] + p->plan.fb_cnt[q])});
+        for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->plan.hseg[2 * q], (size_t)p->plan.hseg[2 * q + 1]});
         if ((rc = grouped(p, p->d_H, bs, segs, false))) return rc;
-      } else if ((rc = allreduce(p, p->d_H, (size_t)p->nHblocks * bs))) return rc;
+      } else if ((rc = allreduce(p, p->d_H, p->plan.hblocks.size() * bs))) return rc;
     }
   }
   return RCVD_OK;
@@ -912,7 +689,7 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
 // Frame-major host vectors in the caller's frame order <-> device vectors in the internal (owner-major) order.
 static int upload_frames(rcvd_problem* p, double* dst, const double* src_user, int stride_dst, int stride_src, int count) {
   std::vector<double> tmp((size_t)p->N * stride_dst, 0.0);
-  for (int i = 0; i < p->N; ++i) memcpy(tmp.data() + (size_t)i * stride_dst, src_user + (size_t)p->uperm[i] * stride_src, (size_t)count * sizeof(double));
+  for (int i = 0; i < p->N; ++i) memcpy(tmp.data() + (size_t)i * stride_dst, src_user + (size_t)p->plan.uperm[i] * stride_src, (size_t)count * sizeof(double));
   CK(cudaMemcpyAsync(dst, tmp.data(), tmp.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
   CK(cudaStreamSynchronize(p->stream));      // tmp goes out of scope
   return RCVD_OK;
@@ -921,7 +698,7 @@ static int download_frames(rcvd_problem* p, double* dst_user, const double* src,
   std::vector<double> tmp((size_t)p->N * stride_src);
   CK(cudaMemcpyAsync(tmp.data(), src, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
   CK(cudaStreamSynchronize(p->stream));
-  for (int i = 0; i < p->N; ++i) memcpy(dst_user + (size_t)p->uperm[i] * stride_dst, tmp.data() + (size_t)i * stride_src, (size_t)count * sizeof(double));
+  for (int i = 0; i < p->N; ++i) memcpy(dst_user + (size_t)p->plan.uperm[i] * stride_dst, tmp.data() + (size_t)i * stride_src, (size_t)count * sizeof(double));
   return RCVD_OK;
 }
 // device state -> h_state (caller's frame order); used before the structure is rebuilt
@@ -1032,9 +809,9 @@ static int enqueue_model_terms(rcvd_problem* p) {
   const int N = p->N, npad = p->L.npad; const size_t Upad = (size_t)N * npad; cudaStream_t st = p->stream;
   k_mul<<<nblk(Upad), 256, 0, st>>>(p->d_S, p->d_y, p->d_Sy, (int)Upad);
   CK(cudaMemsetAsync(p->d_Hy, 0, Upad * sizeof(double), st));
-  k_spmv_sym<<<dim3((npad + 7) / 8, p->dist ? p->n_own_h : p->nHblocks), 256, 0, st>>>(p->d_H, p->d_hblocks, p->d_Sy, p->d_Hy, npad, p->dist ? p->d_own_hblocks : nullptr);
+  k_spmv_sym<<<dim3((npad + 7) / 8, p->plan.dist ? (int)p->plan.own_hblocks.size() : (int)p->plan.hblocks.size()), 256, 0, st>>>(p->d_H, p->d_hblocks, p->d_Sy, p->d_Hy, npad, p->plan.dist ? p->d_own_hblocks : nullptr);
   k_dot2<<<nblk(Upad), 256, 0, st>>>(p->d_gs, p->d_y, p->d_Sy, p->d_Hy, (int)Upad, p->d_scal, SC_GY, SC_YHY);
-  if (p->dist) { int rc = allreduce(p, p->d_scal + SC_YHY, 1); if (rc) return rc; }   // every rank multiplied the H blocks it owns
+  if (p->plan.dist) { int rc = allreduce(p, p->d_scal + SC_YHY, 1); if (rc) return rc; }   // every rank multiplied the H blocks it owns
   k_make_delta<<<nblk(Upad), 256, 0, st>>>(p->d_y, p->d_S, p->d_delta, (int)Upad);
   p->launches += 4;
   return RCVD_OK;
@@ -1242,6 +1019,8 @@ RCVD_API int32_t rcvd_problem_create(const rcvd_config* cfg, int32_t device, rcv
   }
   rcvd_problem* p = new rcvd_problem();
   p->cfg = *cfg; p->L = L; p->N = cfg->num_frames; p->device = device;
+  e = cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, device);   // read once: the plan and the launch shapes use it
+  if (e != cudaSuccess) { delete p; return set_err(RCVD_ERR_CUDA, "cudaDeviceGetAttribute(multiprocessor count): %s", cudaGetErrorString(e)); }
   // the critical chain (potrf -> trsm -> next-level updates) runs at the highest priority, the overlapped updates at the lowest,
   // so that a freed SM goes to the chain first
   int prio_lo = 0, prio_hi = 0; cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
@@ -1362,7 +1141,7 @@ RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
   double* d_out = nullptr;
   CK(cudaMalloc((void**)&d_out, U * U * sizeof(double)));
   CK(cudaMemsetAsync(d_out, 0, U * U * sizeof(double), p->stream));
-  k_h_to_dense<<<dim3(nblk((size_t)p->L.nf * p->L.nf), p->nHblocks), 256, 0, p->stream>>>(p->d_H, p->d_hblocks, p->nHblocks, d_out, p->N, p->L.nf, p->L.npad, p->d_uperm);
+  k_h_to_dense<<<dim3(nblk((size_t)p->L.nf * p->L.nf), (int)p->plan.hblocks.size()), 256, 0, p->stream>>>(p->d_H, p->d_hblocks, (int)p->plan.hblocks.size(), d_out, p->N, p->L.nf, p->L.npad, p->d_uperm);
   cudaError_t e = cudaMemcpyAsync(Hout, d_out, U * U * sizeof(double), cudaMemcpyDeviceToHost, p->stream);
   cudaStreamSynchronize(p->stream); cudaFree(d_out);
   if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "copy failed: %s", cudaGetErrorString(e));
@@ -1372,7 +1151,7 @@ RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
 static int solve_loaded(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y) {
   const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t Upad = (size_t)N * npad;
   std::vector<double> hs(Upad, 1.0), hd(Upad, 1.0), hb(Upad, 0.0);
-  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) { const size_t u = (size_t)p->uperm[f] * nf + l; hs[(size_t)f * npad + l] = S ? S[u] : 1.0; hd[(size_t)f * npad + l] = D2[u]; hb[(size_t)f * npad + l] = b[u]; }
+  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) { const size_t u = (size_t)p->plan.uperm[f] * nf + l; hs[(size_t)f * npad + l] = S ? S[u] : 1.0; hd[(size_t)f * npad + l] = D2[u]; hb[(size_t)f * npad + l] = b[u]; }
   CK(cudaMemcpyAsync(p->d_S, hs.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
   CK(cudaMemcpyAsync(p->d_D2, hd.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
   CK(cudaMemcpyAsync(p->d_gs, hb.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
@@ -1381,7 +1160,7 @@ static int solve_loaded(rcvd_problem* p, const double* S, const double* D2, cons
   std::vector<double> hy(Upad);
   CK(cudaMemcpyAsync(hy.data(), p->d_y, Upad * 8, cudaMemcpyDeviceToHost, p->stream));
   rc = read_scalars(p); if (rc) return rc;
-  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) y[(size_t)p->uperm[f] * nf + l] = hy[(size_t)f * npad + l];
+  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) y[(size_t)p->plan.uperm[f] * nf + l] = hy[(size_t)f * npad + l];
   if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, "factorisation hit a non-positive pivot");
   return RCVD_OK;
 }
@@ -1405,16 +1184,16 @@ RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const
   int rc = ensure_ready(p); if (rc) return rc;
   const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
   std::vector<uint8_t> coupled((size_t)N * N, 0);
-  for (const HBlock& hb : p->hblocks) { const int a = p->uperm[hb.r], c = p->uperm[hb.c]; coupled[(size_t)a * N + c] = coupled[(size_t)c * N + a] = 1; }
+  for (const HBlock& hb : p->plan.hblocks) { const int a = p->plan.uperm[hb.r], c = p->plan.uperm[hb.c]; coupled[(size_t)a * N + c] = coupled[(size_t)c * N + a] = 1; }
   for (int a = 0; a < N; ++a) for (int c = 0; c < N; ++c) {
     if (coupled[(size_t)a * N + c]) continue;
     for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j)
       if (H[((size_t)a * nf + i) * U + (size_t)c * nf + j] != 0.0)
         return set_err(RCVD_ERR_INVALID, "H couples frames %d and %d, which the problem's frame graph does not couple", a, c);
   }
-  std::vector<double> hH((size_t)p->nHblocks * bs, 0.0);
-  for (int h = 0; h < p->nHblocks; ++h) {        // block h holds rows of frame r, columns of frame c (internal ids)
-    const int a = p->uperm[p->hblocks[h].r], c = p->uperm[p->hblocks[h].c];
+  std::vector<double> hH(p->plan.hblocks.size() * bs, 0.0);
+  for (int h = 0; h < (int)p->plan.hblocks.size(); ++h) {        // block h holds rows of frame r, columns of frame c (internal ids)
+    const int a = p->plan.uperm[p->plan.hblocks[h].r], c = p->plan.uperm[p->plan.hblocks[h].c];
     for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) hH[h * bs + (size_t)i * npad + j] = H[((size_t)a * nf + i) * U + (size_t)c * nf + j];
   }
   CK(cudaMemcpyAsync(p->d_H, hH.data(), hH.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
@@ -1424,20 +1203,20 @@ RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const
 RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, double* Linv) {
   if (!p || !order || !L) return set_err(RCVD_ERR_INVALID, "null argument");
   if (!p->structure_ready || !p->factored) return set_err(RCVD_ERR_INVALID, "no factorisation has run on this handle");
-  if (p->dist) return set_err(RCVD_ERR_INVALID, "the distributed factorisation keeps its blocks on their owners");
+  if (p->plan.dist) return set_err(RCVD_ERR_INVALID, "the distributed factorisation keeps its blocks on their owners");
   SET_DEVICE(p->device);
   CK(cudaStreamSynchronize(p->side_stream)); CK(cudaStreamSynchronize(p->stream));
-  const int N = p->N, nf = p->L.nf, npad = p->L.npad, nT = p->nLoff; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
+  const int N = p->N, nf = p->L.nf, npad = p->L.npad, nT = p->plan.nLoff; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
   std::vector<double> hL((size_t)N * bs), hT((size_t)nT * bs);
   CK(cudaMemcpy(hL.data(), p->d_Lb, hL.size() * sizeof(double), cudaMemcpyDeviceToHost));   // the first N blocks: diagonal blocks L_kk
   if (nT > 0) CK(cudaMemcpy(hT.data(), p->d_T, hT.size() * sizeof(double), cudaMemcpyDeviceToHost));
   std::vector<size_t> off(N);
-  for (int q = 0; q < N; ++q) { off[p->elim_order[q]] = (size_t)q * nf; order[q] = p->uperm[p->elim_order[q]]; }
+  for (int q = 0; q < N; ++q) { off[p->plan.elim_order[q]] = (size_t)q * nf; order[q] = p->plan.uperm[p->plan.elim_order[q]]; }
   std::fill(L, L + U * U, 0.0);
   for (int f = 0; f < N; ++f)                      // lower triangle only: the update epilogue may leave values above the diagonal
     for (int i = 0; i < nf; ++i) for (int j = 0; j <= i; ++j) L[(off[f] + i) * U + off[f] + j] = hL[f * bs + (size_t)i * npad + j];
   for (int t = 0; t < nT; ++t) {
-    const HBlock& b = p->lblocks_h[N + t];
+    const HBlock& b = p->plan.lblocks[N + t];
     for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) L[(off[b.r] + i) * U + off[b.c] + j] = hT[t * bs + (size_t)i * npad + j];
   }
   if (Linv) {
@@ -1519,7 +1298,7 @@ RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double
   const bool ov = p->overlap; if (!keep_overlap) p->overlap = false;
   for (int i = 0; i < 8; ++i) out_ms[i] = 0.0;
   std::vector<std::pair<int, cudaEvent_t>> evs;
-  p->level_ms.assign(p->levels.size() * 6, 0.0);
+  p->level_ms.assign(p->plan.levels.size() * 6, 0.0);
   for (int r = -1; r < reps; ++r) {
     CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), p->stream));
     evs.clear(); p->prof = &evs;
@@ -1540,7 +1319,7 @@ RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double
   }
   p->overlap = ov;
   for (int i = 0; i < 6; ++i) out_ms[i] /= reps;
-  out_ms[7] = p->upd_flops;
+  out_ms[7] = p->plan.upd_flops;
   return rc;
 }
 // Bench hook: fp64 tensor-core (DMMA) peak of this device for one mma.sync shape, measured live with a register-only loop on all SMs:
@@ -1623,7 +1402,7 @@ RCVD_API int32_t rcvd_debug_linear_residual(rcvd_problem* p, double radius, doub
   k_lm_prepare<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, p->d_g, p->d_lmdiag, p->d_D2, p->d_gs, (int)Upad, 0, radius, 1e-6, 1e32);
   if ((rc = factor_solve(p))) return rc;
   if ((rc = enqueue_model_terms(p))) return rc;                      // leaves H (S y) in d_Hy
-  if (p->dist && (rc = allreduce(p, p->d_Hy, Upad))) return rc;      // every rank multiplied only the H blocks it owns
+  if (p->plan.dist && (rc = allreduce(p, p->d_Hy, Upad))) return rc;      // every rank multiplied only the H blocks it owns
   double* d_out = p->d_scal + 9;                                      // slots 9..12 are unused by the LM loop
   k_lin_residual<<<nblk(Upad), 256, 0, st>>>(p->d_S, p->d_Hy, p->d_D2, p->d_y, p->d_gs, p->d_g, (int)Upad, d_out);
   p->launches += 4;
@@ -1663,7 +1442,7 @@ RCVD_API int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]) {
   if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
-  out[0] = p->dist ? 1 : 0; out[1] = p->LB; out[2] = (int)p->levels.size(); out[3] = p->dist ? p->fa_cnt[p->rank] + p->fb_cnt[p->rank] : p->N;
+  out[0] = p->plan.dist ? 1 : 0; out[1] = p->plan.LB; out[2] = (int)p->plan.levels.size(); out[3] = p->plan.dist ? p->plan.fa_cnt[p->rank] + p->plan.fb_cnt[p->rank] : p->N;
   return RCVD_OK;
 }
 // Test hook: 0 = generic accumulate kernel (the tests' reference), 1 (default) = specialised kernels (run path on a bilinear depth grid).
@@ -1674,13 +1453,36 @@ RCVD_API int32_t rcvd_solve(rcvd_problem* p, const rcvd_solve_options* opt, rcvd
   rcvd_solve_options o; if (opt) o = *opt; else rcvd_default_solve_options(&o);
   return lm_solve(p, o, *summary);
 }
+// Test hook: the factorisation plan of a frame graph, computed on the host alone -- no handle, no device (see include/rcvd_hooks.h).
+RCVD_API int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                        int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
+                                        int32_t* order, int32_t* level, int32_t* owner, int32_t* perm, int32_t out[12]) {
+  if (!cfg || np < 0 || nt < 0 || (np > 0 && !pairs) || (nt > 0 && !trip_centers) || !order || !level || !owner || !perm || !out)
+    return set_err(RCVD_ERR_INVALID, "null or negative argument");
+  if (nranks < 1 || rank < 0 || rank >= nranks || num_sms < 1) return set_err(RCVD_ERR_INVALID, "bad rank/nranks/num_sms");
+  FactorPlan pl;
+  if (const char* e = make_factor_plan(pl, *cfg, std::vector<int32_t>(pairs, pairs + 2 * (size_t)np), std::vector<int32_t>(trip_centers, trip_centers + nt),
+                                       order_slack, nranks, rank, true, num_sms))
+    return set_err(RCVD_ERR_INVALID, "%s", e);
+  const int N = cfg->num_frames;
+  for (int i = 0; i < N; ++i) {
+    const int f = pl.uperm[i];
+    order[i] = pl.uperm[pl.elim_order[i]]; level[f] = pl.level[i]; owner[f] = pl.owner[i]; perm[i] = f;
+  }
+  int upd = 0; for (const Level& l : pl.levels) upd += l.nupd + l.nupd2;
+  const int32_t v[12] = {(int32_t)pl.levels.size(), pl.nLoff, (int32_t)pl.hblocks.size(), upd, (int32_t)pl.upd_items.size(), (int32_t)pl.sub_tasks.size(),
+                         pl.dist ? 1 : 0, pl.LB, pl.sub_first_level, (int32_t)pl.own_lblocks.size(), (int32_t)pl.own_hblocks.size(),
+                         pl.dist ? pl.fa_cnt[rank] + pl.fb_cnt[rank] : N};
+  std::copy(v, v + 12, out);
+  return RCVD_OK;
+}
 // Structure statistics (for DESIGN.md / bench): frames, off-diagonal factor blocks, levels, H blocks, npad.
 RCVD_API int32_t rcvd_structure_info(rcvd_problem* p, int32_t out[8]) {
   if (!p) return set_err(RCVD_ERR_INVALID, "null argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
-  out[0] = p->N; out[1] = p->nLoff; out[2] = (int)p->levels.size(); out[3] = p->nHblocks; out[4] = p->L.npad; out[5] = p->L.nf; out[6] = p->num_tiles;
-  int upd = 0; for (auto& l : p->levels) upd += l.nupd + l.nupd2; out[7] = upd;
+  out[0] = p->N; out[1] = p->plan.nLoff; out[2] = (int)p->plan.levels.size(); out[3] = (int)p->plan.hblocks.size(); out[4] = p->L.npad; out[5] = p->L.nf; out[6] = p->num_tiles;
+  int upd = 0; for (auto& l : p->plan.levels) upd += l.nupd + l.nupd2; out[7] = upd;
   return RCVD_OK;
 }
 

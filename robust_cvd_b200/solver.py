@@ -57,6 +57,25 @@ def spatial_param_offset(cfg):
     return lib().rcvd_spatial_param_offset(C.byref(cfg))
 
 
+FACTOR_PLAN_COUNTS = ("levels", "offdiag_factor_blocks", "h_blocks", "update_targets", "update_items", "substitution_tasks",
+                      "distributed", "first_replicated_level", "first_substitution_level", "rank_l_blocks", "rank_h_blocks", "rank_frames")
+
+
+def factor_plan(cfg, pairs, trip_centers=(), order_slack=4, nranks=1, rank=0, num_sms=132):
+    """Test hook: the block-Cholesky plan of the frame graph of `pairs` ([P, 2] frame pairs) and `trip_centers` under cfg, computed on
+    the host (no device).  Returns the per-frame arrays order, level, owner, perm (caller's frame ids; perm[i] = caller's frame of
+    internal frame i) and the FACTOR_PLAN_COUNTS."""
+    n = cfg.num_frames
+    pf = np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
+    tc = np.ascontiguousarray(np.asarray(trip_centers, np.int32).reshape(-1))
+    arrays = {k: np.zeros(n, np.int32) for k in ("order", "level", "owner", "perm")}
+    out = (C.c_int32 * len(FACTOR_PLAN_COUNTS))()
+    _check(lib().rcvd_debug_factor_plan(C.byref(cfg), C.c_int32(pf.shape[0]), _p(pf, C.c_int32), C.c_int32(tc.size), _p(tc, C.c_int32),
+                                        C.c_int32(order_slack), C.c_int32(nranks), C.c_int32(rank), C.c_int32(num_sms),
+                                        *(_p(a, C.c_int32) for a in arrays.values()), out))
+    return {**arrays, **dict(zip(FACTOR_PLAN_COUNTS, list(out)))}
+
+
 class Problem:
     def __init__(self, cfg, device=0):
         self.cfg = cfg

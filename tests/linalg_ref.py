@@ -63,8 +63,8 @@ def adjacency(n, pairs):
 
 
 def elimination_order(n, pairs, slack=4):
-    """The solver's multiple-minimum-degree order (rcvd_api.cu, build_structure): each round eliminates a maximal independent set of
-    frames whose degree is within `slack` of the minimum (slack < 0: one frame per round).  Returns (order, cs) with cs[k] the
+    """The solver's multiple-minimum-degree order (robust_cvd_b200/csrc/rcvd_plan.h, make_factor_plan): each round eliminates a maximal
+    independent set of frames whose degree is within `slack` of the minimum (slack < 0: one frame per round).  Returns (order, cs) with cs[k] the
     later-eliminated frames coupled to k after fill, sorted by elimination position."""
     adj = adjacency(n, pairs)
     done = [False] * n; order = []; pos = [-1] * n; cs = [[] for _ in range(n)]
@@ -100,6 +100,34 @@ def levels(order, cs):
         for a in cs[k]:
             lvl[a] = max(lvl[a], lvl[k] + 1)
     return lvl
+
+
+def owners(order, cs, lvl, nranks):
+    """The distributed factorisation's frame owners (rcvd_plan.h): (LB, owner).  Levels >= LB are the replicated tail of levels with
+    fewer than 3 frames; LB = 0 means no distribution.  Owners are greedy LPT, level by level, over each column's incoming phase-A update
+    work (symmetric targets count half) plus 0.6 per off-diagonal block + 0.3 for its own TRSM / POTRF in phase A."""
+    nl = max(lvl.values()) + 1
+    lf = [[k for k in order if lvl[k] == l] for l in range(nl)]
+    LB = nl
+    while LB > 0 and len(lf[LB - 1]) < 3:
+        LB -= 1
+    owner = [0] * len(order)
+    if nranks < 2 or LB == 0:
+        return 0, owner
+    tot_in = [0.0] * len(order)
+    for l in range(LB):
+        for k in lf[l]:
+            for a in range(len(cs[k])):
+                for b in range(a + 1):
+                    tot_in[cs[k][b]] += 0.5 if a == b else 1.0
+    load = [0.0] * nranks
+    for l in range(nl):
+        w = {k: tot_in[k] + (0.6 * len(cs[k]) + 0.3 if l < LB else 0.0) for k in lf[l]}
+        for k in sorted(lf[l], key=lambda k: -w[k]):
+            q = min(range(nranks), key=lambda t: load[t])
+            owner[k] = q
+            load[q] += w[k]
+    return LB, owner
 
 
 # ---------------------------------------------------------------------------------------------------------
