@@ -42,8 +42,8 @@ int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, doub
 /* launches of each factorisation / solve kernel path since the handle was created: {k_potrf_smem, k_potrf_panel, k_trsm_ll<4>,
  * k_trsm_ll<2>, TRSM by explicit inverse (k_gemm_nt), k_update_tma<1>, k_update_tma<2>, update by k_gemm_nt, level-launched
  * substitution (k_fwd_* / k_bwd_*), k_substitution, k_trinv, the rest (k_load_factor, k_potrf_trail), k_update_tma<1> launches with
- * fewer CTAs than items (CTAs that walk several items)} */
-int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]);
+ * fewer CTAs than items (CTAs that walk several items), k_trsm_ll launches (either shape) streamed beside their level's k_potrf_smem} */
+int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[14]);
 
 /* one damped LM step at the current state with trust-region `radius`; out = {|(S H S + D2) y - S g| / |S g| (device SpMV over the
  * assembled H), |S g|, cost, |g|_2, |y|_2, non-positive-pivot flag}: the parity evidence bench.py prints at the size it times */

@@ -174,7 +174,8 @@ __global__ void k_h_to_dense(const double* __restrict__ H, const HBlock* __restr
 
 // launch counters of enqueue_factor_solve by kernel path (rcvd_debug_linear_paths; include/rcvd_hooks.h lists the same order)
 enum { LP_POTRF_SMEM = 0, LP_POTRF_PANEL, LP_TRSM_LL4, LP_TRSM_LL2, LP_TRSM_GEMM, LP_UPD_TMA1, LP_UPD_TMA2, LP_UPD_GEMM, LP_SUB_LEVEL, LP_SUB_FUSED,
-       LP_TRINV, LP_OTHER, LP_UPD_TMA1_MULTI, LP_N };   // LP_UPD_TMA1_MULTI: k_update_tma<1> launches with fewer CTAs than items
+       LP_TRINV, LP_OTHER, LP_UPD_TMA1_MULTI, LP_TRSM_STREAMED, LP_N };   // LP_UPD_TMA1_MULTI: k_update_tma<1> launches with fewer CTAs than
+// items; LP_TRSM_STREAMED: the k_trsm_ll launches (either shape) that run beside their level's k_potrf_smem
 
 // ---------------------------------------------------------------------------
 struct rcvd_problem {
@@ -201,6 +202,8 @@ struct rcvd_problem {
   // matrices
   double *d_H = nullptr, *d_Lb = nullptr, *d_T = nullptr, *d_invL = nullptr, *d_invT = nullptr;
   HBlock *d_hblocks = nullptr, *d_lblocks = nullptr; int* d_fail = nullptr;
+  int* d_potrf_progress = nullptr;   // [N] tile columns of each diagonal block k_potrf_smem has published (read by the streamed k_trsm_ll)
+  int trsm2_ctas_per_sm = 0;          // resident k_trsm_ll<2> CTAs per SM at this npad
   // the block-Cholesky plan (rcvd_plan.h) and its device copies
   FactorPlan plan;
   int *d_lvl_frames = nullptr; GemmTask *d_trsm_tasks = nullptr, *d_upd_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
@@ -213,6 +216,7 @@ struct rcvd_problem {
   int64_t launches = 0, graph_launches = 0;
   std::vector<double> h_state; bool state_dirty = false; bool use_fast = true; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
   cudaStream_t side_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  cudaStream_t inv_stream = nullptr; cudaEvent_t ev_inv_join = nullptr;   // k_trinv, off the critical path and off the side stream's
   double *d_g2 = nullptr, *d_delta = nullptr; int* h_fail = nullptr;
   cudaEvent_t ev[8] = {nullptr};
   std::vector<void*> allocs;
@@ -251,6 +255,7 @@ template <class T> static int upload(rcvd_problem* p, T** ptr, const std::vector
 static void free_all(rcvd_problem* p) {
   if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; }
   if (p->side_stream) cudaStreamSynchronize(p->side_stream);
+  if (p->inv_stream) cudaStreamSynchronize(p->inv_stream);
   for (void* q : p->allocs) cudaFreeAsync(q, p->stream);
   p->allocs.clear();
   if (p->stream) cudaStreamSynchronize(p->stream);
@@ -358,6 +363,7 @@ static int allocate_storage(rcvd_problem* p) {
   DA(p->d_S, Upad); DA(p->d_lmdiag, Upad); DA(p->d_D2, Upad); DA(p->d_gs, Upad); DA(p->d_rhs, Upad);
   DA(p->d_g2, Upad + 8); DA(p->d_delta, Upad);
   DA(p->d_ytmp, Upad); DA(p->d_y, Upad); DA(p->d_Sy, Upad); DA(p->d_Hy, Upad); DA(p->d_scal, SC_N); DA(p->d_active, Upad); DA(p->d_fail, 1);
+  DA(p->d_potrf_progress, (size_t)N);
   const RegCounts rcn = reg_counts(p->cfg, L, N, p->nscale);
   p->npartial = p->num_tiles + (rcn.total + 127) / 128 + p->num_trip_tiles + 1;
   DA(p->d_partial, (size_t)p->npartial);
@@ -412,7 +418,15 @@ static int allocate_storage(rcvd_problem* p) {
   CK(cudaFuncSetAttribute(k_accumulate_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmem));
   CK(cudaFuncSetAttribute(k_accumulate_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, kRunSmem));
   p->use_trsm_ll = trsm_ll_smem_bytes(npad) <= 220 * 1024;
-  if (p->use_trsm_ll) { CK(cudaFuncSetAttribute(k_trsm_ll<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2))); if (trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) CK(cudaFuncSetAttribute(k_trsm_ll<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4))); }
+  if (p->use_trsm_ll) {
+    CK(cudaFuncSetAttribute(k_trsm_ll<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2)));
+    CK(cudaFuncSetAttribute(k_trsm_ll<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2)));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p->trsm2_ctas_per_sm, k_trsm_ll<2, true>, 128, trsm_ll_smem_bytes(npad, 2)));
+    if (trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) {
+      CK(cudaFuncSetAttribute(k_trsm_ll<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4)));
+      CK(cudaFuncSetAttribute(k_trsm_ll<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4)));
+    }
+  }
   if (potrf_smem_bytes(npad) <= 220 * 1024) CK(cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_smem_bytes(npad)));
   return RCVD_OK;
 }
@@ -471,31 +485,60 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     k_gemm_nt<<<dim3(tiles, tiles, ntasks), 128, 0, cs>>>(dstp, A, B, tasks, prs, npad, beta != 0.0 ? neff : npad, alpha, beta);
   };
   mark(-1);
+  CK(cudaMemsetAsync(p->d_potrf_progress, 0, (size_t)N * sizeof(int), st));   // no count of the previous factorisation may read as published
   k_load_factor<<<dim3((npad * npad + 255) / 256, p->plan.dist ? (int)p->plan.own_lblocks.size() : nL), 256, 0, st>>>(p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, L.nf, p->plan.dist ? p->d_own_lblocks : nullptr);
   p->launches += 1; p->paths[LP_OTHER]++; mark(P_LOAD);
   // Two-stream schedule (fork/join inside the captured graph): the non-critical update GEMMs of level l run on `side`
-  // concurrently with potrf / inverse / trsm of level l+1 on `st`.
-  cudaStream_t side = p->side_stream;
-  bool side_pending = false, side_used = false;
+  // concurrently with potrf / trsm of level l+1 on `st`.  The explicit inverses run on a third stream, `inv`: on `side` they would
+  // hold back the next update launch by a k_trinv, and U1(l+1) waits for that update (U2(l)).
+  cudaStream_t side = p->side_stream, inv = p->inv_stream;
+  bool side_pending = false, side_used = false, inv_used = false;
+  auto join_inv = [&]() -> int {
+    if (inv_used) { CK(cudaEventRecord(p->ev_inv_join, inv)); CK(cudaStreamWaitEvent(st, p->ev_inv_join, 0)); inv_used = false; }
+    return RCVD_OK;
+  };
   const size_t bsz = (size_t)npad * npad;
   // phase boundary of the distributed factorisation: the owners' explicit inverses (for the replicated substitution) and their
   // blocks of the trailing matrix go to everybody; from here on every rank factors the same narrow tail
   auto phase_boundary = [&]() -> int {
     if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }
-    std::vector<Seg> inv, tr;
-    for (int q = 0; q < p->nranks; ++q) inv.push_back({(size_t)p->plan.fa_off[q], (size_t)p->plan.fa_cnt[q]});
+    if (int rc = join_inv()) return rc;
+    std::vector<Seg> invs, tr;
+    for (int q = 0; q < p->nranks; ++q) invs.push_back({(size_t)p->plan.fa_off[q], (size_t)p->plan.fa_cnt[q]});
     for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)p->plan.fb_off[q], (size_t)p->plan.fb_cnt[q]});
     for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)N + (size_t)p->plan.bseg[2 * q], (size_t)p->plan.bseg[2 * q + 1]});
-    int rc = grouped(p, p->d_invL, bsz, inv, true); if (rc) return rc;
+    int rc = grouped(p, p->d_invL, bsz, invs, true); if (rc) return rc;
     return grouped(p, p->d_Lb, bsz, tr, true);
   };
+  // A level's TRSM launch that is a single wave (the narrow levels) is streamed behind its k_potrf_smem (see below).
+  const int strips = (npad + kTrsmStrip - 1) / kTrsmStrip;
+  auto trsm_deep = [&](const Level& v) { return strips * v.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024; };
+  auto streamed = [&](const Level& v) {
+    return p->use_trsm_ll && v.nown > 0 && v.ntrsm > 0 && potrf_smem_bytes(npad) <= 220 * 1024 &&
+           strips * v.ntrsm <= (trsm_deep(v) ? 1 : p->trsm2_ctas_per_sm) * p->num_sms;
+  };
+  auto pdl_attr = [](cudaLaunchAttribute& a) { a.id = cudaLaunchAttributeProgrammaticStreamSerialization; a.val.programmaticStreamSerializationAllowed = 1; };
   for (size_t li = 0; li < p->plan.levels.size(); ++li) {
     const Level& lv = p->plan.levels[li]; prof_level = (int)li;
+    // On a streamed level the Cholesky is a programmatic dependent of the previous level's U1 (it waits for it with griddepcontrol.wait
+    // before it reads anything), so its CTAs are resident as soon as U1's SMs drain; and the previous level forked its U2 only after
+    // U1 (below).  Launched beside U1, U2's persistent CTAs (two per SM) took every SM that drained, and k_potrf_smem, which needs a
+    // whole SM, started 15-40 us after U1 had finished.
+    const bool chain = streamed(lv);
+    const bool fork_u2_late = p->overlap && p->gemm_tma && li + 1 < p->plan.levels.size() && streamed(p->plan.levels[li + 1]);
     if (p->plan.dist && (int)li == p->plan.LB) { int rc = phase_boundary(); if (rc) return rc; }
     const int* lframes = p->d_lvl_own + lv.own_off; const int nfr = lv.nown;      // the frames this rank factors at this level
     if (nfr > 0) {
     if (potrf_smem_bytes(npad) <= 220 * 1024) {
-      k_potrf_smem<<<nfr, kPotrfSmemThreads, potrf_smem_bytes(npad), st>>>(p->d_Lb, p->d_invT, lframes, npad, p->d_fail);
+      if (chain && li > 0) {
+        cudaLaunchAttribute attr[1]; pdl_attr(attr[0]);
+        cudaLaunchConfig_t lc = {};
+        lc.gridDim = dim3(nfr); lc.blockDim = dim3(kPotrfSmemThreads); lc.dynamicSmemBytes = potrf_smem_bytes(npad); lc.stream = st;
+        lc.attrs = attr; lc.numAttrs = 1;
+        CK(cudaLaunchKernelEx(&lc, k_potrf_smem, p->d_Lb, p->d_invT, lframes, npad, p->d_fail, p->d_potrf_progress));
+      } else {
+        k_potrf_smem<<<nfr, kPotrfSmemThreads, potrf_smem_bytes(npad), st>>>(p->d_Lb, p->d_invT, lframes, npad, p->d_fail, p->d_potrf_progress);
+      }
       p->paths[LP_POTRF_SMEM]++;
     } else {
       // large blocks: 16-wide panels, panel factor on one CTA per frame, trailing update on the whole machine
@@ -512,18 +555,30 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     if (p->use_trsm_ll) {
       // the explicit inverse is only needed by the (much later) substitution phase: compute it off the critical path
       cudaStream_t is = st;
-      if (p->overlap) { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0)); is = side; side_used = true; }
+      if (p->overlap) { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(inv, p->ev_fork, 0)); is = inv; inv_used = true; }
       k_trinv<<<dim3(npad / 16, nfr), 256, (npad * 16 + 16 * (npad + 1)) * sizeof(double), is>>>(p->d_Lb, p->d_invT, p->d_invL, lframes, npad);
       p->launches += 1; p->paths[LP_TRINV]++; mark(P_TRINV);
       if (lv.ntrsm > 0) {
-        const int strips = (npad + kTrsmStrip - 1) / kTrsmStrip;
-        if (strips * lv.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) {   // a single wave: deep panel prefetch, one CTA per SM
-          k_trsm_ll<4><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 4), st>>>(p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad);
-          p->paths[LP_TRSM_LL4]++;
+        // one CTA per SM fits the launch in a single wave: deep panel prefetch (AHEAD = 4); otherwise two CTAs per SM (AHEAD = 2)
+        const bool deep = trsm_deep(lv);
+        const TrsmTask* tasks = p->d_trsm_ll + lv.trsm_off;
+        // A launch that is a single wave (the narrow levels) starts beside its level's k_potrf_smem as a programmatic dependent launch
+        // and follows the tile columns the Cholesky publishes.  The wide levels' multi-wave launches wait for the Cholesky to finish.
+        if (chain) {
+          cudaLaunchAttribute attr[1]; pdl_attr(attr[0]);
+          cudaLaunchConfig_t lc = {};
+          lc.gridDim = dim3(strips, lv.ntrsm); lc.blockDim = dim3(128); lc.dynamicSmemBytes = trsm_ll_smem_bytes(npad, deep ? 4 : 2); lc.stream = st;
+          lc.attrs = attr; lc.numAttrs = 1;
+          const double *Lb = p->d_Lb, *invT = p->d_invT; const int* progress = p->d_potrf_progress;
+          CK(deep ? cudaLaunchKernelEx(&lc, k_trsm_ll<4, true>, p->d_T, Lb, invT, tasks, npad, progress)
+                  : cudaLaunchKernelEx(&lc, k_trsm_ll<2, true>, p->d_T, Lb, invT, tasks, npad, progress));
+          p->paths[LP_TRSM_STREAMED]++;
+        } else if (deep) {
+          k_trsm_ll<4><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 4), st>>>(p->d_T, p->d_Lb, p->d_invT, tasks, npad, nullptr);
         } else {
-          k_trsm_ll<2><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 2), st>>>(p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad);
-          p->paths[LP_TRSM_LL2]++;
+          k_trsm_ll<2><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 2), st>>>(p->d_T, p->d_Lb, p->d_invT, tasks, npad, nullptr);
         }
+        p->paths[deep ? LP_TRSM_LL4 : LP_TRSM_LL2]++;
         p->launches++; mark(P_TRSM);
       }
     } else {
@@ -538,9 +593,8 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->plan.tseg[(li * p->nranks + q) * 2], (size_t)p->plan.tseg[(li * p->nranks + q) * 2 + 1]});
       int rc = grouped(p, p->d_T, bsz, segs, true); if (rc) return rc;
     }
-    if (lv.nupd2 > 0 && p->overlap) {
-      CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0));
-    }
+    auto fork_u2 = [&]() -> int { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0)); return RCVD_OK; };
+    if (lv.nupd2 > 0 && p->overlap && !fork_u2_late) { if (int rc = fork_u2()) return rc; }
     if (side_pending) { CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }   // U2(l-1) before U1(l)
     auto update = [&](cudaStream_t cs, int off, int n) {   // persistent TMA-fed update kernel
       if (n <= p->num_sms) {   // few items: two DMMA teams per tile, one CTA per SM
@@ -556,6 +610,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     if (p->gemm_tma) {
       if (lv.nit > 0) { update(st, lv.it_off, lv.nit); p->launches++; mark(P_GEMM); }
       if (lv.nit2 > 0) {
+        if (fork_u2_late) { if (int rc = fork_u2()) return rc; }   // after U1
         update(p->overlap ? side : st, lv.it2_off, lv.nit2); p->launches++; mark(P_GEMM);
         if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
       }
@@ -569,6 +624,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   }
   if (p->plan.dist && p->plan.LB >= (int)p->plan.levels.size()) { int rc = phase_boundary(); if (rc) return rc; }
   if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); }
+  if (int rc = join_inv()) return rc;
   CK(cudaMemcpyAsync(p->d_rhs, p->d_gs, (size_t)N * npad * sizeof(double), cudaMemcpyDeviceToDevice, st));
   const int nlv = (int)p->plan.levels.size();
   const int LS = p->plan.sub_first_level;       // levels >= LS: the persistent dataflow kernel (rcvd_linalg.cuh, k_substitution)
@@ -1026,8 +1082,10 @@ RCVD_API int32_t rcvd_problem_create(const rcvd_config* cfg, int32_t device, rcv
   int prio_lo = 0, prio_hi = 0; cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
   e = cudaStreamCreateWithPriority(&p->stream, cudaStreamNonBlocking, prio_hi);
   if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&p->side_stream, cudaStreamNonBlocking, prio_lo);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&p->inv_stream, cudaStreamNonBlocking, prio_lo);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_join, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_inv_join, cudaEventDisableTiming);
   if (e != cudaSuccess) { delete p; return set_err(RCVD_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)); }
   *out = p; return RCVD_OK;
 }
@@ -1039,7 +1097,9 @@ RCVD_API void rcvd_problem_destroy(rcvd_problem* p) {
   if (p->comm && nccl::CommDestroy) nccl::CommDestroy(p->comm);
   if (p->ev_fork) cudaEventDestroy(p->ev_fork);
   if (p->ev_join) cudaEventDestroy(p->ev_join);
+  if (p->ev_inv_join) cudaEventDestroy(p->ev_inv_join);
   if (p->side_stream) cudaStreamDestroy(p->side_stream);
+  if (p->inv_stream) cudaStreamDestroy(p->inv_stream);
   if (p->stream) cudaStreamDestroy(p->stream);
   delete p;
 }
@@ -1205,7 +1265,7 @@ RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double
   if (!p->structure_ready || !p->factored) return set_err(RCVD_ERR_INVALID, "no factorisation has run on this handle");
   if (p->plan.dist) return set_err(RCVD_ERR_INVALID, "the distributed factorisation keeps its blocks on their owners");
   SET_DEVICE(p->device);
-  CK(cudaStreamSynchronize(p->side_stream)); CK(cudaStreamSynchronize(p->stream));
+  CK(cudaStreamSynchronize(p->side_stream)); CK(cudaStreamSynchronize(p->inv_stream)); CK(cudaStreamSynchronize(p->stream));
   const int N = p->N, nf = p->L.nf, npad = p->L.npad, nT = p->plan.nLoff; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
   std::vector<double> hL((size_t)N * bs), hT((size_t)nT * bs);
   CK(cudaMemcpy(hL.data(), p->d_Lb, hL.size() * sizeof(double), cudaMemcpyDeviceToHost));   // the first N blocks: diagonal blocks L_kk
@@ -1228,9 +1288,9 @@ RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double
   }
   return RCVD_OK;
 }
-RCVD_API int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]) {
+RCVD_API int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[14]) {
   if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
-  static_assert(LP_N == 13, "include/rcvd_hooks.h documents thirteen counters");
+  static_assert(LP_N == 14, "include/rcvd_hooks.h documents fourteen counters");
   std::copy(p->paths, p->paths + LP_N, out);
   return RCVD_OK;
 }
@@ -1304,7 +1364,7 @@ RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double
     evs.clear(); p->prof = &evs;
     rc = enqueue_factor_solve(p);
     p->prof = nullptr; p->factored = true;
-    cudaStreamSynchronize(p->stream); cudaStreamSynchronize(p->side_stream);
+    cudaStreamSynchronize(p->stream); cudaStreamSynchronize(p->side_stream); cudaStreamSynchronize(p->inv_stream);
     double ngemm = 0;
     for (size_t i = 1; i < evs.size(); ++i) {
       float ms = 0; cudaEventElapsedTime(&ms, evs[i - 1].second, evs[i].second);

@@ -113,6 +113,11 @@ __device__ __forceinline__ void dmma_8x8x4_fwd(double& c0, double& c1, double a,
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
+// GPU-scope flags between kernels that run at the same time: k_potrf_smem -> streamed k_trsm_ll (per-frame progress), k_substitution.
+// The writer's CTA barrier orders every thread's stores before one thread's release (cumulativity), like cutlass::Semaphore::release.
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) { int v; asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
+__device__ __forceinline__ void st_release_gpu(int* p, int v) { asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ void red_release_add(int* p, int v) { asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
 // C(16x16) = A(16x16) * B(16x16)^T into acc[i8][j8][2] with DMMA; A, B swizzled tiles in smem.
 __device__ __forceinline__ void tile_mma_nt(const double* __restrict__ At, const double* __restrict__ Bt, double acc[2][2][2], int g, int t) {
@@ -224,8 +229,18 @@ __device__ __forceinline__ void warp_chol16_blocked(double* __restrict__ D, doub
 }
 
 
+// Tile column jb of L is final at the end of tile step jb.  The worker warps store it to Lb at the start of step jb + 1, while the
+// chain warp works alone before barrier 2, and then publish progress[frame] = jb + 1 (the last column after the loop): the streamed
+// k_trsm_ll reads row panel jt of L and the tile inverse Di_jt as soon as progress reaches jt + 1.  Every step runs even after a
+// non-positive pivot (*fail is set, the pivot replaced), so the counter always reaches nt.
 __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __restrict__ Lb, double* __restrict__ invT,
-                                                                   const int* __restrict__ frames, int npad, int* __restrict__ fail) {
+                                                                   const int* __restrict__ frames, int npad, int* __restrict__ fail,
+                                                                   int* __restrict__ progress) {
+  // Launched as a programmatic dependent of the previous level's U1 on the narrow levels: wait for it (and its memory) before reading
+  // anything; a no-op after an ordinary launch dependency.  Then this CTA's inputs are complete, and a programmatic dependent launch
+  // (the streamed k_trsm_ll, which reads blocks U1 updated) may start beside it.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   extern __shared__ __align__(16) double tiles[];
   const int frame = frames[blockIdx.x];
   double* A = Lb + (size_t)frame * npad * npad;
@@ -234,6 +249,18 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
   double* pinv = tiles + (size_t)ntl * kTileSz;     // [npad] reciprocal pivots (fits the spare 2 KB tile for npad <= 256)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, nw = kPotrfSmemThreads / 32;
   const int g = lane >> 2, t = lane & 3;
+  // worker warps only: store tile column jc to Lb (16-byte chunks, 128 contiguous bytes per row; the diagonal tile's upper triangle
+  // zeroed), meet on barrier 3, then one thread publishes jc + 1
+  auto publish = [&](int jc) {
+    for (int idx = tid - 32; idx < (nt - jc) * 128; idx += kPotrfSmemThreads - 32) {
+      const int ti = jc + (idx >> 7), e = idx & 127, r = e >> 3, c = (e & 7) * 2;
+      double2 v = *reinterpret_cast<const double2*>(&tiles[(size_t)(ti * (ti + 1) / 2 + jc) * kTileSz + swz(r, c)]);
+      if (ti == jc) { if (c > r) v.x = 0.0; if (c + 1 > r) v.y = 0.0; }
+      *reinterpret_cast<double2*>(&A[(size_t)(ti * 16 + r) * npad + jc * 16 + c]) = v;
+    }
+    asm volatile("bar.sync 3, %0;" ::"n"(kPotrfSmemThreads - 32) : "memory");
+    if (tid == 32) st_release_gpu(progress + frame, jc + 1);
+  };
 #ifdef RCVD_POTRF_PHASES
   long long last_ = clock64();
 #endif
@@ -269,7 +296,10 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
     // warps' trailing update slower by more: 2.77 against 2.68 ms per factorisation)
     const int nwork = nw - 1, widx = warp - 1;       // worker warps beside the chain warp
     if (warp == 0) { if (lane < 16 && rows > 0) prow = lane; } else if (widx * 32 + lane < rows - 16) prow = 16 + widx * 32 + lane;
-    if (warp != 0) asm volatile("bar.sync 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
+    if (warp != 0) {
+      if (jb > 0) publish(jb - 1);                   // in the time the chain warp needs before it arrives on barrier 2
+      asm volatile("bar.sync 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
+    }
     if (prow >= 0) {
       const int ti = jb + 1 + (prow >> 4), r = prow & 15;
       double* Tt = tiles + (size_t)(ti * (ti + 1) / 2 + jb) * kTileSz;
@@ -351,16 +381,7 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
     __syncthreads();
     POTRF_PHASE(7);
   }
-  for (int idx = tid; idx < ntl * 128; idx += kPotrfSmemThreads) {
-    const int tl = idx >> 7, e = idx & 127, r = e >> 3, c = (e & 7) * 2;
-    int ti = (int)((sqrtf(8.f * tl + 1.f) - 1.f) * 0.5f);
-    while ((ti + 1) * (ti + 2) / 2 <= tl) ++ti;
-    while (ti * (ti + 1) / 2 > tl) --ti;
-    const int tj = tl - ti * (ti + 1) / 2;
-    double2 v = *reinterpret_cast<const double2*>(&tiles[(size_t)tl * kTileSz + swz(r, c)]);
-    if (ti == tj) { if (c > r) v.x = 0.0; if (c + 1 > r) v.y = 0.0; }
-    *reinterpret_cast<double2*>(&A[(size_t)(ti * 16 + r) * npad + tj * 16 + c]) = v;
-  }
+  if (warp != 0) publish(nt - 1);
 }
 
 // ---------------------------------------------------------------------------
@@ -604,10 +625,20 @@ constexpr int kTrsmStrip = 4 * kTrsmRW;
 // trsm 2.03 -> 2.72 ms per factorisation, because occupancy halves where throughput counts).
 __host__ __device__ inline size_t trsm_ll_smem_bytes(int npad, int ahead = 2) { return ((size_t)kTrsmStrip * (npad + 4) + ahead * 16 * (size_t)(npad + 4) + ahead * 16 * 20) * sizeof(double); }
 
-template <int kTrsmAhead>
+// cp.async.wait_group with a run-time count of groups that may stay in flight (0..3)
+__device__ __forceinline__ void cp_async_wait_upto3(int n) {
+  if (n >= 3) cp_async_wait<3>(); else if (n == 2) cp_async_wait<2>(); else if (n == 1) cp_async_wait<1>(); else cp_async_wait<0>();
+}
+
+// kStreamed: launched as a programmatic dependent of the k_potrf_smem of the same level, so it runs while the Cholesky of its column
+// frame is still going on.  Step jt reads only row panel jt of L_kk and Di_jt, which k_potrf_smem publishes in progress[kframe] >= jt + 1;
+// a panel is staged once it is published, up to kTrsmAhead steps ahead.  The arithmetic and its order are those of the unstreamed kernel.
+template <int kTrsmAhead, bool kStreamed = false>
 __global__ void __launch_bounds__(128) k_trsm_ll(double* __restrict__ T, const double* __restrict__ Lb, const double* __restrict__ invT,
-                                                  const TrsmTask* __restrict__ tasks, int npad) {
+                                                  const TrsmTask* __restrict__ tasks, int npad, const int* progress) {
+  static_assert(!kStreamed || kTrsmAhead <= 4, "cp_async_wait_upto3 leaves at most three groups in flight");
   extern __shared__ __align__(16) double smx[];
+  __shared__ int s_ready;                        // (kStreamed) the progress thread 0 read last
   const int ld = npad + 4;                       // ld = 4 (mod 16): conflict-free DMMA fragment loads
   double* Xs = smx;                              // [kTrsmStrip][ld]
   double* Ls = smx + (size_t)kTrsmStrip * ld;    // [kTrsmAhead][16][ld]   L[jt*16 .. +15][0 .. jt*16)
@@ -639,12 +670,36 @@ __global__ void __launch_bounds__(128) k_trsm_ll(double* __restrict__ T, const d
     }
     cp_async_commit();
   };
+  if constexpr (kStreamed) {
+    cp_async_commit();                            // the A strip was finished by earlier levels: its own group, in flight at once
+  } else {
 #pragma unroll
-  for (int q = 0; q < kTrsmAhead; ++q) stage(q);         // group 0 also carries the A strip
+    for (int q = 0; q < kTrsmAhead; ++q) stage(q);       // group 0 also carries the A strip
+  }
   constexpr int NI = kTrsmRW / 8;                 // m8 tiles per warp
   const int wr = warp * kTrsmRW;                  // this warp's rows inside the strip
+  int staged = 0, ready = 0;                      // (kStreamed) panels [0, staged) are staged; [0, ready) are known to be published
   for (int jt = 0; jt < nt; ++jt) {
-    cp_async_wait<kTrsmAhead - 1>();              // groups complete in order: panel jt has landed, up to kTrsmAhead - 1 later ones may be in flight
+    if constexpr (kStreamed) {
+      if (ready < min(nt, jt + kTrsmAhead)) {     // a free ring slot may take a panel not known to be published yet: read the counter
+        if (tid == 0) {
+          // Waits only while panel jt itself is unpublished.  This cannot deadlock: a programmatic dependent launch starts only after
+          // every CTA of the k_potrf_smem before it has executed griddepcontrol.launch_dependents, so the producer of this counter is
+          // resident (or done) before any consumer exists, and it never waits on a consumer.  Launched without overlap (the un-captured
+          // profiling and first multi-GPU runs, or a driver that ignores the attribute), k_potrf_smem has finished and every counter is
+          // final.  The counters are zeroed in the factorisation graph before level 0, so a stale count never reads as published.
+          int v = ld_acquire_gpu(progress + task.kframe);
+          while (v <= jt) { __nanosleep(32); v = ld_acquire_gpu(progress + task.kframe); }
+          s_ready = v;
+        }
+        __syncthreads();                          // thread 0's acquire orders every thread's panel loads below after the publication
+        ready = s_ready;
+      }
+      for (; staged < min(ready, jt + kTrsmAhead); ++staged) stage(staged);   // ring slot staged % kTrsmAhead was freed by step staged - kTrsmAhead
+      cp_async_wait_upto3(staged - 1 - jt);       // one group per panel after the A strip's: panel jt has landed
+    } else {
+      cp_async_wait<kTrsmAhead - 1>();            // groups complete in order: panel jt has landed, up to kTrsmAhead - 1 later ones may be in flight
+    }
     __syncthreads();
     const double* ls = Ls + (size_t)(jt % kTrsmAhead) * 16 * ld; const double* dsm = Ds + (jt % kTrsmAhead) * 320;
     double acc[NI][2][2];
@@ -719,8 +774,11 @@ __global__ void __launch_bounds__(128) k_trsm_ll(double* __restrict__ T, const d
         if (r < rows) *reinterpret_cast<double2*>(&X[(size_t)(m0 + r) * npad + cidx]) = v;
       }
     __syncthreads();   // every warp is done with ring slot jt % kTrsmAhead before it is refilled
-    stage(jt + kTrsmAhead);
+    if constexpr (!kStreamed) stage(jt + kTrsmAhead);
   }
+  // k_potrf_smem has published its last panel, so it is (about) done: this wait costs nothing, and it makes the completion of this
+  // kernel imply the completion of k_potrf_smem for whatever follows it with an ordinary dependency
+  if constexpr (kStreamed) asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
 
@@ -822,10 +880,8 @@ constexpr int kSubThreads = 256;
 struct SubTask { int type; int blk; int r; int k; int chunk; };   // type 0 FDIAG, 1 FUPD, 2 BUPD, 3 BDIAG
 struct SubCounters { int* ticket; int* fin; int* fdone; int* bin; int* bdone; const int* fin_need; const int* bin_need; };
 
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) { int v; asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ void sub_wait(const int* c, int need) { while (ld_acquire_gpu(c) < need) __nanosleep(20); }
 
-__device__ __forceinline__ void red_release_add(int* p, int v) { asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ double2 ldcg2(const double* p) { return __ldcg(reinterpret_cast<const double2*>(p)); }
 
 __global__ void __launch_bounds__(kSubThreads) k_substitution(const double* __restrict__ invL, const double* __restrict__ T, double* rhs, double* y, double* x,

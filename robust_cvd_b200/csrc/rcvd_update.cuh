@@ -162,6 +162,9 @@ __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::cta
   // The ring must start on a 1 KB boundary (swizzle atom = 8 rows x 128 B).  It is addressed as the extern array itself: rounding the
   // pointer up through an integer makes the compiler lose the shared address space and emit generic LD.E.64 for every fragment load.
   extern __shared__ __align__(1024) unsigned char ring[];
+  // a programmatic dependent launch (the next narrow level's k_potrf_smem, which waits for this grid before reading) may take the SMs
+  // this launch drains
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (smem_u32(ring) & 1023u) __trap();
   constexpr int kUpdStages = UpdShape<TEAMS>::stages;
   const int tile_bytes = rb * 128, stage_bytes = 2 * tile_bytes;                     // A tile then B tile, [rb][16 doubles]

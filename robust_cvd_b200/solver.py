@@ -173,7 +173,7 @@ class Problem:
         return order, Lf, Li
 
     LINEAR_PATHS = ("potrf_smem", "potrf_panel", "trsm_ll4", "trsm_ll2", "trsm_gemm", "update_tma1", "update_tma2", "update_gemm",
-                    "substitution_levels", "substitution_fused", "trinv", "other", "update_tma1_multi_item")
+                    "substitution_levels", "substitution_fused", "trinv", "other", "update_tma1_multi_item", "trsm_ll_streamed")
 
     def linear_paths(self):
         """Test hook: launches of each factorisation / solve kernel path since the handle was created (LINEAR_PATHS)."""

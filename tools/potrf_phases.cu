@@ -9,14 +9,14 @@ int main() {
   const int n = 208;
   std::vector<double> A((size_t)n * n);
   for (int i = 0; i < n; ++i) for (int j = 0; j <= i; ++j) { double v = std::sin(0.37 * i + 1.3 * j) * 0.5; if (i == j) v = n; A[(size_t)i * n + j] = v; A[(size_t)j * n + i] = v; }
-  double *dA, *dT; int *dF, *dfail; cudaMalloc(&dA, A.size() * 8); cudaMalloc(&dT, n * 16 * 8); cudaMalloc(&dF, 4); cudaMalloc(&dfail, 4);
+  double *dA, *dT; int *dF, *dfail, *dprog; cudaMalloc(&dA, A.size() * 8); cudaMalloc(&dT, n * 16 * 8); cudaMalloc(&dF, 4); cudaMalloc(&dfail, 4); cudaMalloc(&dprog, 4);
   int zero = 0; cudaMemcpy(dF, &zero, 4, cudaMemcpyHostToDevice); cudaMemset(dfail, 0, 4);
   cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_smem_bytes(n));
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   for (int rep = 0; rep < 4; ++rep) {   // rep 0 warms up
     cudaMemcpy(dA, A.data(), A.size() * 8, cudaMemcpyHostToDevice);
     long long z[16] = {0}; cudaMemcpyToSymbol(g_potrf_phase, z, sizeof(z));
-    cudaEventRecord(e0); k_potrf_smem<<<1, kPotrfSmemThreads, potrf_smem_bytes(n)>>>(dA, dT, dF, n, dfail); cudaEventRecord(e1); cudaEventSynchronize(e1);
+    cudaEventRecord(e0); k_potrf_smem<<<1, kPotrfSmemThreads, potrf_smem_bytes(n)>>>(dA, dT, dF, n, dfail, dprog); cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
     long long ph[16]; cudaMemcpyFromSymbol(ph, g_potrf_phase, sizeof(ph));
     printf("rep %d: %.1f us; cycles: load %lld, first chol %lld, panel(thread0) %lld, wait-panel %lld, update-to-lookahead %lld, lookahead chol %lld, rest of update %lld, wait-update %lld  (%s)\n",
