@@ -310,6 +310,31 @@ int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t device, c
                                int64_t* pair_offsets, float* pair_out, int64_t pair_capacity,
                                int64_t* trip_offsets, float* trip_out, int64_t trip_capacity);
 
+/* ---- long point tracks (DESIGN.md section 1 row 8f-6) ----
+ * Replaces DepthVideoProcessor::computeTracks (lib/Processor.cpp:646-886) for a frame range.  Arrays are indexed by a local frame
+ * index 0..num_frames-1 over [range.firstFrame(), range.lastFrame()]: local 0 is the first frame of the range, num_frames-1 the last.
+ *   color_bgr   [num_frames][height][width][3] f32  "down" colour stream (BGR, CV_32FC3)
+ *   dyn_masks   [num_frames][dyn_height][dyn_width] u8  raw dynamic_mask frames (< 127 = dynamic), or NULL without that stream
+ *   flow        [num_frames][height][width][2] f32, flow_mask [num_frames][height][width] u8: slot i holds the flow and mask of
+ *               (first + i - 1 -> first + i); read only where frame_flags says they are usable
+ *   frame_flags [num_frames] bits RCVD_TRACK_IN_RANGE, RCVD_TRACK_HAS_COLOR, RCVD_TRACK_FLOW (flow file present at colour size),
+ *               RCVD_TRACK_MASK (mask file present at colour size)
+ * Outputs: frame_offsets [num_frames+1]; obs_track [n] i32 track ids, ascending within each frame; obs_loc [n][2] f32 normalised
+ * locations (x / w, y / h * inv_aspect); *num_tracks = ids created (short tracks are not deleted here).  If capacity (observations)
+ * is too small the offsets are still filled and RCVD_ERR_INVALID is returned.  Ids and locations equal the reference's bit for bit;
+ * where it reads outside an image (dynamic distance at -1, a track row rounded to height) the nearest pixel is read. */
+enum { RCVD_TRACK_IN_RANGE = 1, RCVD_TRACK_HAS_COLOR = 2, RCVD_TRACK_FLOW = 4, RCVD_TRACK_MASK = 8 };
+typedef struct rcvd_track_params {
+  int32_t num_frames, width, height, dyn_width, dyn_height;
+  int32_t spawn_distance;          /* Params::trackSpawnDistance (>= 0) */
+  int32_t prune_distance;          /* Params::trackPruneDistance (>= 0) */
+  float min_dynamic_distance;      /* Params::minDynamicDistance */
+  float inv_aspect;                /* DepthVideo::invAspect() */
+} rcvd_track_params;
+int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t device, const float* color_bgr, const uint8_t* dyn_masks,
+                            const float* flow, const uint8_t* flow_mask, const uint8_t* frame_flags,
+                            int64_t* frame_offsets, int32_t* obs_track, float* obs_loc, int64_t capacity, int64_t* num_tracks);
+
 /* Static flags of flow constraints on the device: replaces FlowConstraintsCollection::setStaticFlagFromDynamicMask
  * (reference lib/FlowConstraints.cpp:573-660) and the distance images of ::dynamicDistance (:257-286).
  * masks [F][h][w] u8 (dynamic-mask frames: < 127 = dynamic); a constraint is static when

@@ -12,6 +12,7 @@ int64_t rcvd_launch_count(rcvd_problem* p);
 int64_t rcvd_filter_launch_count(void);
 int64_t rcvd_builder_launch_count(void);
 int64_t rcvd_static_flag_launch_count(void);
+int64_t rcvd_tracks_launch_count(void);
 int64_t rcvd_builder_last_rounds(void);          /* selection rounds of the last rcvd_build_constraints call */
 
 /* {frames, off-diagonal factor blocks, levels, H blocks, npad, stride, tiles, update tasks} */

@@ -89,6 +89,15 @@ class BuilderParams(C.Structure):
                [("min_dynamic_distance", C.c_float), ("inv_aspect", C.c_float)]
 
 
+class TrackParams(C.Structure):
+    """rcvd_track_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("num_frames", "width", "height", "dyn_width", "dyn_height", "spawn_distance", "prune_distance")] + \
+               [("min_dynamic_distance", C.c_float), ("inv_aspect", C.c_float)]
+
+
+TRACK_IN_RANGE, TRACK_HAS_COLOR, TRACK_FLOW, TRACK_MASK = 1, 2, 4, 8   # rcvd_compute_tracks frame flags
+
+
 def default_config(num_frames, aspect, **kw):
     """Config with the reference's Params defaults (lib/PoseOptimizer.h:55-103)."""
     focal_long = kw.pop("focal_long", 0.3461538376301239)

@@ -15,6 +15,7 @@
 #include <string>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 #include "rcvd_eval.cuh"
 #include "rcvd_linalg.cuh"
@@ -24,6 +25,7 @@
 #include "rcvd_filter.cuh"
 #include "rcvd_bilateral.cuh"
 #include "rcvd_builder.cuh"
+#include "rcvd_tracks.cuh"
 static int64_t g_filter_launches = 0;
 
 using namespace rcvd;
@@ -1976,5 +1978,163 @@ RCVD_API int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t
   if (e == cudaSuccess) e = cudaGetLastError();
   cleanup();
   if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "static-flag kernels failed: %s", cudaGetErrorString(e));
+  return RCVD_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Long point tracks (rcvd_tracks.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_track_launches = 0;
+RCVD_API int64_t rcvd_tracks_launch_count() { return g_track_launches; }
+RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t device, const float* color_bgr, const uint8_t* dyn_masks,
+                                     const float* flow, const uint8_t* flow_mask, const uint8_t* frame_flags,
+                                     int64_t* frame_offsets, int32_t* obs_track, float* obs_loc, int64_t capacity, int64_t* num_tracks) {
+  if (!prm || !color_bgr || !frame_flags || !frame_offsets || !num_tracks) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_track_params& q = *prm;
+  const int F = q.num_frames, W = q.width, H = q.height;
+  if (F <= 0 || W <= 0 || H <= 0 || q.spawn_distance < 0 || q.prune_distance < 0 || !(q.inv_aspect > 0.f) || (size_t)W * H >= (1u << 31))
+    return set_err(RCVD_ERR_INVALID, "bad track parameters");
+  if (dyn_masks && (q.dyn_width <= 0 || q.dyn_height <= 0)) return set_err(RCVD_ERR_INVALID, "bad dynamic-mask size");
+  bool need_flow = false, need_mask = false;
+  for (int f = 0; f < F; ++f) { need_flow |= (frame_flags[f] & RCVD_TRACK_FLOW) != 0; need_mask |= (frame_flags[f] & RCVD_TRACK_MASK) != 0; }
+  if ((need_flow && !flow) || (need_mask && !flow_mask)) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int f = 0; f <= F; ++f) frame_offsets[f] = 0;
+  *num_tracks = 0;
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev)
+    return set_err(RCVD_ERR_NO_DEVICE, "no usable CUDA device (%s); this library has no CPU fallback", e != cudaSuccess ? cudaGetErrorString(e) : "device ordinal out of range");
+  SET_DEVICE(device);
+  const int plane = W * H;
+  const size_t FP = (size_t)F * plane, dplane = dyn_masks ? (size_t)q.dyn_width * q.dyn_height : 0;
+  const int max_rounds = 4 * (W + H) + 16, max_live = 2 * plane;   // at most one continued and one spawned track per pixel
+  // the re-derived pixel of a spawn candidate (:844-845): x -> int(float(x / float(w)) * w), y -> int(float(float(y / float(h)) * ia) / ia * h)
+  std::vector<int> mxv(W), myv(H);
+  for (int x = 0; x < W; ++x) { volatile float u = x / float(W); volatile float v = u * W; mxv[x] = (int)v; }
+  for (int y = 0; y < H; ++y) { volatile float u = y / float(H); volatile float v = u * q.inv_aspect; volatile float t = v / q.inv_aspect; volatile float z = t * H; myv[y] = (int)z; }
+  cudaStream_t st; CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  std::vector<void*> bufs; bool ok = true;
+  auto dev = [&](size_t bytes) -> void* { void* ptr = nullptr; if (cudaMallocAsync(&ptr, std::max<size_t>(bytes, 16), st) != cudaSuccess) { ok = false; cudaGetLastError(); return nullptr; } bufs.push_back(ptr); return ptr; };
+  auto up = [&](const void* src, size_t bytes) -> void* { void* d = dev(bytes); if (d && src && bytes) cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, st); return d; };
+  auto cleanup = [&]() { for (void* b : bufs) cudaFreeAsync(b, st); cudaStreamSynchronize(st); cudaStreamDestroy(st); };
+  // ---- corner scores and distance images of every frame, batched ----
+  float* d_bgr = (float*)up(color_bgr, FP * 12);
+  float* d_gray = (float*)dev(FP * 4), *d_pl = (float*)dev(FP * 12), *d_corner = (float*)dev(FP * 4); double* d_tmp = (double*)dev(FP * 24);
+  uint8_t* d_dmask = dyn_masks ? (uint8_t*)up(dyn_masks, (size_t)F * dplane) : nullptr;
+  unsigned* d_cscratch = dyn_masks ? (unsigned*)dev((size_t)F * dplane * 4) : nullptr;
+  float* d_dist = dyn_masks ? (float*)dev((size_t)F * dplane * 4) : nullptr;
+  const float* d_flow = need_flow ? (const float*)up(flow, FP * 8) : nullptr;
+  const uint8_t* d_fmask = need_mask ? (const uint8_t*)up(flow_mask, FP) : nullptr;
+  const int* d_mx = (const int*)up(mxv.data(), (size_t)W * 4), *d_my = (const int*)up(myv.data(), (size_t)H * 4);
+  // ---- per-frame working set ----
+  int* d_id[2] = {(int*)dev((size_t)max_live * 4), (int*)dev((size_t)max_live * 4)};
+  float* d_loc[2] = {(float*)dev((size_t)max_live * 8), (float*)dev((size_t)max_live * 8)};
+  int* d_pix = (int*)dev((size_t)max_live * 4); float* d_cloc = (float*)dev((size_t)max_live * 8); uint8_t* d_cstate = (uint8_t*)dev(max_live);
+  unsigned* d_acc = (unsigned*)dev((size_t)plane * 4);
+  unsigned* d_und[3] = {(unsigned*)dev((size_t)plane * 4), (unsigned*)dev((size_t)plane * 4), (unsigned*)dev((size_t)plane * 4)};
+  uint8_t* d_smask = (uint8_t*)dev(plane); uint8_t* d_sstate = (uint8_t*)dev(plane);
+  unsigned long long* d_keys = (unsigned long long*)dev((size_t)plane * 8), *d_sorted = (unsigned long long*)dev((size_t)plane * 8);
+  unsigned* d_cnt = (unsigned*)dev((size_t)2 * max_rounds * 4);   // [0, max_rounds) prune rounds, then spawn rounds
+  int* d_counts = (int*)dev(8);
+  size_t sort_bytes = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, d_keys, d_sorted, plane, 0, 64, st);
+  void* d_sort_tmp = dev(sort_bytes);
+  if (!ok) { cleanup(); return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_compute_tracks"); }
+  k_gray<<<(unsigned)((FP + 255) / 256), 256, 0, st>>>(d_bgr, d_gray, FP);
+  k_sobel_products<<<(unsigned)((FP + 255) / 256), 256, 0, st>>>(d_gray, d_pl, F, H, W);
+  k_box_h<<<(unsigned)((FP * 3 + 255) / 256), 256, 0, st>>>(d_pl, d_tmp, (size_t)3 * F * H, W);
+  k_box_v_eig<<<(unsigned)(((size_t)F * W + 127) / 128), 128, 0, st>>>(d_tmp, d_corner, F, H, W);
+  g_track_launches += 4;
+  if (dyn_masks) { k_chamfer5<<<F, kChamThreads, 0, st>>>(d_dmask, d_cscratch, d_dist, q.dyn_height, q.dyn_width); g_track_launches++; }
+  TrackArgs a{};
+  a.w = W; a.h = H; a.dw = dyn_masks ? q.dyn_width : W; a.dh = dyn_masks ? q.dyn_height : H;
+  a.spawn_r = q.spawn_distance; a.prune_r = q.prune_distance; a.min_dyn = q.min_dynamic_distance; a.ia = q.inv_aspect;
+  // dynamic-mask scale (:657-663); without a mask the distance is FLT_MAX at colour size
+  a.dsx = dyn_masks ? q.dyn_width / float(W) : 1.f; a.dsy = dyn_masks ? q.dyn_height / float(H) : 1.f;
+  // ---- the frame loop: one host round trip per frame (round convergence + list sizes) ----
+  std::vector<int32_t> ids; std::vector<float> locs;
+  int cur = 0, n_prev = 0, next_id = 0, rp = 4, rs = 16;
+  std::vector<unsigned> cnt_h((size_t)2 * max_rounds);
+  int counts_h[2] = {0, 0};
+  int rc = RCVD_OK;
+  // copies the finished list of local frame g (n entries, buffer slot b) into the outputs
+  auto flush = [&](int g, int b, int n) -> cudaError_t {
+    frame_offsets[g + 1] = frame_offsets[g] + n;
+    if (n == 0) return cudaSuccess;
+    ids.resize((size_t)frame_offsets[g + 1]); locs.resize((size_t)frame_offsets[g + 1] * 2);
+    cudaError_t e1 = cudaMemcpyAsync(ids.data() + frame_offsets[g], d_id[b], (size_t)n * 4, cudaMemcpyDeviceToHost, st);
+    if (e1 == cudaSuccess) e1 = cudaMemcpyAsync(locs.data() + 2 * frame_offsets[g], d_loc[b], (size_t)n * 8, cudaMemcpyDeviceToHost, st);
+    return e1;
+  };
+  for (int f = 0; f < F && rc == RCVD_OK; ++f) {
+    const uint8_t fl = frame_flags[f];
+    const int prev = cur, nxt = cur ^ 1;
+    if (!(fl & RCVD_TRACK_IN_RANGE) || !(fl & RCVD_TRACK_HAS_COLOR)) {   // the frame gets no tracks (:714-727)
+      if (f > 0) { e = flush(f - 1, prev, n_prev); if (e == cudaSuccess) e = cudaStreamSynchronize(st); if (e != cudaSuccess) { rc = set_err(RCVD_ERR_CUDA, "track read-back failed: %s", cudaGetErrorString(e)); break; } }
+      n_prev = 0; cur = nxt;
+      continue;
+    }
+    a.dist = dyn_masks ? d_dist + (size_t)f * dplane : nullptr;
+    const bool cont = f > 0 && n_prev > 0 && (fl & RCVD_TRACK_FLOW) && (fl & RCVD_TRACK_MASK);
+    const bool spawn = f < F - 1;
+    const float* score = d_corner + (size_t)f * plane;
+    if (spawn) {
+      k_tr_sort_keys<<<nblk(plane), 256, 0, st>>>(score, plane, d_keys); g_track_launches++;
+      cub::DeviceRadixSort::SortKeys(d_sort_tmp, sort_bytes, d_keys, d_sorted, plane, 0, 64, st);
+    }
+    for (;;) {   // rounds enqueued blind (they stop early on the device); a frame whose rounds did not all finish is run again with more
+      cudaMemsetAsync(d_cnt, 0, (size_t)2 * max_rounds * 4, st);
+      cudaMemsetAsync(d_smask, 0, plane, st);
+      if (cont) {
+        cudaMemsetAsync(d_acc, 0xff, (size_t)plane * 4, st); cudaMemsetAsync(d_und[0], 0xff, (size_t)plane * 4, st); cudaMemsetAsync(d_und[1], 0xff, (size_t)plane * 4, st);
+        k_tr_continue<<<nblk(n_prev), 256, 0, st>>>(a, n_prev, d_loc[prev], d_flow + (size_t)f * plane * 2, d_fmask + (size_t)f * plane, d_pix, d_cloc, d_cstate, d_und[0]);
+        g_track_launches++;
+        for (int k = 0; k < rp; ++k) {
+          k_tr_prune_round<<<nblk(std::max(n_prev, plane)), 256, 0, st>>>(a, n_prev, k, d_pix, d_cstate, d_acc, d_und[k % 3], d_und[(k + 1) % 3], d_und[(k + 2) % 3], d_cnt);
+          g_track_launches++;
+        }
+        k_tr_stamp<<<n_prev, 256, 0, st>>>(a, d_pix, d_cstate, d_smask); g_track_launches++;
+      }
+      if (spawn) {
+        const uint8_t* sm = (fl & RCVD_TRACK_MASK) ? d_fmask + (size_t)f * plane : nullptr;
+        k_tr_spawn_init<<<nblk(plane), 256, 0, st>>>(a, sm, d_smask, d_mx, d_my, d_sstate); g_track_launches++;
+        for (int k = 0; k < rs; ++k) { k_tr_spawn_round<<<nblk(plane), 256, 0, st>>>(a, k, score, d_mx, d_my, d_sstate, d_cnt + max_rounds); g_track_launches++; }
+      }
+      k_tr_emit<<<1, kTrEmitThreads, 0, st>>>(a, cont ? n_prev : 0, d_id[prev], d_cstate, d_cloc, spawn ? 1 : 0, d_sorted, d_sstate, next_id, d_id[nxt], d_loc[nxt], d_counts);
+      g_track_launches++;
+      e = cudaGetLastError();
+      if (e == cudaSuccess && f > 0) e = flush(f - 1, prev, n_prev);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(cnt_h.data(), d_cnt, (size_t)2 * max_rounds * 4, cudaMemcpyDeviceToHost, st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(counts_h, d_counts, 8, cudaMemcpyDeviceToHost, st);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+      if (e != cudaSuccess) { rc = set_err(RCVD_ERR_CUDA, "track computation failed: %s", cudaGetErrorString(e)); break; }
+      const bool p_done = !cont || cnt_h[rp - 1] == 0, s_done = !spawn || cnt_h[max_rounds + rs - 1] == 0;
+      if (p_done && s_done) {
+        // next frame: a few rounds more than this one needed
+        if (cont) { int used = 1; while (used < rp && cnt_h[used - 1] != 0) ++used; rp = std::max(2, used + 1); }
+        if (spawn) { int used = 1; while (used < rs && cnt_h[max_rounds + used - 1] != 0) ++used; rs = std::max(2, used + 2); }
+        break;
+      }
+      if ((!p_done && rp >= max_rounds) || (!s_done && rs >= max_rounds)) { rc = set_err(RCVD_ERR_CUDA, "track selection did not converge"); break; }
+      if (!p_done) rp = std::min(max_rounds, 2 * rp);
+      if (!s_done) rs = std::min(max_rounds, 2 * rs);
+      if (f > 0) frame_offsets[f] = frame_offsets[f - 1];   // the previous list is copied again
+    }
+    if (rc != RCVD_OK) break;
+    n_prev = counts_h[0] + counts_h[1];
+    next_id += counts_h[1];
+    cur = nxt;
+  }
+  if (rc == RCVD_OK) {
+    e = flush(F - 1, cur, n_prev);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) rc = set_err(RCVD_ERR_CUDA, "track read-back failed: %s", cudaGetErrorString(e));
+  }
+  cleanup();
+  if (rc != RCVD_OK) return rc;
+  *num_tracks = next_id;
+  const int64_t total = frame_offsets[F];
+  if (total > capacity || (total > 0 && (!obs_track || !obs_loc))) return set_err(RCVD_ERR_INVALID, "output capacity too small: %lld observations", (long long)total);
+  if (total > 0) { std::memcpy(obs_track, ids.data(), (size_t)total * 4); std::memcpy(obs_loc, locs.data(), (size_t)total * 8); }
   return RCVD_OK;
 }

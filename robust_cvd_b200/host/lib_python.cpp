@@ -157,6 +157,20 @@ PYBIND11_MODULE(lib_python, m) {
         }
         return d; });
 
+  py::class_<DepthVideoTrackTable>(m, "DepthVideoTrackTable")
+      .def(py::init<>())
+      .def("save", &DepthVideoTrackTable::save).def("load", &DepthVideoTrackTable::load)
+      // test/debug accessor (not in the reference): per track id None (deleted) or (first frame, locations [n,2] float32)
+      .def("_tracks", [](const DepthVideoTrackTable& t) {
+        py::list l;
+        for (const auto& tr : t.tracks) {
+          if (!tr.valid) { l.append(py::none()); continue; }
+          py::array_t<float> a({(py::ssize_t)tr.obs.size(), (py::ssize_t)2});
+          if (!tr.obs.empty()) std::memcpy(a.mutable_data(), tr.obs.data(), tr.obs.size() * sizeof(tr.obs[0]));
+          l.append(py::make_tuple(tr.firstFrame, a));
+        }
+        return l; });
+
   struct DepthVideoImporter {};
   py::class_<DepthVideoImporter>(m, "DepthVideoImporter")
       .def_static("importVideo", [](DepthVideo& v, const std::string& path, bool discover) { importVideo(v, path, discover); })
@@ -229,7 +243,7 @@ PYBIND11_MODULE(lib_python, m) {
   dvp.def(py::init<DepthVideo*>(), py::keep_alive<1, 2>())
       .def("process", &DepthVideoProcessor::process).def("gridXformSplit", &DepthVideoProcessor::gridXformSplit)
       .def("reset", &DepthVideoProcessor::reset).def("copy", &DepthVideoProcessor::copy).def("bilateralFilter", &DepthVideoProcessor::bilateralFilter)
-      .def("flowGuidedFilter", &DepthVideoProcessor::flowGuidedFilter)
+      .def("flowGuidedFilter", &DepthVideoProcessor::flowGuidedFilter).def("computeTracks", &DepthVideoProcessor::computeTracks)
       .def("resetPoses", &DepthVideoProcessor::resetPoses).def("resetDepthXforms", &DepthVideoProcessor::resetDepthXforms)
       .def("resetSpatialXforms", &DepthVideoProcessor::resetSpatialXforms)
       .def("normalizeDepth", &DepthVideoProcessor::normalizeDepth).def("optimizePoses", &DepthVideoProcessor::optimizePoses);

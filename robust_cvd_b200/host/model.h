@@ -365,6 +365,20 @@ class DepthVideoPoseOptimizer {
   std::vector<std::array<double, 7>> poseParams_;
 };
 
+// --- DepthVideoTrackTable (lib/Processor.h:17-28, lib/core/TrackTable.h): tracks by id, a deleted id stays as an empty slot ---
+struct DepthVideoTrack {
+  bool valid = false;
+  int firstFrame = 0;
+  std::vector<std::array<float, 2>> obs;   // one normalised location per frame firstFrame, firstFrame + 1, ...
+};
+class DepthVideoTrackTable {
+ public:
+  void save(const std::string& fileName) const;   // TrackTable::save / load (lib/core/TrackTable-impl.h:565-636)
+  void load(const std::string& fileName);
+  std::vector<DepthVideoTrack> tracks;
+  std::vector<std::set<int>> frames;              // ids observed in each frame of the video
+};
+
 class DepthVideoProcessor {
  public:
   enum class Op { None, Reset, Copy, BilateralFilter, FlowGuidedFilter, ComputeConstraints, ResetConstraintStaticFlag,
@@ -384,6 +398,7 @@ class DepthVideoProcessor {
   void copy(const Params& params);                // :152-180
   void bilateralFilter(const Params& params);     // :183-313, on the GPU (rcvd_bilateral_filter)
   void flowGuidedFilter(const Params& params);    // :315-590, on the GPU (rcvd_flow_guided_filter)
+  std::unique_ptr<DepthVideoTrackTable> computeTracks(const Params& params);   // :646-886, on the GPU (rcvd_compute_tracks)
   void gridXformSplit(const Params& params);      // lib/Processor.cpp:888-985
   void resetPoses(const Params& params);          // :987-1003
   void resetDepthXforms(const Params& params);    // :1005-1008

@@ -5,6 +5,8 @@
 // write-back -- but "ceres::Solve" is the CUDA library behind include/rcvd.h.  No CPU solver here.
 #include "model.h"
 #include <dirent.h>
+#include <sys/stat.h>
+#include <fstream>
 #include <cstring>
 
 #include <algorithm>
@@ -400,6 +402,134 @@ void DepthVideoProcessor::bilateralFilter(const Params& params) {
     dstDs.frame(base + outFrames[i]).setDepth(img);
   }
 }
+// Long point tracks (:646-886).  The reference tracks frame by frame on the CPU; here the host gathers the colour frames, dynamic
+// masks and consecutive-frame flows of the range once and one call (rcvd_compute_tracks, csrc/rcvd_tracks.cuh) tracks every frame
+// on the device.  Missing or wrongly sized flows and masks count as absent, as in the reference; short tracks are deleted here.
+std::unique_ptr<DepthVideoTrackTable> DepthVideoProcessor::computeTracks(const Params& params) {
+  struct Trim { ~Trim() { rcvd_trim_device_memory(currentDevice()); } } trimAtExit;
+  logInfo("Computing tracks...");
+  if (params.trackSpawnDistance < 0 || params.trackPruneDistance < 0) throw std::runtime_error("Track spawn and prune distances must not be negative.");
+  params.frameRange.checkEmpty();
+  const int N = video_->numFrames();
+  const int first = params.frameRange.firstFrame(), last = params.frameRange.lastFrame();
+  if (first < 0 || last >= N) throw std::runtime_error("Frame range contains out-of-range frame indices.");
+  ColorStream& cs = video_->colorStream("down");
+  if (cs.type() != cvMakeType(CV_32F, 3)) throw std::runtime_error("Tracking needs the 'down' color stream as CV_32FC3.");
+  const int w = cs.width(), h = cs.height();
+  auto table = std::make_unique<DepthVideoTrackTable>();
+  table->frames.resize(N);
+  if (w <= 0 || h <= 0) return table;   // no colour frame at all: no frame gets tracks
+  const int F = last - first + 1;
+  const size_t plane = size_t(w) * h;
+  // dynamic masks of every frame of the range (checked before any device work)
+  const bool hasDyn = video_->hasColorStream("dynamic_mask");
+  int dw = 0, dh = 0;
+  std::vector<uint8_t> dyn;
+  if (hasDyn) {
+    ColorStream& ms = video_->colorStream("dynamic_mask");
+    for (int i = 0; i < F; ++i) {
+      if (!params.frameRange.inRange(first + i)) continue;
+      const Image* m = ms.frame(first + i).image();
+      if (!m) throw std::runtime_error("Dynamic mask stream is missing frame " + std::to_string(first + i) + ".");
+      if (m->type != cvMakeType(CV_8U, 1)) throw std::runtime_error("Dynamic masks must be single-channel 8-bit images.");
+      if (dyn.empty()) { dw = m->cols; dh = m->rows; dyn.assign(size_t(F) * dw * dh, 255); }
+      if (m->cols != dw || m->rows != dh) throw std::runtime_error("Dynamic masks have inconsistent dimensions.");
+      std::memcpy(dyn.data() + size_t(i) * dw * dh, m->data.data(), size_t(dw) * dh);
+    }
+  }
+  auto exists = [](const std::string& f) { struct stat st; return stat(f.c_str(), &st) == 0; };
+  auto pairFile = [&](const char* fmt, int a) { char buf[96]; snprintf(buf, sizeof(buf), fmt, a - 1, a); return video_->path() + buf; };
+  std::vector<float> color(size_t(F) * plane * 3), flow(size_t(F) * plane * 2);
+  std::vector<uint8_t> mask(size_t(F) * plane), flags(F, 0);
+  parallelFor(size_t(F), [&](size_t i) {
+    const int a = first + int(i);
+    uint8_t fl = 0;
+    if (params.frameRange.inRange(a)) fl |= RCVD_TRACK_IN_RANGE;
+    const Image* c = (fl & RCVD_TRACK_IN_RANGE) ? cs.frame(a).image() : nullptr;
+    if (c && c->cols == w && c->rows == h) { fl |= RCVD_TRACK_HAS_COLOR; std::memcpy(color.data() + i * plane * 3, c->ptr<float>(), plane * 3 * sizeof(float)); }
+    else if (c) throw std::runtime_error("Color frame " + std::to_string(a) + " of stream 'down' has the wrong size.");
+    if (a > first) {   // only a continuation reads the flow
+      const std::string ff = pairFile("/flow/flow_%06d_%06d.raw", a);
+      if (exists(ff)) {
+        Image fimg; freadim(ff, fimg);
+        if (fimg.cols == w && fimg.rows == h && fimg.type == cvMakeType(CV_32F, 2)) { fl |= RCVD_TRACK_FLOW; std::memcpy(flow.data() + i * plane * 2, fimg.ptr<float>(), plane * 2 * sizeof(float)); }
+      }
+    }
+    if (a > 0) {       // frame 0 would read mask_-00001_000000.png, which never exists
+      const std::string mf = pairFile("/flow_mask/mask_%06d_%06d.png", a);
+      if (exists(mf)) {
+        Image m = imreadPng(mf, true);
+        if (m.cols == w && m.rows == h) { fl |= RCVD_TRACK_MASK; std::memcpy(mask.data() + i * plane, m.ptr<uint8_t>(), plane); }
+      }
+    }
+    flags[i] = fl;
+  });
+  rcvd_track_params prm{};
+  prm.num_frames = F; prm.width = w; prm.height = h; prm.dyn_width = dw; prm.dyn_height = dh;
+  prm.spawn_distance = params.trackSpawnDistance; prm.prune_distance = params.trackPruneDistance;
+  prm.min_dynamic_distance = float(params.minDynamicDistance); prm.inv_aspect = video_->invAspect();
+  std::vector<int64_t> offsets(F + 1, 0);
+  std::vector<int32_t> ids; std::vector<float> locs;
+  int64_t numTracks = 0, cap = int64_t(2 * plane);
+  for (int attempt = 0; attempt < 2; ++attempt) {
+    ids.resize(size_t(cap)); locs.resize(size_t(cap) * 2);
+    const int rc = rcvd_compute_tracks(&prm, currentDevice(), color.data(), hasDyn ? dyn.data() : nullptr, flow.data(), mask.data(), flags.data(),
+                                       offsets.data(), ids.data(), locs.data(), cap, &numTracks);
+    if (rc == RCVD_OK) break;
+    if (attempt == 0 && rc == RCVD_ERR_INVALID && offsets[F] > cap) { cap = offsets[F]; continue; }   // the size is known now
+    throw std::runtime_error(std::string("track computation failed: ") + rcvd_last_error());
+  }
+  // the table: observations arrive frame by frame, each track's in consecutive frames
+  table->tracks.resize(size_t(numTracks));
+  for (int i = 0; i < F; ++i)
+    for (int64_t k = offsets[i]; k < offsets[i + 1]; ++k) {
+      DepthVideoTrack& t = table->tracks[size_t(ids[k])];
+      if (!t.valid) { t.valid = true; t.firstFrame = first + i; }
+      t.obs.push_back({locs[2 * k], locs[2 * k + 1]});
+    }
+  for (size_t id = 0; id < table->tracks.size(); ++id) {   // prune short tracks (:874-883)
+    DepthVideoTrack& t = table->tracks[id];
+    if (int(t.obs.size()) < params.minTrackLength) { t = DepthVideoTrack(); continue; }
+    for (size_t k = 0; k < t.obs.size(); ++k) table->frames[size_t(t.firstFrame) + k].insert(int(id));
+  }
+  return table;
+}
+
+template <class T> static void putLE(std::ofstream& os, T v) { os.write(reinterpret_cast<const char*>(&v), sizeof(T)); }
+template <class T> static T getLE(std::ifstream& is) { T v{}; if (!is.read(reinterpret_cast<char*>(&v), sizeof(T))) throw std::runtime_error("Track file is truncated."); return v; }
+void DepthVideoTrackTable::save(const std::string& fileName) const {
+  std::ofstream os(fileName, std::ios::binary);
+  putLE<uint64_t>(os, tracks.size());
+  for (const DepthVideoTrack& t : tracks) {
+    putLE<uint8_t>(os, t.valid ? 1 : 0);
+    if (!t.valid) continue;
+    putLE<uint64_t>(os, uint64_t(t.firstFrame)); putLE<uint64_t>(os, t.obs.size());
+    os.write(reinterpret_cast<const char*>(t.obs.data()), std::streamsize(t.obs.size() * sizeof(t.obs[0])));
+  }
+  putLE<uint64_t>(os, 0); putLE<uint64_t>(os, frames.size());
+}
+void DepthVideoTrackTable::load(const std::string& fileName) {
+  std::ifstream is(fileName, std::ios::binary);
+  if (!is) throw std::runtime_error("Could not open file.");
+  std::vector<DepthVideoTrack> tr(getLE<uint64_t>(is));
+  for (DepthVideoTrack& t : tr) {
+    t.valid = getLE<uint8_t>(is) != 0;
+    if (!t.valid) continue;
+    t.firstFrame = int(getLE<uint64_t>(is));
+    t.obs.resize(getLE<uint64_t>(is));
+    if (!is.read(reinterpret_cast<char*>(t.obs.data()), std::streamsize(t.obs.size() * sizeof(t.obs[0])))) throw std::runtime_error("Track file is truncated.");
+  }
+  const uint64_t offset = getLE<uint64_t>(is), count = getLE<uint64_t>(is);
+  std::vector<std::set<int>> fr(count);
+  for (size_t id = 0; id < tr.size(); ++id)
+    for (size_t k = 0; k < tr[id].obs.size(); ++k) {
+      const uint64_t f = uint64_t(tr[id].firstFrame) + k - offset;
+      if (f >= count) throw std::runtime_error("Track file has an observation outside its frames.");
+      fr[f].insert(int(id));
+    }
+  tracks = std::move(tr); frames = std::move(fr);
+}
+
 // Flow-guided temporal filter (:315-590).  The reference walks frame by frame and pixel by pixel on the CPU; here the host
 // gathers the depth images, cameras and consecutive-frame flows of the whole range once and one kernel launch
 // (rcvd_flow_guided_filter, csrc/rcvd_filter.cuh) filters every frame.

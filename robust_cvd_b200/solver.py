@@ -360,6 +360,38 @@ def build_constraints(color_bgr, pair_frames,pair_flow, pair_mask, match_separat
     return poff, pout[:poff[P]], toff, tout[:toff[T]]
 
 
+def compute_tracks(color_bgr, frame_flags, flow=None, flow_mask=None, dyn_masks=None, spawn_distance=20, prune_distance=5, min_dynamic_distance=3.0,
+                   inv_aspect=1.0, device=0):
+    """rcvd_compute_tracks (DepthVideoProcessor::computeTracks, reference lib/Processor.cpp:646-886) on the GPU, before the deletion of short
+    tracks.  Local stacks over the frame range: color_bgr [F,h,w,3] f32, frame_flags [F] u8 (abi.TRACK_*), flow [F,h,w,2] f32 and
+    flow_mask [F,h,w] u8 (slot f: pair f-1 -> f), dyn_masks [F,dh,dw] u8 or None.
+    Returns (frame_offsets [F+1] i64, track ids [n] i32, locations [n,2] f32, number of ids created)."""
+    color = np.ascontiguousarray(color_bgr, np.float32)
+    F, h, w = color.shape[:3]
+    fl = np.ascontiguousarray(frame_flags, np.uint8).reshape(-1)
+    if fl.size != F:
+        raise ValueError(f"{fl.size} frame flags for {F} frames")
+    fw = None if flow is None else np.ascontiguousarray(flow, np.float32)
+    fm = None if flow_mask is None else np.ascontiguousarray(flow_mask, np.uint8)
+    dm = None if dyn_masks is None else np.ascontiguousarray(dyn_masks, np.uint8)
+    prm = abi.TrackParams(num_frames=F, width=w, height=h, dyn_width=0 if dm is None else dm.shape[2], dyn_height=0 if dm is None else dm.shape[1],
+                          spawn_distance=spawn_distance, prune_distance=prune_distance, min_dynamic_distance=min_dynamic_distance, inv_aspect=inv_aspect)
+    off = np.zeros(F + 1, np.int64)
+    n = C.c_int64(0)
+    cap = F * h * w // 128 + 1024     # ample at the default spawn distance; a larger result is reported and the call repeated
+    for attempt in range(2):
+        ids = np.zeros(max(cap, 1), np.int32); locs = np.zeros((max(cap, 1), 2), np.float32)
+        rc = lib().rcvd_compute_tracks(C.byref(prm), C.c_int32(device), _p(color, C.c_float), _p(dm, C.c_uint8), _p(fw, C.c_float), _p(fm, C.c_uint8),
+                                       _p(fl, C.c_uint8), _p(off, C.c_int64), _p(ids, C.c_int32), _p(locs, C.c_float), C.c_int64(cap), C.byref(n))
+        if rc == 0:
+            break
+        if attempt == 0 and off[F] > cap:
+            cap = int(off[F])      # the first call reports the size
+            continue
+        _check(rc)
+    return off, ids[:off[F]], locs[:off[F]], int(n.value)
+
+
 def static_flags(masks, distance, pair_frames=None, pair_offsets=None, pair_locs=None, trip_frames=None, trip_offsets=None, trip_locs=None, want_distance=False, device=0):
     """rcvd_static_flags (FlowConstraintsCollection::setStaticFlagFromDynamicMask + dynamicDistance, reference lib/FlowConstraints.cpp:573-660,
     :257-286) on the GPU.  masks [F,h,w] u8.  Returns (pair_static u8[n], trip_static u8[m], distance images [F,h,w] f32 or None)."""
