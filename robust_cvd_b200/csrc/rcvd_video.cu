@@ -1,0 +1,580 @@
+// rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
+// and bilateral depth filters, the flow-constraint builder, static flags and long point tracks.  Like the solver (rcvd_api.cu) they
+// have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+#include <optional>
+#include <vector>
+
+#include <cub/device/device_radix_sort.cuh>
+#include "rcvd_host.h"
+#include "rcvd_dense.cuh"
+#include "rcvd_filter.cuh"
+#include "rcvd_bilateral.cuh"
+#include "rcvd_builder.cuh"
+#include "rcvd_tracks.cuh"
+
+using namespace rcvd;
+
+// The device side of one video entry point: the device made current, a stream of its own and every buffer allocated on it.
+// The destructor frees the buffers, waits for the stream and destroys it, and only then makes the caller's device current again.
+struct VideoCall {
+  std::optional<DevGuard> guard;
+  cudaStream_t st = nullptr;
+  std::vector<void*> bufs;
+  bool ok = true;
+  VideoCall() = default;
+  VideoCall(const VideoCall&) = delete;
+  VideoCall& operator=(const VideoCall&) = delete;
+  int open(int device) {
+    if (int rc = check_device(device)) return rc;
+    guard.emplace(device);
+    if (guard->err != cudaSuccess) return set_err(RCVD_ERR_CUDA, "cudaSetDevice(%d) failed: %s", device, cudaGetErrorString(guard->err));
+    cudaStream_t s;
+    CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    st = s;
+    return RCVD_OK;
+  }
+  // at least 16 bytes; a failure is remembered for allocated() and cleared from the runtime's last error
+  void* alloc(size_t bytes) {
+    void* ptr = nullptr;
+    if (cudaMallocAsync(&ptr, std::max<size_t>(bytes, 16), st) != cudaSuccess) { ok = false; cudaGetLastError(); return nullptr; }
+    bufs.push_back(ptr);
+    return ptr;
+  }
+  void* upload(const void* src, size_t bytes) {
+    void* d = alloc(bytes);
+    if (d && src && bytes) cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, st);
+    return d;
+  }
+  // checked before the first launch: a kernel on a null buffer faults with an illegal address, a sticky error of the whole
+  // context, and PyTorch shares this context
+  bool allocated() const { return ok; }
+  // launch errors, then the stream's; both always run, so no copy into host memory is pending when this returns
+  int sync(const char* what) {
+    const cudaError_t launch = cudaGetLastError();
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (launch != cudaSuccess || e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(launch != cudaSuccess ? launch : e));
+    return RCVD_OK;
+  }
+  ~VideoCall() {
+    if (!st) return;
+    for (void* b : bufs) cudaFreeAsync(b, st);
+    cudaStreamSynchronize(st); cudaStreamDestroy(st);
+  }
+};
+
+// ---- dense transform application (next-row kernels) ----
+template <int MODE>
+static int dense_run(const rcvd_config* cfg, int device, const double* params_in, int nparams, int param_off, const float* src, void* out, size_t out_bytes, int h, int w) {
+  Layout L;
+  if (!cfg || !make_layout(*cfg, L)) return set_err(RCVD_ERR_INVALID, "unsupported transform configuration");
+  if (int rc = check_device(device)) return rc;
+  SET_DEVICE(device);
+  std::vector<double> pv(L.nf, 0.0);
+  for (int i = 0; i < nparams; ++i) pv[param_off + i] = params_in[i];
+  double* d_p = nullptr; float* d_src = nullptr; void* d_out = nullptr;
+  const size_t n = (size_t)w * h;
+  // per-frame calls (DepthFrame::depth(), paramMap, warp for every frame of a video): stream-ordered pool allocations and one
+  // synchronisation instead of three cudaMalloc/cudaFree pairs per call
+  static thread_local cudaStream_t st = nullptr; static thread_local int st_dev = -1;
+  if (!st || st_dev != device) {
+    if (st) cudaStreamDestroy(st);
+    CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); st_dev = device;
+    cudaMemPool_t pool; unsigned long long keep = ~0ull;
+    if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+  }
+  CK(cudaMallocAsync((void**)&d_p, pv.size() * 8, st)); CK(cudaMallocAsync(&d_out, out_bytes, st));
+  CK(cudaMemcpyAsync(d_p, pv.data(), pv.size() * 8, cudaMemcpyHostToDevice, st));
+  if (src) { CK(cudaMallocAsync((void**)&d_src, n * 4, st)); CK(cudaMemcpyAsync(d_src, src, n * 4, cudaMemcpyHostToDevice, st)); }
+  k_dense<MODE><<<nblk(n), 256, 0, st>>>(*cfg, L, d_p, d_src, d_out, h, w);
+  cudaError_t e = cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st);
+  cudaFreeAsync(d_p, st); cudaFreeAsync(d_out, st); if (d_src) cudaFreeAsync(d_src, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "dense kernel failed: %s", cudaGetErrorString(e));
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_depth_apply(const rcvd_config* cfg, int32_t device, const double* dp, const float* src, float* dst, int32_t h, int32_t w) {
+  Layout L; if (!cfg || !make_layout(*cfg, L)) return set_err(RCVD_ERR_INVALID, "unsupported transform configuration");
+  return dense_run<0>(cfg, device, dp, L.nd, L.offD, src, dst, (size_t)w * h * 4, h, w);
+}
+RCVD_API int32_t rcvd_depth_param_map(const rcvd_config* cfg, int32_t device, const double* dp, double* out, int32_t h, int32_t w) {
+  Layout L; if (!cfg || !make_layout(*cfg, L)) return set_err(RCVD_ERR_INVALID, "unsupported transform configuration");
+  if (cfg->depth_type != RCVD_DEPTH_GRID) return set_err(RCVD_ERR_INVALID, "Parameter map not implemented for this transform type.");
+  return dense_run<1>(cfg, device, dp, L.nd, L.offD, nullptr, out, (size_t)w * h * L.k * 8, h, w);
+}
+RCVD_API int32_t rcvd_spatial_warp(const rcvd_config* cfg, int32_t device, const double* sp, float* out, int32_t h, int32_t w) {
+  Layout L; if (!cfg || !make_layout(*cfg, L)) return set_err(RCVD_ERR_INVALID, "unsupported transform configuration");
+  return dense_run<2>(cfg, device, sp, L.ns, L.offS, nullptr, out, (size_t)w * h * 8, h, w);
+}
+
+RCVD_API int32_t rcvd_trim_device_memory(int32_t device) {
+  if (int rc = check_device(device)) return rc;
+  SET_DEVICE(device);
+  CK(cudaDeviceSynchronize());
+  cudaMemPool_t pool;
+  CK(cudaDeviceGetDefaultMemPool(&pool, device));
+  CK(cudaMemPoolTrimTo(pool, 0));
+  unsigned long long none = 0;                       // rcvd_problem_create raises the threshold again for the next solve
+  cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &none);
+  return RCVD_OK;
+}
+// The device the host layer should work on: RCVD_DEVICE if set, else the caller's current CUDA device (so that a process launched
+// per GPU -- torchrun LOCAL_RANK + torch.cuda.set_device -- lands on its own GPU); -1 without a usable device.
+RCVD_API int32_t rcvd_current_device(void) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { cudaGetLastError(); return -1; }
+  if (const char* e = getenv("RCVD_DEVICE")) { const int d = atoi(e); return (d >= 0 && d < ndev) ? d : -1; }
+  int d = 0;
+  if (cudaGetDevice(&d) != cudaSuccess) { cudaGetLastError(); return -1; }
+  return d;
+}
+
+// ---------------------------------------------------------------------------
+// Flow-guided temporal depth filter (rcvd_filter.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_filter_launches = 0;
+RCVD_API int32_t rcvd_flow_guided_filter(const rcvd_filter_params* prm, int32_t device, const float* depth, const float* cams,
+                                         const float* fwd_flow, const uint8_t* fwd_mask, const float* bwd_flow, const uint8_t* bwd_mask,
+                                         const int32_t* far_pairs, const float* far_flow, const uint8_t* far_mask, float* out) {
+  if (!prm || !depth || !cams || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_filter_params& q = *prm;
+  if (q.num_frames <= 0 || q.num_out <= 0 || q.first_out < 0 || q.first_out + q.num_out > q.num_frames || q.width <= 0 || q.height <= 0 ||
+      q.depth_width <= 0 || q.depth_height <= 0 || q.frame_radius < 0 || q.spatial_radius < 0 || q.num_far < 0 || !(q.inv_aspect > 0.f))
+    return set_err(RCVD_ERR_INVALID, "bad filter parameters");
+  if (q.frame_radius > 0 && q.num_frames > 1 && (!fwd_flow || !fwd_mask || !bwd_flow || !bwd_mask)) return set_err(RCVD_ERR_INVALID, "flow stacks missing");
+  if (q.num_far > 0 && (!far_pairs || !far_flow || !far_mask)) return set_err(RCVD_ERR_INVALID, "far-connection arrays missing");
+  VideoCall call;
+  if (int rc = call.open(device)) return rc;
+  const int F = q.num_frames; const size_t plane = (size_t)q.width * q.height, dplane = (size_t)q.depth_width * q.depth_height;
+  // cameras: tan(fov / 2) in float on the host, like DepthVideo::project (lib/DepthVideo.cpp:640-641)
+  std::vector<float> hc((size_t)F * 12, 0.f);
+  for (int f = 0; f < F; ++f) {
+    for (int i = 0; i < 7; ++i) hc[(size_t)f * 12 + i] = cams[(size_t)f * 9 + i];
+    hc[(size_t)f * 12 + 7] = std::tan(cams[(size_t)f * 9 + 7] / 2.f);
+    hc[(size_t)f * 12 + 8] = std::tan(cams[(size_t)f * 9 + 8] / 2.f);
+  }
+  // far connections grouped by source frame (stable: the caller's order within a frame is kept)
+  std::vector<int> far_begin(F + 1, 0), order(q.num_far), pairs_sorted((size_t)2 * q.num_far);
+  int maxfar = 0;
+  for (int k = 0; k < q.num_far; ++k) {
+    const int s = far_pairs[2 * k], d = far_pairs[2 * k + 1];
+    if (s < 0 || s >= F || d < 0 || d >= F) return set_err(RCVD_ERR_INVALID, "far connection %d out of range", k);
+    far_begin[s + 1]++;
+  }
+  for (int f = 0; f < F; ++f) { maxfar = std::max(maxfar, far_begin[f + 1]); far_begin[f + 1] += far_begin[f]; }
+  { std::vector<int> cur(far_begin.begin(), far_begin.end() - 1); for (int k = 0; k < q.num_far; ++k) order[cur[far_pairs[2 * k]]++] = k; }
+  FilterArgs a{};
+  a.depth = (const float*)call.upload(depth, (size_t)F * dplane * 4);
+  a.cams = (const float*)call.upload(hc.data(), hc.size() * 4);
+  const bool chains = q.frame_radius > 0 && F > 1;
+  a.fwd_flow = (const float*)call.upload(chains ? fwd_flow : nullptr, chains ? (size_t)F * plane * 8 : 0); a.fwd_mask = (const uint8_t*)call.upload(chains ? fwd_mask : nullptr, chains ? (size_t)F * plane : 0);
+  a.bwd_flow = (const float*)call.upload(chains ? bwd_flow : nullptr, chains ? (size_t)F * plane * 8 : 0); a.bwd_mask = (const uint8_t*)call.upload(chains ? bwd_mask : nullptr, chains ? (size_t)F * plane : 0);
+  if (q.num_far > 0) {
+    float* ff = (float*)call.alloc((size_t)q.num_far * plane * 8); uint8_t* fm = (uint8_t*)call.alloc((size_t)q.num_far * plane);
+    if (ff && fm)
+      for (int k = 0; k < q.num_far; ++k) {   // sorted order on the device
+        cudaMemcpyAsync(ff + (size_t)k * plane * 2, far_flow + (size_t)order[k] * plane * 2, plane * 8, cudaMemcpyHostToDevice, call.st);
+        cudaMemcpyAsync(fm + (size_t)k * plane, far_mask + (size_t)order[k] * plane, plane, cudaMemcpyHostToDevice, call.st);
+        pairs_sorted[2 * k] = far_pairs[2 * order[k]]; pairs_sorted[2 * k + 1] = far_pairs[2 * order[k] + 1];
+      }
+    a.far_flow = ff; a.far_mask = fm;
+    a.far_pairs = (const int*)call.upload(pairs_sorted.data(), pairs_sorted.size() * 4);
+    a.far_begin = (const int*)call.upload(far_begin.data(), far_begin.size() * 4);
+  }
+  float* const out_dev = (float*)call.alloc((size_t)q.num_out * plane * 4);
+  const int win = 2 * q.spatial_radius + 1;
+  a.max_samples = win * win * (1 + 2 * q.frame_radius + maxfar);
+  // the weighted median sorts a per-pixel sample row: the scratch is bounded to ~1 GiB by filtering the range in frame chunks
+  const size_t per_frame_scratch = plane * (size_t)a.max_samples * sizeof(float2);
+  const int chunk = q.median ? (int)std::max<size_t>(1, std::min<size_t>((size_t)q.num_out, ((size_t)1 << 30) / std::max<size_t>(per_frame_scratch, 1))) : q.num_out;
+  if (q.median) a.scratch = (float2*)call.alloc((size_t)chunk * per_frame_scratch);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_flow_guided_filter");
+  cudaMemsetAsync(out_dev, 0, (size_t)q.num_out * plane * 4, call.st);
+  a.F = F; a.last_frame = q.first_out + q.num_out - 1;
+  a.w = q.width; a.h = q.height; a.wd = q.depth_width; a.hd = q.depth_height;
+  a.frame_radius = q.frame_radius; a.spatial_radius = q.spatial_radius; a.median = q.median; a.inv_aspect = q.inv_aspect;
+  for (int c0 = 0; c0 < q.num_out; c0 += chunk) {
+    a.first_out = q.first_out + c0; a.num_out = std::min(chunk, q.num_out - c0); a.out = out_dev + (size_t)c0 * plane;
+    const dim3 grid((q.width + 31) / 32, (q.height + 3) / 4, a.num_out);
+    if (q.median) k_flow_guided_filter<true><<<grid, 128, 0, call.st>>>(a); else k_flow_guided_filter<false><<<grid, 128, 0, call.st>>>(a);
+    g_filter_launches++;
+  }
+  cudaMemcpyAsync(out, out_dev, (size_t)q.num_out * plane * 4, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("flow-guided filter");
+}
+RCVD_API int64_t rcvd_filter_launch_count() { return g_filter_launches; }
+
+// ---------------------------------------------------------------------------
+// Joint depth / colour bilateral filter (rcvd_bilateral.cuh)
+// ---------------------------------------------------------------------------
+RCVD_API int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t device, const float* depth, const float* color_bgr,
+                                       const int32_t* out_frames, const rcvd_config* xform_cfg, const double* xform_params, float* out) {
+  if (!prm || !depth || !out_frames || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_bilateral_params& q = *prm;
+  const int F = q.num_frames;
+  if (F <= 0 || q.width <= 0 || q.height <= 0 || q.num_out <= 0 || q.frame_radius < 0 || q.spatial_radius < 0 || (q.median != 0 && q.median != 1))
+    return set_err(RCVD_ERR_INVALID, "bad bilateral filter parameters");
+  for (int i = 0; i < q.num_out; ++i)
+    if (out_frames[i] < 0 || out_frames[i] >= F || (i > 0 && out_frames[i] <= out_frames[i - 1]))
+      return set_err(RCVD_ERR_INVALID, "output frames must be ascending local indices in [0, num_frames)");
+  const bool color = q.color_sigma > 0.f;
+  if (color && !color_bgr) return set_err(RCVD_ERR_INVALID, "color_sigma > 0 needs the colour stack");
+  // in place, a later output frame reads xform(filtered) of the frames before it (the reference writes into the stream it reads)
+  const bool recur = q.in_place != 0 && q.frame_radius > 0;
+  Layout L{};
+  if (recur) {
+    if (!xform_cfg || !make_layout(*xform_cfg, L)) return set_err(RCVD_ERR_INVALID, "in-place filtering needs a supported depth-transform configuration");
+    if (L.nd > 0 && !xform_params) return set_err(RCVD_ERR_INVALID, "in-place filtering needs the per-frame depth-transform parameters");
+  }
+  const long long r = q.spatial_radius, fr = q.frame_radius;
+  const long long max_samples = std::min<long long>(2 * r + 1, q.width) * std::min<long long>(2 * r + 1, q.height) * std::min<long long>(2 * fr + 1, F);
+  if (q.median && max_samples > kBilateralMaxSamples)
+    return set_err(RCVD_ERR_INVALID, "the weighted median supports at most %d samples per pixel; this window has %lld", kBilateralMaxSamples, max_samples);
+  VideoCall call;
+  if (int rc = call.open(device)) return rc;
+  const size_t plane = (size_t)q.width * q.height;
+  // launch geometry and shared memory
+  BilateralArgs a{};
+  a.F = F; a.w = q.width; a.h = q.height; a.frame_radius = q.frame_radius; a.radius = q.spatial_radius;
+  a.use_depth = q.depth_sigma > 0.f; a.depth_sigma = q.depth_sigma; a.color_sigma = q.color_sigma;
+  size_t smem = 0; bool staged = false;
+  if (q.median) {
+    a.P = 32; while (a.P < max_samples) a.P <<= 1;
+    smem = (size_t)kBfMedianWarps * a.P * sizeof(unsigned long long);
+  } else {
+    a.sw = kBfTx + 2 * q.spatial_radius; a.sh = kBfTy + 2 * q.spatial_radius;
+    const size_t bytes = 2 * (size_t)a.sw * a.sh * (color ? 4 : 1) * sizeof(float);   // two frame buffers
+    staged = bytes <= 200 * 1024;
+    smem = staged ? bytes : 0;
+  }
+  auto launch_filter = [&](cudaStream_t s, int base, int n) {
+    a.out_base = base;
+    if (q.median) {
+      const dim3 grid((unsigned)((plane + kBfMedianWarps - 1) / kBfMedianWarps), 1, n);
+      if (color) k_bilateral_median<true><<<grid, 32 * kBfMedianWarps, smem, s>>>(a); else k_bilateral_median<false><<<grid, 32 * kBfMedianWarps, smem, s>>>(a);
+    } else {
+      const dim3 grid((q.width + kBfTx - 1) / kBfTx, (q.height + kBfTy - 1) / kBfTy, n);
+      if (color) { if (staged) k_bilateral_mean<true, true><<<grid, kBfTx * kBfTy, smem, s>>>(a); else k_bilateral_mean<true, false><<<grid, kBfTx * kBfTy, 0, s>>>(a); }
+      else { if (staged) k_bilateral_mean<false, true><<<grid, kBfTx * kBfTy, smem, s>>>(a); else k_bilateral_mean<false, false><<<grid, kBfTx * kBfTy, 0, s>>>(a); }
+    }
+    g_filter_launches++;
+  };
+  if (smem > 48 * 1024) {
+    const void* fn = q.median ? (color ? (const void*)k_bilateral_median<true> : (const void*)k_bilateral_median<false>)
+                              : (color ? (const void*)k_bilateral_mean<true, true> : (const void*)k_bilateral_mean<false, true>);
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  // per-frame transform vectors in the dense kernel's frame layout (depth parameters at offD)
+  std::vector<double> pv;
+  if (recur) {
+    pv.assign((size_t)F * L.nf, 0.0);
+    for (int f = 0; f < F; ++f) for (int i = 0; i < L.nd; ++i) pv[(size_t)f * L.nf + L.offD + i] = xform_params[(size_t)f * L.nd + i];
+  }
+  float* d_depth = (float*)call.upload(depth, (size_t)F * plane * 4);
+  a.depth = d_depth;
+  a.color = color ? (const float*)call.upload(color_bgr, (size_t)F * plane * 12) : nullptr;
+  a.out_frames = (const int*)call.upload(out_frames, (size_t)q.num_out * 4);
+  float* const out_dev = (float*)call.alloc((size_t)q.num_out * plane * 4);
+  const double* d_pv = recur ? (const double*)call.upload(pv.data(), pv.size() * 8) : nullptr;
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_bilateral_filter");
+  if (recur) {
+    // frame-sequential: filter output o, then rewrite its slot of the depth stack with xform_o(filtered) for the frames after it
+    for (int o = 0; o < q.num_out; ++o) {
+      a.out = out_dev + (size_t)o * plane;
+      launch_filter(call.st, o, 1);
+      const int f = out_frames[o];
+      k_dense<0><<<nblk(plane), 256, 0, call.st>>>(*xform_cfg, L, d_pv + (size_t)f * L.nf, a.out, d_depth + (size_t)f * plane, q.height, q.width);
+    }
+  } else {
+    for (int o = 0; o < q.num_out; o += 65535) {   // grid.z limit
+      a.out = out_dev + (size_t)o * plane;
+      launch_filter(call.st, o, std::min(65535, q.num_out - o));
+    }
+  }
+  cudaMemcpyAsync(out, out_dev, (size_t)q.num_out * plane * 4, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("bilateral filter");
+}
+
+// ---------------------------------------------------------------------------
+// Corner scores, shared by the constraint builder and the tracks (rcvd_builder.cuh)
+// ---------------------------------------------------------------------------
+// cv::cornerMinEigenVal(cv::cvtColor(BGR2GRAY), 3) of F colour frames [F][H][W][3] f32 in one batched pass; returns the [F][H][W]
+// scores, or nullptr without launching anything once an allocation of the call has failed.
+static float* enqueue_corner_scores(VideoCall& call, const float* color_bgr, int F, int H, int W, int64_t& launches) {
+  const size_t FP = (size_t)F * H * W;
+  float* d_bgr = (float*)call.upload(color_bgr, FP * 12);
+  float* d_gray = (float*)call.alloc(FP * 4), *d_pl = (float*)call.alloc(FP * 12), *d_corner = (float*)call.alloc(FP * 4); double* d_tmp = (double*)call.alloc(FP * 24);
+  if (!call.allocated()) return nullptr;
+  k_gray<<<(unsigned)((FP + 255) / 256), 256, 0, call.st>>>(d_bgr, d_gray, FP);
+  k_sobel_products<<<(unsigned)((FP + 255) / 256), 256, 0, call.st>>>(d_gray, d_pl, F, H, W);
+  k_box_h<<<(unsigned)((FP * 3 + 255) / 256), 256, 0, call.st>>>(d_pl, d_tmp, (size_t)3 * F * H, W);
+  k_box_v_eig<<<(unsigned)(((size_t)F * W + 127) / 128), 128, 0, call.st>>>(d_tmp, d_corner, F, H, W);
+  launches += 4;
+  return d_corner;
+}
+
+// ---------------------------------------------------------------------------
+// GPU flow-constraint builder (rcvd_builder.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_builder_launches = 0, g_builder_rounds = 0;
+RCVD_API int64_t rcvd_builder_launch_count() { return g_builder_launches; }
+RCVD_API int64_t rcvd_builder_last_rounds() { return g_builder_rounds; }
+RCVD_API int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t device, const float* color_bgr, const float* dyn_dist,
+                                        const int32_t* pair_frames, const float* pair_flow, const uint8_t* pair_mask,
+                                        const int32_t* trip_frames, const float* trip_flow, const uint8_t* trip_mask,
+                                        int64_t* pair_offsets, float* pair_out, int64_t pair_capacity,
+                                        int64_t* trip_offsets, float* trip_out, int64_t trip_capacity) {
+  if (!prm || !color_bgr) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_builder_params& q = *prm;
+  const int P = q.num_pairs, T = q.num_triplets, F = q.num_frames, I = P + T;
+  if (F <= 0 || q.width <= 0 || q.height <= 0 || P < 0 || T < 0 || q.match_separation < 0 || !(q.inv_aspect > 0.f)) return set_err(RCVD_ERR_INVALID, "bad builder parameters");
+  if ((P > 0 && (!pair_frames || !pair_flow || !pair_mask || !pair_offsets)) || (T > 0 && (!trip_frames || !trip_flow || !trip_mask || !trip_offsets)))
+    return set_err(RCVD_ERR_INVALID, "null argument");
+  if (dyn_dist && (q.dyn_width <= 0 || q.dyn_height <= 0)) return set_err(RCVD_ERR_INVALID, "bad dynamic-distance size");
+  for (int i = 0; i < P; ++i) if (pair_frames[2 * i] < 0 || pair_frames[2 * i] >= F || pair_frames[2 * i + 1] < 0 || pair_frames[2 * i + 1] >= F) return set_err(RCVD_ERR_INVALID, "pair %d out of range", i);
+  for (int i = 0; i < T; ++i) if (trip_frames[i] < 1 || trip_frames[i] >= F) return set_err(RCVD_ERR_INVALID, "triplet %d out of range", i);
+  if (pair_offsets) pair_offsets[0] = 0;
+  if (trip_offsets) trip_offsets[0] = 0;
+  if (I == 0) return RCVD_OK;
+  VideoCall call;
+  if (int rc = call.open(device)) return rc;
+  const int W = q.width, H = q.height;
+  const size_t plane = (size_t)W * H;
+  BuilderArgs a{};
+  a.corner = enqueue_corner_scores(call, color_bgr, F, H, W, g_builder_launches);
+  a.dyn = dyn_dist ? (const float*)call.upload(dyn_dist, (size_t)F * q.dyn_width * q.dyn_height * 4) : nullptr;
+  a.pair_frames = (const int*)call.upload(pair_frames, (size_t)P * 8); a.pair_flow = (const float*)call.upload(pair_flow, (size_t)P * plane * 8); a.pair_mask = (const uint8_t*)call.upload(pair_mask, (size_t)P * plane);
+  a.trip_frames = (const int*)call.upload(trip_frames, (size_t)T * 4); a.trip_flow = (const float*)call.upload(trip_flow, (size_t)T * 2 * plane * 8); a.trip_mask = (const uint8_t*)call.upload(trip_mask, (size_t)T * 2 * plane);
+  a.prio = (float*)call.alloc((size_t)I * plane * 4); a.state = (uint8_t*)call.alloc((size_t)I * plane);
+  unsigned long long* d_cnt = (unsigned long long*)call.alloc((size_t)(2 * I + 2) * 8);   // [0] undecided, [1..I] counts / offsets, [I+1..2I] cursors
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_build_constraints");
+  a.P = P; a.T = T; a.h = H; a.w = W; a.dh = q.dyn_height; a.dw = q.dyn_width; a.sep = q.match_separation; a.min_dyn = q.min_dynamic_distance;
+  // dynamic-mask scale (lib/FlowConstraints.cpp:415-417); without a dynamic mask the distance image has the colour size (:277-285)
+  a.dsx = dyn_dist ? q.dyn_width / float(W) : 1.f; a.dsy = dyn_dist ? q.dyn_height / float(H) : 1.f;
+  a.sx = 1.f / W; a.sy = q.inv_aspect / H;
+  const unsigned gx = (unsigned)((plane + 255) / 256);
+  if (P > 0) { k_pair_candidates<<<dim3(gx, P), 256, 0, call.st>>>(a); g_builder_launches++; }
+  if (T > 0) { k_triplet_candidates<<<dim3(gx, T), 256, 0, call.st>>>(a); g_builder_launches++; }
+  // ---- selection rounds until nothing is undecided ----
+  int rounds = 0;
+  for (;;) {
+    cudaMemsetAsync(d_cnt, 0, 8, call.st);
+    k_select_round<<<dim3(gx, I), 256, 0, call.st>>>(a, d_cnt); g_builder_launches++; ++rounds;
+    unsigned long long und = 0;
+    cudaMemcpyAsync(&und, d_cnt, 8, cudaMemcpyDeviceToHost, call.st);
+    if (int rc = call.sync("constraint selection")) return rc;
+    if (und == 0) break;
+    if (rounds > 4 * (W + H) + 16) return set_err(RCVD_ERR_CUDA, "constraint selection did not converge");
+  }
+  g_builder_rounds = rounds;
+  // ---- counts, offsets, emission ----
+  cudaMemsetAsync(d_cnt, 0, (size_t)(2 * I + 2) * 8, call.st);
+  k_count_accepted<<<dim3(gx, I), 256, 0, call.st>>>(a, d_cnt + 1); g_builder_launches++;
+  std::vector<unsigned long long> cnt(I), off(I + 1, 0);
+  cudaMemcpyAsync(cnt.data(), d_cnt + 1, (size_t)I * 8, cudaMemcpyDeviceToHost, call.st);
+  if (int rc = call.sync("constraint count read-back")) return rc;
+  for (int i = 0; i < I; ++i) off[i + 1] = off[i] + cnt[i];
+  const unsigned long long pair_total = off[P], total = off[I];
+  for (int i = 0; i < P; ++i) pair_offsets[i + 1] = (int64_t)off[i + 1];
+  for (int i = 0; i < T; ++i) trip_offsets[i + 1] = (int64_t)(off[P + i + 1] - pair_total);
+  if ((int64_t)pair_total > pair_capacity || (int64_t)(total - pair_total) > trip_capacity || (pair_total > 0 && !pair_out) || (total > pair_total && !trip_out))
+    return set_err(RCVD_ERR_INVALID, "output capacity too small: %llu pair and %llu triplet constraints", pair_total, total - pair_total);
+  if (total == 0) return RCVD_OK;
+  unsigned long long* d_off = (unsigned long long*)call.upload(off.data(), (size_t)(I + 1) * 8);
+  int* d_idx = (int*)call.alloc(total * 4); float* d_score = (float*)call.alloc(total * 4);
+  float* d_po = (float*)call.alloc(std::max<size_t>(pair_total, 1) * 16); float* d_to = (float*)call.alloc(std::max<size_t>(total - pair_total, 1) * 24);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_build_constraints");
+  k_emit<<<dim3(gx, I), 256, 0, call.st>>>(a, d_off, d_cnt + 1 + I, d_idx, d_score, d_po, d_to, pair_total); g_builder_launches++;
+  std::vector<int> idx(total); std::vector<float> score(total), po(pair_total * 4), to((total - pair_total) * 6);
+  cudaMemcpyAsync(idx.data(), d_idx, total * 4, cudaMemcpyDeviceToHost, call.st); cudaMemcpyAsync(score.data(), d_score, total * 4, cudaMemcpyDeviceToHost, call.st);
+  if (pair_total) cudaMemcpyAsync(po.data(), d_po, pair_total * 16, cudaMemcpyDeviceToHost, call.st);
+  if (total > pair_total) cudaMemcpyAsync(to.data(), d_to, (total - pair_total) * 24, cudaMemcpyDeviceToHost, call.st);
+  if (int rc = call.sync("constraint emission")) return rc;
+  // order each item's survivors by priority (host: a few hundred entries per item)
+  std::vector<unsigned long long> perm;
+  for (int i = 0; i < I; ++i) {
+    const unsigned long long b = off[i], n = cnt[i];
+    perm.resize(n); for (unsigned long long k = 0; k < n; ++k) perm[k] = b + k;
+    std::sort(perm.begin(), perm.end(), [&](unsigned long long x, unsigned long long y) { return score[x] > score[y] || (score[x] == score[y] && idx[x] < idx[y]); });
+    for (unsigned long long k = 0; k < n; ++k) {
+      if (i < P) std::memcpy(pair_out + (b + k) * 4, po.data() + perm[k] * 4, 16);
+      else std::memcpy(trip_out + (b - pair_total + k) * 6, to.data() + (perm[k] - pair_total) * 6, 24);
+    }
+  }
+  return RCVD_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Dynamic-mask distance transform + static flags on the device (rcvd_builder.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_flag_launches = 0;
+RCVD_API int64_t rcvd_static_flag_launch_count() { return g_flag_launches; }
+// dist_out (optional): [F][h][w] float32 = cv::distanceTransform(mask >= 127 ? 255 : 0, DIST_L2, 5) of every frame (fixed-point chamfer).
+// pair_static / trip_static (optional): one byte per constraint.
+RCVD_API int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t F, int32_t h, int32_t w, float distance,
+                                   int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
+                                   int32_t num_triplets, const int32_t* trip_frames, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static,
+                                   float* dist_out) {
+  if (!masks || F <= 0 || h <= 0 || w <= 0 || num_pairs < 0 || num_triplets < 0) return set_err(RCVD_ERR_INVALID, "bad static-flag arguments");
+  if ((num_pairs > 0 && (!pair_frames || !pair_offsets || !pair_static)) || (num_triplets > 0 && (!trip_frames || !trip_offsets || !trip_static))) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int i = 0; i < num_pairs; ++i) if (pair_frames[2 * i] < 0 || pair_frames[2 * i] >= F || pair_frames[2 * i + 1] < 0 || pair_frames[2 * i + 1] >= F || pair_offsets[i + 1] < pair_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad pair %d", i);
+  for (int i = 0; i < num_triplets; ++i) if (trip_frames[i] < 1 || trip_frames[i] + 1 >= F || trip_offsets[i + 1] < trip_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad triplet %d", i);
+  VideoCall call;
+  if (int rc = call.open(device)) return rc;
+  const size_t plane = (size_t)w * h;
+  const uint8_t* d_masks = (const uint8_t*)call.upload(masks, (size_t)F * plane);
+  unsigned* d_scratch = (unsigned*)call.alloc((size_t)F * plane * 4); float* d_dist = (float*)call.alloc((size_t)F * plane * 4);
+  const int64_t np_total = num_pairs ? pair_offsets[num_pairs] : 0, nt_total = num_triplets ? trip_offsets[num_triplets] : 0;
+  std::vector<int32_t> pf3((size_t)num_pairs * 3, -1), tf3((size_t)num_triplets * 3, -1);
+  for (int i = 0; i < num_pairs; ++i) { pf3[3 * i] = pair_frames[2 * i]; pf3[3 * i + 1] = pair_frames[2 * i + 1]; }
+  for (int i = 0; i < num_triplets; ++i) { tf3[3 * i] = trip_frames[i] - 1; tf3[3 * i + 1] = trip_frames[i]; tf3[3 * i + 2] = trip_frames[i] + 1; }
+  int* d_pf = (int*)call.upload(pf3.data(), pf3.size() * 4); int* d_tf = (int*)call.upload(tf3.data(), tf3.size() * 4);
+  long long* d_po = (long long*)call.upload(pair_offsets, (size_t)(num_pairs + 1) * 8 * (num_pairs > 0)); long long* d_to = (long long*)call.upload(trip_offsets, (size_t)(num_triplets + 1) * 8 * (num_triplets > 0));
+  float* d_pl = (float*)call.upload(pair_locs, (size_t)np_total * 16); float* d_tl = (float*)call.upload(trip_locs, (size_t)nt_total * 24);
+  uint8_t* d_ps = (uint8_t*)call.alloc((size_t)np_total); uint8_t* d_ts = (uint8_t*)call.alloc((size_t)nt_total);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_static_flags");
+  k_chamfer5<<<F, kChamThreads, 0, call.st>>>(d_masks, d_scratch, d_dist, h, w); g_flag_launches++;
+  if (np_total > 0) { k_static_flags<<<dim3(8, num_pairs), 256, 0, call.st>>>(d_dist, h, w, distance, 2, d_pf, d_po, num_pairs, d_pl, d_ps); g_flag_launches++; }
+  if (nt_total > 0) { k_static_flags<<<dim3(8, num_triplets), 256, 0, call.st>>>(d_dist, h, w, distance, 3, d_tf, d_to, num_triplets, d_tl, d_ts); g_flag_launches++; }
+  if (np_total > 0) cudaMemcpyAsync(pair_static, d_ps, (size_t)np_total, cudaMemcpyDeviceToHost, call.st);
+  if (nt_total > 0) cudaMemcpyAsync(trip_static, d_ts, (size_t)nt_total, cudaMemcpyDeviceToHost, call.st);
+  if (dist_out) cudaMemcpyAsync(dist_out, d_dist, (size_t)F * plane * 4, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("static-flag kernels");
+}
+
+// ---------------------------------------------------------------------------
+// Long point tracks (rcvd_tracks.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_track_launches = 0;
+RCVD_API int64_t rcvd_tracks_launch_count() { return g_track_launches; }
+RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t device, const float* color_bgr, const uint8_t* dyn_masks,
+                                     const float* flow, const uint8_t* flow_mask, const uint8_t* frame_flags,
+                                     int64_t* frame_offsets, int32_t* obs_track, float* obs_loc, int64_t capacity, int64_t* num_tracks) {
+  if (!prm || !color_bgr || !frame_flags || !frame_offsets || !num_tracks) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_track_params& q = *prm;
+  const int F = q.num_frames, W = q.width, H = q.height;
+  if (F <= 0 || W <= 0 || H <= 0 || q.spawn_distance < 0 || q.prune_distance < 0 || !(q.inv_aspect > 0.f) || (size_t)W * H >= (1u << 31))
+    return set_err(RCVD_ERR_INVALID, "bad track parameters");
+  if (dyn_masks && (q.dyn_width <= 0 || q.dyn_height <= 0)) return set_err(RCVD_ERR_INVALID, "bad dynamic-mask size");
+  bool need_flow = false, need_mask = false;
+  for (int f = 0; f < F; ++f) { need_flow |= (frame_flags[f] & RCVD_TRACK_FLOW) != 0; need_mask |= (frame_flags[f] & RCVD_TRACK_MASK) != 0; }
+  if ((need_flow && !flow) || (need_mask && !flow_mask)) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int f = 0; f <= F; ++f) frame_offsets[f] = 0;
+  *num_tracks = 0;
+  VideoCall call;
+  if (int rc = call.open(device)) return rc;
+  const int plane = W * H;
+  const size_t FP = (size_t)F * plane, dplane = dyn_masks ? (size_t)q.dyn_width * q.dyn_height : 0;
+  const int max_rounds = 4 * (W + H) + 16, max_live = 2 * plane;   // at most one continued and one spawned track per pixel
+  // the re-derived pixel of a spawn candidate (:844-845): x -> int(float(x / float(w)) * w), y -> int(float(float(y / float(h)) * ia) / ia * h)
+  std::vector<int> mxv(W), myv(H);
+  for (int x = 0; x < W; ++x) { volatile float u = x / float(W); volatile float v = u * W; mxv[x] = (int)v; }
+  for (int y = 0; y < H; ++y) { volatile float u = y / float(H); volatile float v = u * q.inv_aspect; volatile float t = v / q.inv_aspect; volatile float z = t * H; myv[y] = (int)z; }
+  // ---- corner scores and distance images of every frame, batched ----
+  const float* d_corner = enqueue_corner_scores(call, color_bgr, F, H, W, g_track_launches);
+  uint8_t* d_dmask = dyn_masks ? (uint8_t*)call.upload(dyn_masks, (size_t)F * dplane) : nullptr;
+  unsigned* d_cscratch = dyn_masks ? (unsigned*)call.alloc((size_t)F * dplane * 4) : nullptr;
+  float* d_dist = dyn_masks ? (float*)call.alloc((size_t)F * dplane * 4) : nullptr;
+  const float* d_flow = need_flow ? (const float*)call.upload(flow, FP * 8) : nullptr;
+  const uint8_t* d_fmask = need_mask ? (const uint8_t*)call.upload(flow_mask, FP) : nullptr;
+  const int* d_mx = (const int*)call.upload(mxv.data(), (size_t)W * 4), *d_my = (const int*)call.upload(myv.data(), (size_t)H * 4);
+  // ---- per-frame working set ----
+  int* d_id[2] = {(int*)call.alloc((size_t)max_live * 4), (int*)call.alloc((size_t)max_live * 4)};
+  float* d_loc[2] = {(float*)call.alloc((size_t)max_live * 8), (float*)call.alloc((size_t)max_live * 8)};
+  int* d_pix = (int*)call.alloc((size_t)max_live * 4); float* d_cloc = (float*)call.alloc((size_t)max_live * 8); uint8_t* d_cstate = (uint8_t*)call.alloc(max_live);
+  unsigned* d_acc = (unsigned*)call.alloc((size_t)plane * 4);
+  unsigned* d_und[3] = {(unsigned*)call.alloc((size_t)plane * 4), (unsigned*)call.alloc((size_t)plane * 4), (unsigned*)call.alloc((size_t)plane * 4)};
+  uint8_t* d_smask = (uint8_t*)call.alloc(plane); uint8_t* d_sstate = (uint8_t*)call.alloc(plane);
+  unsigned long long* d_keys = (unsigned long long*)call.alloc((size_t)plane * 8), *d_sorted = (unsigned long long*)call.alloc((size_t)plane * 8);
+  unsigned* d_cnt = (unsigned*)call.alloc((size_t)2 * max_rounds * 4);   // [0, max_rounds) prune rounds, then spawn rounds
+  int* d_counts = (int*)call.alloc(8);
+  size_t sort_bytes = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, d_keys, d_sorted, plane, 0, 64, call.st);
+  void* d_sort_tmp = call.alloc(sort_bytes);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_compute_tracks");
+  if (dyn_masks) { k_chamfer5<<<F, kChamThreads, 0, call.st>>>(d_dmask, d_cscratch, d_dist, q.dyn_height, q.dyn_width); g_track_launches++; }
+  TrackArgs a{};
+  a.w = W; a.h = H; a.dw = dyn_masks ? q.dyn_width : W; a.dh = dyn_masks ? q.dyn_height : H;
+  a.spawn_r = q.spawn_distance; a.prune_r = q.prune_distance; a.min_dyn = q.min_dynamic_distance; a.ia = q.inv_aspect;
+  // dynamic-mask scale (:657-663); without a mask the distance is FLT_MAX at colour size
+  a.dsx = dyn_masks ? q.dyn_width / float(W) : 1.f; a.dsy = dyn_masks ? q.dyn_height / float(H) : 1.f;
+  // ---- the frame loop: one host round trip per frame (round convergence + list sizes) ----
+  std::vector<int32_t> ids; std::vector<float> locs;
+  int cur = 0, n_prev = 0, next_id = 0, rp = 4, rs = 16;
+  std::vector<unsigned> cnt_h((size_t)2 * max_rounds);
+  int counts_h[2] = {0, 0};
+  // enqueues the copy of the finished list of local frame g (n entries, buffer slot b) into the outputs
+  auto flush = [&](int g, int b, int n) {
+    frame_offsets[g + 1] = frame_offsets[g] + n;
+    if (n == 0) return;
+    ids.resize((size_t)frame_offsets[g + 1]); locs.resize((size_t)frame_offsets[g + 1] * 2);
+    cudaMemcpyAsync(ids.data() + frame_offsets[g], d_id[b], (size_t)n * 4, cudaMemcpyDeviceToHost, call.st);
+    cudaMemcpyAsync(locs.data() + 2 * frame_offsets[g], d_loc[b], (size_t)n * 8, cudaMemcpyDeviceToHost, call.st);
+  };
+  for (int f = 0; f < F; ++f) {
+    const uint8_t fl = frame_flags[f];
+    const int prev = cur, nxt = cur ^ 1;
+    if (!(fl & RCVD_TRACK_IN_RANGE) || !(fl & RCVD_TRACK_HAS_COLOR)) {   // the frame gets no tracks (:714-727)
+      if (f > 0) { flush(f - 1, prev, n_prev); if (int rc = call.sync("track read-back")) return rc; }
+      n_prev = 0; cur = nxt;
+      continue;
+    }
+    a.dist = dyn_masks ? d_dist + (size_t)f * dplane : nullptr;
+    const bool cont = f > 0 && n_prev > 0 && (fl & RCVD_TRACK_FLOW) && (fl & RCVD_TRACK_MASK);
+    const bool spawn = f < F - 1;
+    const float* score = d_corner + (size_t)f * plane;
+    if (spawn) {
+      k_tr_sort_keys<<<nblk(plane), 256, 0, call.st>>>(score, plane, d_keys); g_track_launches++;
+      cub::DeviceRadixSort::SortKeys(d_sort_tmp, sort_bytes, d_keys, d_sorted, plane, 0, 64, call.st);
+    }
+    for (;;) {   // rounds enqueued blind (they stop early on the device); a frame whose rounds did not all finish is run again with more
+      cudaMemsetAsync(d_cnt, 0, (size_t)2 * max_rounds * 4, call.st);
+      cudaMemsetAsync(d_smask, 0, plane, call.st);
+      if (cont) {
+        cudaMemsetAsync(d_acc, 0xff, (size_t)plane * 4, call.st); cudaMemsetAsync(d_und[0], 0xff, (size_t)plane * 4, call.st); cudaMemsetAsync(d_und[1], 0xff, (size_t)plane * 4, call.st);
+        k_tr_continue<<<nblk(n_prev), 256, 0, call.st>>>(a, n_prev, d_loc[prev], d_flow + (size_t)f * plane * 2, d_fmask + (size_t)f * plane, d_pix, d_cloc, d_cstate, d_und[0]);
+        g_track_launches++;
+        for (int k = 0; k < rp; ++k) {
+          k_tr_prune_round<<<nblk(std::max(n_prev, plane)), 256, 0, call.st>>>(a, n_prev, k, d_pix, d_cstate, d_acc, d_und[k % 3], d_und[(k + 1) % 3], d_und[(k + 2) % 3], d_cnt);
+          g_track_launches++;
+        }
+        k_tr_stamp<<<n_prev, 256, 0, call.st>>>(a, d_pix, d_cstate, d_smask); g_track_launches++;
+      }
+      if (spawn) {
+        const uint8_t* sm = (fl & RCVD_TRACK_MASK) ? d_fmask + (size_t)f * plane : nullptr;
+        k_tr_spawn_init<<<nblk(plane), 256, 0, call.st>>>(a, sm, d_smask, d_mx, d_my, d_sstate); g_track_launches++;
+        for (int k = 0; k < rs; ++k) { k_tr_spawn_round<<<nblk(plane), 256, 0, call.st>>>(a, k, score, d_mx, d_my, d_sstate, d_cnt + max_rounds); g_track_launches++; }
+      }
+      k_tr_emit<<<1, kTrEmitThreads, 0, call.st>>>(a, cont ? n_prev : 0, d_id[prev], d_cstate, d_cloc, spawn ? 1 : 0, d_sorted, d_sstate, next_id, d_id[nxt], d_loc[nxt], d_counts);
+      g_track_launches++;
+      if (f > 0) flush(f - 1, prev, n_prev);
+      cudaMemcpyAsync(cnt_h.data(), d_cnt, (size_t)2 * max_rounds * 4, cudaMemcpyDeviceToHost, call.st);
+      cudaMemcpyAsync(counts_h, d_counts, 8, cudaMemcpyDeviceToHost, call.st);
+      if (int rc = call.sync("track computation")) return rc;
+      const bool p_done = !cont || cnt_h[rp - 1] == 0, s_done = !spawn || cnt_h[max_rounds + rs - 1] == 0;
+      if (p_done && s_done) {
+        // next frame: a few rounds more than this one needed
+        if (cont) { int used = 1; while (used < rp && cnt_h[used - 1] != 0) ++used; rp = std::max(2, used + 1); }
+        if (spawn) { int used = 1; while (used < rs && cnt_h[max_rounds + used - 1] != 0) ++used; rs = std::max(2, used + 2); }
+        break;
+      }
+      if ((!p_done && rp >= max_rounds) || (!s_done && rs >= max_rounds)) return set_err(RCVD_ERR_CUDA, "track selection did not converge");
+      if (!p_done) rp = std::min(max_rounds, 2 * rp);
+      if (!s_done) rs = std::min(max_rounds, 2 * rs);
+      if (f > 0) frame_offsets[f] = frame_offsets[f - 1];   // the previous list is copied again
+    }
+    n_prev = counts_h[0] + counts_h[1];
+    next_id += counts_h[1];
+    cur = nxt;
+  }
+  flush(F - 1, cur, n_prev);
+  if (int rc = call.sync("track read-back")) return rc;
+  *num_tracks = next_id;
+  const int64_t total = frame_offsets[F];
+  if (total > capacity || (total > 0 && (!obs_track || !obs_loc))) return set_err(RCVD_ERR_INVALID, "output capacity too small: %lld observations", (long long)total);
+  if (total > 0) { std::memcpy(obs_track, ids.data(), (size_t)total * 4); std::memcpy(obs_loc, locs.data(), (size_t)total * 8); }
+  return RCVD_OK;
+}

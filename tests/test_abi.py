@@ -67,18 +67,31 @@ def test_no_device_fails_loudly():
 
 def test_filter_and_builder_fail_loudly_without_a_device():
     """No CPU fallback anywhere behind the C ABI: on a box without a usable GPU every compute entry point reports
-    RCVD_ERR_NO_DEVICE (skipped where a GPU is present -- the -m gpu tests cover the real calls)."""
+    RCVD_ERR_NO_DEVICE with one message (skipped where a GPU is present -- the -m gpu tests cover the real calls)."""
     import numpy as np
-    from robust_cvd_b200 import solver
+    from robust_cvd_b200 import abi, solver
     try:
         import torch
         if torch.cuda.is_available():
             pytest.skip("a CUDA device is present")
     except ImportError:
         pass
+    no_device = rf"^rcvd error {abi.ERR_NO_DEVICE}: no usable CUDA device \(.+\); this library has no CPU fallback$"
     depth = np.ones((2, 4, 4), np.float32); cams = np.zeros((2, 9), np.float32); cams[:, 6] = 1; cams[:, 7:] = 0.6
     fl = np.zeros((2, 4, 4, 2), np.float32); mk = np.full((2, 4, 4), 255, np.uint8)
-    with pytest.raises(RuntimeError, match="no usable CUDA device|CUDA"):
+    with pytest.raises(RuntimeError, match=no_device):
         solver.flow_guided_filter(depth, cams, fl, mk, fl, mk, first_out=0, num_out=2, frame_radius=1)
-    with pytest.raises(RuntimeError, match="no usable CUDA device|CUDA"):
+    with pytest.raises(RuntimeError, match=no_device):
         solver.build_constraints(np.zeros((2, 4, 4, 3), np.float32), [(0, 1)], fl[:1], mk[:1], 2, 1.0)
+    grid = abi.default_config(1, 1.5, depth_type=abi.DEPTH_GRID, depth_grid_x=4, depth_grid_y=4)
+    with pytest.raises(RuntimeError, match=no_device):
+        solver.depth_param_map(grid, np.ones(solver.frame_stride(grid)), 4, 4)
+    plain = abi.default_config(1, 1.5)
+    with pytest.raises(RuntimeError, match=no_device):
+        solver.spatial_warp(plain, np.zeros(solver.frame_stride(plain)), 4, 4)
+    with pytest.raises(RuntimeError, match=no_device):
+        solver.static_flags(mk, 1.0, want_distance=True)
+    with pytest.raises(RuntimeError, match=no_device):
+        solver._check(solver.lib().rcvd_trim_device_memory(0))
+    with pytest.raises(RuntimeError, match=no_device):
+        solver.fp64_tensor_peaks(0)
