@@ -98,7 +98,8 @@ PYBIND11_MODULE(lib_python, m) {
       .def("resetDepthXform", &DepthFrame::resetDepthXform)
       .def("spatialXform", [](DepthFrame& f) -> Xform& { return f.spatialXform(); }, py::return_value_policy::reference)
       .def("resetSpatialXform", &DepthFrame::resetSpatialXform)
-      .def_readwrite("intrinsics", &DepthFrame::intrinsics).def_readwrite("extrinsics", &DepthFrame::extrinsics);
+      .def_readwrite("intrinsics", &DepthFrame::intrinsics).def_readwrite("extrinsics", &DepthFrame::extrinsics)
+      .def_readonly("_enabled", &DepthFrame::enabled);   // test/debug accessor (not in the reference): set by the pose importers
   py::class_<DepthStream>(m, "DepthStream")
       .def("frame", &DepthStream::frame, py::return_value_policy::reference)
       .def("name", &DepthStream::name).def("path", &DepthStream::path)
@@ -174,9 +175,8 @@ PYBIND11_MODULE(lib_python, m) {
   struct DepthVideoImporter {};
   py::class_<DepthVideoImporter>(m, "DepthVideoImporter")
       .def_static("importVideo", [](DepthVideo& v, const std::string& path, bool discover) { importVideo(v, path, discover); })
-      .def_static("importPoses", [](DepthVideo&, const std::string&, int) { throw std::runtime_error("importPoses (ground-truth pose import) is outside the pose-optimization path and not implemented in this build."); })
-      .def_static("importColmapDepth", [](DepthVideo&) { throw std::runtime_error("COLMAP import is not implemented in this build."); })
-      .def_static("importColmapRecon", [](DepthVideo&, const std::string&, int, bool) { throw std::runtime_error("COLMAP import is not implemented in this build."); });
+      .def_static("importPoses", &importPoses).def_static("loadScale", &loadScale)
+      .def_static("importColmapDepth", &importColmapDepth).def_static("importColmapRecon", &importColmapRecon);
 
   py::enum_<StaticLossType>(m, "StaticLossType").value("Euclidean", StaticLossType::Euclidean).value("ReproDisparity", StaticLossType::ReproDisparity)
       .value("ReproDepthRatio", StaticLossType::ReproDepthRatio).value("ReproLogDepth", StaticLossType::ReproLogDepth);

@@ -3,9 +3,11 @@
 #include "model.h"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <filesystem>
 #include <fstream>
 #include <iostream>
 #include <sstream>
@@ -14,6 +16,7 @@
 #include <zlib.h>
 
 namespace rcvdh {
+namespace fs = std::filesystem;
 
 static bool g_logStdout = false;
 void setLogToStdout(bool v) { g_logStdout = v; }
@@ -529,6 +532,240 @@ void importVideo(DepthVideo& video, const std::string& path, bool discoverStream
   if (discoverStreams) throw std::runtime_error("Stream discovery is not supported in this build (pose_optimization.py passes discoverStreams=False).");
 }
 
+// Entries of a directory sorted by name: std::filesystem (like boost::filesystem in the reference) iterates in no specified order.
+static std::vector<fs::directory_entry> sortedEntries(const std::string& dir) {
+  std::vector<fs::directory_entry> v{fs::directory_iterator(dir), fs::directory_iterator()};
+  std::sort(v.begin(), v.end(), [](const fs::directory_entry& a, const fs::directory_entry& b) { return a.path().filename() < b.path().filename(); });
+  return v;
+}
+
+void importPoses(DepthVideo& video, const std::string& posesFile, int stream) {
+  logInfo("Importing poses from '" + posesFile + "' to stream " + std::to_string(stream) + ".");
+  DepthStream& ds = video.depthStream(stream);
+  std::ifstream is(posesFile, std::ios::binary);
+  if (is.fail()) throw std::runtime_error("Could not open poses file.");
+  int n = -1; is >> n;
+  if (n > video.numFrames()) throw std::runtime_error("Poses file has more frames than the video.");
+  for (int i = 0; i < n; ++i) {   // position x y z, quaternion x y z w, hFov, vFov
+    float v[9] = {};
+    for (float& x : v) is >> x;
+    DepthFrame& f = ds.frame(i);
+    f.enabled = true;
+    f.extrinsics.position = {v[0], v[1], v[2]};
+    f.extrinsics.orientation.x = v[3]; f.extrinsics.orientation.y = v[4]; f.extrinsics.orientation.z = v[5]; f.extrinsics.orientation.w = v[6];
+    f.intrinsics.hFov = v[7]; f.intrinsics.vFov = v[8];
+  }
+  for (int i = std::max(n, 0); i < video.numFrames(); ++i) ds.frame(i).enabled = false;
+}
+
+float loadScale(const std::string& path) {
+  logInfo("Searching 'scales.csv'...");
+  // When several scales.csv exist below path, the last one visited wins, as in the reference; entries are visited in sorted name order
+  // so that which one that is does not depend on the file system.
+  std::string csv;
+  std::function<void(const std::string&)> visit = [&](const std::string& dir) {
+    for (const fs::directory_entry& e : sortedEntries(dir)) {
+      if (e.path().filename() == "scales.csv") csv = e.path().string();
+      else if (e.is_directory()) visit(e.path().string());
+    }
+  };
+  visit(path);
+  // The reference starts the sum at 1, so the scale is (1 + sum) / count rather than the mean of the listed scales; kept as it is.
+  float scale = 1.f;
+  if (csv.empty()) { logInfo("Could not find 'scales.csv'. Using default scale."); return scale; }
+  std::ifstream f(csv);
+  if (f.fail()) throw std::runtime_error("Could not open 'scales.csv'.");
+  int count = 0;
+  for (std::string line; std::getline(f, line);) {
+    const std::vector<std::string> parts = explode(line, ',');
+    if (parts.size() != 2) { logInfo("ERROR: invalid line '" + line + "'."); continue; }
+    scale += float(std::atof(parts[1].c_str()));
+    ++count;
+  }
+  if (count > 0) scale /= count;
+  logInfo("  Scale = " + std::to_string(scale) + ".");
+  return scale;
+}
+
+void importColmapDepth(DepthVideo& video) {
+  logInfo("Importing COLMAP depth maps...");
+  const std::string src = video.path() + "/depth_colmap_dense/depth", dst = video.path() + "/depth_colmap_dense_imported/depth";
+  if (fileExists(dst)) { logInfo("  Destination directory already exists, skipping."); return; }
+  if (!fs::is_directory(src)) throw std::runtime_error("COLMAP depth directory '" + src + "' does not exist.");
+  makeDirs(dst);
+  const float scale = loadScale(video.path());
+  for (const fs::directory_entry& e : sortedEntries(src)) {
+    const std::string name = e.path().stem().string();   // the reference reads <stem>.raw whatever the entry's extension
+    Image depth; freadim(src + "/" + name + ".raw", depth);
+    if (depth.type != cvMakeType(CV_32F, 1)) throw std::runtime_error("COLMAP depth image '" + name + ".raw' is not single-channel float.");
+    float* d = depth.ptr<float>();
+    for (size_t i = 0; i < size_t(depth.rows) * depth.cols; ++i) d[i] = (!std::isfinite(d[i]) || d[i] < 0.f) ? 0.f : d[i] * scale;
+    fwriteim(dst + "/" + name + ".raw", depth);
+  }
+  logInfo("  Done.");
+}
+
+void importColmapRecon(DepthVideo& video, const std::string& npzFile, int stream, bool silent) {
+  DepthStream& ds = video.depthStream(stream);
+  const float scale = loadScale(video.path());
+  // The reconstructed frames are the ones with a depth file.  Everything is checked before the stream is changed.
+  std::vector<int> frames;
+  for (const fs::directory_entry& e : sortedEntries(ds.path() + "/depth")) {
+    const std::string name = e.path().stem().string();
+    if (name.size() != 12 || name.compare(0, 6, "frame_") != 0 || name.find_first_not_of("0123456789", 6) != std::string::npos)
+      throw std::runtime_error("Depth file name '" + e.path().filename().string() + "' does not have the expected format 'frame_NNNNNN.*'.");
+    const int index = std::stoi(name.substr(6));
+    if (index >= video.numFrames()) throw std::runtime_error("Depth file '" + e.path().filename().string() + "' is past the last frame of the video.");
+    frames.push_back(index);
+  }
+  std::sort(frames.begin(), frames.end());
+  const NpyF64 extr = npzLoadF64(npzFile, "extrinsics"), intr = npzLoadF64(npzFile, "intrinsics");
+  auto shapeStr = [](const NpyF64& a) { std::string s = "("; for (size_t i = 0; i < a.shape.size(); ++i) s += (i ? ", " : "") + std::to_string(a.shape[i]); return s + ")"; };
+  if (extr.shape.size() != 3 || extr.shape[1] != 3 || extr.shape[2] != 4) throw std::runtime_error("'extrinsics' in '" + npzFile + "' has shape " + shapeStr(extr) + "; expected (N, 3, 4).");
+  if (intr.shape.size() != 2 || intr.shape[1] != 4) throw std::runtime_error("'intrinsics' in '" + npzFile + "' has shape " + shapeStr(intr) + "; expected (N, 4).");
+  if (extr.shape[0] != intr.shape[0]) throw std::runtime_error("'" + npzFile + "' has " + std::to_string(extr.shape[0]) + " extrinsics but " + std::to_string(intr.shape[0]) + " intrinsics.");
+  if (extr.shape[0] != frames.size())
+    throw std::runtime_error("'" + npzFile + "' has " + std::to_string(extr.shape[0]) + " cameras but '" + ds.path() + "/depth' has " + std::to_string(frames.size()) + " depth files.");
+  if (extr.fortranOrder || intr.fortranOrder) throw std::runtime_error("'" + npzFile + "' holds Fortran-order arrays; only C order is supported.");
+  for (int i = 0; i < video.numFrames(); ++i) ds.frame(i).enabled = false;
+  // Both the metadata and the extrinsics have +x pointing right and +y up, and the camera faces -z: the rotation's columns are the camera's
+  // right, up and backward vectors in world space, the fourth column its position.
+  if (!silent) logInfo("Loading Extrinsics...");
+  for (size_t i = 0; i < frames.size(); ++i) {
+    const double* P = &extr.data[12 * i];
+    float R[3][3], q[4];
+    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) R[r][c] = float(P[4 * r + c]);
+    matrixToQuat(R, q);
+    DepthFrame& df = ds.frame(frames[i]);
+    df.enabled = true;
+    df.extrinsics.position = {float(P[3]) / scale, float(P[7]) / scale, float(P[11]) / scale};
+    df.extrinsics.orientation.x = q[0]; df.extrinsics.orientation.y = q[1]; df.extrinsics.orientation.z = q[2]; df.extrinsics.orientation.w = q[3];
+    if (!silent) {
+      char b[200]; const Extrinsics& x = df.extrinsics;
+      snprintf(b, sizeof(b), "  Frame %d: position %g %g %g, orientation %g %g %g %g", frames[i], x.position.x, x.position.y, x.position.z, x.orientation.x, x.orientation.y, x.orientation.z, x.orientation.w);
+      logInfo(b);
+    }
+  }
+  if (!silent) logInfo("Loading Intrinsics...");
+  const int w = ds.width(), h = ds.height();
+  for (size_t i = 0; i < frames.size(); ++i) {
+    const double fx = intr.data[4 * i], fy = intr.data[4 * i + 1];
+    Intrinsics in;
+    in.hFov = float(2 * std::atan2(w / 2.0, fx));
+    in.vFov = float(2 * std::atan2(h / 2.0, fy));
+    ds.frame(frames[i]).intrinsics = in;
+    if (!silent) { char b[160]; snprintf(b, sizeof(b), "  Frame %d: fx %g fy %g -> hFov %g vFov %g", frames[i], fx, fy, in.hFov, in.vFov); logInfo(b); }
+  }
+}
+
+// --- .npz archives: a zip file (PKWARE APPNOTE) of .npy members, stored (np.savez) or deflated (np.savez_compressed).  numpy writes
+// every member with zip64 extra fields; the central directory gives each member's sizes and local header offset. ---
+static uint16_t le16(const uint8_t* p) { return uint16_t(p[0] | (p[1] << 8)); }
+static uint32_t le32(const uint8_t* p) { return uint32_t(le16(p)) | (uint32_t(le16(p + 2)) << 16); }
+static uint64_t le64(const uint8_t* p) { return uint64_t(le32(p)) | (uint64_t(le32(p + 4)) << 32); }
+
+// .npy: magic, version, header length, then a Python dict literal {'descr': '<f8', 'fortran_order': False, 'shape': (3, 4), } and the data
+static NpyF64 parseNpy(const std::vector<uint8_t>& b, const std::string& what) {
+  auto bad = [&](const std::string& why) { return std::runtime_error(what + " is not a readable .npy array: " + why + "."); };
+  if (b.size() < 10 || memcmp(b.data(), "\x93NUMPY", 6) != 0) throw bad("no .npy magic");
+  size_t hoff = 10, hlen = le16(&b[8]);
+  if (b[6] == 2 || b[6] == 3) { if (b.size() < 12) throw bad("truncated header"); hoff = 12; hlen = le32(&b[8]); }
+  else if (b[6] != 1) throw bad("unknown format version " + std::to_string(b[6]));
+  if (hlen > b.size() - hoff) throw bad("truncated header");
+  const std::string h(b.begin() + hoff, b.begin() + hoff + hlen);
+  auto value = [&](const char* key) {
+    size_t p = h.find(std::string("'") + key + "'");
+    if (p != std::string::npos) p = h.find(':', p);
+    if (p != std::string::npos) p = h.find_first_not_of(' ', p + 1);
+    if (p == std::string::npos) throw bad(std::string("no '") + key + "' in the header");
+    return p;
+  };
+  NpyF64 a;
+  size_t p = value("descr"), q = h.find('\'', p + 1);
+  if (h[p] != '\'' || q == std::string::npos) throw bad("malformed 'descr'");
+  const std::string descr = h.substr(p + 1, q - p - 1);
+  p = value("fortran_order");
+  if (h.compare(p, 4, "True") == 0) a.fortranOrder = true;
+  else if (h.compare(p, 5, "False") != 0) throw bad("malformed 'fortran_order'");
+  p = value("shape"); q = h.find(')', p);
+  if (h[p] != '(' || q == std::string::npos) throw bad("malformed 'shape'");
+  size_t count = 1;
+  for (std::string d : explode(h.substr(p + 1, q - p - 1), ',')) {
+    trim(d);
+    if (d.empty()) continue;
+    if (d.find_first_not_of("0123456789") != std::string::npos) throw bad("malformed 'shape'");
+    a.shape.push_back(std::stoull(d));
+    if (__builtin_mul_overflow(count, a.shape.back(), &count)) throw bad("the shape is too large");
+  }
+  if (descr != "<f8") throw std::runtime_error(what + " has dtype '" + descr + "'; only little-endian float64 ('<f8') is supported.");
+  if (b.size() - hoff - hlen != count * sizeof(double)) throw bad("the data size does not match the shape");
+  a.data.resize(count);
+  if (count) memcpy(a.data.data(), &b[hoff + hlen], count * sizeof(double));   // the host is little-endian (x86-64, aarch64)
+  return a;
+}
+
+NpyF64 npzLoadF64(const std::string& fileName, const std::string& key) {
+  std::ifstream is(fileName, std::ios::binary);
+  if (!is) throw std::runtime_error("Could not open '" + fileName + "'.");
+  const std::vector<uint8_t> buf((std::istreambuf_iterator<char>(is)), std::istreambuf_iterator<char>());
+  auto bad = [&](const std::string& why) { return std::runtime_error("'" + fileName + "' is not a readable .npz archive: " + why + "."); };
+  auto at = [&](uint64_t off, uint64_t len) { if (off > buf.size() || len > buf.size() - off) throw bad("truncated"); return buf.data() + off; };
+  // end-of-central-directory record: the last one in the final 22 + 65535 (longest comment) bytes
+  if (buf.size() < 22) throw bad("too short");
+  size_t eocd = buf.size() - 22;
+  while (le32(&buf[eocd]) != 0x06054b50) { if (eocd == 0 || buf.size() - eocd >= 22 + 65535) throw bad("no end-of-central-directory record"); --eocd; }
+  uint64_t entries = le16(&buf[eocd + 10]), off = le32(&buf[eocd + 16]);
+  if (entries == 0xFFFF || off == 0xFFFFFFFF) {   // zip64: the locator just before the record points to the zip64 record
+    if (eocd < 20 || le32(&buf[eocd - 20]) != 0x07064b50) throw bad("no zip64 end-of-central-directory locator");
+    const uint8_t* z = at(le64(&buf[eocd - 12]), 56);
+    if (le32(z) != 0x06064b50) throw bad("bad zip64 end-of-central-directory record");
+    entries = le64(z + 32); off = le64(z + 48);
+  }
+  const std::string member = key + ".npy";
+  for (uint64_t e = 0; e < entries; ++e) {
+    const uint8_t* c = at(off, 46);
+    if (le32(c) != 0x02014b50) throw bad("bad central directory entry");
+    const uint16_t method = le16(c + 10), nameLen = le16(c + 28), extraLen = le16(c + 30), commentLen = le16(c + 32);
+    const uint32_t crc = le32(c + 16);
+    uint64_t csize = le32(c + 20), usize = le32(c + 24), local = le32(c + 42);
+    const uint8_t* name = at(off + 46, uint64_t(nameLen) + extraLen + commentLen);
+    off += 46 + uint64_t(nameLen) + extraLen + commentLen;
+    if (std::string(reinterpret_cast<const char*>(name), nameLen) != member) continue;
+    // zip64 extended information (id 1): the 64-bit values of the saturated fields, in this order
+    for (const uint8_t *x = name + nameLen, *end = x + extraLen; x + 4 <= end;) {
+      const uint8_t *v = x + 4, *ve = v + le16(x + 2);
+      if (ve > end) throw bad("malformed extra field");
+      if (le16(x) == 1) {
+        auto take = [&](uint64_t& f) { if (f != 0xFFFFFFFF) return; if (v + 8 > ve) throw bad("short zip64 field"); f = le64(v); v += 8; };
+        take(usize); take(csize); take(local);
+      }
+      x = ve;
+    }
+    const uint8_t* lh = at(local, 30);
+    if (le32(lh) != 0x04034b50) throw bad("bad local header");
+    const uint8_t* data = at(local + 30 + le16(lh + 26) + le16(lh + 28), csize);
+    if (usize > UINT_MAX || csize > UINT_MAX) throw bad("member '" + member + "' is larger than 4 GiB");
+    std::vector<uint8_t> raw(usize);
+    if (method == 0) {
+      if (csize != usize) throw bad("stored member '" + member + "' has inconsistent sizes");
+      if (usize) memcpy(raw.data(), data, usize);
+    } else if (method == 8) {
+      z_stream zs{}; int rc = inflateInit2(&zs, -MAX_WBITS);   // raw deflate, no zlib header
+      if (rc == Z_OK) {
+        zs.next_in = const_cast<Bytef*>(data); zs.avail_in = uInt(csize); zs.next_out = raw.data(); zs.avail_out = uInt(usize);
+        rc = inflate(&zs, Z_FINISH);
+        inflateEnd(&zs);
+      }
+      if (rc != Z_STREAM_END || zs.total_out != usize) throw bad("member '" + member + "' does not inflate");
+    } else {
+      throw bad("member '" + member + "' uses compression method " + std::to_string(method) + "; only stored and deflated members are supported");
+    }
+    if (crc32(0L, raw.data(), uInt(usize)) != crc) throw bad("member '" + member + "' fails its CRC check");
+    return parseNpy(raw, "'" + key + "' in '" + fileName + "'");
+  }
+  throw std::runtime_error("'" + fileName + "' has no array '" + key + "'.");
+}
+
 // --- pose conversions (lib/PoseOptimizer.cpp:769-781, :968-974) ---
 void quatToAngleAxis(const Quatf& qf, double aa[3]) {
   const double qx = qf.x, qy = qf.y, qz = qf.z, qw = qf.w;
@@ -566,13 +803,7 @@ Quatf angleAxisToQuat(const double aa[3]) {
   } else {
     R[0][0] = 1; R[1][0] = aa[2]; R[2][0] = -aa[1]; R[0][1] = -aa[2]; R[1][1] = 1; R[2][1] = aa[0]; R[0][2] = aa[1]; R[1][2] = -aa[0]; R[2][2] = 1;
   }
-  // Eigen::Quaterniond(Matrix3d)
-  double q[4] /* x y z w */; double t = R[0][0] + R[1][1] + R[2][2];
-  if (t > 0.0) { t = std::sqrt(t + 1.0); q[3] = 0.5 * t; t = 0.5 / t; q[0] = (R[2][1] - R[1][2]) * t; q[1] = (R[0][2] - R[2][0]) * t; q[2] = (R[1][0] - R[0][1]) * t; }
-  else {
-    int i = 0; if (R[1][1] > R[0][0]) i = 1; if (R[2][2] > R[i][i]) i = 2; const int j = (i + 1) % 3, k = (j + 1) % 3;
-    t = std::sqrt(R[i][i] - R[j][j] - R[k][k] + 1.0); q[i] = 0.5 * t; t = 0.5 / t; q[3] = (R[k][j] - R[j][k]) * t; q[j] = (R[j][i] + R[i][j]) * t; q[k] = (R[k][i] + R[i][k]) * t;
-  }
+  double q[4]; matrixToQuat(R, q);   // Eigen::Quaterniond(Matrix3d)
   Quatf o; o.x = float(q[0]); o.y = float(q[1]); o.z = float(q[2]); o.w = float(q[3]); return o;
 }
 

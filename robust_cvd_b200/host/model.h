@@ -9,6 +9,7 @@
 #pragma once
 #include <array>
 #include <atomic>
+#include <cmath>
 #include <cstdlib>
 #include <exception>
 #include <functional>
@@ -284,7 +285,16 @@ class DepthVideo {
   std::vector<std::unique_ptr<ColorStream>> colorStreams_;
   std::vector<std::unique_ptr<DepthStream>> depthStreams_;
 };
+// --- DepthVideoImporter (lib/Importer.cpp) ---
 void importVideo(DepthVideo& video, const std::string& path, bool discoverStreams);   // lib/Importer.cpp:25-37, :197-238
+void importPoses(DepthVideo& video, const std::string& posesFile, int stream);        // :438-479 (depth_gt/poses.txt)
+float loadScale(const std::string& path);                                             // :240-288 (scales.csv below path)
+void importColmapDepth(DepthVideo& video);                                            // :390-436
+void importColmapRecon(DepthVideo& video, const std::string& npzFile, int stream, bool silent);   // :290-388 (colmap_dense/metadata.npz)
+
+// One array of a numpy .npz archive (np.savez / np.savez_compressed); only little-endian float64 ('<f8') arrays are read.
+struct NpyF64 { std::vector<size_t> shape; bool fortranOrder = false; std::vector<double> data; };
+NpyF64 npzLoadF64(const std::string& fileName, const std::string& key);
 
 // --- flow constraints (lib/FlowConstraints.{h,cpp}) ---
 struct FlowConstraintsParams {
@@ -412,6 +422,17 @@ class DepthVideoProcessor {
 // Conversions restated from Ceres / Eigen (host side of lib/PoseOptimizer.cpp:748-783, :964-987)
 void quatToAngleAxis(const Quatf& q, double aa[3]);          // Eigen q -> rotation(right, up, -front) -> ceres::RotationMatrixToAngleAxis
 Quatf angleAxisToQuat(const double aa[3]);                   // ceres::AngleAxisToRotationMatrix -> Eigen::Quaterniond(R).cast<float>()
+
+// Eigen::Quaternion<T>(Matrix3<T>) (Shoemake's algorithm, Eigen/src/Geometry/Quaternion.h): R[i][j] is row i, column j; q is x, y, z, w.
+// Eigen's unrolled reduction sums the trace as R00 + (R11 + R22), which decides the last bit in float.
+template <class T> void matrixToQuat(const T R[3][3], T q[4]) {
+  T t = R[0][0] + (R[1][1] + R[2][2]);
+  if (t > T(0)) { t = std::sqrt(t + T(1)); q[3] = T(0.5) * t; t = T(0.5) / t; q[0] = (R[2][1] - R[1][2]) * t; q[1] = (R[0][2] - R[2][0]) * t; q[2] = (R[1][0] - R[0][1]) * t; }
+  else {
+    int i = 0; if (R[1][1] > R[0][0]) i = 1; if (R[2][2] > R[i][i]) i = 2; const int j = (i + 1) % 3, k = (j + 1) % 3;
+    t = std::sqrt(R[i][i] - R[j][j] - R[k][k] + T(1)); q[i] = T(0.5) * t; t = T(0.5) / t; q[3] = (R[k][j] - R[j][k]) * t; q[j] = (R[j][i] + R[i][j]) * t; q[k] = (R[k][i] + R[i][k]) * t;
+  }
+}
 
 void logInfo(const std::string& s);
 void setLogToStdout(bool v);
