@@ -15,18 +15,28 @@ int64_t rcvd_static_flag_launch_count(void);
 int64_t rcvd_tracks_launch_count(void);
 int64_t rcvd_builder_last_rounds(void);          /* selection rounds of the last rcvd_build_constraints call */
 
-/* {frames, off-diagonal factor blocks, levels, H blocks, npad, stride, tiles, update tasks} */
+/* {frames, off-diagonal factor blocks, levels, H blocks, npad, stride, tiles, update targets ((source level, target block) pairs)} */
 int32_t rcvd_structure_info(rcvd_problem* p, int32_t out[8]);
 
 /* the block-Cholesky plan (robust_cvd_b200/csrc/rcvd_plan.h) of the frame graph of np pairs and nt triplet centres under cfg (shared
  * intrinsics, position regulariser, stride), as rank `rank` of `nranks` with the distributed factorisation enabled, on a device of
  * num_sms SMs.  Host only: no handle, no device.  Per frame, in the caller's frame ids: order[N] = elimination order, level[N] = level,
  * owner[N] = owning rank, perm[N] = caller's frame of each internal frame id.  out = {levels, off-diagonal factor blocks, H blocks,
- * update targets, k_update_tma items, k_substitution tasks, distributed, first replicated level, first k_substitution level,
- * this rank's L blocks, H blocks, frames}.  An out-of-range pair or triplet centre: RCVD_ERR_INVALID. */
+ * update targets ((source level, target block) pairs), k_update_tma items, k_substitution tasks, distributed, first replicated level,
+ * first k_substitution level, this rank's L blocks, H blocks, frames, update passes}.  An out-of-range pair or triplet centre:
+ * RCVD_ERR_INVALID. */
 int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
                                int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
-                               int32_t* order, int32_t* level, int32_t* owner, int32_t* perm, int32_t out[12]);
+                               int32_t* order, int32_t* level, int32_t* owner, int32_t* perm, int32_t out[13]);
+/* the update passes of the same plan, in launch order, caller's frame ids: passes[P][5] = {target row frame, target column frame (equal
+ * on a diagonal block), apply level, stream (0: late pass, main stream; 1 / 2: deferred pass in the first / second side-stream launch of
+ * its level), source count}; sources = the source frame of every product, pass after pass; join[2 * levels] = per level and side
+ * launch, the level whose late passes wait for it (levels: none).  counts = {passes P, products, 2 * levels, tail boundary level,
+ * source levels per deferred window below the tail} on return; with passes non-null, counts[0..2] are the capacities of passes (in
+ * passes), sources and join on entry. */
+int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                 int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
+                                 int32_t* passes, int32_t* sources, int32_t* join, int32_t counts[5]);
 
 /* y = (S H S + diag(D2))^-1 b with the current H (exercises factorisation + substitution alone) */
 int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y);

@@ -200,6 +200,7 @@ struct rcvd_problem {
   int64_t launches = 0, graph_launches = 0;
   std::vector<double> h_state; bool state_dirty = false; bool use_fast = true; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
   cudaStream_t side_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  std::vector<cudaEvent_t> ev_side;   // per level, two each: recorded after the level's side-stream update launches (Level::join waits on them)
   cudaStream_t inv_stream = nullptr; cudaEvent_t ev_inv_join = nullptr;   // k_trinv, off the critical path and off the side stream's
   double *d_g2 = nullptr, *d_delta = nullptr; int* h_fail = nullptr;
   cudaEvent_t ev[8] = {nullptr};
@@ -421,6 +422,7 @@ static int build_structure(rcvd_problem* p) {
   if (const char* e = make_factor_plan(p->plan, p->cfg, p->struct_pairs.empty() ? p->pair_frames : p->struct_pairs, p->trip_centers, p->order_slack,
                                        p->nranks, p->rank, p->dist_enabled, p->num_sms))
     return set_err(RCVD_ERR_INVALID, "%s", e);
+  while (p->ev_side.size() < 2 * p->plan.levels.size()) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); p->ev_side.push_back(e); }
   int rc;
   if ((rc = upload_plan(p)) || (rc = set_up_problem_data(p)) || (rc = allocate_storage(p))) return rc;
   CK(cudaStreamSynchronize(p->stream));
@@ -472,11 +474,13 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   CK(cudaMemsetAsync(p->d_potrf_progress, 0, (size_t)N * sizeof(int), st));   // no count of the previous factorisation may read as published
   k_load_factor<<<dim3((npad * npad + 255) / 256, p->plan.dist ? (int)p->plan.own_lblocks.size() : nL), 256, 0, st>>>(p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, L.nf, p->plan.dist ? p->d_own_lblocks : nullptr);
   p->launches += 1; p->paths[LP_OTHER]++; mark(P_LOAD);
-  // Two-stream schedule (fork/join inside the captured graph): the non-critical update GEMMs of level l run on `side`
-  // concurrently with potrf / trsm of level l+1 on `st`.  The explicit inverses run on a third stream, `inv`: on `side` they would
-  // hold back the next update launch by a k_trinv, and U1(l+1) waits for that update (U2(l)).
+  // Two-stream schedule (fork/join inside the captured graph): the deferred update passes of level l (U2) run on `side` concurrently
+  // with the later levels on `st`; the late passes (U1) of level Level::join are the first main-stream work that touches one of their
+  // targets, and wait for them there (the side stream runs in order: one wait covers every earlier side launch).  The explicit
+  // inverses run on a third stream, `inv`: on `side` they would hold back the next update launch by a k_trinv.
   cudaStream_t side = p->side_stream, inv = p->inv_stream;
-  bool side_pending = false, side_used = false, inv_used = false;
+  bool side_used = false, inv_used = false;
+  int side_joined = -1;   // the main stream has waited for the side launches (2 * level + launch) up to this one
   auto join_inv = [&]() -> int {
     if (inv_used) { CK(cudaEventRecord(p->ev_inv_join, inv)); CK(cudaStreamWaitEvent(st, p->ev_inv_join, 0)); inv_used = false; }
     return RCVD_OK;
@@ -485,7 +489,7 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   // phase boundary of the distributed factorisation: the owners' explicit inverses (for the replicated substitution) and their
   // blocks of the trailing matrix go to everybody; from here on every rank factors the same narrow tail
   auto phase_boundary = [&]() -> int {
-    if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }
+    if (side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_joined = 2 * p->plan.LB - 1; }
     if (int rc = join_inv()) return rc;
     std::vector<Seg> invs, tr;
     for (int q = 0; q < p->nranks; ++q) invs.push_back({(size_t)p->plan.fa_off[q], (size_t)p->plan.fa_cnt[q]});
@@ -578,8 +582,12 @@ static int enqueue_factor_solve(rcvd_problem* p) {
       int rc = grouped(p, p->d_T, bsz, segs, true); if (rc) return rc;
     }
     auto fork_u2 = [&]() -> int { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0)); return RCVD_OK; };
-    if (lv.nupd2 > 0 && p->overlap && !fork_u2_late) { if (int rc = fork_u2()) return rc; }
-    if (side_pending) { CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_pending = false; }   // U2(l-1) before U1(l)
+    if (lv.nupd2[0] + lv.nupd2[1] > 0 && p->overlap && !fork_u2_late) { if (int rc = fork_u2()) return rc; }
+    if (p->overlap) {   // U2 launch s of level q before U1(join[s] of q)
+      int s = -1;
+      for (int q = side_joined + 1; q < 2 * (int)li; ++q) { const Level& v = p->plan.levels[q / 2]; if (v.nupd2[q % 2] > 0 && v.join[q % 2] <= (int)li) s = q; }
+      if (s >= 0) { CK(cudaStreamWaitEvent(st, p->ev_side[s], 0)); side_joined = s; }
+    }
     auto update = [&](cudaStream_t cs, int off, int n) {   // persistent TMA-fed update kernel
       if (n <= p->num_sms) {   // few items: two DMMA teams per tile, one CTA per SM
         k_update_tma<2><<<n, UpdShape<2>::threads, upd_smem_bytes(p->plan.upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->plan.upd_neff, p->plan.upd_rb, 0);
@@ -593,21 +601,21 @@ static int enqueue_factor_solve(rcvd_problem* p) {
     };
     if (p->gemm_tma) {
       if (lv.nit > 0) { update(st, lv.it_off, lv.nit); p->launches++; mark(P_GEMM); }
-      if (lv.nit2 > 0) {
-        if (fork_u2_late) { if (int rc = fork_u2()) return rc; }   // after U1
-        update(p->overlap ? side : st, lv.it2_off, lv.nit2); p->launches++; mark(P_GEMM);
-        if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
+      if (fork_u2_late && lv.nit2[0] + lv.nit2[1] > 0) { if (int rc = fork_u2()) return rc; }   // after U1
+      for (int h = 0; h < 2; ++h) if (lv.nit2[h] > 0) {
+        update(p->overlap ? side : st, lv.it2_off[h], lv.nit2[h]); p->launches++; mark(P_GEMM);
+        if (p->overlap) { CK(cudaEventRecord(p->ev_side[2 * li + h], side)); side_used = true; }
       }
       continue;
     }
     if (lv.nupd > 0) { gemm(st, lv.nupd, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM); }
-    if (lv.nupd2 > 0) {
-      gemm(p->overlap ? side : st, lv.nupd2, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM);
-      if (p->overlap) { CK(cudaEventRecord(p->ev_join, side)); side_pending = true; side_used = true; }
+    for (int h = 0; h < 2; ++h) if (lv.nupd2[h] > 0) {
+      gemm(p->overlap ? side : st, lv.nupd2[h], p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off[h], p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM);
+      if (p->overlap) { CK(cudaEventRecord(p->ev_side[2 * li + h], side)); side_used = true; }
     }
   }
   if (p->plan.dist && p->plan.LB >= (int)p->plan.levels.size()) { int rc = phase_boundary(); if (rc) return rc; }
-  if (side_pending || side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); }
+  if (side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); }
   if (int rc = join_inv()) return rc;
   CK(cudaMemcpyAsync(p->d_rhs, p->d_gs, (size_t)N * npad * sizeof(double), cudaMemcpyDeviceToDevice, st));
   const int nlv = (int)p->plan.levels.size();
@@ -1076,6 +1084,7 @@ RCVD_API void rcvd_problem_destroy(rcvd_problem* p) {
   if (p->comm && nccl::CommDestroy) nccl::CommDestroy(p->comm);
   if (p->ev_fork) cudaEventDestroy(p->ev_fork);
   if (p->ev_join) cudaEventDestroy(p->ev_join);
+  for (cudaEvent_t e : p->ev_side) cudaEventDestroy(e);
   if (p->ev_inv_join) cudaEventDestroy(p->ev_inv_join);
   if (p->side_stream) cudaStreamDestroy(p->side_stream);
   if (p->inv_stream) cudaStreamDestroy(p->inv_stream);
@@ -1491,27 +1500,58 @@ RCVD_API int32_t rcvd_solve(rcvd_problem* p, const rcvd_solve_options* opt, rcvd
   rcvd_solve_options o; if (opt) o = *opt; else rcvd_default_solve_options(&o);
   return lm_solve(p, o, *summary);
 }
-// Test hook: the factorisation plan of a frame graph, computed on the host alone -- no handle, no device (see include/rcvd_hooks.h).
-RCVD_API int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
-                                        int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
-                                        int32_t* order, int32_t* level, int32_t* owner, int32_t* perm, int32_t out[12]) {
-  if (!cfg || np < 0 || nt < 0 || (np > 0 && !pairs) || (nt > 0 && !trip_centers) || !order || !level || !owner || !perm || !out)
-    return set_err(RCVD_ERR_INVALID, "null or negative argument");
+// The plan of rcvd_debug_factor_plan / rcvd_debug_update_passes: host only, no handle, no device.
+static int32_t debug_plan(FactorPlan& pl, const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                          int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms) {
+  if (!cfg || np < 0 || nt < 0 || (np > 0 && !pairs) || (nt > 0 && !trip_centers)) return set_err(RCVD_ERR_INVALID, "null or negative argument");
   if (nranks < 1 || rank < 0 || rank >= nranks || num_sms < 1) return set_err(RCVD_ERR_INVALID, "bad rank/nranks/num_sms");
-  FactorPlan pl;
   if (const char* e = make_factor_plan(pl, *cfg, std::vector<int32_t>(pairs, pairs + 2 * (size_t)np), std::vector<int32_t>(trip_centers, trip_centers + nt),
                                        order_slack, nranks, rank, true, num_sms))
     return set_err(RCVD_ERR_INVALID, "%s", e);
+  return RCVD_OK;
+}
+// Test hook: the factorisation plan of a frame graph, computed on the host alone -- no handle, no device (see include/rcvd_hooks.h).
+RCVD_API int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                        int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
+                                        int32_t* order, int32_t* level, int32_t* owner, int32_t* perm, int32_t out[13]) {
+  if (!order || !level || !owner || !perm || !out) return set_err(RCVD_ERR_INVALID, "null or negative argument");
+  FactorPlan pl;
+  if (int32_t rc = debug_plan(pl, cfg, np, pairs, nt, trip_centers, order_slack, nranks, rank, num_sms)) return rc;
   const int N = cfg->num_frames;
   for (int i = 0; i < N; ++i) {
     const int f = pl.uperm[i];
     order[i] = pl.uperm[pl.elim_order[i]]; level[f] = pl.level[i]; owner[f] = pl.owner[i]; perm[i] = f;
   }
-  int upd = 0; for (const Level& l : pl.levels) upd += l.nupd + l.nupd2;
-  const int32_t v[12] = {(int32_t)pl.levels.size(), pl.nLoff, (int32_t)pl.hblocks.size(), upd, (int32_t)pl.upd_items.size(), (int32_t)pl.sub_tasks.size(),
+  const int32_t v[13] = {(int32_t)pl.levels.size(), pl.nLoff, (int32_t)pl.hblocks.size(), pl.upd_targets, (int32_t)pl.upd_items.size(), (int32_t)pl.sub_tasks.size(),
                          pl.dist ? 1 : 0, pl.LB, pl.sub_first_level, (int32_t)pl.own_lblocks.size(), (int32_t)pl.own_hblocks.size(),
-                         pl.dist ? pl.fa_cnt[rank] + pl.fb_cnt[rank] : N};
-  std::copy(v, v + 12, out);
+                         pl.dist ? pl.fa_cnt[rank] + pl.fb_cnt[rank] : N, (int32_t)pl.upd_tasks.size()};
+  std::copy(v, v + 13, out);
+  return RCVD_OK;
+}
+// Test hook: the update passes of the plan of a frame graph (see include/rcvd_hooks.h).
+RCVD_API int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                          int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
+                                          int32_t* passes, int32_t* sources, int32_t* join, int32_t counts[5]) {
+  if (!counts) return set_err(RCVD_ERR_INVALID, "null argument");
+  FactorPlan pl;
+  if (int32_t rc = debug_plan(pl, cfg, np, pairs, nt, trip_centers, order_slack, nranks, rank, num_sms)) return rc;
+  const int32_t need[3] = {(int32_t)pl.upd_tasks.size(), (int32_t)pl.upd_pairs.size(), 2 * (int32_t)pl.levels.size()};
+  if (passes) {
+    if (!sources || !join || counts[0] < need[0] || counts[1] < need[1] || counts[2] < need[2]) return set_err(RCVD_ERR_INVALID, "null or short output array");
+    const int N = cfg->num_frames;
+    for (size_t l = 0; l < pl.levels.size(); ++l) {
+      const Level& lv = pl.levels[l];
+      join[2 * l] = lv.join[0]; join[2 * l + 1] = lv.join[1];
+      for (int q = lv.upd_off; q < lv.upd2_off[1] + lv.nupd2[1]; ++q) {
+        const GemmTask& t = pl.upd_tasks[q];
+        const HBlock& b = pl.lblocks[t.dst];
+        int32_t* o = passes + 5 * (size_t)q;
+        o[0] = pl.uperm[b.r]; o[1] = pl.uperm[b.c]; o[2] = (int32_t)l; o[3] = q >= lv.upd2_off[1] ? 2 : q >= lv.upd2_off[0] ? 1 : 0; o[4] = t.count;
+        for (int i = 0; i < t.count; ++i) sources[t.first + i] = pl.uperm[pl.lblocks[N + pl.upd_pairs[t.first + i].x].c];
+      }
+    }
+  }
+  std::copy(need, need + 3, counts); counts[3] = pl.TB; counts[4] = pl.upd_window;
   return RCVD_OK;
 }
 // Structure statistics (for DESIGN.md / bench): frames, off-diagonal factor blocks, levels, H blocks, npad.
@@ -1520,6 +1560,6 @@ RCVD_API int32_t rcvd_structure_info(rcvd_problem* p, int32_t out[8]) {
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
   out[0] = p->N; out[1] = p->plan.nLoff; out[2] = (int)p->plan.levels.size(); out[3] = (int)p->plan.hblocks.size(); out[4] = p->L.npad; out[5] = p->L.nf; out[6] = p->num_tiles;
-  int upd = 0; for (auto& l : p->plan.levels) upd += l.nupd + l.nupd2; out[7] = upd;
+  out[7] = p->plan.upd_targets;
   return RCVD_OK;
 }

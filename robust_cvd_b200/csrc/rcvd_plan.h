@@ -12,9 +12,17 @@
 
 namespace rcvd {
 
-// frame_off: every frame of the level (substitution); own_off: the frames this rank factors; upd: targets consumed by the next level;
-// upd2: the rest; it / it2: the k_update_tma items of upd / upd2
-struct Level { int frame_off, nframes; int trsm_off, ntrsm; int upd_off, nupd; int upd2_off, nupd2; int fwd_off, nfwd; int it_off, nit, it2_off, nit2; int own_off, nown; };
+// frame_off: every frame of the level (substitution); own_off: the frames this rank factors; upd: the late update passes (main stream);
+// upd2[0], upd2[1]: the deferred passes applied at this level (side stream), two launches in this order: [0] the passes into the
+// columns of level + 2, which the next level's late passes need, [1] the rest; it / it2: the k_update_tma items of upd / upd2;
+// join[s]: the first level whose late passes (U1) must wait for launch s -- one of its targets is in a column of level join[s] + 1
+struct Level { int frame_off, nframes; int trsm_off, ntrsm; int upd_off, nupd; int upd2_off[2], nupd2[2]; int fwd_off, nfwd; int it_off, nit, it2_off[2], nit2[2]; int own_off, nown; int join[2]; };
+
+// Deferred update passes group the wide levels (below the narrow tail) in aligned windows of kUpdWindow source levels when a frame block
+// has at most kUpdWindowMaxNf unknowns; otherwise, and in the tail, one pass per source level.  A pass's read-modify-write of its target
+// is amortised over its products; at nf = 775 the products are long enough that batching them saves nothing, and piling them onto fewer
+// levels delays the main stream, as it would in the tail, whose side work must finish within the next level's potrf (DESIGN.md section 4).
+constexpr int kUpdWindow = 2, kUpdWindowMaxNf = 256;
 
 // Every frame id below is internal: frames are numbered owner-major (uperm / iperm map to and from the caller's ids).
 struct FactorPlan {
@@ -35,6 +43,9 @@ struct FactorPlan {
   std::vector<GemmTask> trsm_tasks, upd_tasks; std::vector<int2> trsm_pairs, upd_pairs;
   std::vector<TrsmTask> trsm_ll; std::vector<SolveTask> fwd_tasks;
   std::vector<UpdItem> upd_items; int upd_rb = 0, upd_neff = 0;
+  int upd_targets = 0;      // (source level, target block) pairs of the elimination structure this rank updates
+  int upd_window = 1;       // source levels per window of the deferred update passes
+  int TB = 0;               // tail boundary: levels >= TB are the trailing run of levels with fewer than 3 frames (= LB when distributed)
   double upd_flops = 0.0;   // algorithmic flops of the update GEMMs of one factorisation (2 nf^3 per product, nf^2 (nf+1) on symmetric targets)
   std::vector<SubTask> sub_tasks; std::vector<int> sub_need; int sub_first_level = 0;   // k_substitution: levels >= sub_first_level
 };
@@ -104,9 +115,10 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
   // at the boundary every owner broadcasts its trailing blocks.  H is reduced to the owners only (no all-reduce of the matrix).
   const int R = nranks;
   bool dist = R > 1 && dist_enabled && cfg.intr_opt != RCVD_INTR_SHARED && !(cfg.position_reg > 0.0) && trip_centers.empty();
+  int TB = nl; while (TB > 0 && (int)lf[TB - 1].size() < 3) --TB;
   int LB = 0;
-  if (dist) { LB = nl; while (LB > 0 && (int)lf[LB - 1].size() < 3) --LB; if (LB == 0) dist = false; }
-  P.dist = dist; P.LB = LB;
+  if (dist) { LB = TB; if (LB == 0) dist = false; }
+  P.dist = dist; P.LB = LB; P.TB = TB;
   std::vector<int> own(N, 0);
   if (dist) {
     // incoming update work of every column over the phase-A levels (block products; symmetric targets count half)
@@ -187,11 +199,44 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
   const int upd_nt = (upd_neff + kUpdMaxTile - 1) / kUpdMaxTile;
   const int upd_tile = std::min(kUpdMaxTile, upd_neff);          // 80-row tiles (balanced 5 x 5 units per warp), the remainder last
   P.upd_rb = upd_tile; P.upd_neff = upd_neff;
+  // The block products (source frame k, target (r, c)) of every target, in source-level order.  c is eliminated before r: the target
+  // lives in column c, and a rank updates only the columns it owns in phase A.
+  auto col_of = [&](int target) { return target < N ? target : lcol[target - N]; };
+  std::map<int, std::vector<std::pair<int, int2>>> prod;   // target L block id -> (source level, source pair)
+  for (int l = 0; l < nl; ++l) {
+    const bool shared_level = !dist || l >= LB;   // replicated work: every rank does all of it
+    std::set<int> targets;
+    for (int k : lf[l]) for (size_t a = 0; a < cs[k].size(); ++a) for (size_t b = 0; b <= a; ++b) {
+      const int r = cs[k][a], c = cs[k][b];
+      if (!shared_level && own[c] != rank) continue;
+      const int target = (r == c) ? r : lid[{r, c}];
+      prod[target].push_back({l, make_int2(lid[{r, k}] - N, lid[{c, k}] - N)});
+      targets.insert(target);
+    }
+    P.upd_targets += (int)targets.size();
+  }
+  // Update passes.  The products from level Lc - 1 (Lc: the level of the target's column) are the late pass: it runs on the main stream
+  // at Lc - 1, on the critical path.  The earlier products are deferred to the side stream, grouped in level windows (wide levels only,
+  // see kUpdWindow), each window one pass applied at the level of its latest source: every pass reads and writes the whole target, so
+  // fewer, longer passes move less of it through memory.  Within a level the passes are in target order.
+  const int W = P.upd_window = L.nf <= kUpdWindowMaxNf ? kUpdWindow : 1;
+  auto window = [&](int l) { return l < TB ? l / W : nl + l; };
+  std::vector<std::vector<std::pair<int, std::vector<int2>>>> late(nl), deferred(nl);   // per apply level: (target, source pairs)
+  for (auto& kv : prod) {
+    const int Lc = lvl[col_of(kv.first)];
+    const auto& v = kv.second;
+    for (size_t i = 0, j; i < v.size(); i = j) {
+      const bool is_late = v[i].first == Lc - 1;
+      for (j = i + 1; j < v.size() && (v[j].first == Lc - 1) == is_late && (is_late || window(v[j].first) == window(v[i].first)); ++j) {}
+      auto& pass = (is_late ? late : deferred)[v[j - 1].first];
+      pass.push_back({kv.first, {}});
+      for (size_t q = i; q < j; ++q) pass.back().second.push_back(v[q].second);
+    }
+  }
   for (int l = 0; l < nl; ++l) {
     Level lv; lv.frame_off = (int)P.lvl_frames.size(); lv.nframes = (int)lf[l].size(); lv.own_off = (int)P.lvl_own.size();
     lv.trsm_off = (int)P.trsm_tasks.size(); lv.upd_off = (int)P.upd_tasks.size(); lv.fwd_off = (int)P.fwd_tasks.size();
-    std::map<int, std::vector<int2>> upd;   // target L block id -> source pairs
-    const bool shared_level = !dist || l >= LB;   // replicated work: every rank does all of it
+    const bool shared_level = !dist || l >= LB;
     for (int k : lf[l]) {
       P.lvl_frames.push_back(k);
       const bool mine = shared_level || own[k] == rank;
@@ -205,32 +250,28 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
         }
         P.fwd_tasks.push_back({id - N, r, k});
       }
-      for (size_t a = 0; a < cs[k].size(); ++a) for (size_t b = 0; b <= a; ++b) {
-        const int r = cs[k][a], c = cs[k][b];                     // c is eliminated before r: the target lives in column c
-        if (!shared_level && own[c] != rank) continue;
-        const int target = (r == c) ? r : lid[{r, c}];
-        upd[target].push_back(make_int2(lid[{r, k}] - N, lid[{c, k}] - N));
-      }
     }
     lv.nown = (int)P.lvl_own.size() - lv.own_off;
-    // targets whose column frame is eliminated in the very next level must be complete before that level starts (critical);
-    // all other updates may overlap the next level's potrf / inverse / trsm on a second stream.
-    for (int pass = 0; pass < 2; ++pass) {
-      if (pass == 1) lv.upd2_off = (int)P.upd_tasks.size();
-      for (auto& kv : upd) {
-        const int cframe = kv.first < N ? kv.first : lcol[kv.first - N];
-        const bool critical = (lvl[cframe] == l + 1);
-        if (critical != (pass == 0)) continue;
-        P.upd_tasks.push_back({kv.first, (int)P.upd_pairs.size(), (int)kv.second.size(), kv.first < N ? 1 : 0});
-        { const double n = (double)L.nf; P.upd_flops += (double)kv.second.size() * (kv.first < N ? n * n * (n + 1.0) : 2.0 * n * n * n); }
-        P.upd_pairs.insert(P.upd_pairs.end(), kv.second.begin(), kv.second.end());
+    // the deferred passes of a batched level are two launches, so that the next level's late passes wait only for the first
+    lv.join[0] = lv.join[1] = nl;
+    const bool split = W > 1 && l < TB;
+    for (int pass = 0; pass < 3; ++pass) {
+      if (pass > 0) lv.upd2_off[pass - 1] = (int)P.upd_tasks.size();
+      for (auto& tp : (pass ? deferred : late)[l]) {
+        const int Lc = lvl[col_of(tp.first)];
+        if (pass > 0 && (!split || Lc == l + 2) != (pass == 1)) continue;
+        if (pass > 0) lv.join[pass - 1] = std::min(lv.join[pass - 1], Lc - 1);
+        P.upd_tasks.push_back({tp.first, (int)P.upd_pairs.size(), (int)tp.second.size(), tp.first < N ? 1 : 0});
+        { const double n = (double)L.nf; P.upd_flops += (double)tp.second.size() * (tp.first < N ? n * n * (n + 1.0) : 2.0 * n * n * n); }
+        P.upd_pairs.insert(P.upd_pairs.end(), tp.second.begin(), tp.second.end());
       }
     }
-    lv.ntrsm = (int)P.trsm_tasks.size() - lv.trsm_off; lv.nupd = lv.upd2_off - lv.upd_off; lv.nupd2 = (int)P.upd_tasks.size() - lv.upd2_off; lv.nfwd = (int)P.fwd_tasks.size() - lv.fwd_off;
-    // work items of the persistent update kernel: one per (target tile, source-pair list), heaviest first
+    lv.ntrsm = (int)P.trsm_tasks.size() - lv.trsm_off; lv.nupd = lv.upd2_off[0] - lv.upd_off; lv.nfwd = (int)P.fwd_tasks.size() - lv.fwd_off;
+    lv.nupd2[0] = lv.upd2_off[1] - lv.upd2_off[0]; lv.nupd2[1] = (int)P.upd_tasks.size() - lv.upd2_off[1];
+    // work items of the persistent update kernel: one per (target tile, source-pair list), heaviest first within each launch
     std::vector<UpdItem>& items = P.upd_items;
-    for (int pass = 0; pass < 2; ++pass) {
-      const int t0 = pass ? lv.upd2_off : lv.upd_off, tn = pass ? lv.nupd2 : lv.nupd;
+    for (int pass = 0; pass < 3; ++pass) {
+      const int t0 = pass ? lv.upd2_off[pass - 1] : lv.upd_off, tn = pass ? lv.nupd2[pass - 1] : lv.nupd;
       const size_t i0 = items.size();
       for (int q = t0; q < t0 + tn; ++q) {
         const GemmTask& tk = P.upd_tasks[q];
@@ -243,7 +284,7 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
       }
       auto cost = [](const UpdItem& a) { return (long)a.count * (a.mrows / 8) * (a.ncols / 8) * ((a.flags & 1) ? 3 : 4); };
       std::stable_sort(items.begin() + i0, items.end(), [&](const UpdItem& a, const UpdItem& b) { return cost(a) > cost(b); });
-      if (pass) { lv.it2_off = (int)i0; lv.nit2 = (int)(items.size() - i0); } else { lv.it_off = (int)i0; lv.nit = (int)(items.size() - i0); }
+      if (pass) { lv.it2_off[pass - 1] = (int)i0; lv.nit2[pass - 1] = (int)(items.size() - i0); } else { lv.it_off = (int)i0; lv.nit = (int)(items.size() - i0); }
     }
     P.levels.push_back(lv);
   }
