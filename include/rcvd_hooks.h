@@ -51,10 +51,10 @@ int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* 
  * = the N * stride * stride explicit inverses of the diagonal blocks (k_trinv), same order.  RCVD_ERR_INVALID before any factorisation. */
 int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, double* Linv);
 /* launches of each factorisation / solve kernel path since the handle was created: {k_potrf_smem, k_potrf_panel, k_trsm_ll<4>,
- * k_trsm_ll<2>, TRSM by explicit inverse (k_gemm_nt), k_update_tma<1>, k_update_tma<2>, update by k_gemm_nt, level-launched
- * substitution (k_fwd_* / k_bwd_*), k_substitution, k_trinv, the rest (k_load_factor, k_potrf_trail), k_update_tma<1> launches with
- * fewer CTAs than items (CTAs that walk several items), k_trsm_ll launches (either shape) streamed beside their level's k_potrf_smem} */
-int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[14]);
+ * k_trsm_ll<2>, TRSM by explicit inverse (k_gemm_nt), k_update_tma<1>, k_update_tma<2>, level-launched substitution
+ * (k_fwd_* / k_bwd_*), k_substitution, k_trinv, the rest (k_load_factor, k_potrf_trail), k_update_tma<1> launches with fewer CTAs
+ * than items (CTAs that walk several items), k_trsm_ll launches (either shape) streamed beside their level's k_potrf_smem} */
+int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]);
 
 /* one damped LM step at the current state with trust-region `radius`; out = {|(S H S + D2) y - S g| / |S g| (device SpMV over the
  * assembled H), |S g|, cost, |g|_2, |y|_2, non-positive-pivot flag}: the parity evidence bench.py prints at the size it times */
@@ -81,7 +81,7 @@ int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack);   /* (4) mul
 int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on);        /* (0) cost / gradient evaluations only: no matrix storage (the whole-problem check of a multi-GPU bench) */
 int32_t rcvd_debug_set_distributed(rcvd_problem* p, int32_t on);      /* (1) nranks > 1: distributed factorisation; 0 = all-reduce H + replicated factorisation */
 int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]);       /* {distributed, first replicated level, levels, frames owned by this rank} */
-int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta); /* (1, 0) persistent TMA-fed update kernel / cp.async kernel; items-per-CTA cap of the one-team launches (0: none) */
+int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta); /* (1, 0) tma must be 1 (0: RCVD_ERR_INVALID, the cp.async update path was removed); items-per-CTA cap of the one-team launches (0: none) */
 
 #ifdef __cplusplus
 }

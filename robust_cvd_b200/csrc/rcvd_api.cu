@@ -157,7 +157,7 @@ __global__ void k_h_to_dense(const double* __restrict__ H, const HBlock* __restr
 }
 
 // launch counters of enqueue_factor_solve by kernel path (rcvd_debug_linear_paths; include/rcvd_hooks.h lists the same order)
-enum { LP_POTRF_SMEM = 0, LP_POTRF_PANEL, LP_TRSM_LL4, LP_TRSM_LL2, LP_TRSM_GEMM, LP_UPD_TMA1, LP_UPD_TMA2, LP_UPD_GEMM, LP_SUB_LEVEL, LP_SUB_FUSED,
+enum { LP_POTRF_SMEM = 0, LP_POTRF_PANEL, LP_TRSM_LL4, LP_TRSM_LL2, LP_TRSM_GEMM, LP_UPD_TMA1, LP_UPD_TMA2, LP_SUB_LEVEL, LP_SUB_FUSED,
        LP_TRINV, LP_OTHER, LP_UPD_TMA1_MULTI, LP_TRSM_STREAMED, LP_N };   // LP_UPD_TMA1_MULTI: k_update_tma<1> launches with fewer CTAs than
 // items; LP_TRSM_STREAMED: the k_trsm_ll launches (either shape) that run beside their level's k_potrf_smem
 
@@ -190,7 +190,7 @@ struct rcvd_problem {
   int trsm2_ctas_per_sm = 0;          // resident k_trsm_ll<2> CTAs per SM at this npad
   // the block-Cholesky plan (rcvd_plan.h) and its device copies
   FactorPlan plan;
-  int *d_lvl_frames = nullptr; GemmTask *d_trsm_tasks = nullptr, *d_upd_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
+  int *d_lvl_frames = nullptr; GemmTask* d_trsm_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
   SubTask* d_sub_tasks = nullptr; int* d_sub_counters = nullptr; int* d_sub_need = nullptr;
   SolveTask* d_fwd_tasks = nullptr; TrsmTask* d_trsm_ll = nullptr; bool use_trsm_ll = false;
   cudaGraphExec_t solve_graph = nullptr;
@@ -213,7 +213,7 @@ struct rcvd_problem {
   // distributed factorisation (nranks > 1): the frames this rank factors per level, the blocks it owns, internal -> caller's frame ids
   int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr;
   // TMA-fed persistent update kernel (rcvd_update.cuh)
-  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; bool gemm_tma = true, tmap_ok = false; int num_sms = 0, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
+  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; int num_sms = 0, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
   // test hooks (rcvd_debug_factor_dense, rcvd_debug_linear_paths): whether a factorisation has run, per-kernel-path launch counters
   // (enqueue_factor_solve counts, graph replays add graph_paths)
@@ -265,7 +265,7 @@ static int upload_plan(rcvd_problem* p) {
   const FactorPlan& pl = p->plan; int rc;
   UP(p->d_blk_of, pl.blk_of); UP(p->d_hblocks, pl.hblocks); UP(p->d_lblocks, pl.lblocks); UP(p->d_lvl_frames, pl.lvl_frames); UP(p->d_lvl_own, pl.lvl_own);
   UP(p->d_own_lblocks, pl.own_lblocks); UP(p->d_own_hblocks, pl.own_hblocks); UP(p->d_uperm, pl.uperm);
-  UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_upd_tasks, pl.upd_tasks); UP(p->d_trsm_pairs, pl.trsm_pairs); UP(p->d_upd_pairs, pl.upd_pairs);
+  UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_trsm_pairs, pl.trsm_pairs); UP(p->d_upd_pairs, pl.upd_pairs);
   UP(p->d_sub_tasks, pl.sub_tasks); UP(p->d_sub_need, pl.sub_need); DA(p->d_sub_counters, (size_t)4 * p->N + 4);
   UP(p->d_fwd_tasks, pl.fwd_tasks); UP(p->d_trsm_ll, pl.trsm_ll); UP(p->d_upd_items, pl.upd_items);
   return RCVD_OK;
@@ -360,7 +360,7 @@ static int allocate_storage(rcvd_problem* p) {
 #undef DA
   {
     // 2-D TMA view of the T buffer (off-diagonal factor blocks X_rk, row-major): inner = k, outer = block * npad + row, box [rb][16], 128-B swizzle
-    p->tmap_ok = false;
+    bool encoded = false;
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
     void* fn = nullptr; cudaDriverEntryPointQueryResult qres;
@@ -371,11 +371,12 @@ static int allocate_storage(rcvd_problem* p) {
       const cuuint32_t estr[2] = {1u, 1u};
       const CUresult r = ((EncodeFn)fn)(&p->tmapT, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, p->d_T, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      p->tmap_ok = (r == CUDA_SUCCESS);
+      encoded = (r == CUDA_SUCCESS);
     }
     cudaGetLastError();
-    if (p->tmap_ok) { CK(cudaFuncSetAttribute(k_update_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->plan.upd_rb, 1))); CK(cudaFuncSetAttribute(k_update_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->plan.upd_rb, 2))); }
-    else if (p->gemm_tma) return set_err(RCVD_ERR_CUDA, "cuTensorMapEncodeTiled unavailable or failed: the TMA update kernel cannot run");
+    if (!encoded) return set_err(RCVD_ERR_CUDA, "cuTensorMapEncodeTiled unavailable or failed: the TMA update kernel cannot run");
+    CK(cudaFuncSetAttribute(k_update_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->plan.upd_rb, 1)));
+    CK(cudaFuncSetAttribute(k_update_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)upd_smem_bytes(p->plan.upd_rb, 2)));
   }
   CK(cudaMallocHost((void**)&p->h_scal, (SC_N + 2) * sizeof(double)));
   p->h_fail = (int*)(p->h_scal + SC_N);
@@ -455,191 +456,214 @@ static int grouped(rcvd_problem* p, double* base, size_t unit, const std::vector
 }
 
 // Enqueues factorisation of (S H S + D2) and the solve y = A^{-1} gs on p->stream.
-static int enqueue_factor_solve(rcvd_problem* p) {
-  const Layout& L = p->L; const int N = p->N, npad = L.npad; cudaStream_t st = p->stream;
-  const int nL = N + p->plan.nLoff;
-  const int tiles = (npad + 63) / 64;
-  enum { P_LOAD = 0, P_POTRF, P_TRINV, P_TRSM, P_GEMM, P_SOLVE };
+//
+// Two-stream schedule (fork/join inside the captured graph): the deferred update passes of level l (U2) run on `side` concurrently
+// with the later levels on `st`; the late passes (U1) of level Level::join are the first main-stream work that touches one of their
+// targets, and wait for them there (the side stream runs in order: one wait covers every earlier side launch).  The explicit
+// inverses run on a third stream, `inv`: on `side` they would hold back the next update launch by a k_trinv.
+struct FactorSolve {
+  enum { P_LOAD = 0, P_POTRF, P_TRINV, P_TRSM, P_GEMM, P_SOLVE };   // kernel classes of rcvd_debug_profile_linear
+  rcvd_problem* p; const FactorPlan& pl; const int N, npad, strips; cudaStream_t st, side, inv;
   int prof_level = 0;
-  auto mark = [&](int cls) {   // profiling mode only (single stream, not captured)
+  bool side_used = false, inv_used = false;   // work was enqueued on `side` / on `inv` since the main stream last waited for it
+  int side_joined = -1;                        // the main stream has waited for the side launches (2 * level + launch) up to this one
+
+  explicit FactorSolve(rcvd_problem* p_)
+      : p(p_), pl(p_->plan), N(p_->N), npad(p_->L.npad), strips((npad + kTrsmStrip - 1) / kTrsmStrip), st(p_->stream), side(p_->side_stream),
+        inv(p_->inv_stream) {}
+
+  void mark(int cls) {   // profiling mode only (single stream, not captured)
     if (!p->prof) return;
     cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); p->prof->push_back({cls < 0 ? cls : (cls | (prof_level << 8)), e});
-  };
-  const int neff = std::min(npad, (L.nf + 7) / 8 * 8);
-  auto gemm = [&](cudaStream_t cs, int ntasks, double* dstp, const double* A, const double* B, const GemmTask* tasks, const int2* prs, double alpha, double beta) {
-    // trimming applies to the update products only (beta != 0): the inverse-times-block TRSM of large blocks must write every padded row of T
-    k_gemm_nt<<<dim3(tiles, tiles, ntasks), 128, 0, cs>>>(dstp, A, B, tasks, prs, npad, beta != 0.0 ? neff : npad, alpha, beta);
-  };
-  mark(-1);
-  CK(cudaMemsetAsync(p->d_potrf_progress, 0, (size_t)N * sizeof(int), st));   // no count of the previous factorisation may read as published
-  k_load_factor<<<dim3((npad * npad + 255) / 256, p->plan.dist ? (int)p->plan.own_lblocks.size() : nL), 256, 0, st>>>(p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, L.nf, p->plan.dist ? p->d_own_lblocks : nullptr);
-  p->launches += 1; p->paths[LP_OTHER]++; mark(P_LOAD);
-  // Two-stream schedule (fork/join inside the captured graph): the deferred update passes of level l (U2) run on `side` concurrently
-  // with the later levels on `st`; the late passes (U1) of level Level::join are the first main-stream work that touches one of their
-  // targets, and wait for them there (the side stream runs in order: one wait covers every earlier side launch).  The explicit
-  // inverses run on a third stream, `inv`: on `side` they would hold back the next update launch by a k_trinv.
-  cudaStream_t side = p->side_stream, inv = p->inv_stream;
-  bool side_used = false, inv_used = false;
-  int side_joined = -1;   // the main stream has waited for the side launches (2 * level + launch) up to this one
-  auto join_inv = [&]() -> int {
-    if (inv_used) { CK(cudaEventRecord(p->ev_inv_join, inv)); CK(cudaStreamWaitEvent(st, p->ev_inv_join, 0)); inv_used = false; }
+  }
+  // Every kernel of the factorisation and the solve is launched here and counted in p->launches and p->paths[path].  pdl: a
+  // programmatic dependent launch, which may start before its predecessor on the stream ends (it waits with griddepcontrol.wait).
+  template <class... Params, class... Args>
+  int launch(int path, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
+    cudaLaunchAttribute attr = {};
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization; attr.val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = s; lc.attrs = &attr; lc.numAttrs = pdl ? 1 : 0;
+    CK(cudaLaunchKernelEx(&lc, kernel, args...));
+    p->launches += 1; p->paths[path]++;
     return RCVD_OK;
-  };
-  const size_t bsz = (size_t)npad * npad;
-  // phase boundary of the distributed factorisation: the owners' explicit inverses (for the replicated substitution) and their
-  // blocks of the trailing matrix go to everybody; from here on every rank factors the same narrow tail
-  auto phase_boundary = [&]() -> int {
-    if (side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); side_joined = 2 * p->plan.LB - 1; }
-    if (int rc = join_inv()) return rc;
-    std::vector<Seg> invs, tr;
-    for (int q = 0; q < p->nranks; ++q) invs.push_back({(size_t)p->plan.fa_off[q], (size_t)p->plan.fa_cnt[q]});
-    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)p->plan.fb_off[q], (size_t)p->plan.fb_cnt[q]});
-    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)N + (size_t)p->plan.bseg[2 * q], (size_t)p->plan.bseg[2 * q + 1]});
-    int rc = grouped(p, p->d_invL, bsz, invs, true); if (rc) return rc;
-    return grouped(p, p->d_Lb, bsz, tr, true);
-  };
-  // A level's TRSM launch that is a single wave (the narrow levels) is streamed behind its k_potrf_smem (see below).
-  const int strips = (npad + kTrsmStrip - 1) / kTrsmStrip;
-  auto trsm_deep = [&](const Level& v) { return strips * v.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024; };
-  auto streamed = [&](const Level& v) {
+  }
+  // `waiter` waits for the work enqueued on `from` so far
+  int wait(cudaStream_t waiter, cudaStream_t from, cudaEvent_t e) {
+    CK(cudaEventRecord(e, from)); CK(cudaStreamWaitEvent(waiter, e, 0));
+    return RCVD_OK;
+  }
+  // the main stream waits for `side` (every side launch of the levels before `level`) and `inv`
+  int join_all(int level) {
+    if (side_used) { if (int rc = wait(st, side, p->ev_join)) return rc; side_joined = 2 * level - 1; }
+    if (inv_used) { if (int rc = wait(st, inv, p->ev_inv_join)) return rc; inv_used = false; }
+    return RCVD_OK;
+  }
+
+  // A level's TRSM launch that is a single wave (the narrow levels) is streamed behind its k_potrf_smem (see trsm).
+  bool trsm_deep(const Level& v) const { return strips * v.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024; }
+  bool streamed(const Level& v) const {
     return p->use_trsm_ll && v.nown > 0 && v.ntrsm > 0 && potrf_smem_bytes(npad) <= 220 * 1024 &&
            strips * v.ntrsm <= (trsm_deep(v) ? 1 : p->trsm2_ctas_per_sm) * p->num_sms;
-  };
-  auto pdl_attr = [](cudaLaunchAttribute& a) { a.id = cudaLaunchAttributeProgrammaticStreamSerialization; a.val.programmaticStreamSerializationAllowed = 1; };
-  for (size_t li = 0; li < p->plan.levels.size(); ++li) {
-    const Level& lv = p->plan.levels[li]; prof_level = (int)li;
-    // On a streamed level the Cholesky is a programmatic dependent of the previous level's U1 (it waits for it with griddepcontrol.wait
-    // before it reads anything), so its CTAs are resident as soon as U1's SMs drain; and the previous level forked its U2 only after
-    // U1 (below).  Launched beside U1, U2's persistent CTAs (two per SM) took every SM that drained, and k_potrf_smem, which needs a
-    // whole SM, started 15-40 us after U1 had finished.
-    const bool chain = streamed(lv);
-    const bool fork_u2_late = p->overlap && p->gemm_tma && li + 1 < p->plan.levels.size() && streamed(p->plan.levels[li + 1]);
-    if (p->plan.dist && (int)li == p->plan.LB) { int rc = phase_boundary(); if (rc) return rc; }
-    const int* lframes = p->d_lvl_own + lv.own_off; const int nfr = lv.nown;      // the frames this rank factors at this level
-    if (nfr > 0) {
-    if (potrf_smem_bytes(npad) <= 220 * 1024) {
-      if (chain && li > 0) {
-        cudaLaunchAttribute attr[1]; pdl_attr(attr[0]);
-        cudaLaunchConfig_t lc = {};
-        lc.gridDim = dim3(nfr); lc.blockDim = dim3(kPotrfSmemThreads); lc.dynamicSmemBytes = potrf_smem_bytes(npad); lc.stream = st;
-        lc.attrs = attr; lc.numAttrs = 1;
-        CK(cudaLaunchKernelEx(&lc, k_potrf_smem, p->d_Lb, p->d_invT, lframes, npad, p->d_fail, p->d_potrf_progress));
-      } else {
-        k_potrf_smem<<<nfr, kPotrfSmemThreads, potrf_smem_bytes(npad), st>>>(p->d_Lb, p->d_invT, lframes, npad, p->d_fail, p->d_potrf_progress);
-      }
-      p->paths[LP_POTRF_SMEM]++;
-    } else {
-      // large blocks: 16-wide panels, panel factor on one CTA per frame, trailing update on the whole machine
-      const int nt16 = npad / 16;
-      for (int jb = 0; jb < nt16; ++jb) {
-        k_potrf_panel<<<nfr, kPotrfThreads, 0, st>>>(p->d_Lb, p->d_invT, lframes, npad, jb, p->d_fail);
-        p->launches += 1; p->paths[LP_POTRF_PANEL]++;
-        const int m = npad - (jb + 1) * 16;
-        if (m > 0) { const int n64 = (m + 63) / 64; k_potrf_trail<<<dim3(n64 * (n64 + 1) / 2, nfr), 128, 0, st>>>(p->d_Lb, lframes, npad, jb); p->launches += 1; p->paths[LP_OTHER]++; }
-      }
-      p->launches -= 1;   // (the common increment below)
+  }
+
+  // the Cholesky of the level's diagonal blocks
+  int factor_diagonal(const int* frames, int nfr, bool pdl) {
+    if (potrf_smem_bytes(npad) <= 220 * 1024)
+      return launch(LP_POTRF_SMEM, k_potrf_smem, dim3(nfr), dim3(kPotrfSmemThreads), potrf_smem_bytes(npad), st, pdl, p->d_Lb, p->d_invT, frames, npad,
+                    p->d_fail, p->d_potrf_progress);
+    // large blocks: 16-wide panels, panel factor on one CTA per frame, trailing update on the whole machine
+    for (int jb = 0; jb < npad / 16; ++jb) {
+      if (int rc = launch(LP_POTRF_PANEL, k_potrf_panel, dim3(nfr), dim3(kPotrfThreads), 0, st, false, p->d_Lb, p->d_invT, frames, npad, jb, p->d_fail)) return rc;
+      const int m = npad - (jb + 1) * 16, n64 = (m + 63) / 64;
+      if (m > 0) { if (int rc = launch(LP_OTHER, k_potrf_trail, dim3(n64 * (n64 + 1) / 2, nfr), dim3(128), 0, st, false, p->d_Lb, frames, npad, jb)) return rc; }
     }
-    p->launches += 1; mark(P_POTRF);
+    return RCVD_OK;
+  }
+
+  // the explicit inverses of the level's diagonal blocks, then the TRSM X_rk = A_rk L_kk^-T of its off-diagonal blocks
+  int trsm(const Level& lv, const int* frames, int nfr, bool chain) {
+    // k_trsm_ll does not read the explicit inverse, only the (much later) substitution does: compute it off the critical path
+    const bool inv_stream = p->use_trsm_ll && p->overlap;
+    if (inv_stream) { if (int rc = wait(inv, st, p->ev_fork)) return rc; inv_used = true; }
+    if (int rc = launch(LP_TRINV, k_trinv, dim3(npad / 16, nfr), dim3(256), (npad * 16 + 16 * (npad + 1)) * sizeof(double), inv_stream ? inv : st, false,
+                        p->d_Lb, p->d_invT, p->d_invL, frames, npad)) return rc;
+    mark(P_TRINV);
+    if (lv.ntrsm == 0) return RCVD_OK;
+    int rc;
     if (p->use_trsm_ll) {
-      // the explicit inverse is only needed by the (much later) substitution phase: compute it off the critical path
-      cudaStream_t is = st;
-      if (p->overlap) { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(inv, p->ev_fork, 0)); is = inv; inv_used = true; }
-      k_trinv<<<dim3(npad / 16, nfr), 256, (npad * 16 + 16 * (npad + 1)) * sizeof(double), is>>>(p->d_Lb, p->d_invT, p->d_invL, lframes, npad);
-      p->launches += 1; p->paths[LP_TRINV]++; mark(P_TRINV);
-      if (lv.ntrsm > 0) {
-        // one CTA per SM fits the launch in a single wave: deep panel prefetch (AHEAD = 4); otherwise two CTAs per SM (AHEAD = 2)
-        const bool deep = trsm_deep(lv);
-        const TrsmTask* tasks = p->d_trsm_ll + lv.trsm_off;
-        // A launch that is a single wave (the narrow levels) starts beside its level's k_potrf_smem as a programmatic dependent launch
-        // and follows the tile columns the Cholesky publishes.  The wide levels' multi-wave launches wait for the Cholesky to finish.
-        if (chain) {
-          cudaLaunchAttribute attr[1]; pdl_attr(attr[0]);
-          cudaLaunchConfig_t lc = {};
-          lc.gridDim = dim3(strips, lv.ntrsm); lc.blockDim = dim3(128); lc.dynamicSmemBytes = trsm_ll_smem_bytes(npad, deep ? 4 : 2); lc.stream = st;
-          lc.attrs = attr; lc.numAttrs = 1;
-          const double *Lb = p->d_Lb, *invT = p->d_invT; const int* progress = p->d_potrf_progress;
-          CK(deep ? cudaLaunchKernelEx(&lc, k_trsm_ll<4, true>, p->d_T, Lb, invT, tasks, npad, progress)
-                  : cudaLaunchKernelEx(&lc, k_trsm_ll<2, true>, p->d_T, Lb, invT, tasks, npad, progress));
-          p->paths[LP_TRSM_STREAMED]++;
-        } else if (deep) {
-          k_trsm_ll<4><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 4), st>>>(p->d_T, p->d_Lb, p->d_invT, tasks, npad, nullptr);
-        } else {
-          k_trsm_ll<2><<<dim3(strips, lv.ntrsm), 128, trsm_ll_smem_bytes(npad, 2), st>>>(p->d_T, p->d_Lb, p->d_invT, tasks, npad, nullptr);
-        }
-        p->paths[deep ? LP_TRSM_LL4 : LP_TRSM_LL2]++;
-        p->launches++; mark(P_TRSM);
-      }
+      // One CTA per SM fits the launch in a single wave: deep panel prefetch (AHEAD = 4); otherwise two CTAs per SM (AHEAD = 2).
+      // A launch that is a single wave (`chain`: the narrow levels) starts beside its level's k_potrf_smem as a programmatic dependent
+      // launch and follows the tile columns the Cholesky publishes.  The wide levels' multi-wave launches wait for the Cholesky to finish.
+      const bool deep = trsm_deep(lv);
+      decltype(&k_trsm_ll<2>) kernel = deep ? (chain ? k_trsm_ll<4, true> : k_trsm_ll<4>) : (chain ? k_trsm_ll<2, true> : k_trsm_ll<2>);
+      if (chain) p->paths[LP_TRSM_STREAMED]++;
+      rc = launch(deep ? LP_TRSM_LL4 : LP_TRSM_LL2, kernel, dim3(strips, lv.ntrsm), dim3(128), trsm_ll_smem_bytes(npad, deep ? 4 : 2), st, chain,
+                  p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad, chain ? p->d_potrf_progress : nullptr);
     } else {
-      k_trinv<<<dim3(npad / 16, nfr), 256, (npad * 16 + 16 * (npad + 1)) * sizeof(double), st>>>(p->d_Lb, p->d_invT, p->d_invL, lframes, npad);
-      p->launches += 1; p->paths[LP_TRINV]++; mark(P_TRINV);
-      if (lv.ntrsm > 0) { gemm(st, lv.ntrsm, p->d_T, p->d_Lb, p->d_invL, p->d_trsm_tasks + lv.trsm_off, p->d_trsm_pairs, 1.0, 0.0); p->launches++; p->paths[LP_TRSM_GEMM]++; mark(P_TRSM); }
+      const int tiles = (npad + 63) / 64;
+      rc = launch(LP_TRSM_GEMM, k_gemm_nt, dim3(tiles, tiles, lv.ntrsm), dim3(128), 0, st, false, p->d_T, p->d_Lb, p->d_invL,
+                  p->d_trsm_tasks + lv.trsm_off, p->d_trsm_pairs, npad);
     }
-    }
-    if (p->plan.dist && (int)li < p->plan.LB) {
-      // the off-diagonal factor blocks of this level, from their owners to everybody (one fused NCCL launch)
-      std::vector<Seg> segs;
-      for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)p->plan.tseg[(li * p->nranks + q) * 2], (size_t)p->plan.tseg[(li * p->nranks + q) * 2 + 1]});
-      int rc = grouped(p, p->d_T, bsz, segs, true); if (rc) return rc;
-    }
-    auto fork_u2 = [&]() -> int { CK(cudaEventRecord(p->ev_fork, st)); CK(cudaStreamWaitEvent(side, p->ev_fork, 0)); return RCVD_OK; };
-    if (lv.nupd2[0] + lv.nupd2[1] > 0 && p->overlap && !fork_u2_late) { if (int rc = fork_u2()) return rc; }
+    if (rc) return rc;
+    mark(P_TRSM);
+    return RCVD_OK;
+  }
+
+  // the persistent TMA-fed update kernel over the items [off, off + n)
+  int update(cudaStream_t s, int off, int n) {
+    if (n <= p->num_sms)   // few items: two DMMA teams per tile, one CTA per SM
+      return launch(LP_UPD_TMA2, k_update_tma<2>, dim3(n), dim3(UpdShape<2>::threads), upd_smem_bytes(pl.upd_rb, 2), s, false,
+                    p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, pl.upd_neff, pl.upd_rb, 0);
+    int grid = std::min(n, 2 * p->num_sms);
+    if (p->upd_ipc > 0) grid = std::max(grid, (n + p->upd_ipc - 1) / p->upd_ipc);
+    if (grid < n) p->paths[LP_UPD_TMA1_MULTI]++;
+    return launch(LP_UPD_TMA1, k_update_tma<1>, dim3(grid), dim3(UpdShape<1>::threads), upd_smem_bytes(pl.upd_rb, 1), s, false,
+                  p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, pl.upd_neff, pl.upd_rb, 0);
+  }
+
+  // The update passes of level li: after the waits for the earlier levels' U2 launches it needs, U1 on the main stream, then the
+  // two U2 launches (on `side` when overlapping)
+  int updates(int li) {
+    const Level& lv = pl.levels[li];
+    const bool u2 = lv.nit2[0] + lv.nit2[1] > 0;
+    // Before a streamed level U2 forks only after U1: launched beside U1, U2's persistent CTAs (two per SM) took every SM that drained,
+    // and the next level's k_potrf_smem, which needs a whole SM, started 15-40 us after U1 had finished.
+    const bool fork_late = li + 1 < (int)pl.levels.size() && streamed(pl.levels[li + 1]);
+    if (p->overlap && u2 && !fork_late) { if (int rc = wait(side, st, p->ev_fork)) return rc; }
     if (p->overlap) {   // U2 launch s of level q before U1(join[s] of q)
       int s = -1;
-      for (int q = side_joined + 1; q < 2 * (int)li; ++q) { const Level& v = p->plan.levels[q / 2]; if (v.nupd2[q % 2] > 0 && v.join[q % 2] <= (int)li) s = q; }
+      for (int q = side_joined + 1; q < 2 * li; ++q) { const Level& v = pl.levels[q / 2]; if (v.nit2[q % 2] > 0 && v.join[q % 2] <= li) s = q; }
       if (s >= 0) { CK(cudaStreamWaitEvent(st, p->ev_side[s], 0)); side_joined = s; }
     }
-    auto update = [&](cudaStream_t cs, int off, int n) {   // persistent TMA-fed update kernel
-      if (n <= p->num_sms) {   // few items: two DMMA teams per tile, one CTA per SM
-        k_update_tma<2><<<n, UpdShape<2>::threads, upd_smem_bytes(p->plan.upd_rb, 2), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->plan.upd_neff, p->plan.upd_rb, 0);
-        p->paths[LP_UPD_TMA2]++;
-      } else {
-        int grid = std::min(n, 2 * p->num_sms);
-        if (p->upd_ipc > 0) grid = std::max(grid, (n + p->upd_ipc - 1) / p->upd_ipc);
-        k_update_tma<1><<<grid, UpdShape<1>::threads, upd_smem_bytes(p->plan.upd_rb, 1), cs>>>(p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, p->plan.upd_neff, p->plan.upd_rb, 0);
-        p->paths[LP_UPD_TMA1]++; if (grid < n) p->paths[LP_UPD_TMA1_MULTI]++;
-      }
-    };
-    if (p->gemm_tma) {
-      if (lv.nit > 0) { update(st, lv.it_off, lv.nit); p->launches++; mark(P_GEMM); }
-      if (fork_u2_late && lv.nit2[0] + lv.nit2[1] > 0) { if (int rc = fork_u2()) return rc; }   // after U1
-      for (int h = 0; h < 2; ++h) if (lv.nit2[h] > 0) {
-        update(p->overlap ? side : st, lv.it2_off[h], lv.nit2[h]); p->launches++; mark(P_GEMM);
-        if (p->overlap) { CK(cudaEventRecord(p->ev_side[2 * li + h], side)); side_used = true; }
-      }
-      continue;
-    }
-    if (lv.nupd > 0) { gemm(st, lv.nupd, p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd_off, p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM); }
-    for (int h = 0; h < 2; ++h) if (lv.nupd2[h] > 0) {
-      gemm(p->overlap ? side : st, lv.nupd2[h], p->d_Lb, p->d_T, p->d_T, p->d_upd_tasks + lv.upd2_off[h], p->d_upd_pairs, -1.0, 1.0); p->launches++; p->paths[LP_UPD_GEMM]++; mark(P_GEMM);
+    if (lv.nit > 0) { if (int rc = update(st, lv.it_off, lv.nit)) return rc; mark(P_GEMM); }
+    if (p->overlap && u2 && fork_late) { if (int rc = wait(side, st, p->ev_fork)) return rc; }
+    for (int h = 0; h < 2; ++h) if (lv.nit2[h] > 0) {
+      if (int rc = update(p->overlap ? side : st, lv.it2_off[h], lv.nit2[h])) return rc;
+      mark(P_GEMM);
       if (p->overlap) { CK(cudaEventRecord(p->ev_side[2 * li + h], side)); side_used = true; }
     }
+    return RCVD_OK;
   }
-  if (p->plan.dist && p->plan.LB >= (int)p->plan.levels.size()) { int rc = phase_boundary(); if (rc) return rc; }
-  if (side_used) { CK(cudaEventRecord(p->ev_join, side)); CK(cudaStreamWaitEvent(st, p->ev_join, 0)); }
-  if (int rc = join_inv()) return rc;
-  CK(cudaMemcpyAsync(p->d_rhs, p->d_gs, (size_t)N * npad * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  const int nlv = (int)p->plan.levels.size();
-  const int LS = p->plan.sub_first_level;       // levels >= LS: the persistent dataflow kernel (rcvd_linalg.cuh, k_substitution)
-  for (int l = 0; l < LS; ++l) {
-    const Level& lv = p->plan.levels[l];
-    k_fwd_diag<<<dim3((npad + 7) / 8, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_rhs, p->d_ytmp, p->d_lvl_frames + lv.frame_off, npad);
-    p->launches++; p->paths[LP_SUB_LEVEL]++;
-    if (lv.nfwd > 0) { k_fwd_update<<<dim3((npad + 7) / 8, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_ytmp, p->d_rhs, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; p->paths[LP_SUB_LEVEL]++; }
+
+  // distributed factorisation, levels < LB: the level's off-diagonal factor blocks from their owners to everybody (one fused NCCL launch)
+  int broadcast_level(int li) {
+    std::vector<Seg> segs;
+    for (int q = 0; q < p->nranks; ++q) segs.push_back({(size_t)pl.tseg[(li * p->nranks + q) * 2], (size_t)pl.tseg[(li * p->nranks + q) * 2 + 1]});
+    return grouped(p, p->d_T, (size_t)npad * npad, segs, true);
   }
-  if (LS < nlv && !p->plan.sub_tasks.empty()) {
-    CK(cudaMemsetAsync(p->d_sub_counters, 0, ((size_t)4 * N + 4) * sizeof(int), st));
-    SubCounters cn; cn.ticket = p->d_sub_counters; cn.fin = p->d_sub_counters + 4; cn.fdone = cn.fin + N; cn.bin = cn.fdone + N; cn.bdone = cn.bin + N;
-    cn.fin_need = p->d_sub_need; cn.bin_need = p->d_sub_need + N;
-    k_substitution<<<std::min((int)p->plan.sub_tasks.size(), p->num_sms), kSubThreads, substitution_smem_bytes(npad), st>>>(p->d_invL, p->d_T, p->d_rhs, p->d_ytmp, p->d_y, p->d_sub_tasks, (int)p->plan.sub_tasks.size(), cn, npad);
-    p->launches++; p->paths[LP_SUB_FUSED]++;
+  // phase boundary of the distributed factorisation: the owners' explicit inverses (for the replicated substitution) and their
+  // blocks of the trailing matrix go to everybody; from here on every rank factors the same narrow tail
+  int phase_boundary() {
+    if (int rc = join_all(pl.LB)) return rc;
+    const size_t bsz = (size_t)npad * npad;
+    std::vector<Seg> invs, tr;
+    for (int q = 0; q < p->nranks; ++q) invs.push_back({(size_t)pl.fa_off[q], (size_t)pl.fa_cnt[q]});
+    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)pl.fb_off[q], (size_t)pl.fb_cnt[q]});
+    for (int q = 0; q < p->nranks; ++q) tr.push_back({(size_t)N + (size_t)pl.bseg[2 * q], (size_t)pl.bseg[2 * q + 1]});
+    if (int rc = grouped(p, p->d_invL, bsz, invs, true)) return rc;
+    return grouped(p, p->d_Lb, bsz, tr, true);
   }
-  for (int l = LS - 1; l >= 0; --l) {
-    const Level& lv = p->plan.levels[l];
-    if (lv.nfwd > 0) { k_bwd_update<<<dim3((npad + 31) / 32, lv.nfwd), 256, 0, st>>>(p->d_T, p->d_y, p->d_ytmp, p->d_fwd_tasks + lv.fwd_off, npad); p->launches++; p->paths[LP_SUB_LEVEL]++; }
-    k_bwd_diag<<<dim3((npad + 31) / 32, lv.nframes), 256, 0, st>>>(p->d_invL, p->d_ytmp, p->d_y, p->d_lvl_frames + lv.frame_off, npad);
-    p->launches += 1; p->paths[LP_SUB_LEVEL]++;
+
+  // y = A^{-1} gs by GEMVs with the explicit inverses: the wide levels level by level, the levels >= sub_first_level in the persistent
+  // dataflow kernel (rcvd_linalg.cuh, k_substitution)
+  int substitution() {
+    CK(cudaMemcpyAsync(p->d_rhs, p->d_gs, (size_t)N * npad * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    const int LS = pl.sub_first_level;
+    int rc;
+    for (int l = 0; l < LS; ++l) {
+      const Level& lv = pl.levels[l];
+      if ((rc = launch(LP_SUB_LEVEL, k_fwd_diag, dim3((npad + 7) / 8, lv.nframes), dim3(256), 0, st, false, p->d_invL, p->d_rhs, p->d_ytmp,
+                       p->d_lvl_frames + lv.frame_off, npad))) return rc;
+      if (lv.nfwd > 0 && (rc = launch(LP_SUB_LEVEL, k_fwd_update, dim3((npad + 7) / 8, lv.nfwd), dim3(256), 0, st, false, p->d_T, p->d_ytmp, p->d_rhs,
+                                      p->d_fwd_tasks + lv.fwd_off, npad))) return rc;
+    }
+    if (LS < (int)pl.levels.size() && !pl.sub_tasks.empty()) {
+      CK(cudaMemsetAsync(p->d_sub_counters, 0, ((size_t)4 * N + 4) * sizeof(int), st));
+      SubCounters cn; cn.ticket = p->d_sub_counters; cn.fin = p->d_sub_counters + 4; cn.fdone = cn.fin + N; cn.bin = cn.fdone + N; cn.bdone = cn.bin + N;
+      cn.fin_need = p->d_sub_need; cn.bin_need = p->d_sub_need + N;
+      const int ntasks = (int)pl.sub_tasks.size();
+      if ((rc = launch(LP_SUB_FUSED, k_substitution, dim3(std::min(ntasks, p->num_sms)), dim3(kSubThreads), substitution_smem_bytes(npad), st, false,
+                       p->d_invL, p->d_T, p->d_rhs, p->d_ytmp, p->d_y, p->d_sub_tasks, ntasks, cn, npad))) return rc;
+    }
+    for (int l = LS - 1; l >= 0; --l) {
+      const Level& lv = pl.levels[l];
+      if (lv.nfwd > 0 && (rc = launch(LP_SUB_LEVEL, k_bwd_update, dim3((npad + 31) / 32, lv.nfwd), dim3(256), 0, st, false, p->d_T, p->d_y, p->d_ytmp,
+                                      p->d_fwd_tasks + lv.fwd_off, npad))) return rc;
+      if ((rc = launch(LP_SUB_LEVEL, k_bwd_diag, dim3((npad + 31) / 32, lv.nframes), dim3(256), 0, st, false, p->d_invL, p->d_ytmp, p->d_y,
+                       p->d_lvl_frames + lv.frame_off, npad))) return rc;
+    }
+    mark(P_SOLVE);
+    return RCVD_OK;
   }
-  mark(P_SOLVE);
+};
+
+static int enqueue_factor_solve(rcvd_problem* p) {
+  FactorSolve f(p);
+  const FactorPlan& pl = p->plan; const int npad = p->L.npad, nlv = (int)pl.levels.size();
+  f.mark(-1);
+  CK(cudaMemsetAsync(p->d_potrf_progress, 0, (size_t)p->N * sizeof(int), p->stream));   // no count of the previous factorisation may read as published
+  if (int rc = f.launch(LP_OTHER, k_load_factor, dim3((npad * npad + 255) / 256, pl.dist ? (int)pl.own_lblocks.size() : p->N + pl.nLoff), dim3(256), 0,
+                        p->stream, false, p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, p->L.nf, pl.dist ? p->d_own_lblocks : nullptr)) return rc;
+  f.mark(FactorSolve::P_LOAD);
+  for (int li = 0; li < nlv; ++li) {
+    const Level& lv = pl.levels[li]; f.prof_level = li;
+    if (pl.dist && li == pl.LB) { if (int rc = f.phase_boundary()) return rc; }
+    if (lv.nown > 0) {
+      const int* frames = p->d_lvl_own + lv.own_off;      // the frames this rank factors at this level
+      // On a streamed level the Cholesky is a programmatic dependent of the previous level's U1 (it waits for it with griddepcontrol.wait
+      // before it reads anything), so its CTAs are resident as soon as U1's SMs drain; the previous level forked its U2 only after U1.
+      const bool chain = f.streamed(lv);
+      if (int rc = f.factor_diagonal(frames, lv.nown, chain && li > 0)) return rc;
+      f.mark(FactorSolve::P_POTRF);
+      if (int rc = f.trsm(lv, frames, lv.nown, chain)) return rc;
+    }
+    if (pl.dist && li < pl.LB) { if (int rc = f.broadcast_level(li)) return rc; }
+    if (int rc = f.updates(li)) return rc;
+  }
+  if (pl.dist && pl.LB >= nlv) { if (int rc = f.phase_boundary()) return rc; }
+  if (int rc = f.join_all(nlv)) return rc;
+  if (int rc = f.substitution()) return rc;
   CK(cudaGetLastError());
   return RCVD_OK;
 }
@@ -1276,9 +1300,9 @@ RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double
   }
   return RCVD_OK;
 }
-RCVD_API int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[14]) {
+RCVD_API int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]) {
   if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
-  static_assert(LP_N == 14, "include/rcvd_hooks.h documents fourteen counters");
+  static_assert(LP_N == 13, "include/rcvd_hooks.h documents thirteen counters");
   std::copy(p->paths, p->paths + LP_N, out);
   return RCVD_OK;
 }
@@ -1334,8 +1358,8 @@ RCVD_API int32_t rcvd_debug_last_iteration(rcvd_problem* p, double* g, double* x
   return download_frames(p, xc, p->d_xc, p->L.nf, p->L.nf, p->L.nf);
 }
 // Bench hook: one factorisation + solve, un-captured on a single stream with one CUDA event per launch; returns the
-// summed device time per kernel class: out_ms[0..5] = load, potrf, trinv, trsm, update GEMM (k_gemm_nt), substitution;
-// out_ms[6] = number of k_gemm_nt update launches, out_ms[7] = algorithmic flops of those GEMMs.
+// summed device time per kernel class: out_ms[0..5] = load, potrf, trinv, trsm, update GEMM (k_update_tma), substitution;
+// out_ms[6] = number of k_update_tma launches, out_ms[7] = algorithmic flops of those GEMMs.
 // reps < 0: keep the two-stream overlap (events on the main stream only: side-stream classes read ~0 and every wait for
 // the side stream is charged to the next main-stream launch) -- shows where the chain is delayed by the overlapped work.
 RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double out_ms[8]) {
@@ -1471,13 +1495,13 @@ RCVD_API int64_t rcvd_launch_count(rcvd_problem* p) { return p ? p->launches : 0
 RCVD_API int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack) { if (!p) return RCVD_ERR_INVALID; p->order_slack = slack; p->structure_ready = false; return RCVD_OK; }
 // Test / bench hook: 0 = single-stream factorisation graph, 1 (default) = overlap non-critical updates on a second stream.
 RCVD_API int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->overlap = on != 0; if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; } return RCVD_OK; }
-// Test / bench hook: 1 (default) = persistent TMA-fed update kernel (k_update_tma), 0 = cp.async tile kernel (k_gemm_nt).
-// side_items_per_cta > 0 caps the items per CTA of the one-team update launches (a larger grid); 0 (default) = no cap.
+// Test / bench hook: side_items_per_cta > 0 caps the items per CTA of the one-team update launches (a larger grid); 0 (default) = no cap.
+// tma must be 1: the persistent TMA-fed kernel (k_update_tma) is the only update kernel.
 RCVD_API int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta) {
   if (!p) return RCVD_ERR_INVALID;
-  p->gemm_tma = tma != 0; p->upd_ipc = side_items_per_cta;
+  if (!tma) return set_err(RCVD_ERR_INVALID, "the cp.async update path was removed: k_update_tma is the only update kernel");
+  p->upd_ipc = side_items_per_cta;
   if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; }
-  if (p->gemm_tma && !p->tmap_ok) p->structure_ready = false;
   return RCVD_OK;
 }
 // Test / bench hook (nranks > 1): 1 (default) = distributed factorisation (owner-computes phase A, reduce-to-owner of H), 0 = replicated scheme

@@ -7,7 +7,8 @@
 // the numeric work runs as batched per-level kernels:
 //   k_potrf   (one CTA per diagonal block)      L_kk, plus 16x16 diagonal-tile inverses
 //   k_trinv   (one CTA per 16-column panel)     inv(L_kk)
-//   k_gemm_nt (fp64 tensor-core DMMA, 64x64)    X_rk = A_rk inv(L_kk)^T ;  A_rc -= X_rk X_ck^T
+//   k_gemm_nt (fp64 tensor-core DMMA, 64x64)    X_rk = A_rk inv(L_kk)^T  (large blocks; k_trsm_ll below otherwise)
+//   k_update_tma (rcvd_update.cuh)              A_rc -= X_rk X_ck^T
 // and the triangular solves become GEMVs with inv(L_kk).
 #pragma once
 #include "rcvd_device.cuh"
@@ -430,14 +431,13 @@ __global__ void __launch_bounds__(256) k_trinv(const double* __restrict__ Lb, co
 }
 
 // ---------------------------------------------------------------------------
-// k_gemm_nt: dst[t.dst] = beta*dst + alpha * sum_p A[pairs[p].x] * B[pairs[p].y]^T
+// k_gemm_nt: the TRSM of the large-block path (npad > 416, where a k_trsm_ll strip no longer fits in shared memory),
+// dst[t.dst] = sum_p A[pairs[p].x] * B[pairs[p].y]^T with B = inv(L_kk) lower triangular.
 // fp64 tensor cores (mma.sync m8n8k4 -> DMMA), CTA tile 64x64, 4 warps of 32x32,
-// K staged 16 at a time through a cp.async double buffer.
+// K staged 16 at a time through a cp.async double buffer.  The short last tile row is cheap because out-of-range mma tiles
+// are never issued.
 // ---------------------------------------------------------------------------
-// Measured alternatives that lost at npad = 208 (config 2, 91 update launches, 133.7 GFLOP algorithmic): 96x96 CTA tiles with
-// 3x3-unit warp tiles (250 registers, 2 CTAs/SM): 12.8 TFLOP/s; balanced <=64-row chunks (3,3,3,4 units): 16.1 TFLOP/s;
-// this kernel: 16.7 TFLOP/s.  The short last tile row is cheap because out-of-range mma tiles are never issued.
-struct GemmTask { int dst; int first; int count; int lower_only; };   // lower_only bit0: symmetric target (skip tiles above the diagonal); bit1: B is lower triangular
+struct GemmTask { int dst; int first; int count; int lower_only; };   // lower_only bit0: symmetric update target (tiles above the diagonal are never read)
 
 constexpr int kGemmLd = 20;   // padded leading dimension of the 64x16 smem tiles (conflict-free DMMA fragment loads)
 
@@ -462,10 +462,10 @@ __device__ __forceinline__ void dmma_16x8x4(double& c0, double& c1, double& c2, 
 
 // One 16-deep K stage of a warp's (NI*8) x (NJ*8) sub-tile: NI/NJ are compile-time so that no tensor instruction is predicated
 // (a predicated mma.sync costs a WARPSYNC + branch pair each).
-template <int NI, int NJ, int K4 = 4>
+template <int NI, int NJ>
 __device__ __forceinline__ void gemm_stage(const double* __restrict__ as, const double* __restrict__ bsm, double (&acc)[4][4][2], int wm, int wn, int g, int t) {
 #pragma unroll
-  for (int k4 = 0; k4 < K4; ++k4) {
+  for (int k4 = 0; k4 < 4; ++k4) {
     double af[NI > 0 ? NI : 1], bf[NJ > 0 ? NJ : 1];
 #pragma unroll
     for (int i = 0; i < NI; ++i) af[i] = as[(wm + i * 8 + g) * kGemmLd + k4 * 4 + t];
@@ -479,26 +479,20 @@ __device__ __forceinline__ void gemm_stage(const double* __restrict__ as, const 
 }
 
 __global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, const double* __restrict__ Abase, const double* __restrict__ Bbase,
-                                                  const GemmTask* __restrict__ tasks, const int2* __restrict__ pairs,
-                                                  int npad, int neff, double alpha, double beta) {
-  // neff = per-frame unknowns rounded up to 8 (<= npad): rows / columns / K beyond it are exact zeros in every operand
-  // (padding of the factor blocks), so their mma tiles and the tail K steps are never issued (199 -> 200 of 208: -11 % DMMA)
+                                                  const GemmTask* __restrict__ tasks, const int2* __restrict__ pairs, int npad) {
   __shared__ __align__(16) double As[2][64 * kGemmLd];
   __shared__ __align__(16) double Bs[2][64 * kGemmLd];
   const GemmTask task = tasks[blockIdx.z];
   const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
-  if ((task.lower_only & 1) && n0 > m0) return;   // symmetric target: tiles strictly above the diagonal are never read
   const size_t bs = (size_t)npad * npad;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wm = (warp >> 1) * 32, wn = (warp & 1) * 32;
   const int g = lane >> 2, t = lane & 3;
   // B lower triangular (inv(L_kk)): B[n][k] = 0 for k > n, so only K chunks up to this tile's last column matter
-  const int kchunks = (task.lower_only & 2) ? min(npad, n0 + 64) / 16 : npad / 16;
+  const int kchunks = min(npad, n0 + 64) / 16;
   const int total = task.count * kchunks;
-  // 8-row / 8-column mma tiles of this warp that lie inside the matrix (npad is a multiple of 16, tiles are 64)
-  const int ni = min(4, max(0, (neff - (m0 + wm)) / 8)), nj = min(4, max(0, (neff - (n0 + wn)) / 8));
-  const int lastk = (task.lower_only & 2) ? -1 : kchunks - 1;          // K chunk that holds the tail of neff
-  const int tailk4 = (neff - 16 * (npad / 16 - 1) + 3) / 4;            // 1..4 valid 4-deep K steps in that chunk
+  // 8-row / 8-column mma tiles of this warp that lie inside the matrix (npad is a multiple of 16, tiles are 64 -> ni, nj in {0, 2, 4})
+  const int ni = min(4, max(0, (npad - (m0 + wm)) / 8)), nj = min(4, max(0, (npad - (n0 + wn)) / 8));
   double acc[4][4][2];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -527,34 +521,23 @@ __global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, co
     if (kk + 1 < total) { load_stage(st ^ 1, kk + 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
     __syncthreads();
     const double* as = As[st]; const double* bsm = Bs[st];
-    // warp-uniform dispatch on the number of in-range 8-wide mma tiles (npad is a multiple of 16 -> ni, nj in {0, 2, 4})
-    const bool tail = (kk % kchunks) == lastk && tailk4 == 2;       // neff = 8 (mod 16): only two K steps of the last chunk are non-zero
-#define RCVD_GS(NI_, NJ_) case NI_ * 8 + NJ_: if (tail) gemm_stage<NI_, NJ_, 2>(as, bsm, acc, wm, wn, g, t); else gemm_stage<NI_, NJ_, 4>(as, bsm, acc, wm, wn, g, t); break;
-    if (ni == 4 && nj == 4 && !tail) gemm_stage<4, 4, 4>(as, bsm, acc, wm, wn, g, t);   // interior tiles: the hot path, tested first
-    else switch (ni * 8 + nj) {
-      RCVD_GS(4, 4) RCVD_GS(4, 3) RCVD_GS(4, 2) RCVD_GS(4, 1)
-      RCVD_GS(3, 4) RCVD_GS(3, 3) RCVD_GS(3, 2) RCVD_GS(3, 1)
-      RCVD_GS(2, 4) RCVD_GS(2, 3) RCVD_GS(2, 2) RCVD_GS(2, 1)
-      RCVD_GS(1, 4) RCVD_GS(1, 3) RCVD_GS(1, 2) RCVD_GS(1, 1)
-      default: break;
-    }
-#undef RCVD_GS
+    // warp-uniform dispatch on the number of in-range 8-wide mma tiles; interior tiles, the hot path, are tested first
+    if (ni == 4 && nj == 4) gemm_stage<4, 4>(as, bsm, acc, wm, wn, g, t);
+    else if (ni == 4 && nj == 2) gemm_stage<4, 2>(as, bsm, acc, wm, wn, g, t);
+    else if (ni == 2 && nj == 4) gemm_stage<2, 4>(as, bsm, acc, wm, wn, g, t);
+    else if (ni == 2 && nj == 2) gemm_stage<2, 2>(as, bsm, acc, wm, wn, g, t);
     __syncthreads();
   }
   double* C = dst + (size_t)task.dst * bs;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int row = m0 + wm + i * 8 + g;
-    if (row >= neff) continue;
+    if (row >= npad) continue;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int col = n0 + wn + j * 8 + 2 * t;
-      if (col >= neff) continue;
-      double2* ptr = reinterpret_cast<double2*>(C + (size_t)row * npad + col);
-      double2 o;
-      if (beta != 0.0) { o = *ptr; o.x = beta * o.x + alpha * acc[i][j][0]; o.y = beta * o.y + alpha * acc[i][j][1]; }
-      else { o.x = alpha * acc[i][j][0]; o.y = alpha * acc[i][j][1]; }
-      *ptr = o;
+      if (col >= npad) continue;
+      *reinterpret_cast<double2*>(C + (size_t)row * npad + col) = make_double2(acc[i][j][0], acc[i][j][1]);
     }
   }
 }

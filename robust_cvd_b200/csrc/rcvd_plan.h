@@ -244,7 +244,7 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
       for (int r : cs[k]) {
         const int id = lid[{r, k}];
         if (mine) {
-          P.trsm_tasks.push_back({id - N, (int)P.trsm_pairs.size(), 1, 2});
+          P.trsm_tasks.push_back({id - N, (int)P.trsm_pairs.size(), 1, 0});
           P.trsm_pairs.push_back(make_int2(id, k));
           P.trsm_ll.push_back({id - N, id, k});
         }

@@ -189,8 +189,7 @@ class Problem:
         _check(self.L.rcvd_debug_factor_dense(self.h, _p(order, C.c_int32), _p(Lf, C.c_double), _p(Li, C.c_double)))
         return order, Lf, Li
 
-    LINEAR_PATHS = ("potrf_smem", "potrf_panel", "trsm_ll4", "trsm_ll2", "trsm_gemm", "update_tma1", "update_tma2", "update_gemm",
-                    "substitution_levels", "substitution_fused", "trinv", "other", "update_tma1_multi_item", "trsm_ll_streamed")
+    LINEAR_PATHS = ("potrf_smem", "potrf_panel", "trsm_ll4", "trsm_ll2", "trsm_gemm", "update_tma1", "update_tma2", "substitution_levels", "substitution_fused", "trinv", "other", "update_tma1_multi_item", "trsm_ll_streamed")
 
     def linear_paths(self):
         """Test hook: launches of each factorisation / solve kernel path since the handle was created (LINEAR_PATHS)."""
@@ -245,8 +244,8 @@ class Problem:
         _check(self.L.rcvd_debug_set_fast_path(self.h, C.c_int32(int(on))))
 
     def set_update_kernel(self, tma=True, side_items_per_cta=0):
-        """Test / bench hook: persistent TMA-fed update kernel (default) or the cp.async kernel; side_items_per_cta > 0 caps the
-        work items per CTA of the one-team update launches."""
+        """Test / bench hook: side_items_per_cta > 0 caps the work items per CTA of the one-team update launches.  tma must be True:
+        the persistent TMA-fed kernel is the only update kernel (False raises)."""
         _check(self.L.rcvd_debug_set_update_kernel(self.h, C.c_int32(1 if tma else 0), C.c_int32(side_items_per_cta)))
 
     def set_eval_only(self, on=True):

@@ -123,7 +123,7 @@ def test_entry_outside_the_frame_graph_is_refused():
 UPDATE_NF = {40: 37, 104: 104, 136: 133, 48: 48}
 
 
-UPDATE_CASES = [("chain", "tma"), ("chain", "gemm"), ("complete", "tma"), ("complete", "items_per_cta_1"), ("complete", "gemm")]
+UPDATE_CASES = [("chain", "tma"), ("complete", "tma"), ("complete", "items_per_cta_1")]
 
 
 @pytest.mark.parametrize("graph,variant", UPDATE_CASES, ids=[f"{g}-{v}" for g, v in UPDATE_CASES])
@@ -132,25 +132,23 @@ def test_update_shapes(neff, graph, variant):
     """A chain has a few update items per level (k_update_tma<2>).  A complete graph puts every pair of the remaining frames into level
     0's side-stream launch: K_25 at one 80-row tile per block (neff <= 80) has 276 items, K_14 at 2 x 2 tiles 300, more than the
     2 x 132 CTAs of a k_update_tma<1> launch on an H100, so CTAs walk several items; capping at one item per CTA widens the grid
-    instead.  The cp.async kernel k_gemm_nt runs the same updates."""
+    instead."""
     nf = UPDATE_NF[neff]
     n = 6 if graph == "chain" else (14 if neff > 80 else 25)
     pairs = R.GRAPHS[graph](n)
     P = _problem(nf, n, pairs)
+    with pytest.raises(RuntimeError, match="cp.async update path was removed"):
+        P.set_update_kernel(False)
     if variant == "items_per_cta_1":
         P.set_update_kernel(True, 1)
-    elif variant == "gemm":
-        P.set_update_kernel(False)
     _well(P, n, nf, pairs, seed=neff, tag=f"update-{graph}-{variant}")
     p = P.linear_paths()
-    if variant == "gemm":
-        assert p["update_gemm"] > 0 and p["update_tma1"] == 0 and p["update_tma2"] == 0
-    elif graph == "chain":
-        assert p["update_tma2"] > 0 and p["update_tma1"] == 0 and p["update_gemm"] == 0
+    if graph == "chain":
+        assert p["update_tma2"] > 0 and p["update_tma1"] == 0
     elif variant == "tma":
-        assert p["update_tma1_multi_item"] > 0 and p["update_gemm"] == 0
+        assert p["update_tma1_multi_item"] > 0
     else:
-        assert p["update_tma1"] > 0 and p["update_tma1_multi_item"] == 0 and p["update_gemm"] == 0
+        assert p["update_tma1"] > 0 and p["update_tma1_multi_item"] == 0
 
 
 # ---------------------------------------------------------------------------------------------------------
