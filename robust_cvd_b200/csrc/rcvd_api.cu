@@ -222,6 +222,19 @@ struct rcvd_problem {
   rcvd_problem() {}
 };
 
+// Every kernel this file runs for a handle is launched here: the launch is checked and counted in p->launches (rcvd_launch_count).
+// pdl: a programmatic dependent launch, which may start before its predecessor on the stream ends (it waits with griddepcontrol.wait).
+template <class... Params, class... Args>
+static int launch(rcvd_problem* p, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
+  cudaLaunchAttribute attr = {};
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization; attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t lc = {};
+  lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = s; lc.attrs = &attr; lc.numAttrs = pdl ? 1 : 0;
+  CK(cudaLaunchKernelEx(&lc, kernel, args...));
+  p->launches += 1;
+  return RCVD_OK;
+}
+
 template <class T> static int dalloc(rcvd_problem* p, T** ptr, size_t count) {
   *ptr = nullptr;
   if (count == 0) count = 1;
@@ -294,12 +307,12 @@ static int set_up_problem_data(rcvd_problem* p) {
     int rcs;
     if ((rcs = dalloc(p, &d_k0, (size_t)n)) || (rcs = dalloc(p, &d_k1, (size_t)n)) || (rcs = dalloc(p, &d_i0, (size_t)n)) || (rcs = dalloc(p, &d_i1, (size_t)n)) || (rcs = dalloc(p, &d_sorted, (size_t)n * 6)) ||
         (rcs = upload(p, &d_off, p->offsets))) return rcs;
-    k_record_keys<<<(unsigned)((n + 255) / 256), 256, 0, p->stream>>>(p->cfg, p->d_records, n, d_k0, d_i0);
+    if ((rcs = launch(p, k_record_keys, (unsigned)((n + 255) / 256), 256, 0, p->stream, false, p->cfg, p->d_records, n, d_k0, d_i0))) return rcs;
     size_t tmp_bytes = 0;
     CK(cub::DeviceSegmentedSort::SortPairs(nullptr, tmp_bytes, d_k0, d_k1, d_i0, d_i1, (int)n, np, d_off, d_off + 1, p->stream));
     CK(cudaMallocAsync(&d_tmp, std::max<size_t>(tmp_bytes, 16), p->stream));
     CK(cub::DeviceSegmentedSort::SortPairs(d_tmp, tmp_bytes, d_k0, d_k1, d_i0, d_i1, (int)n, np, d_off, d_off + 1, p->stream));
-    k_gather_records<<<(unsigned)((n * 6 + 255) / 256), 256, 0, p->stream>>>(p->d_records, d_i1, n, d_sorted);
+    if ((rcs = launch(p, k_gather_records, (unsigned)((n * 6 + 255) / 256), 256, 0, p->stream, false, p->d_records, d_i1, n, d_sorted))) return rcs;
     CK(cudaFreeAsync(d_tmp, p->stream));
     CK(cudaGetLastError());
     p->d_records = d_sorted; p->records_sorted = true;      // (the unsorted copy and the sort buffers go back to the pool with the handle's other allocations)
@@ -386,14 +399,13 @@ static int allocate_storage(rcvd_problem* p) {
   // active mask
   CK(cudaMemsetAsync(p->d_active, 0, Upad, p->stream));
   DevProblem d = dev_problem(p);
-  if (p->num_tiles > 0) k_mark_static<<<p->num_tiles, kTile, 0, p->stream>>>(d, p->d_active);
+  if (p->num_tiles > 0 && (rc = launch(p, k_mark_static, p->num_tiles, kTile, 0, p->stream, false, d, p->d_active))) return rc;
   if (rcn.total > 0) {
     DevProblem d1 = d; d1.nranks = 1; d1.rank = 0;   // mark regardless of rank ownership
-    k_regularisers<2><<<(rcn.total + 127) / 128, 128, 0, p->stream>>>(d1, rcn, p->d_x, nullptr, nullptr, nullptr, p->d_active, p->first_frame, p->last_frame);
+    if ((rc = launch(p, k_regularisers<2>, (rcn.total + 127) / 128, 128, 0, p->stream, false, d1, rcn, p->d_x, nullptr, nullptr, nullptr, p->d_active, p->first_frame, p->last_frame))) return rc;
   }
-  if (p->num_trip_tiles > 0) k_triplets<2><<<p->num_trip_tiles, kTile, 0, p->stream>>>(d, p->d_x, nullptr, nullptr, nullptr, p->d_active);
-  k_finalize_mask<<<(int)((Upad + 255) / 256), 256, 0, p->stream>>>(p->cfg, L, p->d_active, N);
-  CK(cudaGetLastError());
+  if (p->num_trip_tiles > 0 && (rc = launch(p, k_triplets<2>, p->num_trip_tiles, kTile, 0, p->stream, false, d, p->d_x, nullptr, nullptr, nullptr, p->d_active))) return rc;
+  if ((rc = launch(p, k_finalize_mask, (int)((Upad + 255) / 256), 256, 0, p->stream, false, p->cfg, L, p->d_active, N))) return rc;
   if (p->nranks > 1) {   // the parameter set of the program is the union over the ranks' constraint shards (norms and stopping tests must agree on every rank)
     const int r = nccl::AllReduce(p->d_active, p->d_active, Upad, nccl::kUint8, nccl::kMax, p->comm, p->stream);
     if (r != 0) return set_err(RCVD_ERR_NCCL, "ncclAllReduce(active mask) failed");
@@ -476,16 +488,11 @@ struct FactorSolve {
     if (!p->prof) return;
     cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); p->prof->push_back({cls < 0 ? cls : (cls | (prof_level << 8)), e});
   }
-  // Every kernel of the factorisation and the solve is launched here and counted in p->launches and p->paths[path].  pdl: a
-  // programmatic dependent launch, which may start before its predecessor on the stream ends (it waits with griddepcontrol.wait).
+  // every kernel of the factorisation and the solve is launched here and also counted in p->paths[path]
   template <class... Params, class... Args>
   int launch(int path, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
-    cudaLaunchAttribute attr = {};
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization; attr.val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t lc = {};
-    lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = s; lc.attrs = &attr; lc.numAttrs = pdl ? 1 : 0;
-    CK(cudaLaunchKernelEx(&lc, kernel, args...));
-    p->launches += 1; p->paths[path]++;
+    if (int rc = ::launch(p, kernel, grid, block, smem, s, pdl, args...)) return rc;
+    p->paths[path]++;
     return RCVD_OK;
   }
   // `waiter` waits for the work enqueued on `from` so far
@@ -710,38 +717,36 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
   const int regblocks = (rcn.total + 127) / 128;
   if (wantH) CK(cudaMemsetAsync(p->d_H, 0, p->plan.hblocks.size() * bs * sizeof(double), st));
   if (wantG) CK(cudaMemsetAsync(gout, 0, (Upad + 8) * sizeof(double), st));
+  int rc;
   if (p->num_tiles > 0) {
-    if (wantH && p->use_fast && p->records_sorted) k_accumulate_runs<<<p->num_tiles, kTile, kRunSmem, st>>>(d, x, p->d_H, gout, p->d_partial);
-    else if (wantH && p->use_fast && fast_path_ok_host(p->cfg, L)) k_accumulate_fast<<<p->num_tiles, kTile, kFastSmem, st>>>(d, x, p->d_H, gout, p->d_partial);
-    else if (wantH) k_accumulate_generic<true><<<p->num_tiles, kTile, 0, st>>>(d, x, p->d_H, gout, p->d_partial);
-    else if (wantG) k_accumulate_generic<false><<<p->num_tiles, kTile, 0, st>>>(d, x, nullptr, gout, p->d_partial);
-    else k_cost_static<<<p->num_tiles, kTile, 0, st>>>(d, x, p->d_partial);
-    p->launches++;
+    if (wantH && p->use_fast && p->records_sorted) rc = launch(p, k_accumulate_runs, p->num_tiles, kTile, kRunSmem, st, false, d, x, p->d_H, gout, p->d_partial);
+    else if (wantH && p->use_fast && fast_path_ok_host(p->cfg, L)) rc = launch(p, k_accumulate_fast, p->num_tiles, kTile, kFastSmem, st, false, d, x, p->d_H, gout, p->d_partial);
+    else if (wantH) rc = launch(p, k_accumulate_generic<true>, p->num_tiles, kTile, 0, st, false, d, x, p->d_H, gout, p->d_partial);
+    else if (wantG) rc = launch(p, k_accumulate_generic<false>, p->num_tiles, kTile, 0, st, false, d, x, nullptr, gout, p->d_partial);
+    else rc = launch(p, k_cost_static, p->num_tiles, kTile, 0, st, false, d, x, p->d_partial);
+    if (rc) return rc;
   }
   if (regblocks > 0) {
     double* part = p->d_partial + p->num_tiles;
-    if (wantH) k_regularisers<1><<<regblocks, 128, 0, st>>>(d, rcn, x, p->d_H, gout, part, nullptr, p->first_frame, p->last_frame);
-    else if (wantG) k_regularisers<3><<<regblocks, 128, 0, st>>>(d, rcn, x, nullptr, gout, part, nullptr, p->first_frame, p->last_frame);
-    else k_regularisers<0><<<regblocks, 128, 0, st>>>(d, rcn, x, nullptr, nullptr, part, nullptr, p->first_frame, p->last_frame);
-    p->launches++;
+    if (wantH) rc = launch(p, k_regularisers<1>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, gout, part, nullptr, p->first_frame, p->last_frame);
+    else if (wantG) rc = launch(p, k_regularisers<3>, regblocks, 128, 0, st, false, d, rcn, x, nullptr, gout, part, nullptr, p->first_frame, p->last_frame);
+    else rc = launch(p, k_regularisers<0>, regblocks, 128, 0, st, false, d, rcn, x, nullptr, nullptr, part, nullptr, p->first_frame, p->last_frame);
+    if (rc) return rc;
   }
   if (p->num_trip_tiles > 0) {
     double* part = p->d_partial + p->num_tiles + regblocks;
-    if (wantH) k_triplets<1><<<p->num_trip_tiles, kTile, 0, st>>>(d, x, p->d_H, gout, part, nullptr);
-    else if (wantG) k_triplets<3><<<p->num_trip_tiles, kTile, 0, st>>>(d, x, nullptr, gout, part, nullptr);
-    else k_triplets<0><<<p->num_trip_tiles, kTile, 0, st>>>(d, x, nullptr, nullptr, part, nullptr);
-    p->launches++;
+    if (wantH) rc = launch(p, k_triplets<1>, p->num_trip_tiles, kTile, 0, st, false, d, x, p->d_H, gout, part, nullptr);
+    else if (wantG) rc = launch(p, k_triplets<3>, p->num_trip_tiles, kTile, 0, st, false, d, x, nullptr, gout, part, nullptr);
+    else rc = launch(p, k_triplets<0>, p->num_trip_tiles, kTile, 0, st, false, d, x, nullptr, nullptr, part, nullptr);
+    if (rc) return rc;
   }
-  k_reduce_partials<<<1, 1024, 0, st>>>(p->d_partial, p->num_tiles + regblocks + p->num_trip_tiles, p->d_scal, slot);
-  p->launches++;
-  CK(cudaGetLastError());
+  if ((rc = launch(p, k_reduce_partials, 1, 1024, 0, st, false, p->d_partial, p->num_tiles + regblocks + p->num_trip_tiles, p->d_scal, slot))) return rc;
   if (p->nranks > 1) {
-    int rc;
     if (wantG) {
       // ONE packed all-reduce: [gradient (Upad) | cost + 7 spare | diagonal of H (Upad, only with H into d_g)]
       CK(cudaMemcpyAsync(gout + Upad, p->d_scal + slot, sizeof(double), cudaMemcpyDeviceToDevice, st));
       size_t cnt = Upad + 8;
-      if (wantH && gout == p->d_g) { k_extract_diag<<<(int)((Upad + 255) / 256), 256, 0, st>>>(p->d_H, p->d_diagH, N, npad); p->launches++; cnt = 2 * Upad + 8; }
+      if (wantH && gout == p->d_g) { if ((rc = launch(p, k_extract_diag, (int)((Upad + 255) / 256), 256, 0, st, false, p->d_H, p->d_diagH, N, npad))) return rc; cnt = 2 * Upad + 8; }
       if ((rc = allreduce(p, gout, cnt))) return rc;
       CK(cudaMemcpyAsync(p->d_scal + slot, gout + Upad, sizeof(double), cudaMemcpyDeviceToDevice, st));
     } else if ((rc = allreduce(p, p->d_scal + slot, 1))) return rc;
@@ -874,19 +879,6 @@ __global__ void k_make_delta(const double* __restrict__ y, const double* __restr
   if (i < n) delta[i] = -y[i] * S[i];
 }
 
-// model = gs.y - 1/2 (Sy)^T H (Sy); leaves GY, YHY in d_scal
-static int enqueue_model_terms(rcvd_problem* p) {
-  const int N = p->N, npad = p->L.npad; const size_t Upad = (size_t)N * npad; cudaStream_t st = p->stream;
-  k_mul<<<nblk(Upad), 256, 0, st>>>(p->d_S, p->d_y, p->d_Sy, (int)Upad);
-  CK(cudaMemsetAsync(p->d_Hy, 0, Upad * sizeof(double), st));
-  k_spmv_sym<<<dim3((npad + 7) / 8, p->plan.dist ? (int)p->plan.own_hblocks.size() : (int)p->plan.hblocks.size()), 256, 0, st>>>(p->d_H, p->d_hblocks, p->d_Sy, p->d_Hy, npad, p->plan.dist ? p->d_own_hblocks : nullptr);
-  k_dot2<<<nblk(Upad), 256, 0, st>>>(p->d_gs, p->d_y, p->d_Sy, p->d_Hy, (int)Upad, p->d_scal, SC_GY, SC_YHY);
-  if (p->plan.dist) { int rc = allreduce(p, p->d_scal + SC_YHY, 1); if (rc) return rc; }   // every rank multiplied the H blocks it owns
-  k_make_delta<<<nblk(Upad), 256, 0, st>>>(p->d_y, p->d_S, p->d_delta, (int)Upad);
-  p->launches += 4;
-  return RCVD_OK;
-}
-
 // xc = Plus(x, alpha * delta) with bounds projection, delta = -y*S (k_make_delta); accumulates |x - xc|^2 over active params,
 // g . delta and max|delta| (for the line search).  delta, g have npad stride; x, xc nf stride.
 __global__ void __launch_bounds__(256) k_candidate(rcvd_config cfg, Layout L, const uint8_t* __restrict__ in_range, const uint8_t* __restrict__ active,
@@ -912,11 +904,38 @@ __global__ void __launch_bounds__(256) k_candidate(rcvd_config cfg, Layout L, co
   }
 }
 
-static int enqueue_candidate(rcvd_problem* p, double alpha, const double* g) {
-  const size_t U = (size_t)p->N * p->L.nf;
-  k_candidate<<<nblk(U), 256, 0, p->stream>>>(p->cfg, p->L, p->d_in_range, p->d_active, p->d_x, p->d_delta, g, alpha, p->d_xc, p->d_scal, p->N);
-  p->launches++;
-  return RCVD_OK;
+// The three parts of an LM step.  rcvd_solve, rcvd_time_iteration and rcvd_debug_linear_residual all build their steps from them.
+
+// Assemble: cost (SC_COST), gradient (d_g) and H at d_x, and diag H into d_diagH (at N > 1 enqueue_evaluate extracts it for its all-reduce)
+static int enqueue_assemble(rcvd_problem* p) {
+  if (int rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST)) return rc;
+  if (p->nranks > 1) return RCVD_OK;
+  return launch(p, k_extract_diag, nblk((size_t)p->N * p->L.npad), 256, 0, p->stream, false, p->d_H, p->d_diagH, p->N, p->L.npad);
+}
+
+// Damped step: the LM diagonal (clamped S^2 diag H unless `reuse`), D2 = diagonal / radius and gs = S g; y = (S H S + D2)^-1 gs; the
+// model terms gs.y (GY) and (Sy)^T H (Sy) (YHY, with H (S y) left in d_Hy) and delta = -y S.
+static int enqueue_damped_step(rcvd_problem* p, const rcvd_solve_options& o, double radius, bool reuse) {
+  const int npad = p->L.npad; const size_t Upad = (size_t)p->N * npad; cudaStream_t st = p->stream;
+  int rc;
+  if ((rc = launch(p, k_lm_prepare, nblk(Upad), 256, 0, st, false, p->d_diagH, p->d_S, p->d_g, p->d_lmdiag, p->d_D2, p->d_gs, (int)Upad, reuse ? 1 : 0, radius, o.min_lm_diagonal, o.max_lm_diagonal))) return rc;
+  if ((rc = factor_solve(p))) return rc;
+  if ((rc = launch(p, k_mul, nblk(Upad), 256, 0, st, false, p->d_S, p->d_y, p->d_Sy, (int)Upad))) return rc;
+  CK(cudaMemsetAsync(p->d_Hy, 0, Upad * sizeof(double), st));
+  if ((rc = launch(p, k_spmv_sym, dim3((npad + 7) / 8, p->plan.dist ? (int)p->plan.own_hblocks.size() : (int)p->plan.hblocks.size()), 256, 0, st, false, p->d_H, p->d_hblocks, p->d_Sy, p->d_Hy, npad, p->plan.dist ? p->d_own_hblocks : nullptr))) return rc;
+  if ((rc = launch(p, k_dot2, nblk(Upad), 256, 0, st, false, p->d_gs, p->d_y, p->d_Sy, p->d_Hy, (int)Upad, p->d_scal, SC_GY, SC_YHY))) return rc;
+  if (p->plan.dist && (rc = allreduce(p, p->d_scal + SC_YHY, 1))) return rc;   // every rank multiplied the H blocks it owns
+  return launch(p, k_make_delta, nblk(Upad), 256, 0, st, false, p->d_y, p->d_S, p->d_delta, (int)Upad);
+}
+
+// Candidate cost: xc = Plus(x, alpha delta), then the cost at xc (SC_CAND).  `slope` (a line-search trial): also the gradient at xc
+// into d_g2 and its directional derivative g(xc).delta (SC_GY).
+static int enqueue_candidate_cost(rcvd_problem* p, double alpha, bool slope) {
+  const size_t U = (size_t)p->N * p->L.nf, Upad = (size_t)p->N * p->L.npad;
+  if (int rc = launch(p, k_candidate, nblk(U), 256, 0, p->stream, false, p->cfg, p->L, p->d_in_range, p->d_active, p->d_x, p->d_delta, p->d_g, alpha, p->d_xc, p->d_scal, p->N)) return rc;
+  if (int rc = enqueue_evaluate(p, p->d_xc, slope, false, slope ? p->d_g2 : nullptr, SC_CAND)) return rc;
+  if (!slope) return RCVD_OK;
+  return launch(p, k_dot2, nblk(Upad), 256, 0, p->stream, false, p->d_g2, p->d_delta, p->d_g2, p->d_delta, (int)Upad, p->d_scal, SC_GY, SC_YHY);
 }
 
 static float ev_ms(cudaEvent_t a, cudaEvent_t b) { float m = 0; cudaEventElapsedTime(&m, a, b); return m; }
@@ -933,19 +952,16 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
   const int64_t launches0 = p->launches;
   sum.num_constraints = p->C;
   const bool constrained = p->cfg.depth_lower_bound && L.nd > 0;
-  for (int i = 0; i < 8; ++i) if (!p->ev[i]) CK(cudaEventCreate(&p->ev[i]));
-  if (constrained) { k_project_state<<<nblk(U), 256, 0, st>>>(p->cfg, L, p->d_in_range, p->d_x, N); p->launches++; }
+  if (constrained && (rc = launch(p, k_project_state, nblk(U), 256, 0, st, false, p->cfg, L, p->d_in_range, p->d_x, N))) return rc;
   // user-visible minimum-cost iterate
   CK(cudaMemcpyAsync(p->d_xsave, p->d_x, U * sizeof(double), cudaMemcpyDeviceToDevice, st));
 
-  auto full_eval = [&]() -> int {   // cost, gradient, H, diag, norms at d_x
+  auto full_eval = [&]() -> int {   // assemble, then the norms at d_x
     CK(cudaMemsetAsync(p->d_scal, 0, SC_N * sizeof(double), st));
     CK(cudaEventRecord(p->ev[0], st));
-    int r = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST); if (r) return r;
+    int r = enqueue_assemble(p); if (r) return r;
     CK(cudaEventRecord(p->ev[1], st));
-    if (p->nranks <= 1) k_extract_diag<<<nblk(Upad), 256, 0, st>>>(p->d_H, p->d_diagH, N, npad);
-    k_state_norms<<<nblk(U), 256, 0, st>>>(p->cfg, L, p->d_in_range, p->d_active, p->d_x, p->d_g, p->d_scal, N);
-    p->launches += 2;
+    r = launch(p, k_state_norms, nblk(U), 256, 0, st, false, p->cfg, L, p->d_in_range, p->d_active, p->d_x, p->d_g, p->d_scal, N); if (r) return r;
     r = read_scalars(p); if (r) return r;
     sum.eval_ms += ev_ms(p->ev[0], p->ev[1]);
     return RCVD_OK;
@@ -953,8 +969,7 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
   if ((rc = full_eval())) return rc;
   double xCost = p->h_scal[SC_COST], xNorm = std::sqrt(p->h_scal[SC_X2]), gmax = p->h_scal[SC_GMAX];
   sum.initial_cost = xCost;
-  k_jacobi_scale<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, (int)Upad, o.jacobi_scaling);
-  p->launches++;
+  if ((rc = launch(p, k_jacobi_scale, nblk(Upad), 256, 0, st, false, p->d_diagH, p->d_S, (int)Upad, o.jacobi_scaling))) return rc;
   double radius = o.initial_radius, decrease = 2.0; bool reuseDiag = false;
   double minimumCost = xCost;
   int iter = 0, invalid = 0; bool stepSuccessful = true;
@@ -974,16 +989,12 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
     CK(cudaMemsetAsync(p->d_scal, 0, SC_N * sizeof(double), st));
     CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), st));
     CK(cudaEventRecord(p->ev[2], st));
-    k_lm_prepare<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, p->d_g, p->d_lmdiag, p->d_D2, p->d_gs, (int)Upad, reuseDiag ? 1 : 0, radius, o.min_lm_diagonal, o.max_lm_diagonal);
-    p->launches++;
+    if ((rc = enqueue_damped_step(p, o, radius, reuseDiag))) return rc;
     reuseDiag = true;
-    if ((rc = factor_solve(p))) return rc;
-    if ((rc = enqueue_model_terms(p))) return rc;
     CK(cudaEventRecord(p->ev[3], st));
     double alpha = 1.0;
     if (!constrained) {
-      if ((rc = enqueue_candidate(p, 1.0, p->d_g))) return rc;
-      if ((rc = enqueue_evaluate(p, p->d_xc, false, false, nullptr, SC_CAND))) return rc;
+      if ((rc = enqueue_candidate_cost(p, 1.0, false))) return rc;
       CK(cudaEventRecord(p->ev[4], st));
     }
     if ((rc = read_scalars(p))) return rc;
@@ -1003,10 +1014,7 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
       // DoLineSearch: Armijo with cubic interpolation along the projected path (ceres defaults)
       auto trial = [&](double a, ls::Sample& s) -> int {
         CK(cudaMemsetAsync(p->d_scal, 0, SC_N * sizeof(double), st));
-        int r = enqueue_candidate(p, a, p->d_g); if (r) return r;
-        r = enqueue_evaluate(p, p->d_xc, true, false, p->d_g2, SC_CAND); if (r) return r;
-        k_dot2<<<nblk(Upad), 256, 0, st>>>(p->d_g2, p->d_delta, p->d_g2, p->d_delta, (int)Upad, p->d_scal, SC_GY, SC_YHY);
-        p->launches++;
+        int r = enqueue_candidate_cost(p, a, true); if (r) return r;
         r = read_scalars(p); if (r) return r;
         s.x = a; s.value = p->h_scal[SC_CAND]; s.valueValid = std::isfinite(s.value);
         s.gradient = p->h_scal[SC_GY]; s.gradValid = s.valueValid && std::isfinite(s.gradient);
@@ -1029,8 +1037,7 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
       }
       alpha = success ? cur.x : 1.0;
       CK(cudaMemsetAsync(p->d_scal, 0, SC_N * sizeof(double), st));
-      if ((rc = enqueue_candidate(p, alpha, p->d_g))) return rc;
-      if ((rc = enqueue_evaluate(p, p->d_xc, false, false, nullptr, SC_CAND))) return rc;
+      if ((rc = enqueue_candidate_cost(p, alpha, false))) return rc;
       if ((rc = read_scalars(p))) return rc;
     }
     double candCost = p->h_scal[SC_CAND];
@@ -1097,7 +1104,8 @@ RCVD_API int32_t rcvd_problem_create(const rcvd_config* cfg, int32_t device, rcv
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_join, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_inv_join, cudaEventDisableTiming);
-  if (e != cudaSuccess) { delete p; return set_err(RCVD_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)); }
+  for (int i = 0; i < 8 && e == cudaSuccess; ++i) e = cudaEventCreate(&p->ev[i]);   // the timing events of rcvd_solve and the bench hooks
+  if (e != cudaSuccess) { rcvd_problem_destroy(p); return set_err(RCVD_ERR_CUDA, "cudaStreamCreate / cudaEventCreate: %s", cudaGetErrorString(e)); }
   *out = p; return RCVD_OK;
 }
 RCVD_API void rcvd_problem_destroy(rcvd_problem* p) {
@@ -1213,9 +1221,10 @@ RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
   double* d_out = nullptr;
   CK(cudaMalloc((void**)&d_out, U * U * sizeof(double)));
   CK(cudaMemsetAsync(d_out, 0, U * U * sizeof(double), p->stream));
-  k_h_to_dense<<<dim3(nblk((size_t)p->L.nf * p->L.nf), (int)p->plan.hblocks.size()), 256, 0, p->stream>>>(p->d_H, p->d_hblocks, (int)p->plan.hblocks.size(), d_out, p->N, p->L.nf, p->L.npad, p->d_uperm);
-  cudaError_t e = cudaMemcpyAsync(Hout, d_out, U * U * sizeof(double), cudaMemcpyDeviceToHost, p->stream);
+  rc = launch(p, k_h_to_dense, dim3(nblk((size_t)p->L.nf * p->L.nf), (int)p->plan.hblocks.size()), 256, 0, p->stream, false, p->d_H, p->d_hblocks, (int)p->plan.hblocks.size(), d_out, p->N, p->L.nf, p->L.npad, p->d_uperm);
+  cudaError_t e = rc ? cudaSuccess : cudaMemcpyAsync(Hout, d_out, U * U * sizeof(double), cudaMemcpyDeviceToHost, p->stream);
   cudaStreamSynchronize(p->stream); cudaFree(d_out);
+  if (rc) return rc;
   if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "copy failed: %s", cudaGetErrorString(e));
   return RCVD_OK;
 }
@@ -1310,7 +1319,6 @@ RCVD_API int32_t rcvd_time_accumulate(rcvd_problem* p, int32_t iters, double* ms
   if (!p || iters <= 0) return set_err(RCVD_ERR_INVALID, "bad argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
-  for (int i = 0; i < 2; ++i) if (!p->ev[i]) CK(cudaEventCreate(&p->ev[i]));
   if ((rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST))) return rc;   // warm-up
   CK(cudaEventRecord(p->ev[0], p->stream));
   for (int i = 0; i < iters; ++i) if ((rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST))) return rc;
@@ -1323,23 +1331,20 @@ RCVD_API int32_t rcvd_time_iteration(rcvd_problem* p, int32_t iters, double radi
   if (!p || iters <= 0) return set_err(RCVD_ERR_INVALID, "bad argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
-  const int N = p->N, npad = p->L.npad; const size_t Upad = (size_t)N * npad; cudaStream_t st = p->stream;
-  for (int i = 0; i < 8; ++i) if (!p->ev[i]) CK(cudaEventCreate(&p->ev[i]));
+  const size_t Upad = (size_t)p->N * p->L.npad; cudaStream_t st = p->stream;
+  rcvd_solve_options o; rcvd_default_solve_options(&o);
   double ta = 0, tl = 0, tc = 0, tt = 0;
   for (int it = -1; it < iters; ++it) {   // it == -1: warm-up (also instantiates the graph)
+    // the first iteration of rcvd_solve with the default options: assemble, Jacobi scaling, damped step, candidate cost
     CK(cudaMemsetAsync(p->d_scal, 0, SC_N * sizeof(double), st));
     CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), st));
     CK(cudaEventRecord(p->ev[0], st));
-    if ((rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST))) return rc;
-    if (p->nranks <= 1) k_extract_diag<<<nblk(Upad), 256, 0, st>>>(p->d_H, p->d_diagH, N, npad);
-    k_jacobi_scale<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, (int)Upad, 1);
+    if ((rc = enqueue_assemble(p))) return rc;
+    if ((rc = launch(p, k_jacobi_scale, nblk(Upad), 256, 0, st, false, p->d_diagH, p->d_S, (int)Upad, o.jacobi_scaling))) return rc;
     CK(cudaEventRecord(p->ev[1], st));
-    k_lm_prepare<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, p->d_g, p->d_lmdiag, p->d_D2, p->d_gs, (int)Upad, 0, radius, 1e-6, 1e32);
-    if ((rc = factor_solve(p))) return rc;
-    if ((rc = enqueue_model_terms(p))) return rc;
+    if ((rc = enqueue_damped_step(p, o, radius, false))) return rc;
     CK(cudaEventRecord(p->ev[2], st));
-    if ((rc = enqueue_candidate(p, 1.0, p->d_g))) return rc;
-    if ((rc = enqueue_evaluate(p, p->d_xc, false, false, nullptr, SC_CAND))) return rc;
+    if ((rc = enqueue_candidate_cost(p, 1.0, false))) return rc;
     CK(cudaEventRecord(p->ev[3], st));
     if ((rc = read_scalars(p))) return rc;
     if (it >= 0) { ta += ev_ms(p->ev[0], p->ev[1]); tl += ev_ms(p->ev[1], p->ev[2]); tc += ev_ms(p->ev[2], p->ev[3]); tt += ev_ms(p->ev[0], p->ev[3]); }
@@ -1464,19 +1469,16 @@ RCVD_API int32_t rcvd_debug_linear_residual(rcvd_problem* p, double radius, doub
   if (!p || !out || !(radius > 0.0)) return set_err(RCVD_ERR_INVALID, "bad argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
-  const int N = p->N, npad = p->L.npad; const size_t Upad = (size_t)N * npad; cudaStream_t st = p->stream;
+  const size_t Upad = (size_t)p->N * p->L.npad; cudaStream_t st = p->stream;
+  rcvd_solve_options o; rcvd_default_solve_options(&o);
   CK(cudaMemsetAsync(p->d_scal, 0, SC_N * sizeof(double), st));
   CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), st));
-  if ((rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST))) return rc;
-  if (p->nranks <= 1) k_extract_diag<<<nblk(Upad), 256, 0, st>>>(p->d_H, p->d_diagH, N, npad);
-  k_jacobi_scale<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, (int)Upad, 1);
-  k_lm_prepare<<<nblk(Upad), 256, 0, st>>>(p->d_diagH, p->d_S, p->d_g, p->d_lmdiag, p->d_D2, p->d_gs, (int)Upad, 0, radius, 1e-6, 1e32);
-  if ((rc = factor_solve(p))) return rc;
-  if ((rc = enqueue_model_terms(p))) return rc;                      // leaves H (S y) in d_Hy
+  if ((rc = enqueue_assemble(p))) return rc;
+  if ((rc = launch(p, k_jacobi_scale, nblk(Upad), 256, 0, st, false, p->d_diagH, p->d_S, (int)Upad, o.jacobi_scaling))) return rc;
+  if ((rc = enqueue_damped_step(p, o, radius, false))) return rc;         // leaves H (S y) in d_Hy
   if (p->plan.dist && (rc = allreduce(p, p->d_Hy, Upad))) return rc;      // every rank multiplied only the H blocks it owns
-  double* d_out = p->d_scal + 9;                                      // slots 9..12 are unused by the LM loop
-  k_lin_residual<<<nblk(Upad), 256, 0, st>>>(p->d_S, p->d_Hy, p->d_D2, p->d_y, p->d_gs, p->d_g, (int)Upad, d_out);
-  p->launches += 4;
+  double* d_out = p->d_scal + 9;                                          // slots 9..12 are unused by the LM loop
+  if ((rc = launch(p, k_lin_residual, nblk(Upad), 256, 0, st, false, p->d_S, p->d_Hy, p->d_D2, p->d_y, p->d_gs, p->d_g, (int)Upad, d_out))) return rc;
   if ((rc = read_scalars(p))) return rc;
   const double r2 = p->h_scal[9], b2 = p->h_scal[10];
   out[0] = b2 > 0.0 ? std::sqrt(r2 / b2) : std::sqrt(r2); out[1] = std::sqrt(b2); out[2] = p->h_scal[SC_COST];

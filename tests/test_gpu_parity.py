@@ -308,3 +308,26 @@ def test_last_iteration_returns_what_the_timed_step_computed():
     np.testing.assert_allclose(it["gradient"].ravel(), g, rtol=0, atol=1e-9 * np.abs(g).max())
     step = it["candidate_state"] - G.get_state()
     assert np.isfinite(step).all() and np.abs(step).max() > 0 and np.isfinite(it["candidate_cost"])
+
+
+def test_timed_step_is_the_solvers_step():
+    """The step rcvd_time_iteration times (bench.py's headline) is the step rcvd_solve takes: from one state, one rcvd_solve iteration
+    with the default radius and Jacobi scaling accepts the timed step's candidate state and cost.  The substitution sums with red_add,
+    whose order is not fixed between two runs, hence 1e-12 relative rather than bit equality.  (On this case the first step at radius
+    1e4 is accepted; on the depth-grid cases it is not.)"""
+    from robust_cvd_b200 import solver
+    sc, cfg, pairs, offs, rec, med = helpers.make_case(num_frames=8, **dict(helpers.VARIANTS)["identitydepth_perframe"])
+    off_d, nd = helpers.layout_numbers(cfg)
+    G = solver.Problem(cfg)
+    x = helpers.initial_state(sc, cfg, G.stride, off_d, nd)
+    helpers.setup_problem(G, cfg, pairs, offs, rec, med, x)
+    G.time_iteration(iters=1, radius=1e4)
+    it = G.last_iteration()
+    opt = abi.default_solve_options(max_iterations=1)
+    opt.function_tolerance = 0.0; opt.parameter_tolerance = 0.0; opt.gradient_tolerance = 0.0
+    assert opt.initial_radius == 1e4 and opt.jacobi_scaling == 1
+    s = G.solve(opt)
+    assert s.iterations == 1 and s.num_successful_steps == 2 and s.num_unsuccessful_steps == 0, s.message      # the step was accepted
+    xc = it["candidate_state"]
+    assert np.abs(G.get_state() - xc).max() <= 1e-12 * np.abs(xc).max()
+    assert abs(s.final_cost - it["candidate_cost"]) <= 1e-12 * abs(it["candidate_cost"]), (s.final_cost, it["candidate_cost"])
