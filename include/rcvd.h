@@ -347,6 +347,17 @@ int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t num_fram
                           int32_t num_triplets, const int32_t* trip_frames, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static,
                           float* dist_out);
 
+/* Static-flag pruning on the device: replaces FlowConstraintsCollection::pruneStaticFlag (reference lib/FlowConstraints.cpp:662-748).
+ * Every non-static pair constraint stamps a disc (rx^2 + ry^2 <= distance^2, clipped to the h x w image of the "down" stream) around
+ * its end in each of its frames (end 0 only when both frames are equal); then every pair or triplet constraint with an end on a
+ * stamped pixel of its frame becomes non-static.  An end's pixel is (int(loc.x * w), int(loc.y * w)), y scaled by the WIDTH as the
+ * reference does; the disc centre is used as is, the lookup pixel is clamped to the image (the reference reads past the frame there).
+ * Arrays as in rcvd_static_flags (trip_centres: centre frame t of the triplet t-1, t, t+1); pair_static / trip_static in/out, one
+ * byte per constraint, flags only go from static to non-static.  No pair constraint non-static, or distance < 0: nothing changes. */
+int32_t rcvd_prune_static_flags(int32_t device, int32_t num_frames, int32_t height, int32_t width, int32_t distance,
+                                int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
+                                int32_t num_triplets, const int32_t* trip_centres, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static);
+
 #ifdef __cplusplus
 }
 #endif

@@ -175,8 +175,15 @@ __global__ void __launch_bounds__(kChamThreads) k_chamfer5(const uint8_t* __rest
   }
 }
 
-// isStatic of every pair / triplet constraint: dist > distance at all ends; pixel = (int(loc.x * w), int(loc.y * w)) -- the reference
-// scales y by the mask WIDTH as well (:618-621).  items: [n][3] frames (-1 = unused end), locs: [total][2 * ends] float32.
+// The pixel a constraint end is looked up at: (int(loc.x * w), int(loc.y * w)) -- the reference scales y by the image WIDTH as
+// well (:618-621, :725-744) -- clamped to the image, where the reference indexes unchecked.
+__device__ __forceinline__ int2 end_pixel(const float* loc, int h, int w) {
+  const int ix = (int)__fmul_rn(loc[0], (float)w), iy = (int)__fmul_rn(loc[1], (float)w);
+  return make_int2(min(max(ix, 0), w - 1), min(max(iy, 0), h - 1));
+}
+
+// isStatic of every pair / triplet constraint: dist > distance at all ends (end_pixel).  items: [n][3] frames (-1 = unused end),
+// locs: [total][2 * ends] float32.
 __global__ void __launch_bounds__(256) k_static_flags(const float* __restrict__ dist, int h, int w, float distance, int ends, const int* __restrict__ item_frames,
                                                        const long long* __restrict__ offsets, int nitems, const float* __restrict__ locs, uint8_t* __restrict__ flags) {
   const int item = blockIdx.y;
@@ -188,11 +195,68 @@ __global__ void __launch_bounds__(256) k_static_flags(const float* __restrict__ 
     bool st = true;
     for (int e = 0; e < ends; ++e) {
       const int f = item_frames[item * 3 + e];
-      int ix = (int)__fmul_rn(L[2 * e], (float)w), iy = (int)__fmul_rn(L[2 * e + 1], (float)w);
-      ix = min(max(ix, 0), w - 1); iy = min(max(iy, 0), h - 1);     // the reference indexes unchecked
-      st = st && (dist[(size_t)f * plane + (size_t)iy * w + ix] > distance);
+      const int2 p = end_pixel(L + 2 * e, h, w);
+      st = st && (dist[(size_t)f * plane + (size_t)p.y * w + p.x] > distance);
     }
     flags[b + i] = st ? 1 : 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Static-flag pruning (reference FlowConstraintsCollection::pruneStaticFlag, lib/FlowConstraints.cpp:662-748): every non-static pair
+// constraint stamps a disc of radius `distance` around its end in each of its two frames; then every pair / triplet constraint with an
+// end on a stamped pixel becomes non-static.  The per-frame byte masks of the reference are bit planes here, [F][h][words] u32 with
+// words = ceil(w / 32), zeroed before the stamps; a disc row is one span of set bits, so it is stamped with a few word-wide atomicOr.
+// ---------------------------------------------------------------------------------------------------------------------------
+// One warp per non-static pair constraint, its lanes over the rows of each end's disc.  The centre is not clamped: the reference's
+// loop bounds clip the disc to the image, so a centre at or beyond row h stamps only the disc rows that fall inside.  A pair whose two
+// frames are equal stamps end 0 only (key.first == frame picks c[0]).  flags are the input flags, not yet pruned.
+__global__ void __launch_bounds__(256) k_prune_stamp(unsigned* __restrict__ bits, int h, int w, int words, int distance, const int* __restrict__ pair_frames,
+                                                      const long long* __restrict__ offsets, int npairs, const float* __restrict__ locs, const uint8_t* __restrict__ flags) {
+  const int item = blockIdx.y;
+  if (item >= npairs) return;
+  const long long b = offsets[item], n = offsets[item + 1] - b;
+  const int lane = threadIdx.x & 31, f0 = pair_frames[item * 3], f1 = pair_frames[item * 3 + 1];
+  const long long d = distance, d2 = d * d;
+  const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long i = warp0; i < n; i += nwarps) {
+    if (flags[b + i]) continue;
+    const float* L = locs + (size_t)(b + i) * 4;
+    for (int e = 0; e < (f0 == f1 ? 1 : 2); ++e) {
+      const long long cx = (int)__fmul_rn(L[2 * e], (float)w), cy = (int)__fmul_rn(L[2 * e + 1], (float)w);
+      unsigned* plane = bits + (size_t)(e ? f1 : f0) * h * words;
+      for (long long y = max(0ll, cy - d) + lane; y <= min((long long)h - 1, cy + d); y += 32) {
+        // half-width of the disc row: the largest k with k^2 + dy^2 <= d^2 (integer square root, corrected in 64-bit)
+        const long long dy = y - cy, r2 = d2 - dy * dy;
+        long long k = (long long)sqrt((double)r2);
+        while (k * k > r2) --k;
+        while ((k + 1) * (k + 1) <= r2) ++k;
+        const long long x0 = max(0ll, cx - k), x1 = min((long long)w - 1, cx + k);
+        if (x0 > x1) continue;
+        unsigned* row = plane + (size_t)y * words;
+        for (int wd = (int)(x0 >> 5); wd <= (int)(x1 >> 5); ++wd) {
+          const int lo = max((int)x0 - 32 * wd, 0), hi = min((int)x1 - 32 * wd, 31);
+          atomicOr(row + wd, (0xffffffffu >> (31 - hi)) & (0xffffffffu << lo));
+        }
+      }
+    }
+  }
+}
+// Shaped like k_static_flags: a static constraint with any end (end_pixel) on a stamped pixel becomes non-static; others keep their flag.
+__global__ void __launch_bounds__(256) k_prune_lookup(const unsigned* __restrict__ bits, int h, int w, int words, int ends, const int* __restrict__ item_frames,
+                                                       const long long* __restrict__ offsets, int nitems, const float* __restrict__ locs, uint8_t* __restrict__ flags) {
+  const int item = blockIdx.y;
+  if (item >= nitems) return;
+  const long long b = offsets[item], n = offsets[item + 1] - b;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (!flags[b + i]) continue;
+    const float* L = locs + (size_t)(b + i) * 2 * ends;
+    bool hit = false;
+    for (int e = 0; e < ends; ++e) {
+      const int2 p = end_pixel(L + 2 * e, h, w);
+      hit = hit || ((bits[((size_t)item_frames[item * 3 + e] * h + p.y) * words + (p.x >> 5)] >> (p.x & 31)) & 1u);
+    }
+    if (hit) flags[b + i] = 0;
   }
 }
 

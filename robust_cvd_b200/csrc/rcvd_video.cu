@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and long point tracks.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, and long point tracks.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -443,6 +443,42 @@ RCVD_API int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t
   if (nt_total > 0) cudaMemcpyAsync(trip_static, d_ts, (size_t)nt_total, cudaMemcpyDeviceToHost, call.st);
   if (dist_out) cudaMemcpyAsync(dist_out, d_dist, (size_t)F * plane * 4, cudaMemcpyDeviceToHost, call.st);
   return call.sync("static-flag kernels");
+}
+
+// pair_static / trip_static are read and updated in place (flags only go from static to non-static).  Nothing is launched when no
+// pair constraint is non-static or the distance is negative: the flags cannot change then.
+RCVD_API int32_t rcvd_prune_static_flags(int32_t device, int32_t F, int32_t h, int32_t w, int32_t distance,
+                                         int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
+                                         int32_t num_triplets, const int32_t* trip_centres, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static) {
+  if (F <= 0 || h <= 0 || w <= 0 || num_pairs < 0 || num_triplets < 0) return set_err(RCVD_ERR_INVALID, "bad static-flag pruning arguments");
+  if ((num_pairs > 0 && (!pair_frames || !pair_offsets)) || (num_triplets > 0 && (!trip_centres || !trip_offsets))) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int i = 0; i < num_pairs; ++i) if (pair_frames[2 * i] < 0 || pair_frames[2 * i] >= F || pair_frames[2 * i + 1] < 0 || pair_frames[2 * i + 1] >= F || pair_offsets[i + 1] < pair_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad pair %d", i);
+  for (int i = 0; i < num_triplets; ++i) if (trip_centres[i] < 1 || trip_centres[i] + 1 >= F || trip_offsets[i + 1] < trip_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad triplet %d", i);
+  const int64_t np_total = num_pairs ? pair_offsets[num_pairs] : 0, nt_total = num_triplets ? trip_offsets[num_triplets] : 0;
+  if ((np_total > 0 && (!pair_locs || !pair_static)) || (nt_total > 0 && (!trip_locs || !trip_static))) return set_err(RCVD_ERR_INVALID, "null argument");
+  bool stamps = false;
+  for (int64_t i = 0; i < np_total && !stamps; ++i) stamps = pair_static[i] == 0;
+  if (!stamps || distance < 0) return RCVD_OK;
+  VideoCall call;
+  if (int rc = call.open(device)) return rc;
+  const int words = (w + 31) / 32;
+  const size_t bits_bytes = (size_t)F * h * words * 4;
+  unsigned* d_bits = (unsigned*)call.alloc(bits_bytes);
+  std::vector<int32_t> pf3((size_t)num_pairs * 3, -1), tf3((size_t)num_triplets * 3, -1);
+  for (int i = 0; i < num_pairs; ++i) { pf3[3 * i] = pair_frames[2 * i]; pf3[3 * i + 1] = pair_frames[2 * i + 1]; }
+  for (int i = 0; i < num_triplets; ++i) { tf3[3 * i] = trip_centres[i] - 1; tf3[3 * i + 1] = trip_centres[i]; tf3[3 * i + 2] = trip_centres[i] + 1; }
+  int* d_pf = (int*)call.upload(pf3.data(), pf3.size() * 4); int* d_tf = (int*)call.upload(tf3.data(), tf3.size() * 4);
+  long long* d_po = (long long*)call.upload(pair_offsets, (size_t)(num_pairs + 1) * 8); long long* d_to = (long long*)call.upload(trip_offsets, (size_t)(num_triplets + 1) * 8 * (num_triplets > 0));
+  float* d_pl = (float*)call.upload(pair_locs, (size_t)np_total * 16); float* d_tl = (float*)call.upload(trip_locs, (size_t)nt_total * 24);
+  uint8_t* d_ps = (uint8_t*)call.upload(pair_static, (size_t)np_total); uint8_t* d_ts = (uint8_t*)call.upload(trip_static, (size_t)nt_total);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_prune_static_flags");
+  cudaMemsetAsync(d_bits, 0, bits_bytes, call.st);
+  k_prune_stamp<<<dim3(8, num_pairs), 256, 0, call.st>>>(d_bits, h, w, words, distance, d_pf, d_po, num_pairs, d_pl, d_ps); g_flag_launches++;
+  k_prune_lookup<<<dim3(8, num_pairs), 256, 0, call.st>>>(d_bits, h, w, words, 2, d_pf, d_po, num_pairs, d_pl, d_ps); g_flag_launches++;
+  if (nt_total > 0) { k_prune_lookup<<<dim3(8, num_triplets), 256, 0, call.st>>>(d_bits, h, w, words, 3, d_tf, d_to, num_triplets, d_tl, d_ts); g_flag_launches++; }
+  cudaMemcpyAsync(pair_static, d_ps, (size_t)np_total, cudaMemcpyDeviceToHost, call.st);
+  if (nt_total > 0) cudaMemcpyAsync(trip_static, d_ts, (size_t)nt_total, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("static-flag pruning kernels");
 }
 
 // ---------------------------------------------------------------------------

@@ -202,15 +202,21 @@ Image FlowConstraintsCollection::dynamicDistance(int frame) {   // :257-286
   std::fill(d.ptr<float>(), d.ptr<float>() + size_t(d.rows) * d.cols, 3.402823466e+38f);
   return d;
 }
+// RCVD_CONSTRAINT_BUILDER: unset, empty or "gpu" selects the device path of the constraint operations, "host" the sequential
+// restatement; anything else is an error.  There is no automatic fallback.
+static bool hostConstraintPath() {
+  const char* sel = std::getenv("RCVD_CONSTRAINT_BUILDER");
+  if (sel && !(std::string(sel) == "host" || std::string(sel) == "gpu" || std::string(sel).empty())) throw std::runtime_error("RCVD_CONSTRAINT_BUILDER must be 'gpu' or 'host'.");
+  return sel && std::string(sel) == "host";
+}
 void FlowConstraintsCollection::compute() {
   logInfo("Computing constraints...");
-  const char* sel = std::getenv("RCVD_CONSTRAINT_BUILDER");
-  if (sel && std::string(sel) == "host") {
+  if (hostConstraintPath()) {
     for (auto& kv : pairs_) compute(kv.first);
     for (auto& kv : triplets_) computeTriplet(kv.first);
-  } else if (!sel || std::string(sel) == "gpu" || std::string(sel).empty()) {
+  } else {
     computeOnDevice();
-  } else throw std::runtime_error("RCVD_CONSTRAINT_BUILDER must be 'gpu' or 'host'.");
+  }
 }
 
 namespace {
@@ -454,9 +460,7 @@ void FlowConstraintsCollection::setStaticFlagFromDynamicMask(int distance) {   /
   {
     // default: distance transforms + per-constraint lookups on the device (rcvd_static_flags); RCVD_CONSTRAINT_BUILDER=host
     // selects the sequential restatement below (no automatic fallback)
-    const char* sel = std::getenv("RCVD_CONSTRAINT_BUILDER");
-    if (sel && !(std::string(sel) == "host" || std::string(sel) == "gpu" || std::string(sel).empty())) throw std::runtime_error("RCVD_CONSTRAINT_BUILDER must be 'gpu' or 'host'.");
-    if (!sel || std::string(sel) != "host") {
+    if (!hostConstraintPath()) {
       const int F = video_->numFrames(); const size_t plane = size_t(w) * h;
       std::vector<uint8_t> masks(size_t(F) * plane, 255);
       std::vector<uint8_t> used(F, 0);
@@ -505,6 +509,33 @@ void FlowConstraintsCollection::setStaticFlagFromDynamicMask(int distance) {   /
 void FlowConstraintsCollection::pruneStaticFlag(int distance) {   // :662-748
   ColorStream& ds = video_->colorStream("down");
   const int w = ds.width(), h = ds.height();
+  const bool host = hostConstraintPath();
+  // the stamps come from non-static pair constraints only: without one (or with a negative radius, where the reference fails in
+  // OpenCV's Mat allocation) no flag can change
+  bool anyDynamic = false;
+  for (auto& kv : pairs_) for (auto& c : kv.second) anyDynamic = anyDynamic || !c.isStatic;
+  if (!anyDynamic || distance < 0) return;
+  if (!host) {
+    // default: disc stamps into per-frame bit planes + per-constraint lookups on the device (rcvd_prune_static_flags)
+    const int F = video_->numFrames();
+    std::vector<int32_t> pf, tf; std::vector<int64_t> po(1, 0), to(1, 0); std::vector<float> pl, tl; std::vector<uint8_t> ps, ts;
+    for (auto& kv : pairs_) {
+      pf.push_back(kv.first.first); pf.push_back(kv.first.second);
+      for (auto& c : kv.second) { pl.insert(pl.end(), &c.loc[0][0], &c.loc[0][0] + 4); ps.push_back(c.isStatic ? 1 : 0); }
+      po.push_back(po.back() + int64_t(kv.second.size()));
+    }
+    for (auto& kv : triplets_) {
+      tf.push_back(kv.first);
+      for (auto& c : kv.second) { tl.insert(tl.end(), &c.loc[0][0], &c.loc[0][0] + 6); ts.push_back(c.isStatic ? 1 : 0); }
+      to.push_back(to.back() + int64_t(kv.second.size()));
+    }
+    const int rc = rcvd_prune_static_flags(currentDevice(), F, h, w, distance, int(pf.size() / 2), pf.data(), po.data(), pl.data(), ps.data(),
+                                           int(tf.size()), tf.data(), to.data(), tl.data(), ts.data());
+    if (rc != RCVD_OK) throw std::runtime_error(std::string("rcvd_prune_static_flags failed: ") + rcvd_last_error());
+    size_t i = 0; for (auto& kv : pairs_) for (auto& c : kv.second) c.isStatic = ps[i++] != 0;
+    i = 0; for (auto& kv : triplets_) for (auto& c : kv.second) c.isStatic = ts[i++] != 0;
+    return;
+  }
   const int size = 2 * distance + 1;
   std::vector<uint8_t> disk(size_t(size) * size);
   for (int y = 0; y < size; ++y) for (int x = 0; x < size; ++x) { const int rx = x - distance, ry = y - distance; disk[size_t(y) * size + x] = (rx * rx + ry * ry <= distance * distance) ? 255 : 0; }
@@ -520,14 +551,16 @@ void FlowConstraintsCollection::pruneStaticFlag(int distance) {   // :662-748
         for (int my = my0; my <= my1; ++my) for (int mx = mx0; mx <= mx1; ++mx) if (disk[size_t(my - (y - distance)) * size + (mx - (x - distance))]) masks[frame][size_t(my) * w + mx] = 255;
       }
     }
-  for (auto& kv : pairs_) for (auto& c : kv.second) {
-    const int x0 = int(c.loc[0][0] * w), y0 = int(c.loc[0][1] * w), x1 = int(c.loc[1][0] * w), y1 = int(c.loc[1][1] * w);
-    if (masks[kv.first.first][size_t(y0) * w + x0] || masks[kv.first.second][size_t(y1) * w + x1]) c.isStatic = false;
-  }
-  for (auto& kv : triplets_) for (auto& c : kv.second) {
-    const int x0 = int(c.loc[0][0] * w), y0 = int(c.loc[0][1] * w), x1 = int(c.loc[1][0] * w), y1 = int(c.loc[1][1] * w), x2 = int(c.loc[2][0] * w), y2 = int(c.loc[2][1] * w);
-    if (masks[kv.first - 1][size_t(y0) * w + x0] || masks[kv.first][size_t(y1) * w + x1] || masks[kv.first + 1][size_t(y2) * w + x2]) c.isStatic = false;
-  }
+  // lookups clamped to the image like the device's (k_prune_lookup): with a "down" aspect other than the video's, int(loc.y * w)
+  // can reach h, where the reference reads past the frame
+  auto at = [&](int frame, const float* loc) {
+    const int x = std::min(std::max(int(loc[0] * w), 0), w - 1), y = std::min(std::max(int(loc[1] * w), 0), h - 1);
+    return masks[frame][size_t(y) * w + x] != 0;
+  };
+  for (auto& kv : pairs_) for (auto& c : kv.second)
+    if (at(kv.first.first, c.loc[0]) || at(kv.first.second, c.loc[1])) c.isStatic = false;
+  for (auto& kv : triplets_) for (auto& c : kv.second)
+    if (at(kv.first - 1, c.loc[0]) || at(kv.first, c.loc[1]) || at(kv.first + 1, c.loc[2])) c.isStatic = false;
 }
 
 }  // namespace rcvdh

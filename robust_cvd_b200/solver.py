@@ -427,6 +427,26 @@ def static_flags(masks, distance, pair_frames=None, pair_offsets=None, pair_locs
     return ps, ts, dist
 
 
+def prune_static_flags(num_frames, height, width, distance, pair_frames, pair_offsets, pair_locs, pair_static,
+                       trip_centres=None, trip_offsets=None, trip_locs=None, trip_static=None, device=0):
+    """rcvd_prune_static_flags (FlowConstraintsCollection::pruneStaticFlag, reference lib/FlowConstraints.cpp:662-748) on the GPU.
+    height x width: the "down" stream's size.  Arrays as in static_flags; pair_static / trip_static are the input flags (not modified).
+    Returns the pruned (pair_static u8[n], trip_static u8[m])."""
+    P = len(pair_frames); T = 0 if trip_centres is None else len(trip_centres)
+    pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2) if P else None
+    po = np.ascontiguousarray(pair_offsets, np.int64) if P else None
+    pl = np.ascontiguousarray(pair_locs, np.float32).reshape(-1, 4) if P else None
+    ps = np.array(pair_static, np.uint8).reshape(-1) if P else np.zeros(0, np.uint8)
+    tc = np.ascontiguousarray(trip_centres, np.int32) if T else None
+    to = np.ascontiguousarray(trip_offsets, np.int64) if T else None
+    tl = np.ascontiguousarray(trip_locs, np.float32).reshape(-1, 6) if T else None
+    ts = np.array(trip_static, np.uint8).reshape(-1) if T else np.zeros(0, np.uint8)
+    _check(lib().rcvd_prune_static_flags(C.c_int32(device), C.c_int32(num_frames), C.c_int32(height), C.c_int32(width), C.c_int32(distance),
+                                         C.c_int32(P), _p(pf, C.c_int32), _p(po, C.c_int64), _p(pl, C.c_float), _p(ps if P else None, C.c_uint8),
+                                         C.c_int32(T), _p(tc, C.c_int32), _p(to, C.c_int64), _p(tl, C.c_float), _p(ts if T else None, C.c_uint8)))
+    return ps, ts
+
+
 FP64_MMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
 
 
