@@ -76,7 +76,8 @@ int32_t rcvd_debug_level_profile(rcvd_problem* p, double* out, int32_t max_level
 int32_t rcvd_debug_fp64_tensor_peak(int32_t device, int32_t shape, double* tflops);
 
 /* A/B switches (defaults in parentheses) */
-int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on);        /* (1) specialised accumulate kernels; 0 = generic kernel */
+int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on);        /* (1) specialised accumulate kernels; 0 = generic kernel; 2 = k_accumulate_fast
+                                                                          even where the run path applies (bilinear grids) */
 int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on);          /* (1) two-stream factorisation graph */
 int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack);   /* (4) multiple-elimination degree slack; -1 greedy */
 int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on);        /* (0) cost / gradient evaluations only: no matrix storage (the whole-problem check of a multi-GPU bench) */

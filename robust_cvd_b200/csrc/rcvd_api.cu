@@ -24,15 +24,6 @@
 
 using namespace rcvd;
 
-constexpr int kFastSmem = (3 * kTile * kJsLd + 4 * 256) * (int)sizeof(double);
-static bool run_path_ok_host(const rcvd_config& c, const Layout& L);
-static bool fast_path_ok_host(const rcvd_config& c, const Layout& L) {
-  return L.k == 1 && c.spatial_type == RCVD_SPATIAL_IDENTITY && c.intr_opt != RCVD_INTR_SHARED && !c.fix_poses && !c.fix_depth_xforms &&
-         !c.fix_spatial_xforms && (c.depth_type != RCVD_DEPTH_GRID || !c.depth_cubic);
-}
-
-static bool run_path_ok_host(const rcvd_config& c, const Layout& L) { return fast_path_ok_host(c, L) && c.depth_type == RCVD_DEPTH_GRID && L.G < 65535; }
-
 static thread_local std::string g_err = "";
 int set_err(int code, const char* fmt, ...) {
   char buf[512]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof(buf), fmt, ap); va_end(ap);
@@ -198,7 +189,7 @@ struct rcvd_problem {
   // multi GPU
   int nranks = 1, rank = 0; nccl::Comm comm = nullptr;
   int64_t launches = 0, graph_launches = 0;
-  std::vector<double> h_state; bool state_dirty = false; bool use_fast = true; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
+  std::vector<double> h_state; bool state_dirty = false; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
   cudaStream_t side_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   std::vector<cudaEvent_t> ev_side;   // per level, two each: recorded after the level's side-stream update launches (Level::join waits on them)
   cudaStream_t inv_stream = nullptr; cudaEvent_t ev_inv_join = nullptr;   // k_trinv, off the critical path and off the side stream's
@@ -209,6 +200,7 @@ struct rcvd_problem {
   std::vector<std::pair<int, cudaEvent_t>>* prof = nullptr;
   bool eval_only = false;   // test / bench hook: only rcvd_evaluate is used (no H, no factor storage)
   bool records_sorted = false;   // run path of the accumulate kernel (bilinear depth grid): records sorted by cell pair
+  int fast_path = 1;             // rcvd_debug_set_fast_path
   bool dist_enabled = true, graph_warm = false, force_full_H = false;
   // distributed factorisation (nranks > 1): the frames this rank factors per level, the blocks it owns, internal -> caller's frame ids
   int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr;
@@ -262,13 +254,36 @@ static void free_all(rcvd_problem* p) {
 }
 
 static DevProblem dev_problem(const rcvd_problem* p) {
-  DevProblem d; d.cfg = p->cfg; d.L = p->L; d.N = p->N; d.num_tiles = p->num_tiles; d.num_constraints = p->C;
+  DevProblem d; d.cfg = p->cfg; d.L = p->L; d.N = p->N;
   d.records = p->d_records; d.tile_pair = p->d_tile_pair; d.tile_begin = p->d_tile_begin; d.tile_count = p->d_tile_count;
   d.pair_frames = p->d_pair_frames; d.blk_of = p->d_blk_of; d.in_range = p->d_in_range; d.median = p->d_median;
-  d.adaptive = p->adaptive.empty() ? nullptr : p->d_adaptive; d.scale_locs = p->d_scale_locs; d.num_scale_locs = p->nscale;
+  d.adaptive = p->adaptive.empty() ? nullptr : p->d_adaptive; d.scale_locs = p->d_scale_locs;
   d.rank = p->rank; d.nranks = p->nranks;
-  d.trip_records = p->d_trip_records; d.trip_tile_center = p->d_trip_tile_center; d.trip_tile_begin = p->d_trip_tile_begin; d.trip_tile_count = p->d_trip_tile_count; d.num_trip_tiles = p->num_trip_tiles;
+  d.trip_records = p->d_trip_records; d.trip_tile_center = p->d_trip_tile_center; d.trip_tile_begin = p->d_trip_tile_begin; d.trip_tile_count = p->d_trip_tile_count;
   return d;
+}
+
+// Enqueues the three residual families on the main stream in mode MODE: pair constraints (the one place that chooses their
+// kernel), regulariser rows, smoothness triplets.  Their per-block partial costs fill d_partial in that order; MarkActive marks
+// d_active instead.
+template <EvalMode MODE>
+static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
+  const DevProblem d = dev_problem(p);
+  const RegCounts rcn = reg_counts(p->cfg, p->L, p->N, p->nscale);
+  const int regblocks = (rcn.total + 127) / 128;
+  cudaStream_t st = p->stream; double* part = p->d_partial; int rc;
+  if (p->num_tiles > 0) {
+    const bool tc = MODE == EvalMode::CostGradH && p->fast_path != 0;   // a tensor-core kernel (rcvd_debug_set_fast_path)
+    if (tc && p->fast_path == 1 && p->records_sorted) rc = launch(p, k_accumulate_runs, p->num_tiles, kTile, kRunSmem, st, false, d, x, p->d_H, g, part);
+    else if (tc && fast_path_ok(p->cfg, p->L)) rc = launch(p, k_accumulate_fast, p->num_tiles, kTile, kFastSmem, st, false, d, x, p->d_H, g, part);
+    else rc = launch(p, k_pairs<MODE>, p->num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active);
+    if (rc) return rc;
+  }
+  part += p->num_tiles;
+  if (regblocks > 0 && (rc = launch(p, k_regularisers<MODE>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, g, part, p->d_active, p->first_frame, p->last_frame))) return rc;
+  part += regblocks;
+  if (p->num_trip_tiles > 0 && (rc = launch(p, k_triplets<MODE>, p->num_trip_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active))) return rc;
+  return RCVD_OK;
 }
 
 // ---- structure: the plan on the device, the problem data, the storage ----
@@ -300,7 +315,7 @@ static int set_up_problem_data(rcvd_problem* p) {
     UP(p->d_pair_frames, pf_int); UP(p->d_records, p->records_h);
   }
   p->records_sorted = false;
-  if (run_path_ok_host(p->cfg, L) && p->C > 0 && p->C < (int64_t)0x7fffffff) {
+  if (run_path_ok(p->cfg, L) && p->C > 0 && p->C < (int64_t)0x7fffffff) {
     // run path of the accumulate kernel: the records of every pair sorted by (source cell, target cell) -- device segmented sort by pair
     const long long n = p->C;
     unsigned *d_k0 = nullptr, *d_k1 = nullptr; int *d_i0 = nullptr, *d_i1 = nullptr; float* d_sorted = nullptr; int64_t* d_off = nullptr; void* d_tmp = nullptr;
@@ -398,13 +413,7 @@ static int allocate_storage(rcvd_problem* p) {
   CK(cudaMemsetAsync(p->d_S, 0, Upad * sizeof(double), p->stream));
   // active mask
   CK(cudaMemsetAsync(p->d_active, 0, Upad, p->stream));
-  DevProblem d = dev_problem(p);
-  if (p->num_tiles > 0 && (rc = launch(p, k_mark_static, p->num_tiles, kTile, 0, p->stream, false, d, p->d_active))) return rc;
-  if (rcn.total > 0) {
-    DevProblem d1 = d; d1.nranks = 1; d1.rank = 0;   // mark regardless of rank ownership
-    if ((rc = launch(p, k_regularisers<2>, (rcn.total + 127) / 128, 128, 0, p->stream, false, d1, rcn, p->d_x, nullptr, nullptr, nullptr, p->d_active, p->first_frame, p->last_frame))) return rc;
-  }
-  if (p->num_trip_tiles > 0 && (rc = launch(p, k_triplets<2>, p->num_trip_tiles, kTile, 0, p->stream, false, d, p->d_x, nullptr, nullptr, nullptr, p->d_active))) return rc;
+  if ((rc = enqueue_residuals<EvalMode::MarkActive>(p, p->d_x, nullptr))) return rc;
   if ((rc = launch(p, k_finalize_mask, (int)((Upad + 255) / 256), 256, 0, p->stream, false, p->cfg, L, p->d_active, N))) return rc;
   if (p->nranks > 1) {   // the parameter set of the program is the union over the ranks' constraint shards (norms and stopping tests must agree on every rank)
     const int r = nccl::AllReduce(p->d_active, p->d_active, Upad, nccl::kUint8, nccl::kMax, p->comm, p->stream);
@@ -712,34 +721,12 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
   if (wantH && p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no normal matrix");
   const Layout& L = p->L; const int N = p->N, npad = L.npad; cudaStream_t st = p->stream;
   const size_t bs = (size_t)npad * npad, Upad = (size_t)N * npad;
-  DevProblem d = dev_problem(p);
-  const RegCounts rcn = reg_counts(p->cfg, L, N, p->nscale);
-  const int regblocks = (rcn.total + 127) / 128;
+  const int regblocks = (reg_counts(p->cfg, L, N, p->nscale).total + 127) / 128;
   if (wantH) CK(cudaMemsetAsync(p->d_H, 0, p->plan.hblocks.size() * bs * sizeof(double), st));
   if (wantG) CK(cudaMemsetAsync(gout, 0, (Upad + 8) * sizeof(double), st));
-  int rc;
-  if (p->num_tiles > 0) {
-    if (wantH && p->use_fast && p->records_sorted) rc = launch(p, k_accumulate_runs, p->num_tiles, kTile, kRunSmem, st, false, d, x, p->d_H, gout, p->d_partial);
-    else if (wantH && p->use_fast && fast_path_ok_host(p->cfg, L)) rc = launch(p, k_accumulate_fast, p->num_tiles, kTile, kFastSmem, st, false, d, x, p->d_H, gout, p->d_partial);
-    else if (wantH) rc = launch(p, k_accumulate_generic<true>, p->num_tiles, kTile, 0, st, false, d, x, p->d_H, gout, p->d_partial);
-    else if (wantG) rc = launch(p, k_accumulate_generic<false>, p->num_tiles, kTile, 0, st, false, d, x, nullptr, gout, p->d_partial);
-    else rc = launch(p, k_cost_static, p->num_tiles, kTile, 0, st, false, d, x, p->d_partial);
-    if (rc) return rc;
-  }
-  if (regblocks > 0) {
-    double* part = p->d_partial + p->num_tiles;
-    if (wantH) rc = launch(p, k_regularisers<1>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, gout, part, nullptr, p->first_frame, p->last_frame);
-    else if (wantG) rc = launch(p, k_regularisers<3>, regblocks, 128, 0, st, false, d, rcn, x, nullptr, gout, part, nullptr, p->first_frame, p->last_frame);
-    else rc = launch(p, k_regularisers<0>, regblocks, 128, 0, st, false, d, rcn, x, nullptr, nullptr, part, nullptr, p->first_frame, p->last_frame);
-    if (rc) return rc;
-  }
-  if (p->num_trip_tiles > 0) {
-    double* part = p->d_partial + p->num_tiles + regblocks;
-    if (wantH) rc = launch(p, k_triplets<1>, p->num_trip_tiles, kTile, 0, st, false, d, x, p->d_H, gout, part, nullptr);
-    else if (wantG) rc = launch(p, k_triplets<3>, p->num_trip_tiles, kTile, 0, st, false, d, x, nullptr, gout, part, nullptr);
-    else rc = launch(p, k_triplets<0>, p->num_trip_tiles, kTile, 0, st, false, d, x, nullptr, nullptr, part, nullptr);
-    if (rc) return rc;
-  }
+  int rc = wantH ? enqueue_residuals<EvalMode::CostGradH>(p, x, gout)
+           : wantG ? enqueue_residuals<EvalMode::CostGrad>(p, x, gout) : enqueue_residuals<EvalMode::Cost>(p, x, gout);
+  if (rc) return rc;
   if ((rc = launch(p, k_reduce_partials, 1, 1024, 0, st, false, p->d_partial, p->num_tiles + regblocks + p->num_trip_tiles, p->d_scal, slot))) return rc;
   if (p->nranks > 1) {
     if (wantG) {
@@ -1518,8 +1505,14 @@ RCVD_API int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]) {
   out[0] = p->plan.dist ? 1 : 0; out[1] = p->plan.LB; out[2] = (int)p->plan.levels.size(); out[3] = p->plan.dist ? p->plan.fa_cnt[p->rank] + p->plan.fb_cnt[p->rank] : p->N;
   return RCVD_OK;
 }
-// Test hook: 0 = generic accumulate kernel (the tests' reference), 1 (default) = specialised kernels (run path on a bilinear depth grid).
-RCVD_API int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->use_fast = on != 0; return RCVD_OK; }
+// Test hook: 0 = generic accumulate kernel (the tests' reference), 1 (default) = specialised kernels (run path on a bilinear depth grid),
+// 2 = k_accumulate_fast even where the run path applies (sorted records are valid input for it): the only way to run its Grid branch
+// below 65535 grid nodes.
+RCVD_API int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on) {
+  if (!p) return RCVD_ERR_INVALID;
+  if (on < 0 || on > 2) return set_err(RCVD_ERR_INVALID, "fast path switch must be 0, 1 or 2 (got %d)", on);
+  p->fast_path = on; return RCVD_OK;
+}
 RCVD_API int32_t rcvd_solve(rcvd_problem* p, const rcvd_solve_options* opt, rcvd_solve_summary* summary) {
   if (!p || !summary) return set_err(RCVD_ERR_INVALID, "null argument");
   SET_DEVICE(p->device);

@@ -71,14 +71,19 @@ __device__ __forceinline__ void cubic_spline(double w[4], double t) {
   w[2] = __dadd_rn(__dadd_rn(__dmul_rn(-1.5, t3), __dmul_rn(2.0, t2)), __dmul_rn(0.5, t));
   w[3] = __dsub_rn(__dmul_rn(0.5, t3), __dmul_rn(0.5, t2));
 }
-// linearGather spatial branch (:822-840) and bilinearSpatialGridGather (:1253-1286)
-__device__ __forceinline__ void gather_bilinear(float lx, float ly, int gx, int gy, Gather& g) {
+// The bilinear cell holding (lx, ly): returns its top-left node b and the weights of the nodes b, b + 1, b + gx, b + gx + 1.
+// Every bilinear gather goes through here, the run path's sort key included, so all of them agree on the cell and its rounding.
+__device__ __forceinline__ int bilinear_cell(float lx, float ly, int gx, int gy, double w[4]) {
   int ix, iy; double rx, ry;
   cell_coord(lx, gx, ix, rx); cell_coord(ly, gy, iy, ry);
-  g.n = 4;
-  g.idx[0] = ix + iy * gx; g.idx[1] = ix + 1 + iy * gx; g.idx[2] = ix + (iy + 1) * gx; g.idx[3] = ix + 1 + (iy + 1) * gx;
   const double ox = __dsub_rn(1.0, rx), oy = __dsub_rn(1.0, ry);
-  g.w[0] = __dmul_rn(ox, oy); g.w[1] = __dmul_rn(rx, oy); g.w[2] = __dmul_rn(ox, ry); g.w[3] = __dmul_rn(rx, ry);
+  w[0] = __dmul_rn(ox, oy); w[1] = __dmul_rn(rx, oy); w[2] = __dmul_rn(ox, ry); w[3] = __dmul_rn(rx, ry);
+  return ix + iy * gx;
+}
+// linearGather spatial branch (:822-840) and bilinearSpatialGridGather (:1253-1286)
+__device__ __forceinline__ void gather_bilinear(float lx, float ly, int gx, int gy, Gather& g) {
+  const int b = bilinear_cell(lx, ly, gx, gy, g.w);
+  g.n = 4; g.idx[0] = b; g.idx[1] = b + 1; g.idx[2] = b + gx; g.idx[3] = b + gx + 1;
 }
 // cubicGather (:853-948, gz == 1) and bicubicSpatialGridGather (:1288-1343): taps outside the
 // grid are not created; their weight is folded onto the nearest in-range tap.

@@ -240,7 +240,8 @@ class Problem:
         return dict(zip(keys, list(out)))
 
     def set_fast_path(self, on=True):
-        """Test hook: False forces the generic accumulate kernel (the tests' reference); True (default) allows the specialised ones."""
+        """Test hook: False forces the generic accumulate kernel (the tests' reference); True (default) allows the specialised ones;
+        2 selects k_accumulate_fast even on bilinear grids, where the run path would serve."""
         _check(self.L.rcvd_debug_set_fast_path(self.h, C.c_int32(int(on))))
 
     def set_update_kernel(self, tma=True, side_items_per_cta=0):

@@ -104,11 +104,17 @@ def test_adaptive_deformation_cost_with_node_weights(cubic):
     assert np.linalg.norm(O.get_state() - G.get_state()) <= 1e-4 * np.linalg.norm(O.get_state())
 
 
-@pytest.mark.parametrize("name", ["bilinear_perframe_disp", "global_perframe_disp", "bilinear_fixedintr_ratio", "global_euclid", "identitydepth_perframe"])
-def test_fast_kernel_matches_generic(name):
+# fast_path 1: the default choice (run path on bilinear grids, else k_accumulate_fast); 2: k_accumulate_fast on the bilinear grids too
+FAST_CASES = [(n, 1) for n in ["bilinear_perframe_disp", "global_perframe_disp", "bilinear_fixedintr_ratio", "global_euclid", "identitydepth_perframe"]] + \
+             [(n, 2) for n in ["bilinear_perframe_disp", "bilinear_fixedintr_ratio"]]
+
+
+@pytest.mark.parametrize("name,fast_path", FAST_CASES, ids=[n if f == 1 else n + "-fast_kernel" for n, f in FAST_CASES])
+def test_fast_kernel_matches_generic(name, fast_path):
     overrides = dict(helpers.VARIANTS)[name]
     sc, cfg, O, G, x = _both(overrides)
-    Hf = G.normal_matrix_dense(); cf, gf = G.evaluate(True)      # default: run path on bilinear grids (records sorted by cell pair), else k_accumulate_fast
+    G.set_fast_path(fast_path)
+    Hf = G.normal_matrix_dense(); cf, gf = G.evaluate(True)
     G.set_fast_path(0)
     Hg = G.normal_matrix_dense(); cg, gg = G.evaluate(True)      # generic kernel
     assert np.abs(Hf - Hg).max() <= 1e-10 * np.abs(Hg).max()
