@@ -32,12 +32,13 @@ int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t
 /* the update passes of the same plan, in launch order, caller's frame ids: passes[P][5] = {target row frame, target column frame (equal
  * on a diagonal block), apply level, stream (0: late pass, main stream; 1 / 2: deferred pass in the first / second side-stream launch of
  * its level), source count}; sources = the source frame of every product, pass after pass; join[2 * levels] = per level and side
- * launch, the level whose late passes wait for it (levels: none).  counts = {passes P, products, 2 * levels, tail boundary level,
- * source levels per deferred window below the tail} on return; with passes non-null, counts[0..2] are the capacities of passes (in
- * passes), sources and join on entry. */
+ * launch, the level whose late passes wait for it (levels: none); flags[P] = per pass, bit 0: symmetric (diagonal) target, bit 1: the
+ * first pass into a fill block, which writes the target without reading it.  counts = {passes P, products, 2 * levels, tail boundary
+ * level, source levels per deferred window below the tail} on return; with passes non-null, counts[0..2] are the capacities of passes
+ * and flags (in passes), sources and join on entry. */
 int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
                                  int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
-                                 int32_t* passes, int32_t* sources, int32_t* join, int32_t counts[5]);
+                                 int32_t* passes, int32_t* sources, int32_t* join, int32_t* flags, int32_t counts[5]);
 
 /* y = (S H S + diag(D2))^-1 b with the current H (exercises factorisation + substitution alone) */
 int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y);

@@ -202,8 +202,9 @@ struct rcvd_problem {
   bool records_sorted = false;   // run path of the accumulate kernel (bilinear depth grid): records sorted by cell pair
   int fast_path = 1;             // rcvd_debug_set_fast_path
   bool dist_enabled = true, graph_warm = false, force_full_H = false;
-  // distributed factorisation (nranks > 1): the frames this rank factors per level, the blocks it owns, internal -> caller's frame ids
-  int *d_lvl_own = nullptr, *d_own_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr;
+  // the frames this rank factors per level, the L blocks k_load_factor writes (FactorPlan::load_lblocks), the H blocks this rank owns,
+  // internal -> caller's frame ids
+  int *d_lvl_own = nullptr, *d_load_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr;
   // TMA-fed persistent update kernel (rcvd_update.cuh)
   UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; int num_sms = 0, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
@@ -292,7 +293,7 @@ static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
 static int upload_plan(rcvd_problem* p) {
   const FactorPlan& pl = p->plan; int rc;
   UP(p->d_blk_of, pl.blk_of); UP(p->d_hblocks, pl.hblocks); UP(p->d_lblocks, pl.lblocks); UP(p->d_lvl_frames, pl.lvl_frames); UP(p->d_lvl_own, pl.lvl_own);
-  UP(p->d_own_lblocks, pl.own_lblocks); UP(p->d_own_hblocks, pl.own_hblocks); UP(p->d_uperm, pl.uperm);
+  UP(p->d_load_lblocks, pl.load_lblocks); UP(p->d_own_hblocks, pl.own_hblocks); UP(p->d_uperm, pl.uperm);
   UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_trsm_pairs, pl.trsm_pairs); UP(p->d_upd_pairs, pl.upd_pairs);
   UP(p->d_sub_tasks, pl.sub_tasks); UP(p->d_sub_need, pl.sub_need); DA(p->d_sub_counters, (size_t)4 * p->N + 4);
   UP(p->d_fwd_tasks, pl.fwd_tasks); UP(p->d_trsm_ll, pl.trsm_ll); UP(p->d_upd_items, pl.upd_items);
@@ -659,8 +660,10 @@ static int enqueue_factor_solve(rcvd_problem* p) {
   const FactorPlan& pl = p->plan; const int npad = p->L.npad, nlv = (int)pl.levels.size();
   f.mark(-1);
   CK(cudaMemsetAsync(p->d_potrf_progress, 0, (size_t)p->N * sizeof(int), p->stream));   // no count of the previous factorisation may read as published
-  if (int rc = f.launch(LP_OTHER, k_load_factor, dim3((npad * npad + 255) / 256, pl.dist ? (int)pl.own_lblocks.size() : p->N + pl.nLoff), dim3(256), 0,
-                        p->stream, false, p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, p->L.nf, pl.dist ? p->d_own_lblocks : nullptr)) return rc;
+  // the blocks this rank factors; of the fill blocks only the padding, their interior is written by their first update pass
+  const int nfill = (int)pl.load_lblocks.size() - pl.nload;
+  if (int rc = f.launch(LP_OTHER, k_load_factor, dim3((npad * npad + 255) / 256, pl.nload + load_factor_pad_rows(npad, pl.upd_neff, nfill)), dim3(256), 0,
+                        p->stream, false, p->d_H, p->d_Lb, p->d_lblocks, p->d_S, p->d_D2, npad, p->L.nf, pl.upd_neff, p->d_load_lblocks, pl.nload, nfill)) return rc;
   f.mark(FactorSolve::P_LOAD);
   for (int li = 0; li < nlv; ++li) {
     const Level& lv = pl.levels[li]; f.prof_level = li;
@@ -1550,13 +1553,13 @@ RCVD_API int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, cons
 // Test hook: the update passes of the plan of a frame graph (see include/rcvd_hooks.h).
 RCVD_API int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
                                           int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
-                                          int32_t* passes, int32_t* sources, int32_t* join, int32_t counts[5]) {
+                                          int32_t* passes, int32_t* sources, int32_t* join, int32_t* flags, int32_t counts[5]) {
   if (!counts) return set_err(RCVD_ERR_INVALID, "null argument");
   FactorPlan pl;
   if (int32_t rc = debug_plan(pl, cfg, np, pairs, nt, trip_centers, order_slack, nranks, rank, num_sms)) return rc;
   const int32_t need[3] = {(int32_t)pl.upd_tasks.size(), (int32_t)pl.upd_pairs.size(), 2 * (int32_t)pl.levels.size()};
   if (passes) {
-    if (!sources || !join || counts[0] < need[0] || counts[1] < need[1] || counts[2] < need[2]) return set_err(RCVD_ERR_INVALID, "null or short output array");
+    if (!sources || !join || !flags || counts[0] < need[0] || counts[1] < need[1] || counts[2] < need[2]) return set_err(RCVD_ERR_INVALID, "null or short output array");
     const int N = cfg->num_frames;
     for (size_t l = 0; l < pl.levels.size(); ++l) {
       const Level& lv = pl.levels[l];
@@ -1566,6 +1569,7 @@ RCVD_API int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, co
         const HBlock& b = pl.lblocks[t.dst];
         int32_t* o = passes + 5 * (size_t)q;
         o[0] = pl.uperm[b.r]; o[1] = pl.uperm[b.c]; o[2] = (int32_t)l; o[3] = q >= lv.upd2_off[1] ? 2 : q >= lv.upd2_off[0] ? 1 : 0; o[4] = t.count;
+        flags[q] = t.lower_only;
         for (int i = 0; i < t.count; ++i) sources[t.first + i] = pl.uperm[pl.lblocks[N + pl.upd_pairs[t.first + i].x].c];
       }
     }

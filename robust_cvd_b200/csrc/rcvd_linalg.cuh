@@ -437,7 +437,7 @@ __global__ void __launch_bounds__(256) k_trinv(const double* __restrict__ Lb, co
 // K staged 16 at a time through a cp.async double buffer.  The short last tile row is cheap because out-of-range mma tiles
 // are never issued.
 // ---------------------------------------------------------------------------
-struct GemmTask { int dst; int first; int count; int lower_only; };   // lower_only bit0: symmetric update target (tiles above the diagonal are never read)
+struct GemmTask { int dst; int first; int count; int lower_only; };   // lower_only bit0: symmetric update target (tiles above the diagonal are never read); bit1: first pass into a fill block (the target is written, not read)
 
 constexpr int kGemmLd = 20;   // padded leading dimension of the 64x16 smem tiles (conflict-free DMMA fragment loads)
 
@@ -965,18 +965,31 @@ __global__ void __launch_bounds__(kSubThreads) k_substitution(const double* __re
 __host__ __device__ inline size_t substitution_smem_bytes(int) { return (size_t)8 * (kSubChunk + 2) * sizeof(double); }
 
 // ---------------------------------------------------------------------------
-// Factor load: L <- S H S + D2 (lower triangle of diagonal blocks, pad diagonal = 1)
-// grid: (ceil(npad*npad/256), H blocks)
+// Factor load: L <- S H S + D2 (lower triangle of diagonal blocks, pad diagonal = 1) for the blocks blist[0, nload), zeros in the
+// padding of the fill blocks blist[nload, nload + nfill) (rows neff..npad, and columns neff..npad of rows < neff).  The interior of a
+// fill block is written by its first update pass (kUpdFirstFill), which covers rows and columns < neff; the padding still holds the
+// previous factorisation's values.
+// grid: (ceil(npad*npad/256), nload + enough rows of CTAs for the fill padding)
 // ---------------------------------------------------------------------------
 struct HBlock { int lblk; int r; int c; };   // H list: lblk = destination block in L.  L list: lblk = source block in H (or -1: fill)
 __global__ void __launch_bounds__(256) k_load_factor(const double* __restrict__ H, double* __restrict__ Lb, const HBlock* __restrict__ lb,
-                                                      const double* __restrict__ S, const double* __restrict__ D2, int npad, int nf, const int* __restrict__ blist) {
-  const int bid = blist ? blist[blockIdx.y] : blockIdx.y;   // L block id (blist: the blocks this rank owns)
+                                                      const double* __restrict__ S, const double* __restrict__ D2, int npad, int nf, int neff,
+                                                      const int* __restrict__ blist, int nload, int nfill) {
+  const size_t bs = (size_t)npad * npad;
+  if ((int)blockIdx.y >= nload) {
+    const int ph = npad - neff, per = ph * (npad + neff);     // padding elements per fill block: ph full rows, then ph columns of neff rows
+    const long q = ((long)(blockIdx.y - nload) * gridDim.x + blockIdx.x) * 256 + threadIdx.x;
+    if (per == 0 || q >= (long)nfill * per) return;
+    const int f = (int)(q / per), e = (int)(q % per), r = e - ph * npad;
+    const int i = r < 0 ? neff + e / npad : r / ph, j = r < 0 ? e % npad : neff + r % ph;
+    Lb[(size_t)blist[nload + f] * bs + (size_t)i * npad + j] = 0.0;
+    return;
+  }
+  const int bid = blist[blockIdx.y];
   const HBlock b = lb[bid];
   const int e = blockIdx.x * 256 + threadIdx.x;
   if (e >= npad * npad) return;
   const int i = e / npad, j = e % npad;
-  const size_t bs = (size_t)npad * npad;
   double v = 0.0;
   if (b.r == b.c) {
     if (j > i) v = 0.0;
@@ -985,10 +998,14 @@ __global__ void __launch_bounds__(256) k_load_factor(const double* __restrict__ 
       v = H[(size_t)b.lblk * bs + e] * S[(size_t)b.r * npad + i] * S[(size_t)b.c * npad + j];
       if (i == j) v += D2[(size_t)b.r * npad + i];
     }
-  } else if (b.lblk >= 0 && i < nf && j < nf) {
+  } else if (i < nf && j < nf) {
     v = H[(size_t)b.lblk * bs + e] * S[(size_t)b.r * npad + i] * S[(size_t)b.c * npad + j];
   }
   Lb[(size_t)bid * bs + e] = v;
+}
+__host__ __device__ inline int load_factor_pad_rows(int npad, int neff, int nfill) {   // grid rows of k_load_factor for the fill padding
+  const long per = (long)(npad - neff) * (npad + neff), row = (long)((npad * npad + 255) / 256) * 256;
+  return (int)(((long)nfill * per + row - 1) / row);
 }
 
 // out += H v over the original block structure (symmetric; diagonal blocks hold the lower triangle).

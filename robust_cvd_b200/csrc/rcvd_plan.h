@@ -38,6 +38,7 @@ struct FactorPlan {
   std::vector<HBlock> hblocks, lblocks;        // lblocks: every L block with its H source (or -1: fill)
   std::vector<int32_t> blk_of;                 // N x N frame pair -> 2 * H block + (pair's first frame is the row side), or -1
   std::vector<int> own_lblocks, own_hblocks;   // blocks this rank loads into the factor / multiplies in the model term (all without distribution)
+  std::vector<int> load_lblocks; int nload = 0;  // k_load_factor's list: own_lblocks with an H source or diagonal (nload), then the fill blocks
   // task lists of the level schedule
   std::vector<int> lvl_frames, lvl_own;
   std::vector<GemmTask> trsm_tasks, upd_tasks; std::vector<int2> trsm_pairs, upd_pairs;
@@ -194,6 +195,9 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
   P.elim_order = order; P.level = lvl; P.owner = own;
   for (int b = 0; b < N + nLoff; ++b) { const int c = b < N ? b : lcol[b - N]; if (!dist || own[c] == rank) P.own_lblocks.push_back(b); }
   for (int h = 0; h < nHblocks; ++h) if (!dist || own[hblocks[h].c] == rank) P.own_hblocks.push_back(h);
+  for (int b : P.own_lblocks) if (P.lblocks[b].lblk >= 0) P.load_lblocks.push_back(b);
+  P.nload = (int)P.load_lblocks.size();
+  for (int b : P.own_lblocks) if (P.lblocks[b].lblk < 0) P.load_lblocks.push_back(b);
   // tile cut of the update targets: kUpdMaxTile-row tiles over the unknowns (rounded to 8)
   const int upd_neff = std::min(npad, (L.nf + 7) / 8 * 8);
   const int upd_nt = (upd_neff + kUpdMaxTile - 1) / kUpdMaxTile;
@@ -203,13 +207,15 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
   // lives in column c, and a rank updates only the columns it owns in phase A.
   auto col_of = [&](int target) { return target < N ? target : lcol[target - N]; };
   std::map<int, std::vector<std::pair<int, int2>>> prod;   // target L block id -> (source level, source pair)
+  std::map<int, int> first_level;                           // target L block id -> earliest source level of any rank's products into it
   for (int l = 0; l < nl; ++l) {
     const bool shared_level = !dist || l >= LB;   // replicated work: every rank does all of it
     std::set<int> targets;
     for (int k : lf[l]) for (size_t a = 0; a < cs[k].size(); ++a) for (size_t b = 0; b <= a; ++b) {
       const int r = cs[k][a], c = cs[k][b];
-      if (!shared_level && own[c] != rank) continue;
       const int target = (r == c) ? r : lid[{r, c}];
+      first_level.emplace(target, l);
+      if (!shared_level && own[c] != rank) continue;
       prod[target].push_back({l, make_int2(lid[{r, k}] - N, lid[{c, k}] - N)});
       targets.insert(target);
     }
@@ -219,6 +225,11 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
   // at Lc - 1, on the critical path.  The earlier products are deferred to the side stream, grouped in level windows (wide levels only,
   // see kUpdWindow), each window one pass applied at the level of its latest source: every pass reads and writes the whole target, so
   // fewer, longer passes move less of it through memory.  Within a level the passes are in target order.
+  // The first pass into a fill block (an L block without an H source; k_load_factor leaves its interior alone) writes the target without
+  // reading it.  Passes into one target run in launch order (the side stream is in order, and a late pass waits for its target's
+  // deferred passes), so the first one enqueued is the first one executed.  Distributed, a rank's first pass is the block's first only if
+  // it holds the block's earliest product: the phase-A passes into a phase-B column run on its owner alone, and the other ranks receive
+  // the block with the broadcast at the phase boundary.
   const int W = P.upd_window = L.nf <= kUpdWindowMaxNf ? kUpdWindow : 1;
   auto window = [&](int l) { return l < TB ? l / W : nl + l; };
   std::vector<std::vector<std::pair<int, std::vector<int2>>>> late(nl), deferred(nl);   // per apply level: (target, source pairs)
@@ -233,6 +244,7 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
       for (size_t q = i; q < j; ++q) pass.back().second.push_back(v[q].second);
     }
   }
+  std::vector<uint8_t> updated(N + nLoff, 0);   // per L block: a pass into it is enqueued already
   for (int l = 0; l < nl; ++l) {
     Level lv; lv.frame_off = (int)P.lvl_frames.size(); lv.nframes = (int)lf[l].size(); lv.own_off = (int)P.lvl_own.size();
     lv.trsm_off = (int)P.trsm_tasks.size(); lv.upd_off = (int)P.upd_tasks.size(); lv.fwd_off = (int)P.fwd_tasks.size();
@@ -261,7 +273,9 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
         const int Lc = lvl[col_of(tp.first)];
         if (pass > 0 && (!split || Lc == l + 2) != (pass == 1)) continue;
         if (pass > 0) lv.join[pass - 1] = std::min(lv.join[pass - 1], Lc - 1);
-        P.upd_tasks.push_back({tp.first, (int)P.upd_pairs.size(), (int)tp.second.size(), tp.first < N ? 1 : 0});
+        const bool first_fill = P.lblocks[tp.first].lblk < 0 && !updated[tp.first] && prod[tp.first][0].first == first_level[tp.first];
+        updated[tp.first] = 1;
+        P.upd_tasks.push_back({tp.first, (int)P.upd_pairs.size(), (int)tp.second.size(), (tp.first < N ? 1 : 0) | (first_fill ? 2 : 0)});
         { const double n = (double)L.nf; P.upd_flops += (double)tp.second.size() * (tp.first < N ? n * n * (n + 1.0) : 2.0 * n * n * n); }
         P.upd_pairs.insert(P.upd_pairs.end(), tp.second.begin(), tp.second.end());
       }
@@ -278,11 +292,11 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
         for (int ti = 0; ti < upd_nt; ++ti) for (int tj = 0; tj < ((tk.lower_only & 1) ? ti + 1 : upd_nt); ++tj) {
           UpdItem it; it.dst = tk.dst; it.first = tk.first; it.count = tk.count; it.m0 = (short)(ti * upd_tile); it.n0 = (short)(tj * upd_tile);
           it.mrows = (short)std::min(upd_tile, upd_neff - ti * upd_tile); it.ncols = (short)std::min(upd_tile, upd_neff - tj * upd_tile);
-          it.flags = ((tk.lower_only & 1) && ti == tj) ? 1 : 0;
+          it.flags = (((tk.lower_only & 1) && ti == tj) ? kUpdSymDiag : 0) | ((tk.lower_only & 2) ? kUpdFirstFill : 0);
           items.push_back(it);
         }
       }
-      auto cost = [](const UpdItem& a) { return (long)a.count * (a.mrows / 8) * (a.ncols / 8) * ((a.flags & 1) ? 3 : 4); };
+      auto cost = [](const UpdItem& a) { return (long)a.count * (a.mrows / 8) * (a.ncols / 8) * ((a.flags & kUpdSymDiag) ? 3 : 4); };
       std::stable_sort(items.begin() + i0, items.end(), [&](const UpdItem& a, const UpdItem& b) { return cost(a) > cost(b); });
       if (pass) { lv.it2_off[pass - 1] = (int)i0; lv.nit2[pass - 1] = (int)(items.size() - i0); } else { lv.it_off = (int)i0; lv.nit = (int)(items.size() - i0); }
     }

@@ -81,16 +81,18 @@ def update_passes(cfg, pairs, trip_centers=(), order_slack=4, nranks=1, rank=0, 
     """Test hook: the update passes of factor_plan's plan, in launch order (host only).  Returns passes [P, 5] (target row frame, target
     column frame, apply level, stream: 0 late / main, 1 or 2 deferred / the level's first or second side launch, source count), sources
     (the source frame of every product, pass after pass), join ([levels, 2]: per side launch, the level whose late passes wait for it),
-    tail (the tail boundary level) and window (source levels per window of the deferred passes)."""
+    flags ([P]: bit 0 symmetric target, bit 1 the first pass into a fill block, which writes its target without reading it), tail (the
+    tail boundary level) and window (source levels per window of the deferred passes)."""
     pf = np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
     tc = np.ascontiguousarray(np.asarray(trip_centers, np.int32).reshape(-1))
     args = (C.byref(cfg), C.c_int32(pf.shape[0]), _p(pf, C.c_int32), C.c_int32(tc.size), _p(tc, C.c_int32),
             C.c_int32(order_slack), C.c_int32(nranks), C.c_int32(rank), C.c_int32(num_sms))
     counts = (C.c_int32 * 5)()
-    _check(lib().rcvd_debug_update_passes(*args, None, None, None, counts))
+    _check(lib().rcvd_debug_update_passes(*args, None, None, None, None, counts))
     passes, sources, join = np.zeros((counts[0], 5), np.int32), np.zeros(counts[1], np.int32), np.zeros(counts[2], np.int32)
-    _check(lib().rcvd_debug_update_passes(*args, _p(passes, C.c_int32), _p(sources, C.c_int32), _p(join, C.c_int32), counts))
-    return {"passes": passes, "sources": sources, "join": join.reshape(-1, 2), "tail": counts[3], "window": counts[4]}
+    flags = np.zeros(counts[0], np.int32)
+    _check(lib().rcvd_debug_update_passes(*args, _p(passes, C.c_int32), _p(sources, C.c_int32), _p(join, C.c_int32), _p(flags, C.c_int32), counts))
+    return {"passes": passes, "sources": sources, "join": join.reshape(-1, 2), "flags": flags, "tail": counts[3], "window": counts[4]}
 
 
 class Problem:
