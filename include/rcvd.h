@@ -19,6 +19,8 @@
  *   addFocalRegularization (:1524-1549),        |
  *   addPositionRegularization (:1417-1447)      |
  *   addSceneFlowSmoothnessLoss (:1242-1339)     | rcvd_problem_set_triplets
+ *   DisparityDissimilarityCost rows of          | rcvd_problem_set_depth_pairs
+ *     normalizeDepth (:1005-1095)               |
  *   poseParams_ / xform params_ (:748-783)      | rcvd_problem_set_state / get_state
  *   ceres::Solve (:954-962, :1117-1125)         | rcvd_solve
  *
@@ -172,6 +174,15 @@ int32_t rcvd_problem_set_constraints(rcvd_problem* p, int32_t num_pairs, const i
  * smoothDynamicWeight, :1314-1317).  Optional; absent by default as in the reference (both weights 0). */
 int32_t rcvd_problem_set_triplets(rcvd_problem* p, int32_t num_groups, const int32_t* centers,
                                   const int64_t* offsets, const float* records);
+
+/* Pairwise depth normalisation (normalizeDepth with normalizeDepthFromFirstFrame = false, lib/PoseOptimizer.cpp:1005-1095):
+ * one DisparityDissimilarityCost row per constraint, r = 1 / max(D0, 1e-6) - 1 / max(D1, 1e-6) with D the depth of each end
+ * through its frame's depth transform, robustified by robust_type / robustness (the reference: CauchyLoss(robustness)).  Every
+ * constraint of the pair counts, static or not; no pose, focal or static_depth_weight enters.  Arrays and validation as in
+ * rcvd_problem_set_constraints (pair_frames[P][2], offsets[P+1], records[C][6]).  Optional and additive to the other families;
+ * not sharded: with nranks > 1 this call (and a later solve) fails with RCVD_ERR_INVALID. */
+int32_t rcvd_problem_set_depth_pairs(rcvd_problem* p, int32_t num_pairs, const int32_t* pair_frames,
+                                     const int64_t* offsets, const float* records);
 
 /* Multi-GPU: this rank only holds a shard of the pairs; accumulated normal
  * equations and costs are all-reduced over `nranks` ranks with NCCL.

@@ -162,6 +162,9 @@ struct rcvd_problem {
   std::vector<int32_t> struct_pairs;   // global frame-pair graph (multi-GPU); empty -> local pairs
   std::vector<int32_t> trip_centers; std::vector<int64_t> trip_offsets; std::vector<float> trip_records;   // smoothness triplets
   float* d_trip_records = nullptr; int32_t *d_trip_tile_center = nullptr, *d_trip_tile_count = nullptr; int64_t* d_trip_tile_begin = nullptr; int num_trip_tiles = 0;
+  std::vector<int32_t> dp_pair_frames; std::vector<int64_t> dp_offsets; std::vector<float> dp_records;   // pairwise depth normalisation
+  float* d_dp_records = nullptr; int32_t *d_dp_pair_frames = nullptr, *d_dp_tile_pair = nullptr, *d_dp_tile_count = nullptr; int64_t* d_dp_tile_begin = nullptr;
+  int num_dp_tiles = 0;
   int first_frame = 0, last_frame = -1;
   // device problem data
   float* d_records = nullptr; int32_t *d_tile_pair = nullptr, *d_tile_count = nullptr, *d_pair_frames = nullptr, *d_blk_of = nullptr;
@@ -261,12 +264,14 @@ static DevProblem dev_problem(const rcvd_problem* p) {
   d.adaptive = p->adaptive.empty() ? nullptr : p->d_adaptive; d.scale_locs = p->d_scale_locs;
   d.rank = p->rank; d.nranks = p->nranks;
   d.trip_records = p->d_trip_records; d.trip_tile_center = p->d_trip_tile_center; d.trip_tile_begin = p->d_trip_tile_begin; d.trip_tile_count = p->d_trip_tile_count;
+  d.dp_records = p->d_dp_records; d.dp_pair_frames = p->d_dp_pair_frames; d.dp_tile_pair = p->d_dp_tile_pair; d.dp_tile_begin = p->d_dp_tile_begin;
+  d.dp_tile_count = p->d_dp_tile_count;
   return d;
 }
 
-// Enqueues the three residual families on the main stream in mode MODE: pair constraints (the one place that chooses their
-// kernel), regulariser rows, smoothness triplets.  Their per-block partial costs fill d_partial in that order; MarkActive marks
-// d_active instead.
+// Enqueues the four residual families on the main stream in mode MODE: pair constraints (the one place that chooses their
+// kernel), regulariser rows, smoothness triplets, depth-normalisation pairs.  Their per-block partial costs fill d_partial in that
+// order; MarkActive marks d_active instead.
 template <EvalMode MODE>
 static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
   const DevProblem d = dev_problem(p);
@@ -284,6 +289,8 @@ static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
   if (regblocks > 0 && (rc = launch(p, k_regularisers<MODE>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, g, part, p->d_active, p->first_frame, p->last_frame))) return rc;
   part += regblocks;
   if (p->num_trip_tiles > 0 && (rc = launch(p, k_triplets<MODE>, p->num_trip_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active))) return rc;
+  part += p->num_trip_tiles;
+  if (p->num_dp_tiles > 0 && (rc = launch(p, k_depth_pairs<MODE>, p->num_dp_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active))) return rc;
   return RCVD_OK;
 }
 
@@ -341,6 +348,14 @@ static int set_up_problem_data(rcvd_problem* p) {
     UP(p->d_trip_tile_center, tc); UP(p->d_trip_tile_begin, tb); UP(p->d_trip_tile_count, tn); UP(p->d_trip_records, p->trip_records);
   }
   {
+    std::vector<int32_t> tp, tn, pf(p->dp_pair_frames.size()); std::vector<int64_t> tb;
+    for (size_t i = 0; i + 1 < p->dp_offsets.size(); ++i)
+      for (int64_t b = p->dp_offsets[i]; b < p->dp_offsets[i + 1]; b += kTile) { tp.push_back((int32_t)i); tb.push_back(b); tn.push_back((int32_t)std::min<int64_t>(kTile, p->dp_offsets[i + 1] - b)); }
+    for (size_t i = 0; i < pf.size(); ++i) pf[i] = p->plan.iperm[p->dp_pair_frames[i]];
+    p->num_dp_tiles = (int)tp.size();
+    UP(p->d_dp_tile_pair, tp); UP(p->d_dp_tile_begin, tb); UP(p->d_dp_tile_count, tn); UP(p->d_dp_pair_frames, pf); UP(p->d_dp_records, p->dp_records);
+  }
+  {
     std::vector<uint8_t> ir(N); std::vector<double> md(N), ad;
     for (int i = 0; i < N; ++i) { ir[i] = p->in_range[uperm[i]]; md[i] = p->median[uperm[i]]; }
     UP(p->d_in_range, ir); UP(p->d_median, md);
@@ -379,7 +394,7 @@ static int allocate_storage(rcvd_problem* p) {
   DA(p->d_ytmp, Upad); DA(p->d_y, Upad); DA(p->d_Sy, Upad); DA(p->d_Hy, Upad); DA(p->d_scal, SC_N); DA(p->d_active, Upad); DA(p->d_fail, 1);
   DA(p->d_potrf_progress, (size_t)N);
   const RegCounts rcn = reg_counts(p->cfg, L, N, p->nscale);
-  p->npartial = p->num_tiles + (rcn.total + 127) / 128 + p->num_trip_tiles + 1;
+  p->npartial = p->num_tiles + (rcn.total + 127) / 128 + p->num_trip_tiles + p->num_dp_tiles + 1;
   DA(p->d_partial, (size_t)p->npartial);
   if (p->eval_only) { DA(p->d_H, 1); DA(p->d_Lb, 1); DA(p->d_T, 1); DA(p->d_invL, 1); DA(p->d_invT, 1); }   // cost / gradient evaluations only: no matrices
   else {
@@ -440,10 +455,13 @@ static int allocate_storage(rcvd_problem* p) {
 }
 
 static int build_structure(rcvd_problem* p) {
+  if (p->nranks > 1 && !p->dp_pair_frames.empty()) return set_err(RCVD_ERR_INVALID, "depth-normalisation pairs are not sharded: they need a single-GPU problem (nranks = 1)");
   free_all(p);
   CK(cudaSetDevice(p->device));
-  if (const char* e = make_factor_plan(p->plan, p->cfg, p->struct_pairs.empty() ? p->pair_frames : p->struct_pairs, p->trip_centers, p->order_slack,
-                                       p->nranks, p->rank, p->dist_enabled, p->num_sms))
+  // the frame graph: static pairs (or the global structure of a sharded problem) and the depth-normalisation pairs
+  std::vector<int32_t> graph = p->struct_pairs.empty() ? p->pair_frames : p->struct_pairs;
+  graph.insert(graph.end(), p->dp_pair_frames.begin(), p->dp_pair_frames.end());
+  if (const char* e = make_factor_plan(p->plan, p->cfg, graph, p->trip_centers, p->order_slack, p->nranks, p->rank, p->dist_enabled, p->num_sms))
     return set_err(RCVD_ERR_INVALID, "%s", e);
   while (p->ev_side.size() < 2 * p->plan.levels.size()) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); p->ev_side.push_back(e); }
   int rc;
@@ -730,7 +748,7 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
   int rc = wantH ? enqueue_residuals<EvalMode::CostGradH>(p, x, gout)
            : wantG ? enqueue_residuals<EvalMode::CostGrad>(p, x, gout) : enqueue_residuals<EvalMode::Cost>(p, x, gout);
   if (rc) return rc;
-  if ((rc = launch(p, k_reduce_partials, 1, 1024, 0, st, false, p->d_partial, p->num_tiles + regblocks + p->num_trip_tiles, p->d_scal, slot))) return rc;
+  if ((rc = launch(p, k_reduce_partials, 1, 1024, 0, st, false, p->d_partial, p->num_tiles + regblocks + p->num_trip_tiles + p->num_dp_tiles, p->d_scal, slot))) return rc;
   if (p->nranks > 1) {
     if (wantG) {
       // ONE packed all-reduce: [gradient (Upad) | cost + 7 spare | diagonal of H (Upad, only with H into d_g)]
@@ -1147,6 +1165,22 @@ RCVD_API int32_t rcvd_problem_set_triplets(rcvd_problem* p, int32_t nt, const in
   const int64_t n = p->trip_offsets.back();
   if (n > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null triplet records");
   p->trip_records.assign(rec, rec + (size_t)n * 10);
+  p->structure_ready = false;
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_problem_set_depth_pairs(rcvd_problem* p, int32_t np, const int32_t* pf, const int64_t* off, const float* rec) {
+  if (!p || np < 0 || (np > 0 && (!pf || !off))) return set_err(RCVD_ERR_INVALID, "bad depth-pair arrays");
+  if (p->nranks > 1 && np > 0) return set_err(RCVD_ERR_INVALID, "depth-normalisation pairs are not sharded: they need a single-GPU problem (nranks = 1)");
+  for (int i = 0; i < np; ++i) {   // checked before anything is kept: a refused call leaves the problem as it was
+    if (off[i + 1] < off[i] || off[0] != 0) return set_err(RCVD_ERR_INVALID, "offsets must start at 0 and be non-decreasing");
+    if (pf[2 * i] < 0 || pf[2 * i] >= p->N || pf[2 * i + 1] < 0 || pf[2 * i + 1] >= p->N || pf[2 * i] == pf[2 * i + 1]) return set_err(RCVD_ERR_INVALID, "bad frame pair %d", i);
+  }
+  const int64_t C = np > 0 ? off[np] : 0;
+  if (C > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null records");
+  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
+  p->dp_pair_frames.assign(pf, pf + 2 * (size_t)np);
+  if (np > 0) p->dp_offsets.assign(off, off + np + 1); else p->dp_offsets.assign(1, 0);
+  p->dp_records.assign(rec, rec + (size_t)C * 6);
   p->structure_ready = false;
   return RCVD_OK;
 }

@@ -8,6 +8,7 @@
 //   k_accumulate_fast, k_accumulate_runs : the CostGradH pair kernels of the default configuration (pose block on the tensor cores)
 //   k_regularisers<MODE> : scale / deform / spatial / focal / position rows (:488-656, :1341-1549)
 //   k_triplets<MODE>     : scene-flow smoothness rows (:1242-1339)
+//   k_depth_pairs<MODE>  : pairwise depth normalisation, DisparityDissimilarityCost rows (:425-462, added at :1005-1095)
 // The partial costs of all families meet in one deterministic two-stage reduction (k_reduce_partials).
 #pragma once
 #include "rcvd_device.cuh"
@@ -35,6 +36,8 @@ struct DevProblem {
   int rank, nranks;            // regulariser and triplet rows are evaluated by rank f % nranks (every rank marks them all)
   // scene-flow smoothness triplets (optional): records [n][10], tiles of <= kTile constraints with one centre frame
   const float* trip_records; const int32_t* trip_tile_center; const int64_t* trip_tile_begin; const int32_t* trip_tile_count;
+  // pairwise depth-normalisation constraints (optional): records [n][6], tiles of <= kTile constraints of one directed pair
+  const float* dp_records; const int32_t* dp_pair_frames; const int32_t* dp_tile_pair; const int64_t* dp_tile_begin; const int32_t* dp_tile_count;
 };
 
 __device__ __forceinline__ bool is_const_local(const rcvd_config& c, const Layout& L, int l) {
@@ -666,6 +669,94 @@ __global__ void __launch_bounds__(kTile) k_triplets(DevProblem p, const double* 
     }
   }
   if (MODE != EvalMode::MarkActive) block_store_sum(cost, partial + t);
+}
+
+// --- pairwise depth normalisation (normalizeDepth with normalizeDepthFromFirstFrame = false, lib/PoseOptimizer.cpp:1005-1095) ---
+// One DisparityDissimilarityCost row per constraint (:425-462), r = 1 / max(D_a, 1e-6) - 1 / max(D_b, 1e-6), D the transformed depth
+// of each end, over the depth-transform parameters of both frames; robustified as the static rows (robust_loss, sqrt(rho') corrector).
+// max(D, eps) is Jet max, (D < eps) ? eps : D: a clamped end contributes no derivative.  With a Global transform every constraint of
+// the tile touches the same 2k gradient and k (2k + 1) H entries (one pair): they are summed over the tile (warp shuffle, then shared
+// memory) and leave the SM as one RED each.  Grid transforms scatter per constraint over the gathered nodes.
+template <EvalMode MODE>
+__global__ void __launch_bounds__(kTile) k_depth_pairs(DevProblem p, const double* __restrict__ x, double* __restrict__ H, double* __restrict__ g,
+                                                       double* __restrict__ partial, uint8_t* __restrict__ mask) {
+  const rcvd_config& c = p.cfg; const Layout& L = p.L;
+  const int t = blockIdx.x, np = L.npad;
+  const int pr = p.dp_tile_pair[t];
+  const int fr[2] = {p.dp_pair_frames[2 * pr], p.dp_pair_frames[2 * pr + 1]};
+  const bool active = (int)threadIdx.x < p.dp_tile_count[t];
+  const float* rec = p.dp_records + (size_t)(p.dp_tile_begin[t] + (active ? threadIdx.x : 0)) * 6;
+  Gather dg[2];
+  for (int s = 0; s < 2; ++s) {
+    if (active) gather_depth(c, rec[3 * s], rec[3 * s + 1], dg[s]);
+    else dg[s].n = 0;
+  }
+  if constexpr (MODE == EvalMode::MarkActive) {
+    for (int s = 0; s < 2; ++s)
+      for (int q = 0; q < dg[s].n; ++q)
+        for (int j = 0; j < L.k; ++j) mask[(size_t)fr[s] * np + L.offD + dg[s].idx[q] * L.k + j] = 1;
+    return;
+  } else {
+    double cost = 0.0, rs = 0.0, dr[2] = {0.0, 0.0};   // scaled residual and scaled dr/dD of each end (zero on idle threads)
+    if (active) {
+      constexpr double eps = 1e-6;
+      const double D0 = depth_value(c, L, dg[0], rec[2], x + (size_t)fr[0] * L.nf), D1 = depth_value(c, L, dg[1], rec[5], x + (size_t)fr[1] * L.nf);
+      const bool c0 = D0 < eps, c1 = D1 < eps;
+      const double r = 1.0 / (c0 ? eps : D0) - 1.0 / (c1 ? eps : D1);
+      double rho0, rho1;
+      robust_loss(c, r * r, rho0, rho1);
+      cost = 0.5 * rho0;
+      const double sc = sqrt(rho1);
+      rs = r * sc;
+      dr[0] = c0 ? 0.0 : -sc / (D0 * D0);
+      dr[1] = c1 ? 0.0 : sc / (D1 * D1);
+    }
+    if (MODE != EvalMode::Cost && !c.fix_depth_xforms) {
+      constexpr bool WANT_H = MODE == EvalMode::CostGradH;
+      if (c.depth_type == RCVD_DEPTH_GLOBAL) {
+        // columns a = side * k + component (scale: dD/ds = src; shift: dD/do = 1); values: J^T r over a, then H(a, b), b <= a
+        const int k = L.k, nc = 2 * k, nv = nc + (WANT_H ? nc * (nc + 1) / 2 : 0);
+        double j[4];
+        for (int s = 0; s < 2; ++s) { j[s * k] = dr[s] * (double)rec[3 * s + 2]; if (k == 2) j[s * k + 1] = dr[s]; }
+        __shared__ double red[14][kTile / 32];
+        const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+        int i = 0;
+        for (int a = 0; a < nc; ++a, ++i) { const double v = warp_sum(j[a] * rs); if (lane == 0) red[i][wid] = v; }
+        if (WANT_H)
+          for (int a = 0; a < nc; ++a)
+            for (int b = 0; b <= a; ++b, ++i) { const double v = warp_sum(j[a] * j[b]); if (lane == 0) red[i][wid] = v; }
+        __syncthreads();
+        if ((int)threadIdx.x < nv) {
+          i = threadIdx.x;
+          double v = 0.0;
+#pragma unroll
+          for (int w = 0; w < kTile / 32; ++w) v += red[i][w];
+          if (i < nc) red_add(g + (size_t)fr[i / k] * np + L.offD + i % k, v);
+          else {
+            int e = i - nc, a = 0;
+            while (e > a) { e -= a + 1; ++a; }   // e-th entry of the lower triangle, row-major: (a, e)
+            add_h(p, H, fr[a / k], L.offD + a % k, fr[e / k], L.offD + e % k, v);
+          }
+        }
+      } else if (active) {
+        int ef[64]; short el[64]; double ej[64];   // 2 ends x <= 16 nodes x k
+        int E = 0;
+        for (int s = 0; s < 2; ++s) {
+          const double src = (double)rec[3 * s + 2];
+          for (int q = 0; q < dg[s].n; ++q) {
+            const double w = dg[s].w[q];
+            ef[E] = fr[s]; el[E] = (short)(L.offD + dg[s].idx[q] * L.k); ej[E] = dr[s] * w * src; ++E;
+            if (L.k == 2) { ef[E] = fr[s]; el[E] = (short)(L.offD + dg[s].idx[q] * 2 + 1); ej[E] = dr[s] * w; ++E; }
+          }
+        }
+        for (int a = 0; a < E; ++a) {
+          red_add(g + (size_t)ef[a] * np + el[a], ej[a] * rs);
+          if (WANT_H) for (int b = 0; b <= a; ++b) add_h(p, H, ef[a], el[a], ef[b], el[b], ej[a] * ej[b]);
+        }
+      }
+    }
+    block_store_sum(cost, partial + t);
+  }
 }
 
 // Final deterministic reduction of the per-block partial costs: out[slot] = sum(partial[0..n))

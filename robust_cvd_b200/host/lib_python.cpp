@@ -199,7 +199,8 @@ PYBIND11_MODULE(lib_python, m) {
       .def_readwrite("coarseToFine", &P::coarseToFine).def_readwrite("ctfLong", &P::ctfLong).def_readwrite("ctfShort", &P::ctfShort)
       .def_readwrite("deferredSpatialOpt", &P::deferredSpatialOpt).def_readwrite("dsoLong", &P::dsoLong).def_readwrite("dsoShort", &P::dsoShort)
       .def_readwrite("focalLong", &P::focalLong).def_readwrite("intrOpt", &P::intrOpt)
-      .def_readwrite("fixPoses", &P::fixPoses).def_readwrite("fixDepthXforms", &P::fixDepthXforms).def_readwrite("fixSpatialXforms", &P::fixSpatialXforms);
+      .def_readwrite("fixPoses", &P::fixPoses).def_readwrite("fixDepthXforms", &P::fixDepthXforms).def_readwrite("fixSpatialXforms", &P::fixSpatialXforms)
+      .def_readwrite("normalizeDepthFromFirstFrame", &P::normalizeDepthFromFirstFrame);   // not bound by the reference (a C++ option there)
   dvpo.def(py::init<DepthVideo*, int>(), py::keep_alive<1, 2>())
       .def("poseOptimization", &DepthVideoPoseOptimizer::poseOptimization)
       .def("normalizeDepth", &DepthVideoPoseOptimizer::normalizeDepth)
@@ -218,6 +219,9 @@ PYBIND11_MODULE(lib_python, m) {
         d["trip_centers"] = py::array_t<int32_t>(pa.tripCenters.size(), pa.tripCenters.data());
         d["trip_offsets"] = py::array_t<int64_t>(pa.tripOffsets.size(), pa.tripOffsets.data());
         d["trip_records"] = py::array_t<float>(pa.tripRecords.size(), pa.tripRecords.data());
+        d["dpair_frames"] = py::array_t<int32_t>(pa.dpPairFrames.size(), pa.dpPairFrames.data());
+        d["dpair_offsets"] = py::array_t<int64_t>(pa.dpOffsets.size(), pa.dpOffsets.data());
+        d["dpair_records"] = py::array_t<float>(pa.dpRecords.size(), pa.dpRecords.data());
         return d; }, py::arg("params"), py::arg("constraints"), py::arg("depthDeformReg") = 0.1, py::arg("normalize") = false);
 
   py::class_<DepthVideoProcessor> dvp(m, "DepthVideoProcessor");

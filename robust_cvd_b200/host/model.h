@@ -362,6 +362,7 @@ class DepthVideoPoseOptimizer {
     rcvd_config cfg; std::vector<uint8_t> inRange; std::vector<double> median, adaptive, state;
     std::vector<int32_t> pairFrames; std::vector<int64_t> offsets; std::vector<float> records;
     std::vector<int32_t> tripCenters; std::vector<int64_t> tripOffsets; std::vector<float> tripRecords;   // smoothness triplets, 10 floats each
+    std::vector<int32_t> dpPairFrames; std::vector<int64_t> dpOffsets; std::vector<float> dpRecords;   // pairwise depth normalisation, 6 floats each
     int pairCount = 0; int64_t constraintCount = 0;
   };
   ProblemArrays buildProblem(const Params& params, const FlowConstraintsCollection* constraints, double depthDeformReg, bool normalize);
@@ -371,6 +372,8 @@ class DepthVideoPoseOptimizer {
   const std::vector<std::array<double, 7>>& poseParams() const { return poseParams_; }
  private:
   void solveAndWriteBack(ProblemArrays& pa, const Params& params, bool writePoses);
+  void assemblePairRecords(const FlowConstraintsCollection& constraints, const FrameRange& range, bool staticOnly, std::vector<int32_t>& pairFrames,
+                           std::vector<int64_t>& offsets, std::vector<float>& records, int& pairCount, int64_t& constraintCount);
   DepthVideo* video_; int depthStream_; int numFrames_ = 0;
   std::vector<std::array<double, 7>> poseParams_;
 };

@@ -30,6 +30,62 @@ DepthVideoPoseOptimizer::DepthVideoPoseOptimizer(DepthVideo* video, int depthStr
 
 static void checkStatus(int rc) { if (rc != RCVD_OK) throw std::runtime_error(std::string("rcvd: ") + rcvd_last_error()); }
 
+// Observation records {ndc0.x, ndc0.y, depth0, ndc1.x, ndc1.y, depth1} of the flow-constraint pairs with both ends in range, in map
+// order (Observation :104-117; addStaticSceneLoss :1167-1193, the pairwise branch of normalizeDepth :1013-1063).  A constraint whose
+// source depth at either end is non-finite or <= 0 is dropped.  staticOnly: the static-scene rows take the constraints flagged static
+// only; the depth-normalisation rows take all of them.  The pairs' records are assembled in parallel into per-pair slots and
+// concatenated in order; offsets starts at {0}.
+void DepthVideoPoseOptimizer::assemblePairRecords(const FlowConstraintsCollection& constraints, const FrameRange& range, bool staticOnly,
+                                                  std::vector<int32_t>& pairFrames, std::vector<int64_t>& offsets, std::vector<float>& records,
+                                                  int& pairCount, int64_t& constraintCount) {
+  DepthStream& ds = video_->depthStream(depthStream_);
+  const float invAspect = video_->invAspect();
+  struct PairJob { int f0, f1; const std::vector<PairConstraint>* list; const Image* d0; const Image* d1; std::vector<float> rec; };
+  std::vector<PairJob> jobs;
+  { std::set<int> touched;
+    for (const auto& kv : constraints.pairs()) if (range.inRange(kv.first.first) && range.inRange(kv.first.second)) { touched.insert(kv.first.first); touched.insert(kv.first.second); }
+    ds.preloadSourceDepth(std::vector<int>(touched.begin(), touched.end()), false); }
+  for (const auto& kv : constraints.pairs()) {
+    const int f0 = kv.first.first, f1 = kv.first.second;
+    if (!range.inRange(f0) || !range.inRange(f1)) continue;
+    const Image* d0 = ds.frame(f0).sourceDepth(); const Image* d1 = ds.frame(f1).sourceDepth();
+    if (!d0 || !d1) throw std::runtime_error("Missing depth image.");
+    jobs.push_back({f0, f1, &kv.second, d0, d1, {}});
+  }
+  parallelFor(jobs.size(), [&](size_t j) {
+    PairJob& job = jobs[j];
+    job.rec.reserve(job.list->size() * 6);
+    for (const PairConstraint& c : *job.list) {
+      if (staticOnly && !c.isStatic) continue;
+      float rec[6];
+      bool ok = true;
+      for (int o = 0; o < 2; ++o) {
+        const Image* d = o ? job.d1 : job.d0;
+        const float lx = c.loc[o][0], ly = c.loc[o][1];
+        rec[o * 3] = -1.f + 2.f * lx; rec[o * 3 + 1] = 1.f - 2.f * ly / invAspect;
+        int px = int(lx * d->cols), py = int(ly / invAspect * d->rows);
+        // the reference indexes the Mat unchecked (SURVEY A1 quirk for targets in (-1.5,-0.5]); clamp instead of reading out of bounds
+        px = std::min(std::max(px, 0), d->cols - 1); py = std::min(std::max(py, 0), d->rows - 1);
+        const float sd = d->ptr<float>(py)[px];
+        rec[o * 3 + 2] = sd;
+        if (!std::isfinite(sd) || sd <= 0) ok = false;
+      }
+      if (!ok) continue;
+      job.rec.insert(job.rec.end(), rec, rec + 6);
+    }
+  });
+  size_t total = 0; for (const PairJob& job : jobs) total += job.rec.size();
+  records.reserve(total);
+  for (const PairJob& job : jobs) {
+    ++pairCount;
+    records.insert(records.end(), job.rec.begin(), job.rec.end());
+    const int64_t n = int64_t(job.rec.size()) / 6;
+    pairFrames.push_back(job.f0); pairFrames.push_back(job.f1);
+    offsets.push_back(offsets.back() + n);
+    constraintCount += n;
+  }
+}
+
 DepthVideoPoseOptimizer::ProblemArrays DepthVideoPoseOptimizer::buildProblem(const Params& params, const FlowConstraintsCollection* constraints,
                                                                              double depthDeformReg, bool normalize) {
   ProblemArrays pa;
@@ -99,53 +155,15 @@ DepthVideoPoseOptimizer::ProblemArrays DepthVideoPoseOptimizer::buildProblem(con
     // the coarse-to-fine steps of one poseOptimization() call see the same constraints and source depths: the records are assembled once
     pa.pairFrames = cachedPairFrames_; pa.offsets = cachedOffsets_; pa.records = cachedRecords_; pa.pairCount = cachedPairCount_; pa.constraintCount = cachedConstraintCount_;
   } else if (!normalize && constraints) {
-    const float invAspect = video_->invAspect();
-    // pairs with both ends in range, in map order; their records are assembled in parallel into per-pair slots and concatenated in order
-    struct PairJob { int f0, f1; const std::vector<PairConstraint>* list; const Image* d0; const Image* d1; std::vector<float> rec; };
-    std::vector<PairJob> jobs;
-    { std::set<int> touched;
-      for (const auto& kv : constraints->pairs()) if (range.inRange(kv.first.first) && range.inRange(kv.first.second)) { touched.insert(kv.first.first); touched.insert(kv.first.second); }
-      ds.preloadSourceDepth(std::vector<int>(touched.begin(), touched.end()), false); }
-    for (const auto& kv : constraints->pairs()) {
-      const int f0 = kv.first.first, f1 = kv.first.second;
-      if (!range.inRange(f0) || !range.inRange(f1)) continue;
-      const Image* d0 = ds.frame(f0).sourceDepth(); const Image* d1 = ds.frame(f1).sourceDepth();
-      if (!d0 || !d1) throw std::runtime_error("Missing depth image.");
-      jobs.push_back({f0, f1, &kv.second, d0, d1, {}});
-    }
-    parallelFor(jobs.size(), [&](size_t j) {
-      PairJob& job = jobs[j];
-      job.rec.reserve(job.list->size() * 6);
-      for (const PairConstraint& c : *job.list) {
-        if (!c.isStatic) continue;
-        float rec[6];
-        bool ok = true;
-        for (int o = 0; o < 2; ++o) {
-          const Image* d = o ? job.d1 : job.d0;
-          const float lx = c.loc[o][0], ly = c.loc[o][1];
-          rec[o * 3] = -1.f + 2.f * lx; rec[o * 3 + 1] = 1.f - 2.f * ly / invAspect;
-          int px = int(lx * d->cols), py = int(ly / invAspect * d->rows);
-          // the reference indexes the Mat unchecked (SURVEY A1 quirk for targets in (-1.5,-0.5]); clamp instead of reading out of bounds
-          px = std::min(std::max(px, 0), d->cols - 1); py = std::min(std::max(py, 0), d->rows - 1);
-          const float sd = d->ptr<float>(py)[px];
-          rec[o * 3 + 2] = sd;
-          if (!std::isfinite(sd) || sd <= 0) ok = false;
-        }
-        if (!ok) continue;
-        job.rec.insert(job.rec.end(), rec, rec + 6);
-      }
-    });
-    size_t total = 0; for (const PairJob& job : jobs) total += job.rec.size();
-    pa.records.reserve(total);
-    for (const PairJob& job : jobs) {
-      ++pa.pairCount;
-      pa.records.insert(pa.records.end(), job.rec.begin(), job.rec.end());
-      const int64_t n = int64_t(job.rec.size()) / 6;
-      pa.pairFrames.push_back(job.f0); pa.pairFrames.push_back(job.f1);
-      pa.offsets.push_back(pa.offsets.back() + n);
-      pa.constraintCount += n;
-    }
+    assemblePairRecords(*constraints, range, true, pa.pairFrames, pa.offsets, pa.records, pa.pairCount, pa.constraintCount);
     if (recordCacheOn_) { cachedPairFrames_ = pa.pairFrames; cachedOffsets_ = pa.offsets; cachedRecords_ = pa.records; cachedPairCount_ = pa.pairCount; cachedConstraintCount_ = pa.constraintCount; recordCacheValid_ = true; }
+  }
+  // pairwise depth normalisation (:1005-1095): a DisparityDissimilarityCost row for every constraint of every in-range pair
+  pa.dpOffsets.assign(1, 0);
+  if (normalize && !params.normalizeDepthFromFirstFrame) {
+    if (!constraints) throw std::runtime_error("Pairwise depth normalization needs flow constraints.");
+    int pairs = 0; int64_t count = 0;
+    assemblePairRecords(*constraints, range, false, pa.dpPairFrames, pa.dpOffsets, pa.dpRecords, pairs, count);
   }
   // scene-flow smoothness constraints (addSceneFlowSmoothnessLoss :1242-1339): only if either weight is positive (:899-901)
   pa.tripOffsets.assign(1, 0);
@@ -199,6 +217,7 @@ void DepthVideoPoseOptimizer::solveAndWriteBack(ProblemArrays& pa, const Params&
     checkStatus(rcvd_problem_set_frames(p, pa.inRange.data(), pa.median.data(), pa.adaptive.empty() ? nullptr : pa.adaptive.data()));
     checkStatus(rcvd_problem_set_constraints(p, int(pa.pairFrames.size() / 2), pa.pairFrames.data(), pa.offsets.data(), pa.records.data()));
     if (!pa.tripCenters.empty()) checkStatus(rcvd_problem_set_triplets(p, int(pa.tripCenters.size()), pa.tripCenters.data(), pa.tripOffsets.data(), pa.tripRecords.data()));
+    if (!pa.dpPairFrames.empty()) checkStatus(rcvd_problem_set_depth_pairs(p, int(pa.dpPairFrames.size() / 2), pa.dpPairFrames.data(), pa.dpOffsets.data(), pa.dpRecords.data()));
     checkStatus(rcvd_problem_set_state(p, pa.state.data()));
     rcvd_solve_options opt; rcvd_default_solve_options(&opt);
     opt.max_iterations = params.maxIterations; opt.verbose = 1;   // minimizer_progress_to_stdout = true (:957)
@@ -245,14 +264,15 @@ void DepthVideoPoseOptimizer::poseOptimizationStep(const Params& params, const F
 void DepthVideoPoseOptimizer::normalizeDepth(const Params& params, const FlowConstraintsCollection& constraints) {
   logInfo("------------------------");
   logInfo("Depth Normalization (depth stream " + std::to_string(depthStream_) + ")...");
-  if (!params.normalizeDepthFromFirstFrame) throw std::runtime_error("normalizeDepthFromFirstFrame = false is not supported (it is not reachable from Python in the reference either).");
-  (void)constraints;
-  ProblemArrays pa = buildProblem(params, nullptr, 0.0, true);
+  ProblemArrays pa = buildProblem(params, &constraints, 0.0, true);
+  if (!params.normalizeDepthFromFirstFrame) logInfo("    Added " + std::to_string(pa.dpOffsets.back()) + " depth-normalization constraints over " + std::to_string(pa.dpPairFrames.size() / 2) + " frame pairs.");
   solveAndWriteBack(pa, params, false);
   FrameRange range = params.frameRange; if (range.isEmpty()) range.resolve(numFrames_);
   DepthStream& ds = video_->depthStream(depthStream_);
-  const int first = range.firstFrame();   // copy the first frame's transform to all others (:1127-1138)
-  for (int f : range.frames) { if (f != first) ds.frame(f).depthXform().copyFrom(ds.frame(first).depthXform()); }
+  if (params.normalizeDepthFromFirstFrame) {   // copy the first frame's transform to all others (:1127-1138); the pairwise mode keeps each frame's own
+    const int first = range.firstFrame();
+    for (int f : range.frames) { if (f != first) ds.frame(f).depthXform().copyFrom(ds.frame(first).depthXform()); }
+  }
   for (int f : range.frames) ds.frame(f).clearXformedCache();
 }
 

@@ -138,6 +138,15 @@ class Problem:
         assert off.shape[0] == ce.shape[0] + 1 and off[-1] == rec.shape[0]
         _check(self.L.rcvd_problem_set_triplets(self.h, C.c_int32(ce.shape[0]), _p(ce, C.c_int32), _p(off, C.c_int64), _p(rec, C.c_float)))
 
+    def set_depth_pairs(self, pair_frames, offsets, records):
+        """Pairwise depth-normalisation constraints (DisparityDissimilarityCost): pair_frames[P, 2], offsets[P+1], records[C][6] in the
+        layout of set_constraints.  Single-GPU only."""
+        pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
+        off = np.ascontiguousarray(offsets, np.int64)
+        rec = np.ascontiguousarray(records, np.float32).reshape(-1, 6)
+        assert off.shape[0] == pf.shape[0] + 1 and off[-1] == rec.shape[0]
+        _check(self.L.rcvd_problem_set_depth_pairs(self.h, C.c_int32(pf.shape[0]), _p(pf, C.c_int32), _p(off, C.c_int64), _p(rec, C.c_float)))
+
     def set_structure(self, pair_frames):
         pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
         _check(self.L.rcvd_problem_set_structure(self.h, C.c_int32(pf.shape[0]), _p(pf, C.c_int32)))
