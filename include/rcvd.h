@@ -164,14 +164,19 @@ int32_t rcvd_problem_set_frames(rcvd_problem* p, const uint8_t* in_range,
  * (isStatic, both frames in range, finite positive source depths,
  * lib/PoseOptimizer.cpp:1167-1193), grouped by directed frame pair.
  * pair_frames[P][2], offsets[P+1], records[C][6] = {ndc0.x, ndc0.y, depth0,
- * ndc1.x, ndc1.y, depth1} as float32 (Observation, :104-117). */
+ * ndc1.x, ndc1.y, depth1} as float32 (Observation, :104-117).
+ * The two frames of a pair are distinct and in [0, N).  For this call, rcvd_problem_set_triplets and
+ * rcvd_problem_set_depth_pairs: group i owns the records offsets[i] .. offsets[i+1]-1, offsets[0] must be 0,
+ * the offsets must not decrease, and records may be null only if offsets[n] is 0.  A call that fails with
+ * RCVD_ERR_INVALID changes nothing: the problem keeps its earlier constraints of that family. */
 int32_t rcvd_problem_set_constraints(rcvd_problem* p, int32_t num_pairs, const int32_t* pair_frames,
                                      const int64_t* offsets, const float* records);
 
 /* Scene-flow smoothness constraints (addSceneFlowSmoothnessLoss, lib/PoseOptimizer.cpp:1242-1339), grouped by the centre
  * frame f of the triplet (f-1, f, f+1): centers[T], offsets[T+1], records[n][10] float32 =
  * {ndc.x, ndc.y, depth} for the three observations + the ScaledLoss weight (smoothStaticWeight or
- * smoothDynamicWeight, :1314-1317).  Optional; absent by default as in the reference (both weights 0). */
+ * smoothDynamicWeight, :1314-1317).  Every centre is in [1, N-2]; offsets and refusals as in
+ * rcvd_problem_set_constraints.  Optional; absent by default as in the reference (both weights 0). */
 int32_t rcvd_problem_set_triplets(rcvd_problem* p, int32_t num_groups, const int32_t* centers,
                                   const int64_t* offsets, const float* records);
 
@@ -190,7 +195,8 @@ int32_t rcvd_problem_set_depth_pairs(rcvd_problem* p, int32_t num_pairs, const i
 int32_t rcvd_nccl_unique_id(uint8_t out[128]);
 int32_t rcvd_problem_init_comm(rcvd_problem* p, int32_t nranks, int32_t rank, const uint8_t unique_id[128]);
 /* Multi-GPU: the GLOBAL list of directed frame pairs [num_pairs][2] (all ranks pass the same list) so that every rank builds
- * the identical block structure / elimination order although it only holds a shard of the constraints. */
+ * the identical block structure / elimination order although it only holds a shard of the constraints.  A negative num_pairs,
+ * or a null pair_frames with num_pairs > 0, fails with RCVD_ERR_INVALID and changes nothing. */
 int32_t rcvd_problem_set_structure(rcvd_problem* p, int32_t num_pairs, const int32_t* pair_frames);
 /* regulariser terms are evaluated by the rank that owns frame f: f % nranks == rank */
 

@@ -153,30 +153,36 @@ enum { LP_POTRF_SMEM = 0, LP_POTRF_PANEL, LP_TRSM_LL4, LP_TRSM_LL2, LP_TRSM_GEMM
 // items; LP_TRSM_STREAMED: the k_trsm_ll launches (either shape) that run beside their level's k_potrf_smem
 
 // ---------------------------------------------------------------------------
+// One constraint family: groups of `nframes` frames (a directed pair: 2, a triplet's centre: 1), each with a run of consecutive
+// records of `width` floats, as the caller set them, and their tiled device copy (set_up_problem_data).
+struct RecordSet {
+  const int width, nframes;
+  std::vector<int32_t> frames; std::vector<int64_t> offsets{0}; std::vector<float> records;
+  RecordTiles dev = {}; int num_tiles = 0;
+  RecordSet(int width_, int nframes_) : width(width_), nframes(nframes_) {}
+  int groups() const { return (int)offsets.size() - 1; }
+  int64_t count() const { return offsets.back(); }
+};
+
 struct rcvd_problem {
   rcvd_config cfg; Layout L; int N = 0; int device = 0;
   cudaStream_t stream = nullptr;
   // host inputs
   std::vector<uint8_t> in_range; std::vector<double> median, adaptive;
-  std::vector<int32_t> pair_frames; std::vector<int64_t> offsets; std::vector<float> records_h;
+  RecordSet pairs{6, 2}, trips{10, 1}, dpairs{6, 2};   // static-scene pairs, smoothness triplets, pairwise depth normalisation
   std::vector<int32_t> struct_pairs;   // global frame-pair graph (multi-GPU); empty -> local pairs
-  std::vector<int32_t> trip_centers; std::vector<int64_t> trip_offsets; std::vector<float> trip_records;   // smoothness triplets
-  float* d_trip_records = nullptr; int32_t *d_trip_tile_center = nullptr, *d_trip_tile_count = nullptr; int64_t* d_trip_tile_begin = nullptr; int num_trip_tiles = 0;
-  std::vector<int32_t> dp_pair_frames; std::vector<int64_t> dp_offsets; std::vector<float> dp_records;   // pairwise depth normalisation
-  float* d_dp_records = nullptr; int32_t *d_dp_pair_frames = nullptr, *d_dp_tile_pair = nullptr, *d_dp_tile_count = nullptr; int64_t* d_dp_tile_begin = nullptr;
-  int num_dp_tiles = 0;
   int first_frame = 0, last_frame = -1;
   // device problem data
-  float* d_records = nullptr; int32_t *d_tile_pair = nullptr, *d_tile_count = nullptr, *d_pair_frames = nullptr, *d_blk_of = nullptr;
-  int64_t* d_tile_begin = nullptr; uint8_t *d_in_range = nullptr, *d_active = nullptr;
+  int32_t* d_blk_of = nullptr; uint8_t *d_in_range = nullptr, *d_active = nullptr;
   double *d_median = nullptr, *d_adaptive = nullptr; float* d_scale_locs = nullptr; int nscale = 0;
-  int num_tiles = 0; int64_t C = 0;
   // state & vectors
   double *d_x = nullptr, *d_xc = nullptr, *d_xsave = nullptr;
   double *d_g = nullptr, *d_S = nullptr, *d_diagH = nullptr, *d_lmdiag = nullptr, *d_D2 = nullptr, *d_gs = nullptr, *d_rhs = nullptr, *d_ytmp = nullptr,
          *d_y = nullptr, *d_Sy = nullptr, *d_Hy = nullptr, *d_partial = nullptr, *d_scal = nullptr;
   double* h_scal = nullptr;   // pinned
-  int npartial = 0;
+  // d_partial holds one partial cost per CTA: the pair tiles from 0, the regulariser blocks from part_reg, the triplet tiles from
+  // part_trip, the depth-pair tiles from part_dp; npartial in all
+  int part_reg = 0, part_trip = 0, part_dp = 0, npartial = 0;
   // matrices
   double *d_H = nullptr, *d_Lb = nullptr, *d_T = nullptr, *d_invL = nullptr, *d_invT = nullptr;
   HBlock *d_hblocks = nullptr, *d_lblocks = nullptr; int* d_fail = nullptr;
@@ -259,13 +265,10 @@ static void free_all(rcvd_problem* p) {
 
 static DevProblem dev_problem(const rcvd_problem* p) {
   DevProblem d; d.cfg = p->cfg; d.L = p->L; d.N = p->N;
-  d.records = p->d_records; d.tile_pair = p->d_tile_pair; d.tile_begin = p->d_tile_begin; d.tile_count = p->d_tile_count;
-  d.pair_frames = p->d_pair_frames; d.blk_of = p->d_blk_of; d.in_range = p->d_in_range; d.median = p->d_median;
+  d.pairs = p->pairs.dev; d.trips = p->trips.dev; d.dpairs = p->dpairs.dev;
+  d.blk_of = p->d_blk_of; d.in_range = p->d_in_range; d.median = p->d_median;
   d.adaptive = p->adaptive.empty() ? nullptr : p->d_adaptive; d.scale_locs = p->d_scale_locs;
   d.rank = p->rank; d.nranks = p->nranks;
-  d.trip_records = p->d_trip_records; d.trip_tile_center = p->d_trip_tile_center; d.trip_tile_begin = p->d_trip_tile_begin; d.trip_tile_count = p->d_trip_tile_count;
-  d.dp_records = p->d_dp_records; d.dp_pair_frames = p->d_dp_pair_frames; d.dp_tile_pair = p->d_dp_tile_pair; d.dp_tile_begin = p->d_dp_tile_begin;
-  d.dp_tile_count = p->d_dp_tile_count;
   return d;
 }
 
@@ -276,21 +279,19 @@ template <EvalMode MODE>
 static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
   const DevProblem d = dev_problem(p);
   const RegCounts rcn = reg_counts(p->cfg, p->L, p->N, p->nscale);
-  const int regblocks = (rcn.total + 127) / 128;
+  const int regblocks = p->part_trip - p->part_reg, ntiles = p->pairs.num_tiles;
   cudaStream_t st = p->stream; double* part = p->d_partial; int rc;
-  if (p->num_tiles > 0) {
+  if (ntiles > 0) {
     const bool tc = MODE == EvalMode::CostGradH && p->fast_path != 0;   // a tensor-core kernel (rcvd_debug_set_fast_path)
-    if (tc && p->fast_path == 1 && p->records_sorted) rc = launch(p, k_accumulate_runs, p->num_tiles, kTile, kRunSmem, st, false, d, x, p->d_H, g, part);
-    else if (tc && fast_path_ok(p->cfg, p->L)) rc = launch(p, k_accumulate_fast, p->num_tiles, kTile, kFastSmem, st, false, d, x, p->d_H, g, part);
-    else rc = launch(p, k_pairs<MODE>, p->num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active);
+    if (tc && p->fast_path == 1 && p->records_sorted) rc = launch(p, k_accumulate_runs, ntiles, kTile, kRunSmem, st, false, d, x, p->d_H, g, part);
+    else if (tc && fast_path_ok(p->cfg, p->L)) rc = launch(p, k_accumulate_fast, ntiles, kTile, kFastSmem, st, false, d, x, p->d_H, g, part);
+    else rc = launch(p, k_pairs<MODE>, ntiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active);
     if (rc) return rc;
   }
-  part += p->num_tiles;
-  if (regblocks > 0 && (rc = launch(p, k_regularisers<MODE>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, g, part, p->d_active, p->first_frame, p->last_frame))) return rc;
-  part += regblocks;
-  if (p->num_trip_tiles > 0 && (rc = launch(p, k_triplets<MODE>, p->num_trip_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active))) return rc;
-  part += p->num_trip_tiles;
-  if (p->num_dp_tiles > 0 && (rc = launch(p, k_depth_pairs<MODE>, p->num_dp_tiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active))) return rc;
+  if (regblocks > 0 && (rc = launch(p, k_regularisers<MODE>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, g, part + p->part_reg, p->d_active,
+                                    p->first_frame, p->last_frame))) return rc;
+  if (p->trips.num_tiles > 0 && (rc = launch(p, k_triplets<MODE>, p->trips.num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part + p->part_trip, p->d_active))) return rc;
+  if (p->dpairs.num_tiles > 0 && (rc = launch(p, k_depth_pairs<MODE>, p->dpairs.num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part + p->part_dp, p->d_active))) return rc;
   return RCVD_OK;
 }
 
@@ -307,53 +308,42 @@ static int upload_plan(rcvd_problem* p) {
   return RCVD_OK;
 }
 
-// constraint and triplet tiles, the record sort of the run path, the per-frame inputs in internal frame order, the scale lattice
+// A family's records, its group frames in internal frame order and its tiles (<= kTile records of one group each) on the device.
+// Triplet centres pass through iperm like pair frames, and k_triplets also reads the neighbours fc - 1 and fc + 1: that holds
+// because make_factor_plan keeps the caller's frame order (iperm the identity) whenever there are triplets.
+static int upload_record_set(rcvd_problem* p, RecordSet& s) {
+  std::vector<int32_t> frames(s.frames.size()), tile_group, tile_count; std::vector<int64_t> tile_begin;
+  for (size_t i = 0; i < frames.size(); ++i) frames[i] = p->plan.iperm[s.frames[i]];
+  for (int i = 0; i < s.groups(); ++i)
+    for (int64_t b = s.offsets[i]; b < s.offsets[i + 1]; b += kTile) { tile_group.push_back(i); tile_begin.push_back(b); tile_count.push_back((int32_t)std::min<int64_t>(kTile, s.offsets[i + 1] - b)); }
+  s.num_tiles = (int)tile_group.size();
+  float* rec; int32_t *fr, *tg, *tn; int64_t* tb; int rc;
+  UP(rec, s.records); UP(fr, frames); UP(tg, tile_group); UP(tb, tile_begin); UP(tn, tile_count);
+  s.dev = RecordTiles{rec, fr, tg, tb, tn};
+  return RCVD_OK;
+}
+
+// the three families on the device, the record sort of the run path, the per-frame inputs in internal frame order, the scale
+// lattice, the layout of the partial costs
 static int set_up_problem_data(rcvd_problem* p) {
   const int N = p->N; const Layout& L = p->L; const std::vector<int>& uperm = p->plan.uperm; int rc;
-  // tiles
-  const int np = (int)(p->pair_frames.size() / 2);
-  std::vector<int32_t> tile_pair, tile_count; std::vector<int64_t> tile_begin;
-  for (int i = 0; i < np; ++i)
-    for (int64_t b = p->offsets[i]; b < p->offsets[i + 1]; b += kTile) { tile_pair.push_back(i); tile_begin.push_back(b); tile_count.push_back((int32_t)std::min<int64_t>(kTile, p->offsets[i + 1] - b)); }
-  p->num_tiles = (int)tile_pair.size(); p->C = p->offsets.empty() ? 0 : p->offsets.back();
-  UP(p->d_tile_pair, tile_pair); UP(p->d_tile_begin, tile_begin); UP(p->d_tile_count, tile_count);
-  {
-    std::vector<int32_t> pf_int(p->pair_frames.size());
-    for (size_t i = 0; i < pf_int.size(); ++i) pf_int[i] = p->plan.iperm[p->pair_frames[i]];
-    UP(p->d_pair_frames, pf_int); UP(p->d_records, p->records_h);
-  }
+  for (RecordSet* s : {&p->pairs, &p->trips, &p->dpairs}) if ((rc = upload_record_set(p, *s))) return rc;
   p->records_sorted = false;
-  if (run_path_ok(p->cfg, L) && p->C > 0 && p->C < (int64_t)0x7fffffff) {
+  if (run_path_ok(p->cfg, L) && p->pairs.count() > 0 && p->pairs.count() < (int64_t)0x7fffffff) {
     // run path of the accumulate kernel: the records of every pair sorted by (source cell, target cell) -- device segmented sort by pair
-    const long long n = p->C;
+    const long long n = p->pairs.count();
     unsigned *d_k0 = nullptr, *d_k1 = nullptr; int *d_i0 = nullptr, *d_i1 = nullptr; float* d_sorted = nullptr; int64_t* d_off = nullptr; void* d_tmp = nullptr;
-    int rcs;
-    if ((rcs = dalloc(p, &d_k0, (size_t)n)) || (rcs = dalloc(p, &d_k1, (size_t)n)) || (rcs = dalloc(p, &d_i0, (size_t)n)) || (rcs = dalloc(p, &d_i1, (size_t)n)) || (rcs = dalloc(p, &d_sorted, (size_t)n * 6)) ||
-        (rcs = upload(p, &d_off, p->offsets))) return rcs;
-    if ((rcs = launch(p, k_record_keys, (unsigned)((n + 255) / 256), 256, 0, p->stream, false, p->cfg, p->d_records, n, d_k0, d_i0))) return rcs;
+    if ((rc = dalloc(p, &d_k0, (size_t)n)) || (rc = dalloc(p, &d_k1, (size_t)n)) || (rc = dalloc(p, &d_i0, (size_t)n)) || (rc = dalloc(p, &d_i1, (size_t)n)) || (rc = dalloc(p, &d_sorted, (size_t)n * 6)) ||
+        (rc = upload(p, &d_off, p->pairs.offsets))) return rc;
+    if ((rc = launch(p, k_record_keys, (unsigned)((n + 255) / 256), 256, 0, p->stream, false, p->cfg, p->pairs.dev.records, n, d_k0, d_i0))) return rc;
     size_t tmp_bytes = 0;
-    CK(cub::DeviceSegmentedSort::SortPairs(nullptr, tmp_bytes, d_k0, d_k1, d_i0, d_i1, (int)n, np, d_off, d_off + 1, p->stream));
+    CK(cub::DeviceSegmentedSort::SortPairs(nullptr, tmp_bytes, d_k0, d_k1, d_i0, d_i1, (int)n, p->pairs.groups(), d_off, d_off + 1, p->stream));
     CK(cudaMallocAsync(&d_tmp, std::max<size_t>(tmp_bytes, 16), p->stream));
-    CK(cub::DeviceSegmentedSort::SortPairs(d_tmp, tmp_bytes, d_k0, d_k1, d_i0, d_i1, (int)n, np, d_off, d_off + 1, p->stream));
-    if ((rcs = launch(p, k_gather_records, (unsigned)((n * 6 + 255) / 256), 256, 0, p->stream, false, p->d_records, d_i1, n, d_sorted))) return rcs;
+    CK(cub::DeviceSegmentedSort::SortPairs(d_tmp, tmp_bytes, d_k0, d_k1, d_i0, d_i1, (int)n, p->pairs.groups(), d_off, d_off + 1, p->stream));
+    if ((rc = launch(p, k_gather_records, (unsigned)((n * 6 + 255) / 256), 256, 0, p->stream, false, p->pairs.dev.records, d_i1, n, d_sorted))) return rc;
     CK(cudaFreeAsync(d_tmp, p->stream));
     CK(cudaGetLastError());
-    p->d_records = d_sorted; p->records_sorted = true;      // (the unsorted copy and the sort buffers go back to the pool with the handle's other allocations)
-  }
-  {
-    std::vector<int32_t> tc, tn; std::vector<int64_t> tb;
-    for (size_t i = 0; i < p->trip_centers.size(); ++i)
-      for (int64_t b = p->trip_offsets[i]; b < p->trip_offsets[i + 1]; b += kTile) { tc.push_back(p->trip_centers[i]); tb.push_back(b); tn.push_back((int32_t)std::min<int64_t>(kTile, p->trip_offsets[i + 1] - b)); }
-    p->num_trip_tiles = (int)tc.size();
-    UP(p->d_trip_tile_center, tc); UP(p->d_trip_tile_begin, tb); UP(p->d_trip_tile_count, tn); UP(p->d_trip_records, p->trip_records);
-  }
-  {
-    std::vector<int32_t> tp, tn, pf(p->dp_pair_frames.size()); std::vector<int64_t> tb;
-    for (size_t i = 0; i + 1 < p->dp_offsets.size(); ++i)
-      for (int64_t b = p->dp_offsets[i]; b < p->dp_offsets[i + 1]; b += kTile) { tp.push_back((int32_t)i); tb.push_back(b); tn.push_back((int32_t)std::min<int64_t>(kTile, p->dp_offsets[i + 1] - b)); }
-    for (size_t i = 0; i < pf.size(); ++i) pf[i] = p->plan.iperm[p->dp_pair_frames[i]];
-    p->num_dp_tiles = (int)tp.size();
-    UP(p->d_dp_tile_pair, tp); UP(p->d_dp_tile_begin, tb); UP(p->d_dp_tile_count, tn); UP(p->d_dp_pair_frames, pf); UP(p->d_dp_records, p->dp_records);
+    p->pairs.dev.records = d_sorted; p->records_sorted = true;      // (the unsorted copy and the sort buffers go back to the pool with the handle's other allocations)
   }
   {
     std::vector<uint8_t> ir(N); std::vector<double> md(N), ad;
@@ -379,6 +369,10 @@ static int set_up_problem_data(rcvd_problem* p) {
   }
   p->first_frame = 0; p->last_frame = -1;
   { bool any = false; for (int f = 0; f < N; ++f) if (p->in_range[f]) { if (!any) { p->first_frame = f; any = true; } p->last_frame = f; } }
+  p->part_reg = p->pairs.num_tiles;
+  p->part_trip = p->part_reg + (reg_counts(p->cfg, L, N, p->nscale).total + 127) / 128;
+  p->part_dp = p->part_trip + p->trips.num_tiles;
+  p->npartial = p->part_dp + p->dpairs.num_tiles;
   return RCVD_OK;
 }
 #undef UP
@@ -393,8 +387,6 @@ static int allocate_storage(rcvd_problem* p) {
   DA(p->d_g2, Upad + 8); DA(p->d_delta, Upad);
   DA(p->d_ytmp, Upad); DA(p->d_y, Upad); DA(p->d_Sy, Upad); DA(p->d_Hy, Upad); DA(p->d_scal, SC_N); DA(p->d_active, Upad); DA(p->d_fail, 1);
   DA(p->d_potrf_progress, (size_t)N);
-  const RegCounts rcn = reg_counts(p->cfg, L, N, p->nscale);
-  p->npartial = p->num_tiles + (rcn.total + 127) / 128 + p->num_trip_tiles + p->num_dp_tiles + 1;
   DA(p->d_partial, (size_t)p->npartial);
   if (p->eval_only) { DA(p->d_H, 1); DA(p->d_Lb, 1); DA(p->d_T, 1); DA(p->d_invL, 1); DA(p->d_invT, 1); }   // cost / gradient evaluations only: no matrices
   else {
@@ -455,13 +447,13 @@ static int allocate_storage(rcvd_problem* p) {
 }
 
 static int build_structure(rcvd_problem* p) {
-  if (p->nranks > 1 && !p->dp_pair_frames.empty()) return set_err(RCVD_ERR_INVALID, "depth-normalisation pairs are not sharded: they need a single-GPU problem (nranks = 1)");
+  if (p->nranks > 1 && !p->dpairs.frames.empty()) return set_err(RCVD_ERR_INVALID, "depth-normalisation pairs are not sharded: they need a single-GPU problem (nranks = 1)");
   free_all(p);
   CK(cudaSetDevice(p->device));
   // the frame graph: static pairs (or the global structure of a sharded problem) and the depth-normalisation pairs
-  std::vector<int32_t> graph = p->struct_pairs.empty() ? p->pair_frames : p->struct_pairs;
-  graph.insert(graph.end(), p->dp_pair_frames.begin(), p->dp_pair_frames.end());
-  if (const char* e = make_factor_plan(p->plan, p->cfg, graph, p->trip_centers, p->order_slack, p->nranks, p->rank, p->dist_enabled, p->num_sms))
+  std::vector<int32_t> graph = p->struct_pairs.empty() ? p->pairs.frames : p->struct_pairs;
+  graph.insert(graph.end(), p->dpairs.frames.begin(), p->dpairs.frames.end());
+  if (const char* e = make_factor_plan(p->plan, p->cfg, graph, p->trips.frames, p->order_slack, p->nranks, p->rank, p->dist_enabled, p->num_sms))
     return set_err(RCVD_ERR_INVALID, "%s", e);
   while (p->ev_side.size() < 2 * p->plan.levels.size()) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); p->ev_side.push_back(e); }
   int rc;
@@ -742,13 +734,12 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
   if (wantH && p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no normal matrix");
   const Layout& L = p->L; const int N = p->N, npad = L.npad; cudaStream_t st = p->stream;
   const size_t bs = (size_t)npad * npad, Upad = (size_t)N * npad;
-  const int regblocks = (reg_counts(p->cfg, L, N, p->nscale).total + 127) / 128;
   if (wantH) CK(cudaMemsetAsync(p->d_H, 0, p->plan.hblocks.size() * bs * sizeof(double), st));
   if (wantG) CK(cudaMemsetAsync(gout, 0, (Upad + 8) * sizeof(double), st));
   int rc = wantH ? enqueue_residuals<EvalMode::CostGradH>(p, x, gout)
            : wantG ? enqueue_residuals<EvalMode::CostGrad>(p, x, gout) : enqueue_residuals<EvalMode::Cost>(p, x, gout);
   if (rc) return rc;
-  if ((rc = launch(p, k_reduce_partials, 1, 1024, 0, st, false, p->d_partial, p->num_tiles + regblocks + p->num_trip_tiles + p->num_dp_tiles, p->d_scal, slot))) return rc;
+  if ((rc = launch(p, k_reduce_partials, 1, 1024, 0, st, false, p->d_partial, p->npartial, p->d_scal, slot))) return rc;
   if (p->nranks > 1) {
     if (wantG) {
       // ONE packed all-reduce: [gradient (Upad) | cost + 7 spare | diagonal of H (Upad, only with H into d_g)]
@@ -795,7 +786,6 @@ static int save_state(rcvd_problem* p) {
 
 static int ensure_ready(rcvd_problem* p) {
   if (!p->structure_ready) {
-    if (p->offsets.empty()) { p->offsets.assign(1, 0); }
     if (p->in_range.empty()) p->in_range.assign(p->N, 1);
     if (p->median.empty()) p->median.assign(p->N, 1.0);
     int rc = build_structure(p); if (rc) return rc;
@@ -958,7 +948,7 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
   int rc = ensure_ready(p); if (rc) return rc;
   const Layout& L = p->L; const int N = p->N, npad = L.npad; const size_t Upad = (size_t)N * npad, U = (size_t)N * L.nf; cudaStream_t st = p->stream;
   const int64_t launches0 = p->launches;
-  sum.num_constraints = p->C;
+  sum.num_constraints = p->pairs.count();
   const bool constrained = p->cfg.depth_lower_bound && L.nd > 0;
   if (constrained && (rc = launch(p, k_project_state, nblk(U), 256, 0, st, false, p->cfg, L, p->d_in_range, p->d_x, N))) return rc;
   // user-visible minimum-cost iterate
@@ -1141,52 +1131,42 @@ RCVD_API int32_t rcvd_problem_set_frames(rcvd_problem* p, const uint8_t* in_rang
   p->structure_ready = false;
   return RCVD_OK;
 }
-RCVD_API int32_t rcvd_problem_set_constraints(rcvd_problem* p, int32_t np, const int32_t* pf, const int64_t* off, const float* rec) {
-  if (!p || np < 0 || (np > 0 && (!pf || !off))) return set_err(RCVD_ERR_INVALID, "bad constraint arrays");
-  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
-  p->pair_frames.assign(pf, pf + 2 * (size_t)np);
-  if (np > 0) p->offsets.assign(off, off + np + 1); else p->offsets.assign(1, 0);
-  for (int i = 0; i < np; ++i) {
-    if (p->offsets[i + 1] < p->offsets[i]) return set_err(RCVD_ERR_INVALID, "offsets must be non-decreasing");
-    if (pf[2 * i] < 0 || pf[2 * i] >= p->N || pf[2 * i + 1] < 0 || pf[2 * i + 1] >= p->N || pf[2 * i] == pf[2 * i + 1]) return set_err(RCVD_ERR_INVALID, "bad frame pair %d", i);
+// The setter of every family.  Everything is checked before anything is kept, so a refused call leaves the problem as it was:
+// n groups of frames[n][nframes], offsets[n + 1] from 0, non-decreasing, records[offsets[n]][width].
+static int32_t set_records(rcvd_problem* p, RecordSet rcvd_problem::*family, const char* what, int32_t n, const int32_t* frames, const int64_t* off,
+                           const float* rec) {
+  if (!p || n < 0 || (n > 0 && (!frames || !off))) return set_err(RCVD_ERR_INVALID, "bad %s arrays", what);
+  RecordSet& s = p->*family;
+  if (n > 0 && off[0] != 0) return set_err(RCVD_ERR_INVALID, "%s offsets must start at 0", what);
+  for (int i = 0; i < n; ++i) {
+    if (off[i + 1] < off[i]) return set_err(RCVD_ERR_INVALID, "%s offsets must be non-decreasing", what);
+    const int32_t* f = frames + (size_t)i * s.nframes;
+    const bool ok = s.nframes == 2 ? f[0] >= 0 && f[0] < p->N && f[1] >= 0 && f[1] < p->N && f[0] != f[1]   // two distinct frames
+                                   : f[0] >= 1 && f[0] < p->N - 1;                                         // a centre with two neighbours
+    if (!ok) return set_err(RCVD_ERR_INVALID, "bad %s group %d", what, i);
   }
-  const int64_t C = p->offsets.back();
-  if (C > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null records");
-  p->records_h.assign(rec, rec + (size_t)C * 6);
+  const int64_t count = n > 0 ? off[n] : 0;
+  if (count > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null %s records", what);
+  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
+  s.frames.assign(frames, frames + (size_t)n * s.nframes);
+  if (n > 0) s.offsets.assign(off, off + n + 1); else s.offsets.assign(1, 0);
+  s.records.assign(rec, rec + (size_t)count * s.width);
   p->structure_ready = false;
   return RCVD_OK;
+}
+RCVD_API int32_t rcvd_problem_set_constraints(rcvd_problem* p, int32_t np, const int32_t* pf, const int64_t* off, const float* rec) {
+  return set_records(p, &rcvd_problem::pairs, "constraint", np, pf, off, rec);
 }
 RCVD_API int32_t rcvd_problem_set_triplets(rcvd_problem* p, int32_t nt, const int32_t* centers, const int64_t* off, const float* rec) {
-  if (!p || nt < 0 || (nt > 0 && (!centers || !off))) return set_err(RCVD_ERR_INVALID, "bad triplet arrays");
-  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
-  p->trip_centers.assign(centers, centers + nt);
-  if (nt > 0) p->trip_offsets.assign(off, off + nt + 1); else p->trip_offsets.assign(1, 0);
-  for (int i = 0; i < nt; ++i) if (p->trip_offsets[i + 1] < p->trip_offsets[i] || centers[i] < 1 || centers[i] + 1 >= p->N) return set_err(RCVD_ERR_INVALID, "bad triplet group %d", i);
-  const int64_t n = p->trip_offsets.back();
-  if (n > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null triplet records");
-  p->trip_records.assign(rec, rec + (size_t)n * 10);
-  p->structure_ready = false;
-  return RCVD_OK;
+  return set_records(p, &rcvd_problem::trips, "triplet", nt, centers, off, rec);
 }
 RCVD_API int32_t rcvd_problem_set_depth_pairs(rcvd_problem* p, int32_t np, const int32_t* pf, const int64_t* off, const float* rec) {
-  if (!p || np < 0 || (np > 0 && (!pf || !off))) return set_err(RCVD_ERR_INVALID, "bad depth-pair arrays");
-  if (p->nranks > 1 && np > 0) return set_err(RCVD_ERR_INVALID, "depth-normalisation pairs are not sharded: they need a single-GPU problem (nranks = 1)");
-  for (int i = 0; i < np; ++i) {   // checked before anything is kept: a refused call leaves the problem as it was
-    if (off[i + 1] < off[i] || off[0] != 0) return set_err(RCVD_ERR_INVALID, "offsets must start at 0 and be non-decreasing");
-    if (pf[2 * i] < 0 || pf[2 * i] >= p->N || pf[2 * i + 1] < 0 || pf[2 * i + 1] >= p->N || pf[2 * i] == pf[2 * i + 1]) return set_err(RCVD_ERR_INVALID, "bad frame pair %d", i);
-  }
-  const int64_t C = np > 0 ? off[np] : 0;
-  if (C > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null records");
-  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
-  p->dp_pair_frames.assign(pf, pf + 2 * (size_t)np);
-  if (np > 0) p->dp_offsets.assign(off, off + np + 1); else p->dp_offsets.assign(1, 0);
-  p->dp_records.assign(rec, rec + (size_t)C * 6);
-  p->structure_ready = false;
-  return RCVD_OK;
+  if (p && p->nranks > 1 && np > 0) return set_err(RCVD_ERR_INVALID, "depth-normalisation pairs are not sharded: they need a single-GPU problem (nranks = 1)");
+  return set_records(p, &rcvd_problem::dpairs, "depth-pair", np, pf, off, rec);
 }
 // Global frame-pair graph for multi-GPU runs (every rank must build the same block structure).
 RCVD_API int32_t rcvd_problem_set_structure(rcvd_problem* p, int32_t np, const int32_t* pf) {
-  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  if (!p || np < 0 || (np > 0 && !pf)) return set_err(RCVD_ERR_INVALID, "bad structure arrays");
   p->struct_pairs.assign(pf, pf + 2 * (size_t)np);
   p->structure_ready = false;
   return RCVD_OK;
@@ -1616,7 +1596,7 @@ RCVD_API int32_t rcvd_structure_info(rcvd_problem* p, int32_t out[8]) {
   if (!p) return set_err(RCVD_ERR_INVALID, "null argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
-  out[0] = p->N; out[1] = p->plan.nLoff; out[2] = (int)p->plan.levels.size(); out[3] = (int)p->plan.hblocks.size(); out[4] = p->L.npad; out[5] = p->L.nf; out[6] = p->num_tiles;
+  out[0] = p->N; out[1] = p->plan.nLoff; out[2] = (int)p->plan.levels.size(); out[3] = (int)p->plan.hblocks.size(); out[4] = p->L.npad; out[5] = p->L.nf; out[6] = p->pairs.num_tiles;
   out[7] = p->plan.upd_targets;
   return RCVD_OK;
 }

@@ -15,29 +15,33 @@
 
 namespace rcvd {
 
-constexpr int kTile = 128;          // constraints per CTA tile (all from one directed pair)
+constexpr int kTile = 128;          // constraints per CTA tile (all from one group: a directed pair or a triplet centre)
 
 enum class EvalMode { Cost, CostGrad, CostGradH, MarkActive };
+
+// One constraint family on the device: groups of consecutive records (a group is a directed frame pair, or a triplet's centre
+// frame), cut into tiles of <= kTile records of one group.  Tile t is CTA t of the family's kernel.
+struct RecordTiles {
+  const float* records;         // [n][record width]
+  const int32_t* group_frames;  // [groups][frames per group], internal frame ids
+  const int32_t* tile_group;    // [T]
+  const int64_t* tile_begin;    // [T] first record
+  const int32_t* tile_count;    // [T] records
+};
 
 struct DevProblem {
   rcvd_config cfg;
   Layout L;
   int N;
-  const float* records;        // [C][6]
-  const int32_t* tile_pair;    // [T]
-  const int64_t* tile_begin;   // [T]
-  const int32_t* tile_count;   // [T]
-  const int32_t* pair_frames;  // [P][2]
+  RecordTiles pairs;           // static-scene pairs, records [C][6]
+  RecordTiles trips;           // scene-flow smoothness triplets (optional), records [n][10]
+  RecordTiles dpairs;          // pairwise depth-normalisation pairs (optional), records [n][6]
   const int32_t* blk_of;       // [N*N]: (fa,fb) -> H block id*2 + (fa is the row side), -1 if absent
   const uint8_t* in_range;     // [N]
   const double* median;        // [N]
   const double* adaptive;      // [N*G] or null
   const float* scale_locs;     // [M][2]
   int rank, nranks;            // regulariser and triplet rows are evaluated by rank f % nranks (every rank marks them all)
-  // scene-flow smoothness triplets (optional): records [n][10], tiles of <= kTile constraints with one centre frame
-  const float* trip_records; const int32_t* trip_tile_center; const int64_t* trip_tile_begin; const int32_t* trip_tile_count;
-  // pairwise depth-normalisation constraints (optional): records [n][6], tiles of <= kTile constraints of one directed pair
-  const float* dp_records; const int32_t* dp_pair_frames; const int32_t* dp_tile_pair; const int64_t* dp_tile_begin; const int32_t* dp_tile_count;
 };
 
 __device__ __forceinline__ bool is_const_local(const rcvd_config& c, const Layout& L, int l) {
@@ -167,11 +171,11 @@ __global__ void __launch_bounds__(kTile) k_pairs(DevProblem p, const double* __r
                                                  double* __restrict__ partial, uint8_t* __restrict__ mask) {
   const rcvd_config& c = p.cfg;
   const int t = blockIdx.x;
-  const int pr = p.tile_pair[t];
-  const int f0 = p.pair_frames[2 * pr], f1 = p.pair_frames[2 * pr + 1];
+  const int pr = p.pairs.tile_group[t];
+  const int f0 = p.pairs.group_frames[2 * pr], f1 = p.pairs.group_frames[2 * pr + 1];
   double cost = 0.0;
-  if ((int)threadIdx.x < p.tile_count[t]) {
-    const float* rec = p.records + (size_t)(p.tile_begin[t] + threadIdx.x) * 6;
+  if ((int)threadIdx.x < p.pairs.tile_count[t]) {
+    const float* rec = p.pairs.records + (size_t)(p.pairs.tile_begin[t] + threadIdx.x) * 6;
     if constexpr (MODE == EvalMode::MarkActive) {
       for (int side = 0; side < 2; ++side) {
         Gather dg, sg;
@@ -338,16 +342,16 @@ __global__ void __launch_bounds__(kTile) k_accumulate_fast(DevProblem p, const d
   double* Ms = sm + 3 * kTile * kJsLd;              // [4 warps][16][16]
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int t = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int pr = p.tile_pair[t];
-  const int f0 = p.pair_frames[2 * pr], f1 = p.pair_frames[2 * pr + 1];
+  const int pr = p.pairs.tile_group[t];
+  const int f0 = p.pairs.group_frames[2 * pr], f1 = p.pairs.group_frames[2 * pr + 1];
   const int np = L.npad, gx = c.depth_grid_x;
   const PairBlocks hb = pair_blocks(p, H, f0, f1);
-  const bool active = tid < p.tile_count[t];
+  const bool active = tid < p.pairs.tile_count[t];
   const int nn = c.depth_type == RCVD_DEPTH_GRID ? 4 : (c.depth_type == RCVD_DEPTH_GLOBAL ? 1 : 0);
   double Jl[60]; TcEval e = {};
 #pragma unroll
   for (int i = 0; i < 60; ++i) Jl[i] = 0.0;
-  if (active) tc_eval<false>(p, x, f0, f1, p.records + (size_t)(p.tile_begin[t] + tid) * 6, Jl, e);
+  if (active) tc_eval<false>(p, x, f0, f1, p.pairs.records + (size_t)(p.pairs.tile_begin[t] + tid) * 6, Jl, e);
   stage_pose_rows<kJsLd>(Js, tid, Jl, e);
   // ---- per-thread scatter of the spline-node columns ----
   if (active && nn > 0) {
@@ -417,20 +421,20 @@ __global__ void __launch_bounds__(kTile) k_accumulate_runs(DevProblem p, const d
   unsigned* skey = reinterpret_cast<unsigned*>(Ms + 4 * 256);
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int t = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int pr = p.tile_pair[t];
-  const int f0 = p.pair_frames[2 * pr], f1 = p.pair_frames[2 * pr + 1];
+  const int pr = p.pairs.tile_group[t];
+  const int f0 = p.pairs.group_frames[2 * pr], f1 = p.pairs.group_frames[2 * pr + 1];
   const int np = L.npad;
   const PairBlocks hb = pair_blocks(p, H, f0, f1);
   const int gx = c.depth_grid_x;
   double cost = 0.0;
-  const bool active = tid < p.tile_count[t];
+  const bool active = tid < p.pairs.tile_count[t];
   unsigned key = 0xffffffffu;
   {
     double Jl[60]; TcEval e = {};
 #pragma unroll
     for (int i = 0; i < 60; ++i) Jl[i] = 0.0;
     if (active) {
-      tc_eval<true>(p, x, f0, f1, p.records + (size_t)(p.tile_begin[t] + tid) * 6, Jl, e);
+      tc_eval<true>(p, x, f0, f1, p.pairs.records + (size_t)(p.pairs.tile_begin[t] + tid) * 6, Jl, e);
       key = ((unsigned)e.node0 << 16) | (unsigned)e.node1;
     }
     cost = e.cost;
@@ -634,11 +638,11 @@ __global__ void __launch_bounds__(kTile) k_triplets(DevProblem p, const double* 
                                                     double* __restrict__ partial, uint8_t* __restrict__ mask) {
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int t = blockIdx.x;
-  const int fc = p.trip_tile_center[t];
+  const int fc = p.trips.group_frames[p.trips.tile_group[t]];
   const bool mine = MODE == EvalMode::MarkActive || (p.nranks <= 1) || (fc % p.nranks == p.rank);
   double cost = 0.0;
-  if ((int)threadIdx.x < p.trip_tile_count[t] && mine) {
-    const float* rec = p.trip_records + (size_t)(p.trip_tile_begin[t] + threadIdx.x) * 10;
+  if ((int)threadIdx.x < p.trips.tile_count[t] && mine) {
+    const float* rec = p.trips.records + (size_t)(p.trips.tile_begin[t] + threadIdx.x) * 10;
     Gather dg[3], sg[3];
     ObsIn o[3]; const double* pose[3]; double phi[3], D[3], u[3][2];
     for (int i = 0; i < 3; ++i) {
@@ -682,10 +686,10 @@ __global__ void __launch_bounds__(kTile) k_depth_pairs(DevProblem p, const doubl
                                                        double* __restrict__ partial, uint8_t* __restrict__ mask) {
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int t = blockIdx.x, np = L.npad;
-  const int pr = p.dp_tile_pair[t];
-  const int fr[2] = {p.dp_pair_frames[2 * pr], p.dp_pair_frames[2 * pr + 1]};
-  const bool active = (int)threadIdx.x < p.dp_tile_count[t];
-  const float* rec = p.dp_records + (size_t)(p.dp_tile_begin[t] + (active ? threadIdx.x : 0)) * 6;
+  const int pr = p.dpairs.tile_group[t];
+  const int fr[2] = {p.dpairs.group_frames[2 * pr], p.dpairs.group_frames[2 * pr + 1]};
+  const bool active = (int)threadIdx.x < p.dpairs.tile_count[t];
+  const float* rec = p.dpairs.records + (size_t)(p.dpairs.tile_begin[t] + (active ? threadIdx.x : 0)) * 6;
   Gather dg[2];
   for (int s = 0; s < 2; ++s) {
     if (active) gather_depth(c, rec[3 * s], rec[3 * s + 1], dg[s]);

@@ -123,29 +123,26 @@ class Problem:
         aw = None if adaptive_weights is None else np.ascontiguousarray(adaptive_weights, np.float64)
         _check(self.L.rcvd_problem_set_frames(self.h, _p(ir, C.c_uint8), _p(md, C.c_double), _p(aw, C.c_double)))
 
-    def set_constraints(self, pair_frames, offsets, records):
-        pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
+    def _set_records(self, setter, frames, frames_per_group, offsets, records, width):
+        """One constraint family through its C setter: frames[G, frames_per_group], offsets[G+1], records[n][width].  Returns n."""
+        fr = np.ascontiguousarray(frames, np.int32).reshape(-1, frames_per_group)
         off = np.ascontiguousarray(offsets, np.int64)
-        rec = np.ascontiguousarray(records, np.float32).reshape(-1, 6)
-        assert off.shape[0] == pf.shape[0] + 1 and off[-1] == rec.shape[0]
-        self.num_constraints = int(rec.shape[0])
-        _check(self.L.rcvd_problem_set_constraints(self.h, C.c_int32(pf.shape[0]), _p(pf, C.c_int32), _p(off, C.c_int64), _p(rec, C.c_float)))
+        rec = np.ascontiguousarray(records, np.float32).reshape(-1, width)
+        assert off.shape[0] == fr.shape[0] + 1 and off[-1] == rec.shape[0]
+        _check(setter(self.h, C.c_int32(fr.shape[0]), _p(fr, C.c_int32), _p(off, C.c_int64), _p(rec, C.c_float)))
+        return int(rec.shape[0])
+
+    def set_constraints(self, pair_frames, offsets, records):
+        self.num_constraints = self._set_records(self.L.rcvd_problem_set_constraints, pair_frames, 2, offsets, records, 6)
 
     def set_triplets(self, centers, offsets, records):
         """Scene-flow smoothness constraints (addSceneFlowSmoothnessLoss): centers[T], offsets[T+1], records[n][10]."""
-        ce = np.ascontiguousarray(centers, np.int32); off = np.ascontiguousarray(offsets, np.int64)
-        rec = np.ascontiguousarray(records, np.float32).reshape(-1, 10)
-        assert off.shape[0] == ce.shape[0] + 1 and off[-1] == rec.shape[0]
-        _check(self.L.rcvd_problem_set_triplets(self.h, C.c_int32(ce.shape[0]), _p(ce, C.c_int32), _p(off, C.c_int64), _p(rec, C.c_float)))
+        self._set_records(self.L.rcvd_problem_set_triplets, centers, 1, offsets, records, 10)
 
     def set_depth_pairs(self, pair_frames, offsets, records):
         """Pairwise depth-normalisation constraints (DisparityDissimilarityCost): pair_frames[P, 2], offsets[P+1], records[C][6] in the
         layout of set_constraints.  Single-GPU only."""
-        pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
-        off = np.ascontiguousarray(offsets, np.int64)
-        rec = np.ascontiguousarray(records, np.float32).reshape(-1, 6)
-        assert off.shape[0] == pf.shape[0] + 1 and off[-1] == rec.shape[0]
-        _check(self.L.rcvd_problem_set_depth_pairs(self.h, C.c_int32(pf.shape[0]), _p(pf, C.c_int32), _p(off, C.c_int64), _p(rec, C.c_float)))
+        self._set_records(self.L.rcvd_problem_set_depth_pairs, pair_frames, 2, offsets, records, 6)
 
     def set_structure(self, pair_frames):
         pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
