@@ -187,12 +187,11 @@ struct rcvd_problem {
   double *d_H = nullptr, *d_Lb = nullptr, *d_T = nullptr, *d_invL = nullptr, *d_invT = nullptr;
   HBlock *d_hblocks = nullptr, *d_lblocks = nullptr; int* d_fail = nullptr;
   int* d_potrf_progress = nullptr;   // [N] tile columns of each diagonal block k_potrf_smem has published (read by the streamed k_trsm_ll)
-  int trsm2_ctas_per_sm = 0;          // resident k_trsm_ll<2> CTAs per SM at this npad
+  FactorKernels fk = {};              // the factorisation's kernel variants at this npad (allocate_storage)
   // the block-Cholesky plan (rcvd_plan.h) and its device copies
   FactorPlan plan;
-  int *d_lvl_frames = nullptr; GemmTask* d_trsm_tasks = nullptr; int2 *d_trsm_pairs = nullptr, *d_upd_pairs = nullptr;
+  int *d_lvl_frames = nullptr; TrsmTask* d_trsm_tasks = nullptr; int2* d_upd_pairs = nullptr; SolveTask* d_fwd_tasks = nullptr;
   SubTask* d_sub_tasks = nullptr; int* d_sub_counters = nullptr; int* d_sub_need = nullptr;
-  SolveTask* d_fwd_tasks = nullptr; TrsmTask* d_trsm_ll = nullptr; bool use_trsm_ll = false;
   cudaGraphExec_t solve_graph = nullptr;
   bool structure_ready = false, constraints_set = false, frames_set = false;
   // multi GPU
@@ -302,9 +301,9 @@ static int upload_plan(rcvd_problem* p) {
   const FactorPlan& pl = p->plan; int rc;
   UP(p->d_blk_of, pl.blk_of); UP(p->d_hblocks, pl.hblocks); UP(p->d_lblocks, pl.lblocks); UP(p->d_lvl_frames, pl.lvl_frames); UP(p->d_lvl_own, pl.lvl_own);
   UP(p->d_load_lblocks, pl.load_lblocks); UP(p->d_own_hblocks, pl.own_hblocks); UP(p->d_uperm, pl.uperm);
-  UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_trsm_pairs, pl.trsm_pairs); UP(p->d_upd_pairs, pl.upd_pairs);
+  UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_upd_pairs, pl.upd_pairs);
   UP(p->d_sub_tasks, pl.sub_tasks); UP(p->d_sub_need, pl.sub_need); DA(p->d_sub_counters, (size_t)4 * p->N + 4);
-  UP(p->d_fwd_tasks, pl.fwd_tasks); UP(p->d_trsm_ll, pl.trsm_ll); UP(p->d_upd_items, pl.upd_items);
+  UP(p->d_fwd_tasks, pl.fwd_tasks); UP(p->d_upd_items, pl.upd_items);
   return RCVD_OK;
 }
 
@@ -428,21 +427,21 @@ static int allocate_storage(rcvd_problem* p) {
     if (r != 0) return set_err(RCVD_ERR_NCCL, "ncclAllReduce(active mask) failed");
   }
   // kernels that need > 48 KB dynamic smem
-  if ((npad * 16 + 16 * (npad + 1)) * (int)sizeof(double) > 220 * 1024) return set_err(RCVD_ERR_INVALID, "frame block too large for the panel-inverse kernel (npad=%d)", npad);
-  CK(cudaFuncSetAttribute(k_trinv, cudaFuncAttributeMaxDynamicSharedMemorySize, (npad * 16 + 16 * (npad + 1)) * (int)sizeof(double)));
+  FactorKernels& fk = p->fk = factor_kernels(npad);
+  if (fk.trinv_bytes > kMaxDynSmem) return set_err(RCVD_ERR_INVALID, "frame block too large for the panel-inverse kernel (npad=%d)", npad);
+  CK(cudaFuncSetAttribute(k_trinv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fk.trinv_bytes));
   CK(cudaFuncSetAttribute(k_accumulate_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmem));
   CK(cudaFuncSetAttribute(k_accumulate_runs, cudaFuncAttributeMaxDynamicSharedMemorySize, kRunSmem));
-  p->use_trsm_ll = trsm_ll_smem_bytes(npad) <= 220 * 1024;
-  if (p->use_trsm_ll) {
-    CK(cudaFuncSetAttribute(k_trsm_ll<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2)));
-    CK(cudaFuncSetAttribute(k_trsm_ll<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 2)));
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p->trsm2_ctas_per_sm, k_trsm_ll<2, true>, 128, trsm_ll_smem_bytes(npad, 2)));
-    if (trsm_ll_smem_bytes(npad, 4) <= 220 * 1024) {
-      CK(cudaFuncSetAttribute(k_trsm_ll<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4)));
-      CK(cudaFuncSetAttribute(k_trsm_ll<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trsm_ll_smem_bytes(npad, 4)));
-    }
+  if (fk.trsm_ll) {
+    CK(cudaFuncSetAttribute(k_trsm_ll<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fk.trsm_ll2_bytes));
+    CK(cudaFuncSetAttribute(k_trsm_ll<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fk.trsm_ll2_bytes));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fk.trsm2_ctas_per_sm, k_trsm_ll<2, true>, 128, fk.trsm_ll2_bytes));
   }
-  if (potrf_smem_bytes(npad) <= 220 * 1024) CK(cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)potrf_smem_bytes(npad)));
+  if (fk.trsm_ll4) {
+    CK(cudaFuncSetAttribute(k_trsm_ll<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fk.trsm_ll4_bytes));
+    CK(cudaFuncSetAttribute(k_trsm_ll<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fk.trsm_ll4_bytes));
+  }
+  if (fk.potrf_smem) CK(cudaFuncSetAttribute(k_potrf_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fk.potrf_bytes));
   return RCVD_OK;
 }
 
@@ -495,13 +494,13 @@ static int grouped(rcvd_problem* p, double* base, size_t unit, const std::vector
 // inverses run on a third stream, `inv`: on `side` they would hold back the next update launch by a k_trinv.
 struct FactorSolve {
   enum { P_LOAD = 0, P_POTRF, P_TRINV, P_TRSM, P_GEMM, P_SOLVE };   // kernel classes of rcvd_debug_profile_linear
-  rcvd_problem* p; const FactorPlan& pl; const int N, npad, strips; cudaStream_t st, side, inv;
+  rcvd_problem* p; const FactorPlan& pl; const FactorKernels& fk; const int N, npad, strips; cudaStream_t st, side, inv;
   int prof_level = 0;
   bool side_used = false, inv_used = false;   // work was enqueued on `side` / on `inv` since the main stream last waited for it
   int side_joined = -1;                        // the main stream has waited for the side launches (2 * level + launch) up to this one
 
   explicit FactorSolve(rcvd_problem* p_)
-      : p(p_), pl(p_->plan), N(p_->N), npad(p_->L.npad), strips((npad + kTrsmStrip - 1) / kTrsmStrip), st(p_->stream), side(p_->side_stream),
+      : p(p_), pl(p_->plan), fk(p_->fk), N(p_->N), npad(p_->L.npad), strips((npad + kTrsmStrip - 1) / kTrsmStrip), st(p_->stream), side(p_->side_stream),
         inv(p_->inv_stream) {}
 
   void mark(int cls) {   // profiling mode only (single stream, not captured)
@@ -528,16 +527,15 @@ struct FactorSolve {
   }
 
   // A level's TRSM launch that is a single wave (the narrow levels) is streamed behind its k_potrf_smem (see trsm).
-  bool trsm_deep(const Level& v) const { return strips * v.ntrsm <= p->num_sms && trsm_ll_smem_bytes(npad, 4) <= 220 * 1024; }
+  bool trsm_deep(const Level& v) const { return strips * v.ntrsm <= p->num_sms && fk.trsm_ll4; }
   bool streamed(const Level& v) const {
-    return p->use_trsm_ll && v.nown > 0 && v.ntrsm > 0 && potrf_smem_bytes(npad) <= 220 * 1024 &&
-           strips * v.ntrsm <= (trsm_deep(v) ? 1 : p->trsm2_ctas_per_sm) * p->num_sms;
+    return fk.trsm_ll && v.nown > 0 && v.ntrsm > 0 && fk.potrf_smem && strips * v.ntrsm <= (trsm_deep(v) ? 1 : fk.trsm2_ctas_per_sm) * p->num_sms;
   }
 
   // the Cholesky of the level's diagonal blocks
   int factor_diagonal(const int* frames, int nfr, bool pdl) {
-    if (potrf_smem_bytes(npad) <= 220 * 1024)
-      return launch(LP_POTRF_SMEM, k_potrf_smem, dim3(nfr), dim3(kPotrfSmemThreads), potrf_smem_bytes(npad), st, pdl, p->d_Lb, p->d_invT, frames, npad,
+    if (fk.potrf_smem)
+      return launch(LP_POTRF_SMEM, k_potrf_smem, dim3(nfr), dim3(kPotrfSmemThreads), fk.potrf_bytes, st, pdl, p->d_Lb, p->d_invT, frames, npad,
                     p->d_fail, p->d_potrf_progress);
     // large blocks: 16-wide panels, panel factor on one CTA per frame, trailing update on the whole machine
     for (int jb = 0; jb < npad / 16; ++jb) {
@@ -551,26 +549,26 @@ struct FactorSolve {
   // the explicit inverses of the level's diagonal blocks, then the TRSM X_rk = A_rk L_kk^-T of its off-diagonal blocks
   int trsm(const Level& lv, const int* frames, int nfr, bool chain) {
     // k_trsm_ll does not read the explicit inverse, only the (much later) substitution does: compute it off the critical path
-    const bool inv_stream = p->use_trsm_ll && p->overlap;
+    const bool inv_stream = fk.trsm_ll && p->overlap;
     if (inv_stream) { if (int rc = wait(inv, st, p->ev_fork)) return rc; inv_used = true; }
-    if (int rc = launch(LP_TRINV, k_trinv, dim3(npad / 16, nfr), dim3(256), (npad * 16 + 16 * (npad + 1)) * sizeof(double), inv_stream ? inv : st, false,
+    if (int rc = launch(LP_TRINV, k_trinv, dim3(npad / 16, nfr), dim3(256), fk.trinv_bytes, inv_stream ? inv : st, false,
                         p->d_Lb, p->d_invT, p->d_invL, frames, npad)) return rc;
     mark(P_TRINV);
     if (lv.ntrsm == 0) return RCVD_OK;
     int rc;
-    if (p->use_trsm_ll) {
+    if (fk.trsm_ll) {
       // One CTA per SM fits the launch in a single wave: deep panel prefetch (AHEAD = 4); otherwise two CTAs per SM (AHEAD = 2).
       // A launch that is a single wave (`chain`: the narrow levels) starts beside its level's k_potrf_smem as a programmatic dependent
       // launch and follows the tile columns the Cholesky publishes.  The wide levels' multi-wave launches wait for the Cholesky to finish.
       const bool deep = trsm_deep(lv);
       decltype(&k_trsm_ll<2>) kernel = deep ? (chain ? k_trsm_ll<4, true> : k_trsm_ll<4>) : (chain ? k_trsm_ll<2, true> : k_trsm_ll<2>);
       if (chain) p->paths[LP_TRSM_STREAMED]++;
-      rc = launch(deep ? LP_TRSM_LL4 : LP_TRSM_LL2, kernel, dim3(strips, lv.ntrsm), dim3(128), trsm_ll_smem_bytes(npad, deep ? 4 : 2), st, chain,
-                  p->d_T, p->d_Lb, p->d_invT, p->d_trsm_ll + lv.trsm_off, npad, chain ? p->d_potrf_progress : nullptr);
+      rc = launch(deep ? LP_TRSM_LL4 : LP_TRSM_LL2, kernel, dim3(strips, lv.ntrsm), dim3(128), deep ? fk.trsm_ll4_bytes : fk.trsm_ll2_bytes, st, chain,
+                  p->d_T, p->d_Lb, p->d_invT, p->d_trsm_tasks + lv.trsm_off, npad, chain ? p->d_potrf_progress : nullptr);
     } else {
       const int tiles = (npad + 63) / 64;
       rc = launch(LP_TRSM_GEMM, k_gemm_nt, dim3(tiles, tiles, lv.ntrsm), dim3(128), 0, st, false, p->d_T, p->d_Lb, p->d_invL,
-                  p->d_trsm_tasks + lv.trsm_off, p->d_trsm_pairs, npad);
+                  p->d_trsm_tasks + lv.trsm_off, npad);
     }
     if (rc) return rc;
     mark(P_TRSM);
@@ -650,7 +648,7 @@ struct FactorSolve {
       SubCounters cn; cn.ticket = p->d_sub_counters; cn.fin = p->d_sub_counters + 4; cn.fdone = cn.fin + N; cn.bin = cn.fdone + N; cn.bdone = cn.bin + N;
       cn.fin_need = p->d_sub_need; cn.bin_need = p->d_sub_need + N;
       const int ntasks = (int)pl.sub_tasks.size();
-      if ((rc = launch(LP_SUB_FUSED, k_substitution, dim3(std::min(ntasks, p->num_sms)), dim3(kSubThreads), substitution_smem_bytes(npad), st, false,
+      if ((rc = launch(LP_SUB_FUSED, k_substitution, dim3(std::min(ntasks, p->num_sms)), dim3(kSubThreads), fk.substitution_bytes, st, false,
                        p->d_invL, p->d_T, p->d_rhs, p->d_ytmp, p->d_y, p->d_sub_tasks, ntasks, cn, npad))) return rc;
     }
     for (int l = LS - 1; l >= 0; --l) {
@@ -1579,11 +1577,11 @@ RCVD_API int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, co
       const Level& lv = pl.levels[l];
       join[2 * l] = lv.join[0]; join[2 * l + 1] = lv.join[1];
       for (int q = lv.upd_off; q < lv.upd2_off[1] + lv.nupd2[1]; ++q) {
-        const GemmTask& t = pl.upd_tasks[q];
+        const UpdPass& t = pl.upd_tasks[q];
         const HBlock& b = pl.lblocks[t.dst];
         int32_t* o = passes + 5 * (size_t)q;
         o[0] = pl.uperm[b.r]; o[1] = pl.uperm[b.c]; o[2] = (int32_t)l; o[3] = q >= lv.upd2_off[1] ? 2 : q >= lv.upd2_off[0] ? 1 : 0; o[4] = t.count;
-        flags[q] = t.lower_only;
+        flags[q] = t.flags;
         for (int i = 0; i < t.count; ++i) sources[t.first + i] = pl.uperm[pl.lblocks[N + pl.upd_pairs[t.first + i].x].c];
       }
     }

@@ -18,8 +18,7 @@
 // its shared-memory slice, lane 0 sums the weights in window order, the warp sorts the keys (bitonic) and lane 0 walks the running
 // weight in sorted order.  S is at most kBilateralMaxSamples.
 #pragma once
-#include <cuda_runtime.h>
-#include <cstdint>
+#include "rcvd_ptx.cuh"
 
 namespace rcvd {
 
@@ -36,14 +35,6 @@ struct BilateralArgs {
   int sw, sh;                                     // mean: staged tile incl. halo (kBfTx + 2r) x (kBfTy + 2r)
   int P;                                          // median: keys per warp (power of two >= the largest window)
 };
-
-__device__ __forceinline__ void bf_cp_async4(float* sdst, const float* gsrc) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(sdst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(s), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void bf_cp_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bf_cp_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 
 // lib/Processor.cpp:264-280
 template <bool COLOR>
@@ -78,17 +69,17 @@ __global__ void __launch_bounds__(kBfTx * kBfTy) k_bilateral_mean(BilateralArgs 
     const float* gd = a.depth + (size_t)f * plane;
     for (int i = threadIdx.x; i < nx * ny; i += kBfTx * kBfTy) {
       const int yy = cy0 + i / nx, xx = cx0 + i % nx;
-      bf_cp_async4(sd + (yy - sy0) * a.sw + (xx - sx0), gd + (size_t)yy * a.w + xx);
+      cp_async4_ca(sd + (yy - sy0) * a.sw + (xx - sx0), gd + (size_t)yy * a.w + xx);
     }
     if (COLOR) {
       float* sc = sd + tile;
       const float* gc = a.color + (size_t)f * plane * 3;
       for (int i = threadIdx.x; i < 3 * nx * ny; i += kBfTx * kBfTy) {
         const int yy = cy0 + i / (3 * nx), xc = i % (3 * nx);
-        bf_cp_async4(sc + (yy - sy0) * 3 * a.sw + 3 * (cx0 - sx0) + xc, gc + ((size_t)yy * a.w + cx0) * 3 + xc);
+        cp_async4_ca(sc + (yy - sy0) * 3 * a.sw + 3 * (cx0 - sx0) + xc, gc + ((size_t)yy * a.w + cx0) * 3 + xc);
       }
     }
-    bf_cp_commit();
+    cp_async_commit();
   };
   float dref = 0.f, r0 = 0.f, r1 = 0.f, r2 = 0.f;
   if (inside) {
@@ -104,7 +95,7 @@ __global__ void __launch_bounds__(kBfTx * kBfTy) k_bilateral_mean(BilateralArgs 
   for (int f = f0; f <= f1; ++f) {
     const float* sd = bf_smem + ((f - f0) & 1) * buf;
     if (STAGED) {
-      if (f < f1) { stage(f + 1, (f - f0 + 1) & 1); bf_cp_wait<1>(); } else bf_cp_wait<0>();
+      if (f < f1) { stage(f + 1, (f - f0 + 1) & 1); cp_async_wait<1>(); } else cp_async_wait<0>();
       __syncthreads();
     }
     if (inside) {

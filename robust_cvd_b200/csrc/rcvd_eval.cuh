@@ -12,6 +12,7 @@
 // The partial costs of all families meet in one deterministic two-stage reduction (k_reduce_partials).
 #pragma once
 #include "rcvd_device.cuh"
+#include "rcvd_ptx.cuh"
 
 namespace rcvd {
 
@@ -219,11 +220,6 @@ __host__ __device__ inline bool fast_path_ok(const rcvd_config& c, const Layout&
 }
 __host__ __device__ inline bool run_path_ok(const rcvd_config& c, const Layout& L) { return fast_path_ok(c, L) && c.depth_type == RCVD_DEPTH_GRID && L.G < 65535; }
 
-__device__ __forceinline__ void dmma_acc(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
 // The three H blocks a pair (f0, f1) touches: its two diagonal blocks and the cross block, stored with frame 0 or frame 1 as rows.
 struct PairBlocks {
   double *H0, *H1, *Hx; bool f0rows; int np;
@@ -311,7 +307,7 @@ __device__ __forceinline__ void pose_block_mma(const double* Js, double* Ms, int
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
-      for (int j = 0; j < 2; ++j) dmma_acc(acc[i][j][0], acc[i][j][1], i ? a1 : a0, j ? a1 : a0);
+      for (int j = 0; j < 2; ++j) dmma_8x8x4(acc[i][j][0], acc[i][j][1], i ? a1 : a0, j ? a1 : a0);
   }
   double* mw = Ms + warp * 256;
 #pragma unroll
@@ -473,7 +469,7 @@ __global__ void __launch_bounds__(kTile) k_accumulate_runs(DevProblem p, const d
         const bool in = row < row1;                                       // the last K step of a run reaches into the next run: masked
         const double a = in ? rowp[16 + gq] : 0.0;
 #pragma unroll
-        for (int nb = 0; nb < 3; ++nb) dmma_acc(acc[nb][0], acc[nb][1], a, in ? rowp[nb * 8 + gq] : 0.0);
+        for (int nb = 0; nb < 3; ++nb) dmma_8x8x4(acc[nb][0], acc[nb][1], a, in ? rowp[nb * 8 + gq] : 0.0);
       }
       // lane (gq, tq) holds M[node gq][columns nb*8 + 2 tq, + 1]
       const int ba = (int)(rk >> 16), bb = (int)(rk & 0xffffu);

@@ -12,6 +12,7 @@
 // and the triangular solves become GEMVs with inv(L_kk).
 #pragma once
 #include "rcvd_device.cuh"
+#include "rcvd_ptx.cuh"
 
 namespace rcvd {
 
@@ -104,21 +105,9 @@ __global__ void __launch_bounds__(kPotrfThreads) k_potrf_panel(double* __restric
 // ---------------------------------------------------------------------------
 constexpr int kPotrfSmemThreads = 512;
 constexpr int kTileSz = 256;
+constexpr size_t kMaxDynSmem = 220 * 1024;   // dynamic shared memory a factorisation kernel may use (factor_kernels picks the variants by it)
 __host__ __device__ inline size_t potrf_smem_bytes(int npad) { const int nt = npad / 16; return (size_t)(nt * (nt + 1) / 2 + 1) * kTileSz * sizeof(double); }
 __device__ __forceinline__ int swz(int r, int k) { return r * 16 + (k ^ ((r & 3) << 2)); }
-__device__ __forceinline__ void cp_async16_fwd(void* smem, const void* gmem) {
-  const unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void dmma_8x8x4_fwd(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-// GPU-scope flags between kernels that run at the same time: k_potrf_smem -> streamed k_trsm_ll (per-frame progress), k_substitution.
-// The writer's CTA barrier orders every thread's stores before one thread's release (cumulativity), like cutlass::Semaphore::release.
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) { int v; asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
-__device__ __forceinline__ void st_release_gpu(int* p, int v) { asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-__device__ __forceinline__ void red_release_add(int* p, int v) { asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
 // C(16x16) = A(16x16) * B(16x16)^T into acc[i8][j8][2] with DMMA; A, B swizzled tiles in smem.
 __device__ __forceinline__ void tile_mma_nt(const double* __restrict__ At, const double* __restrict__ Bt, double acc[2][2][2], int g, int t) {
@@ -130,7 +119,7 @@ __device__ __forceinline__ void tile_mma_nt(const double* __restrict__ At, const
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
-      for (int j = 0; j < 2; ++j) dmma_8x8x4_fwd(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+      for (int j = 0; j < 2; ++j) dmma_8x8x4(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
   }
 }
 
@@ -222,7 +211,7 @@ __device__ __forceinline__ void warp_chol16_blocked(double* __restrict__ D, doub
 #pragma unroll
       for (int i = 0; i < 2; ++i) { const int r = 8 * i + g; pa[i] = r >= k0 + 4 ? D[swz(r, k0 + t)] : 0.0; }
 #pragma unroll
-      for (int u = 0; u < 3; ++u) dmma_8x8x4_fwd(c[u][0], c[u][1], -pa[ui[u]], pa[uj[u]]);
+      for (int u = 0; u < 3; ++u) dmma_8x8x4(c[u][0], c[u][1], -pa[ui[u]], pa[uj[u]]);
     }
     CHOL_PHASE(11);
   }
@@ -240,8 +229,8 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
   // Launched as a programmatic dependent of the previous level's U1 on the narrow levels: wait for it (and its memory) before reading
   // anything; a no-op after an ordinary launch dependency.  Then this CTA's inputs are complete, and a programmatic dependent launch
   // (the streamed k_trsm_ll, which reads blocks U1 updated) may start beside it.
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  griddep_wait();
+  griddep_launch_dependents();
   extern __shared__ __align__(16) double tiles[];
   const int frame = frames[blockIdx.x];
   double* A = Lb + (size_t)frame * npad * npad;
@@ -259,7 +248,7 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
       if (ti == jc) { if (c > r) v.x = 0.0; if (c + 1 > r) v.y = 0.0; }
       *reinterpret_cast<double2*>(&A[(size_t)(ti * 16 + r) * npad + jc * 16 + c]) = v;
     }
-    asm volatile("bar.sync 3, %0;" ::"n"(kPotrfSmemThreads - 32) : "memory");
+    named_bar_sync<3, kPotrfSmemThreads - 32>();
     if (tid == 32) st_release_gpu(progress + frame, jc + 1);
   };
 #ifdef RCVD_POTRF_PHASES
@@ -268,14 +257,11 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
   // asynchronous tile load: 16-byte chunks (the swizzle keeps aligned pairs together), all in flight at once
   for (int idx = tid; idx < ntl * 128; idx += kPotrfSmemThreads) {
     const int tl = idx >> 7, e = idx & 127, r = e >> 3, c = (e & 7) * 2;
-    int ti = (int)((sqrtf(8.f * tl + 1.f) - 1.f) * 0.5f);
-    while ((ti + 1) * (ti + 2) / 2 <= tl) ++ti;
-    while (ti * (ti + 1) / 2 > tl) --ti;
-    const int tj = tl - ti * (ti + 1) / 2;
-    cp_async16_fwd(&tiles[(size_t)tl * kTileSz + swz(r, c)], &A[(size_t)(ti * 16 + r) * npad + tj * 16 + c]);
+    const int2 tij = tri_index(tl);
+    cp_async16(&tiles[(size_t)tl * kTileSz + swz(r, c)], &A[(size_t)(tij.x * 16 + r) * npad + tij.y * 16 + c]);
   }
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  cp_async_commit();
+  cp_async_wait<0>();
   __syncthreads();
   POTRF_PHASE(0);
   if (warp == 0) warp_chol16_blocked(tiles, pinv, lane, fail);
@@ -299,7 +285,7 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
     if (warp == 0) { if (lane < 16 && rows > 0) prow = lane; } else if (widx * 32 + lane < rows - 16) prow = 16 + widx * 32 + lane;
     if (warp != 0) {
       if (jb > 0) publish(jb - 1);                   // in the time the chain warp needs before it arrives on barrier 2
-      asm volatile("bar.sync 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
+      named_bar_sync<2, kPotrfSmemThreads>();
     }
     if (prow >= 0) {
       const int ti = jb + 1 + (prow >> 4), r = prow & 15;
@@ -340,7 +326,7 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
       for (int r = 0; r < 16; ++r) iT[(size_t)jb * 256 + r * 16 + cidx] = xcol[r];
     }
     POTRF_PHASE(2);
-    if (warp != 0) asm volatile("bar.sync 3, %0;" ::"n"(kPotrfSmemThreads - 32) : "memory");
+    if (warp != 0) named_bar_sync<3, kPotrfSmemThreads - 32>();
     POTRF_PHASE(3);
     // ---- trailing update (DMMA) with lookahead: warp 0 updates tile (jb+1, jb+1) first and factors it at once ----
     const int m = nt - jb - 1, ntr = m * (m + 1) / 2;
@@ -359,24 +345,18 @@ __global__ void __launch_bounds__(kPotrfSmemThreads) k_potrf_smem(double* __rest
         }
       return Ct;
     };
-    auto tile_of = [&](int tl, int& gi, int& gj) {   // tile order: tl = 0 is (jb+1, jb+1)
-      int ti = (int)((sqrtf(8.f * tl + 1.f) - 1.f) * 0.5f);
-      while ((ti + 1) * (ti + 2) / 2 <= tl) ++ti;
-      while (ti * (ti + 1) / 2 > tl) --ti;
-      gi = jb + 1 + ti; gj = jb + 1 + (tl - ti * (ti + 1) / 2);
-    };
     // warp 0 owns the chain (measured: 88.7 -> 83.0 us per 208x208 block in tools/potrf_phases.cu, against every warp taking
     // trailing tiles): its panel rows, tile (jb+1, jb+1) and the next pivot tile, with the SM to itself until it arrives on barrier 2
     if (warp == 0) {
       double* Ct = nullptr;
       if (ntr > 0) { __syncwarp(); Ct = upd_tile(jb + 1, jb + 1); }
       __threadfence_block();
-      asm volatile("bar.arrive 2, %0;" ::"n"(kPotrfSmemThreads) : "memory");
+      named_bar_arrive<2, kPotrfSmemThreads>();
       POTRF_PHASE(4);
       if (ntr > 0) { __syncwarp(); warp_chol16_blocked(Ct, pinv + (jb + 1) * 16, lane, fail); }
       POTRF_PHASE(5);
     } else {
-      for (int tl = 1 + widx; tl < ntr; tl += nwork) { int gi, gj; tile_of(tl, gi, gj); upd_tile(gi, gj); }
+      for (int tl = 1 + widx; tl < ntr; tl += nwork) { const int2 tij = tri_index(tl); upd_tile(jb + 1 + tij.x, jb + 1 + tij.y); }   // tl = 0 is (jb+1, jb+1)
     }
     POTRF_PHASE(6);
     __syncthreads();
@@ -432,33 +412,14 @@ __global__ void __launch_bounds__(256) k_trinv(const double* __restrict__ Lb, co
 
 // ---------------------------------------------------------------------------
 // k_gemm_nt: the TRSM of the large-block path (npad > 416, where a k_trsm_ll strip no longer fits in shared memory),
-// dst[t.dst] = sum_p A[pairs[p].x] * B[pairs[p].y]^T with B = inv(L_kk) lower triangular.
+// T[t.dst] = Lb[t.src] * invL[t.kframe]^T for the task t of blockIdx.z, with inv(L_kk) lower triangular.
 // fp64 tensor cores (mma.sync m8n8k4 -> DMMA), CTA tile 64x64, 4 warps of 32x32,
 // K staged 16 at a time through a cp.async double buffer.  The short last tile row is cheap because out-of-range mma tiles
 // are never issued.
 // ---------------------------------------------------------------------------
-struct GemmTask { int dst; int first; int count; int lower_only; };   // lower_only bit0: symmetric update target (tiles above the diagonal are never read); bit1: first pass into a fill block (the target is written, not read)
+struct TrsmTask { int dst; int src; int kframe; };   // T index, L block id, column frame (the task of k_gemm_nt and of k_trsm_ll)
 
 constexpr int kGemmLd = 20;   // padded leading dimension of the 64x16 smem tiles (conflict-free DMMA fragment loads)
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  const int sz = valid ? 16 : 0;
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void dmma_8x8x4(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-// m16n8k4: two m8n8k4 units stacked in M that share the B fragment -- rows g (a0 -> c0, c1) and g + 8 (a1 -> c2, c3).
-// On the H100 it issues at twice the fp64 rate of m8n8k4 (rcvd_debug_fp64_tensor_peak measures every shape live).
-__device__ __forceinline__ void dmma_16x8x4(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
-  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3) : "d"(a0), "d"(a1), "d"(b));
-}
 
 // One 16-deep K stage of a warp's (NI*8) x (NJ*8) sub-tile: NI/NJ are compile-time so that no tensor instruction is predicated
 // (a predicated mma.sync costs a WARPSYNC + branch pair each).
@@ -478,11 +439,11 @@ __device__ __forceinline__ void gemm_stage(const double* __restrict__ as, const 
   }
 }
 
-__global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, const double* __restrict__ Abase, const double* __restrict__ Bbase,
-                                                  const GemmTask* __restrict__ tasks, const int2* __restrict__ pairs, int npad) {
+__global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ T, const double* __restrict__ Lb, const double* __restrict__ invL,
+                                                  const TrsmTask* __restrict__ tasks, int npad) {
   __shared__ __align__(16) double As[2][64 * kGemmLd];
   __shared__ __align__(16) double Bs[2][64 * kGemmLd];
-  const GemmTask task = tasks[blockIdx.z];
+  const TrsmTask task = tasks[blockIdx.z];
   const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
   const size_t bs = (size_t)npad * npad;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -490,7 +451,6 @@ __global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, co
   const int g = lane >> 2, t = lane & 3;
   // B lower triangular (inv(L_kk)): B[n][k] = 0 for k > n, so only K chunks up to this tile's last column matter
   const int kchunks = min(npad, n0 + 64) / 16;
-  const int total = task.count * kchunks;
   // 8-row / 8-column mma tiles of this warp that lie inside the matrix (npad is a multiple of 16, tiles are 64 -> ni, nj in {0, 2, 4})
   const int ni = min(4, max(0, (npad - (m0 + wm)) / 8)), nj = min(4, max(0, (npad - (n0 + wn)) / 8));
   double acc[4][4][2];
@@ -500,10 +460,8 @@ __global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, co
     for (int j = 0; j < 4; ++j) { acc[i][j][0] = 0.0; acc[i][j][1] = 0.0; }
 
   auto load_stage = [&](int st, int kk) {
-    const int2 pr = pairs[task.first + kk / kchunks];
-    const int k0 = (kk % kchunks) * 16;
-    const double* Ag = Abase + (size_t)pr.x * bs + k0;
-    const double* Bg = Bbase + (size_t)pr.y * bs + k0;
+    const double* Ag = Lb + (size_t)task.src * bs + kk * 16;
+    const double* Bg = invL + (size_t)task.kframe * bs + kk * 16;
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int cidx = tid + q * 128;
@@ -515,10 +473,10 @@ __global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, co
     cp_async_commit();
   };
 
-  if (total > 0) load_stage(0, 0);
-  for (int kk = 0; kk < total; ++kk) {
+  load_stage(0, 0);
+  for (int kk = 0; kk < kchunks; ++kk) {
     const int st = kk & 1;
-    if (kk + 1 < total) { load_stage(st ^ 1, kk + 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
+    if (kk + 1 < kchunks) { load_stage(st ^ 1, kk + 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
     __syncthreads();
     const double* as = As[st]; const double* bsm = Bs[st];
     // warp-uniform dispatch on the number of in-range 8-wide mma tiles; interior tiles, the hot path, are tested first
@@ -528,7 +486,7 @@ __global__ void __launch_bounds__(128, 4) k_gemm_nt(double* __restrict__ dst, co
     else if (ni == 2 && nj == 2) gemm_stage<2, 2>(as, bsm, acc, wm, wn, g, t);
     __syncthreads();
   }
-  double* C = dst + (size_t)task.dst * bs;
+  double* C = T + (size_t)task.dst * bs;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int row = m0 + wm + i * 8 + g;
@@ -549,11 +507,8 @@ __global__ void __launch_bounds__(128, 4) k_potrf_trail(double* __restrict__ Lb,
   const int frame = frames[blockIdx.y];
   double* A = Lb + (size_t)frame * npad * npad;
   const int j0 = jb * 16, j1 = j0 + 16;
-  int ti = (int)((sqrtf(8.f * blockIdx.x + 1.f) - 1.f) * 0.5f);
-  while ((ti + 1) * (ti + 2) / 2 <= (int)blockIdx.x) ++ti;
-  while (ti * (ti + 1) / 2 > (int)blockIdx.x) --ti;
-  const int tj = blockIdx.x - ti * (ti + 1) / 2;
-  const int m0 = j1 + ti * 64, n0 = j1 + tj * 64;
+  const int2 tij = tri_index(blockIdx.x);
+  const int m0 = j1 + tij.x * 64, n0 = j1 + tij.y * 64;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const int wm = (warp >> 1) * 32, wn = (warp & 1) * 32;
   for (int e = tid; e < 64 * 8; e += 128) {     // 64 rows x 8 double2
@@ -596,7 +551,6 @@ __global__ void __launch_bounds__(128, 4) k_potrf_trail(double* __restrict__ Lb,
 // One CTA = one kTrsmStrip-row strip of one block: 4 warps x kTrsmRW rows; the strip of X lives in shared memory
 // (kTrsmStrip x (npad+4) doubles), the L row panel of step jt is staged with cp.async one step ahead.
 // ---------------------------------------------------------------------------
-struct TrsmTask { int dst; int src; int kframe; };   // T index, L block id, column frame
 // strip = 4 warps x RW rows.  RW = 8 (32-row strips, 108 KB -> two CTAs per SM, twice the CTAs): every warp issues one DMMA per
 // 16 clk at best, so its 13-step chain costs (rows/8) x 728 DMMA x 16 clk -- halving the rows per warp halves the latency of a
 // launch that does not fill the machine (the dense tail), and two co-resident CTAs hide each other's staging waits elsewhere.
@@ -606,12 +560,7 @@ constexpr int kTrsmStrip = 4 * kTrsmRW;
 // fill the machine; AHEAD = 4 (169 KB, one CTA per SM) for the narrow levels, where a launch is a single wave and every step of the
 // chain otherwise waits for its panel to come back from L2 (measured: all launches at AHEAD = 4 made the wide levels slower,
 // trsm 2.03 -> 2.72 ms per factorisation, because occupancy halves where throughput counts).
-__host__ __device__ inline size_t trsm_ll_smem_bytes(int npad, int ahead = 2) { return ((size_t)kTrsmStrip * (npad + 4) + ahead * 16 * (size_t)(npad + 4) + ahead * 16 * 20) * sizeof(double); }
-
-// cp.async.wait_group with a run-time count of groups that may stay in flight (0..3)
-__device__ __forceinline__ void cp_async_wait_upto3(int n) {
-  if (n >= 3) cp_async_wait<3>(); else if (n == 2) cp_async_wait<2>(); else if (n == 1) cp_async_wait<1>(); else cp_async_wait<0>();
-}
+__host__ __device__ inline size_t trsm_ll_smem_bytes(int npad, int ahead) { return ((size_t)kTrsmStrip * (npad + 4) + ahead * 16 * (size_t)(npad + 4) + ahead * 16 * 20) * sizeof(double); }
 
 // kStreamed: launched as a programmatic dependent of the k_potrf_smem of the same level, so it runs while the Cholesky of its column
 // frame is still going on.  Step jt reads only row panel jt of L_kk and Di_jt, which k_potrf_smem publishes in progress[kframe] >= jt + 1;
@@ -761,7 +710,7 @@ __global__ void __launch_bounds__(128) k_trsm_ll(double* __restrict__ T, const d
   }
   // k_potrf_smem has published its last panel, so it is (about) done: this wait costs nothing, and it makes the completion of this
   // kernel imply the completion of k_potrf_smem for whatever follows it with an ordinary dependency
-  if constexpr (kStreamed) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if constexpr (kStreamed) griddep_wait();
 }
 
 
@@ -962,7 +911,20 @@ __global__ void __launch_bounds__(kSubThreads) k_substitution(const double* __re
     if (tid == 0) red_release_add(tk.type == 0 ? cn.fdone + tk.k : (tk.type == 1 ? cn.fin + tk.r : (tk.type == 2 ? cn.bin + tk.k : cn.bdone + tk.k)), 1);
   }
 }
-__host__ __device__ inline size_t substitution_smem_bytes(int) { return (size_t)8 * (kSubChunk + 2) * sizeof(double); }
+
+// The factorisation's kernel variants at block size npad and each kernel's dynamic shared memory: k_potrf_smem up to npad 224 (else
+// k_potrf_panel + k_potrf_trail), k_trsm_ll up to 416 (else k_gemm_nt with the inverse from k_trinv), its AHEAD = 4 shape up to 272.
+struct FactorKernels {
+  bool potrf_smem, trsm_ll, trsm_ll4;
+  size_t potrf_bytes, trsm_ll2_bytes, trsm_ll4_bytes, trinv_bytes, substitution_bytes;
+  int trsm2_ctas_per_sm;   // resident k_trsm_ll<2> CTAs per SM: set by allocate_storage (rcvd_api.cu) from an occupancy query
+};
+inline FactorKernels factor_kernels(int npad) {
+  const size_t potrf = potrf_smem_bytes(npad), ll2 = trsm_ll_smem_bytes(npad, 2), ll4 = trsm_ll_smem_bytes(npad, 4);
+  const size_t trinv = (size_t)(npad * 16 + 16 * (npad + 1)) * sizeof(double);   // tile column of the inverse + staged L row panel
+  const size_t sub = (size_t)8 * (kSubChunk + 2) * sizeof(double);                 // k_substitution: [8][kSubChunk + 2] column partials
+  return {potrf <= kMaxDynSmem, ll2 <= kMaxDynSmem, ll4 <= kMaxDynSmem, potrf, ll2, ll4, trinv, sub, 0};
+}
 
 // ---------------------------------------------------------------------------
 // Factor load: L <- S H S + D2 (lower triangle of diagonal blocks, pad diagonal = 1) for the blocks blist[0, nload), zeros in the

@@ -16,6 +16,8 @@ namespace rcvd {
 // upd2[0], upd2[1]: the deferred passes applied at this level (side stream), two launches in this order: [0] the passes into the
 // columns of level + 2, which the next level's late passes need, [1] the rest; it / it2: the k_update_tma items of upd / upd2;
 // join[s]: the first level whose late passes (U1) must wait for launch s -- one of its targets is in a column of level join[s] + 1
+struct UpdPass { int dst; int first; int count; int flags; };   // products upd_pairs[first, first + count) into L block dst; flags bit0: symmetric target (tiles above the diagonal are never read), bit1: first pass into a fill block (the target is written, not read)
+
 struct Level { int frame_off, nframes; int trsm_off, ntrsm; int upd_off, nupd; int upd2_off[2], nupd2[2]; int fwd_off, nfwd; int it_off, nit, it2_off[2], nit2[2]; int own_off, nown; int join[2]; };
 
 // Deferred update passes group the wide levels (below the narrow tail) in aligned windows of kUpdWindow source levels when a frame block
@@ -41,8 +43,7 @@ struct FactorPlan {
   std::vector<int> load_lblocks; int nload = 0;  // k_load_factor's list: own_lblocks with an H source or diagonal (nload), then the fill blocks
   // task lists of the level schedule
   std::vector<int> lvl_frames, lvl_own;
-  std::vector<GemmTask> trsm_tasks, upd_tasks; std::vector<int2> trsm_pairs, upd_pairs;
-  std::vector<TrsmTask> trsm_ll; std::vector<SolveTask> fwd_tasks;
+  std::vector<TrsmTask> trsm_tasks; std::vector<UpdPass> upd_tasks; std::vector<int2> upd_pairs; std::vector<SolveTask> fwd_tasks;
   std::vector<UpdItem> upd_items; int upd_rb = 0, upd_neff = 0;
   int upd_targets = 0;      // (source level, target block) pairs of the elimination structure this rank updates
   int upd_window = 1;       // source levels per window of the deferred update passes
@@ -255,11 +256,7 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
       if (mine) P.lvl_own.push_back(k);
       for (int r : cs[k]) {
         const int id = lid[{r, k}];
-        if (mine) {
-          P.trsm_tasks.push_back({id - N, (int)P.trsm_pairs.size(), 1, 0});
-          P.trsm_pairs.push_back(make_int2(id, k));
-          P.trsm_ll.push_back({id - N, id, k});
-        }
+        if (mine) P.trsm_tasks.push_back({id - N, id, k});
         P.fwd_tasks.push_back({id - N, r, k});
       }
     }
@@ -288,11 +285,11 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
       const int t0 = pass ? lv.upd2_off[pass - 1] : lv.upd_off, tn = pass ? lv.nupd2[pass - 1] : lv.nupd;
       const size_t i0 = items.size();
       for (int q = t0; q < t0 + tn; ++q) {
-        const GemmTask& tk = P.upd_tasks[q];
-        for (int ti = 0; ti < upd_nt; ++ti) for (int tj = 0; tj < ((tk.lower_only & 1) ? ti + 1 : upd_nt); ++tj) {
+        const UpdPass& tk = P.upd_tasks[q];
+        for (int ti = 0; ti < upd_nt; ++ti) for (int tj = 0; tj < ((tk.flags & 1) ? ti + 1 : upd_nt); ++tj) {
           UpdItem it; it.dst = tk.dst; it.first = tk.first; it.count = tk.count; it.m0 = (short)(ti * upd_tile); it.n0 = (short)(tj * upd_tile);
           it.mrows = (short)std::min(upd_tile, upd_neff - ti * upd_tile); it.ncols = (short)std::min(upd_tile, upd_neff - tj * upd_tile);
-          it.flags = (((tk.lower_only & 1) && ti == tj) ? kUpdSymDiag : 0) | ((tk.lower_only & 2) ? kUpdFirstFill : 0);
+          it.flags = (((tk.flags & 1) && ti == tj) ? kUpdSymDiag : 0) | ((tk.flags & 2) ? kUpdFirstFill : 0);
           items.push_back(it);
         }
       }

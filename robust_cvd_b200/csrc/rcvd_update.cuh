@@ -30,9 +30,8 @@
 //   * tiles are 80 x 80 (5 x 5 m8n8 units for each of the 2 x 2 warps: balanced), the remainder of the block last:
 //     neff = 200 -> 80 + 80 + 40, not 64 + 64 + 64 + 8.
 #pragma once
-#include <cuda.h>
-#include <stdint.h>
 #include "rcvd_linalg.cuh"
+#include "rcvd_ptx.cuh"
 
 namespace rcvd {
 
@@ -56,28 +55,6 @@ template <int TEAMS> struct UpdShape { static constexpr int stages = TEAMS == 2 
 __host__ __device__ inline size_t upd_smem_bytes(int rb, int teams) {
   const int stages = teams == 2 ? 8 : 5;
   return (size_t)stages * 2 * rb * 16 * sizeof(double) + (teams == 2 ? (size_t)kUpdPartial * sizeof(double) : 0) + 2 * stages * sizeof(uint64_t) + 1024;
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred P1;\n"
-      "LAB_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-      "@P1 bra DONE;\n"
-      "bra LAB_WAIT;\n"
-      "DONE:\n"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
 // One k4 step of the warp tile: pairs of 8-row units as m16n8k4 (one instruction per pair and column unit), an odd last unit as m8n8k4.
@@ -152,8 +129,6 @@ __device__ __forceinline__ void upd_store_partial(double* __restrict__ part, con
 #pragma unroll
     for (int j = 0; j < NJ; ++j) *reinterpret_cast<double2*>(part + (size_t)(i * 5 + j) * 64) = make_double2(acc[i][j][0], acc[i][j][1]);
 }
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 #define RCVD_UPD_CASES(M) \
   M(1, 1) M(1, 2) M(1, 3) M(1, 4) M(1, 5) M(2, 1) M(2, 2) M(2, 3) M(2, 4) M(2, 5) M(3, 1) M(3, 2) M(3, 3) M(3, 4) M(3, 5) \
@@ -173,7 +148,7 @@ __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::cta
   extern __shared__ __align__(1024) unsigned char ring[];
   // a programmatic dependent launch (the next narrow level's k_potrf_smem, which waits for this grid before reading) may take the SMs
   // this launch drains
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  griddep_launch_dependents();
   if (smem_u32(ring) & 1023u) __trap();
   constexpr int kUpdStages = UpdShape<TEAMS>::stages;
   const int tile_bytes = rb * 128, stage_bytes = 2 * tile_bytes;                     // A tile then B tile, [rb][16 doubles]
@@ -215,7 +190,7 @@ __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::cta
         const double* row = dst + (size_t)it.dst * bs + (size_t)it.m0 * npad + it.n0;
         for (int r = 0; r < it.mrows; ++r, row += npad) {
           const int bytes = ((it.flags & kUpdSymDiag) && r < hm ? hn : it.ncols) * 8;
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(row), "r"(bytes) : "memory");
+          prefetch_l2_bulk(row, bytes);
         }
       }
     }
@@ -230,7 +205,7 @@ __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::cta
   for (int k4 = 0; k4 < 4; ++k4) kc[k4] = (((2 * k4 + (t >> 1)) ^ pg) << 4) + ((t & 1) << 3);
   const int wr = tw >> 1, wc = tw & 1;
   double* mypart = partial + (size_t)tw * (25 * 64) + lane * 2;     // [team-warp][unit][lane][2]
-  if (TEAMS == 2 && team == 0) named_bar_arrive(2, 256);       // "partial buffer is free" for team 1's first item
+  if (TEAMS == 2 && team == 0) named_bar_arrive<2, 256>();     // "partial buffer is free" for team 1's first item
   int stage = 0; uint32_t phase = 0; unsigned sidx = 0;         // sidx: running stage counter (its parity picks the team)
   for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
     const UpdItem it = items[w];
@@ -267,18 +242,18 @@ __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::cta
     }
     if (TEAMS == 2 && team == 1) {
       // hand the partial accumulators to team 0 and go on with the next item
-      named_bar_sync(2, 256);                                  // team 0 has consumed the previous partials
+      named_bar_sync<2, 256>();                                // team 0 has consumed the previous partials
       switch (code) {
 #define RCVD_UPD_PART(NI_, NJ_) case NI_ * 8 + NJ_: upd_store_partial<NI_, NJ_>(mypart, acc); break;
         RCVD_UPD_CASES(RCVD_UPD_PART)
 #undef RCVD_UPD_PART
         default: break;
       }
-      named_bar_arrive(1, 256);                                // "partials are in shared memory"
+      named_bar_arrive<1, 256>();                              // "partials are in shared memory"
       continue;
     }
-    if (TEAMS == 2) named_bar_sync(1, 256);
-    if (dbg & 2) { if (acc[0][0][0] == 1.2345e300) dst[0] = acc[4][4][1] + acc[2][3][0]; if (TEAMS == 2) named_bar_arrive(2, 256); continue; }   // timing experiment: no read-modify-write of the target
+    if (TEAMS == 2) named_bar_sync<1, 256>();
+    if (dbg & 2) { if (acc[0][0][0] == 1.2345e300) dst[0] = acc[4][4][1] + acc[2][3][0]; if (TEAMS == 2) named_bar_arrive<2, 256>(); continue; }   // timing experiment: no read-modify-write of the target
     double* C = dst + (size_t)it.dst * bs + (size_t)(it.m0 + wm + pg) * npad + it.n0 + wn + ((t & 1) << 2) + (t & 2);
     const bool fresh = (it.flags & kUpdFirstFill) != 0;
     switch (code) {
@@ -287,7 +262,7 @@ __global__ void __launch_bounds__(UpdShape<TEAMS>::threads, UpdShape<TEAMS>::cta
 #undef RCVD_UPD_EPI
       default: break;
     }
-    if (TEAMS == 2) named_bar_arrive(2, 256);                  // partial buffer free again
+    if (TEAMS == 2) named_bar_arrive<2, 256>();                // partial buffer free again
   }
 }
 
