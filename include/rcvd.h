@@ -200,7 +200,8 @@ int32_t rcvd_problem_init_comm(rcvd_problem* p, int32_t nranks, int32_t rank, co
 int32_t rcvd_problem_set_structure(rcvd_problem* p, int32_t num_pairs, const int32_t* pair_frames);
 /* regulariser terms are evaluated by the rank that owns frame f: f % nranks == rank */
 
-/* State: params[N * stride] host doubles. */
+/* State: params[N * stride] host doubles, zero at creation.  The state is the later of the last set_state and the last
+ * rcvd_solve's result, and it survives every setter. */
 int32_t rcvd_problem_set_state(rcvd_problem* p, const double* params);
 int32_t rcvd_problem_get_state(rcvd_problem* p, double* params);
 

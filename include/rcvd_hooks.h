@@ -76,7 +76,8 @@ int32_t rcvd_debug_level_profile(rcvd_problem* p, double* out, int32_t max_level
  * measured live */
 int32_t rcvd_debug_fp64_tensor_peak(int32_t device, int32_t shape, double* tflops);
 
-/* A/B switches (defaults in parentheses) */
+/* A/B switches (defaults in parentheses).  A null handle: RCVD_ERR_INVALID.  set_order_slack, set_eval_only and set_distributed
+ * rebuild the structure at the next call that needs it; like every setter of rcvd.h they keep the state (rcvd_problem_get_state). */
 int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on);        /* (1) specialised accumulate kernels; 0 = generic kernel; 2 = k_accumulate_fast
                                                                           even where the run path applies (bilinear grids) */
 int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on);          /* (1) two-stream factorisation graph */

@@ -167,7 +167,7 @@ struct RecordSet {
 struct rcvd_problem {
   rcvd_config cfg; Layout L; int N = 0; int device = 0;
   cudaStream_t stream = nullptr;
-  // host inputs
+  // host inputs (in_range all 1 and median all 1.0 from rcvd_problem_create on)
   std::vector<uint8_t> in_range; std::vector<double> median, adaptive;
   RecordSet pairs{6, 2}, trips{10, 1}, dpairs{6, 2};   // static-scene pairs, smoothness triplets, pairwise depth normalisation
   std::vector<int32_t> struct_pairs;   // global frame-pair graph (multi-GPU); empty -> local pairs
@@ -193,11 +193,13 @@ struct rcvd_problem {
   int *d_lvl_frames = nullptr; TrsmTask* d_trsm_tasks = nullptr; int2* d_upd_pairs = nullptr; SolveTask* d_fwd_tasks = nullptr;
   SubTask* d_sub_tasks = nullptr; int* d_sub_counters = nullptr; int* d_sub_need = nullptr;
   cudaGraphExec_t solve_graph = nullptr;
-  bool structure_ready = false, constraints_set = false, frames_set = false;
+  bool structure_ready = false;
   // multi GPU
   int nranks = 1, rank = 0; nccl::Comm comm = nullptr;
   int64_t launches = 0, graph_launches = 0;
-  std::vector<double> h_state; bool state_dirty = false; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
+  // The caller-visible state (N x nf, caller's frame order) is h_state whenever !structure_ready || state_dirty, and d_x otherwise:
+  // drop_structure saves d_x to h_state before it invalidates the structure, ensure_ready uploads h_state when state_dirty.
+  std::vector<double> h_state; bool state_dirty = true; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
   cudaStream_t side_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   std::vector<cudaEvent_t> ev_side;   // per level, two each: recorded after the level's side-stream update launches (Level::join waits on them)
   cudaStream_t inv_stream = nullptr; cudaEvent_t ev_inv_join = nullptr;   // k_trinv, off the critical path and off the side stream's
@@ -251,8 +253,39 @@ template <class T> static int upload(rcvd_problem* p, T** ptr, const std::vector
   if (!v.empty()) CK(cudaMemcpyAsync(*ptr, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, p->stream));
   return RCVD_OK;
 }
-static void free_all(rcvd_problem* p) {
+// Frame-major vectors between the caller's frame order and the internal one (internal frame i is the caller's frame uperm[i]): `count`
+// elements of each frame, frames `src_stride` / `dst_stride` elements apart.  frames_to_internal fills the rest of each row with `pad`.
+template <class T> static std::vector<T> frames_to_internal(const std::vector<int>& uperm, const T* src, size_t src_stride, size_t dst_stride, size_t count, T pad = T()) {
+  std::vector<T> out(uperm.size() * dst_stride, pad);
+  for (size_t i = 0; i < uperm.size(); ++i) std::copy_n(src + (size_t)uperm[i] * src_stride, count, out.begin() + i * dst_stride);
+  return out;
+}
+template <class T> static void frames_to_caller(const std::vector<int>& uperm, const T* src, size_t src_stride, T* dst, size_t dst_stride, size_t count) {
+  for (size_t i = 0; i < uperm.size(); ++i) std::copy_n(src + i * src_stride, count, dst + (size_t)uperm[i] * dst_stride);
+}
+// A device vector of src_stride doubles per internal frame -> dst, nf per frame in the caller's order.
+static int download_frames(rcvd_problem* p, double* dst, const double* src, int src_stride) {
+  std::vector<double> tmp((size_t)p->N * src_stride);
+  CK(cudaMemcpyAsync(tmp.data(), src, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  CK(cudaStreamSynchronize(p->stream));
+  frames_to_caller(p->plan.uperm, tmp.data(), src_stride, dst, p->L.nf, p->L.nf);
+  return RCVD_OK;
+}
+// The factor+solve graph captures the switches of enqueue_factor_solve and the device buffers: it goes when either changes.
+static void drop_graph(rcvd_problem* p) {
   if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; }
+}
+// Every setter of something build_structure reads calls this after its own checks; the state survives (see rcvd_problem).
+static int drop_structure(rcvd_problem* p) {
+  if (p->structure_ready && !p->state_dirty) {
+    SET_DEVICE(p->device);
+    if (int rc = download_frames(p, p->h_state.data(), p->d_x, p->L.nf)) return rc;
+  }
+  p->state_dirty = true; p->structure_ready = false;
+  return RCVD_OK;
+}
+static void free_all(rcvd_problem* p) {
+  drop_graph(p);
   if (p->side_stream) cudaStreamSynchronize(p->side_stream);
   if (p->inv_stream) cudaStreamSynchronize(p->inv_stream);
   for (void* q : p->allocs) cudaFreeAsync(q, p->stream);
@@ -344,15 +377,11 @@ static int set_up_problem_data(rcvd_problem* p) {
     CK(cudaGetLastError());
     p->pairs.dev.records = d_sorted; p->records_sorted = true;      // (the unsorted copy and the sort buffers go back to the pool with the handle's other allocations)
   }
-  {
-    std::vector<uint8_t> ir(N); std::vector<double> md(N), ad;
-    for (int i = 0; i < N; ++i) { ir[i] = p->in_range[uperm[i]]; md[i] = p->median[uperm[i]]; }
-    UP(p->d_in_range, ir); UP(p->d_median, md);
-    if (!p->adaptive.empty()) {
-      const size_t G = p->adaptive.size() / N; ad.resize(p->adaptive.size());
-      for (int i = 0; i < N; ++i) std::copy(p->adaptive.begin() + (size_t)uperm[i] * G, p->adaptive.begin() + (size_t)(uperm[i] + 1) * G, ad.begin() + (size_t)i * G);
-      UP(p->d_adaptive, ad);
-    }
+  UP(p->d_in_range, frames_to_internal(uperm, p->in_range.data(), 1, 1, 1));
+  UP(p->d_median, frames_to_internal(uperm, p->median.data(), 1, 1, 1));
+  if (!p->adaptive.empty()) {
+    const size_t G = p->adaptive.size() / N;
+    UP(p->d_adaptive, frames_to_internal(uperm, p->adaptive.data(), G, G, G));
   }
   {
     // scale-regulariser lattice in float32, lib/PoseOptimizer.cpp:1382-1385
@@ -760,38 +789,12 @@ static int enqueue_evaluate(rcvd_problem* p, const double* x, bool wantG, bool w
   return RCVD_OK;
 }
 
-// Frame-major host vectors in the caller's frame order <-> device vectors in the internal (owner-major) order.
-static int upload_frames(rcvd_problem* p, double* dst, const double* src_user, int stride_dst, int stride_src, int count) {
-  std::vector<double> tmp((size_t)p->N * stride_dst, 0.0);
-  for (int i = 0; i < p->N; ++i) memcpy(tmp.data() + (size_t)i * stride_dst, src_user + (size_t)p->plan.uperm[i] * stride_src, (size_t)count * sizeof(double));
-  CK(cudaMemcpyAsync(dst, tmp.data(), tmp.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-  CK(cudaStreamSynchronize(p->stream));      // tmp goes out of scope
-  return RCVD_OK;
-}
-static int download_frames(rcvd_problem* p, double* dst_user, const double* src, int stride_dst, int stride_src, int count) {
-  std::vector<double> tmp((size_t)p->N * stride_src);
-  CK(cudaMemcpyAsync(tmp.data(), src, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
-  CK(cudaStreamSynchronize(p->stream));
-  for (int i = 0; i < p->N; ++i) memcpy(dst_user + (size_t)p->plan.uperm[i] * stride_dst, tmp.data() + (size_t)i * stride_src, (size_t)count * sizeof(double));
-  return RCVD_OK;
-}
-// device state -> h_state (caller's frame order); used before the structure is rebuilt
-static int save_state(rcvd_problem* p) {
-  DevGuard g(p->device); cudaStreamSynchronize(p->stream);
-  if (p->h_state.size() != (size_t)p->N * p->L.nf) p->h_state.assign((size_t)p->N * p->L.nf, 0.0);
-  return download_frames(p, p->h_state.data(), p->d_x, p->L.nf, p->L.nf, p->L.nf);
-}
-
 static int ensure_ready(rcvd_problem* p) {
-  if (!p->structure_ready) {
-    if (p->in_range.empty()) p->in_range.assign(p->N, 1);
-    if (p->median.empty()) p->median.assign(p->N, 1.0);
-    int rc = build_structure(p); if (rc) return rc;
-    p->state_dirty = true;
-  }
+  if (!p->structure_ready) { if (int rc = build_structure(p)) return rc; }
   if (p->state_dirty) {
-    if (p->h_state.size() != (size_t)p->N * p->L.nf) p->h_state.assign((size_t)p->N * p->L.nf, 0.0);
-    { int rc = upload_frames(p, p->d_x, p->h_state.data(), p->L.nf, p->L.nf, p->L.nf); if (rc) return rc; }
+    const std::vector<double> x = frames_to_internal(p->plan.uperm, p->h_state.data(), p->L.nf, p->L.nf, p->L.nf);
+    CK(cudaMemcpyAsync(p->d_x, x.data(), x.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaStreamSynchronize(p->stream));      // x goes out of scope
     p->state_dirty = false;
   }
   return RCVD_OK;
@@ -1089,6 +1092,7 @@ RCVD_API int32_t rcvd_problem_create(const rcvd_config* cfg, int32_t device, rcv
   }
   rcvd_problem* p = new rcvd_problem();
   p->cfg = *cfg; p->L = L; p->N = cfg->num_frames; p->device = device;
+  p->in_range.assign(p->N, 1); p->median.assign(p->N, 1.0); p->h_state.assign((size_t)p->N * L.nf, 0.0);
   cudaError_t e = cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, device);   // read once: the plan and the launch shapes use it
   if (e != cudaSuccess) { delete p; return set_err(RCVD_ERR_CUDA, "cudaDeviceGetAttribute(multiprocessor count): %s", cudaGetErrorString(e)); }
   // the critical chain (potrf -> trsm -> next-level updates) runs at the highest priority, the overlapped updates at the lowest,
@@ -1121,12 +1125,12 @@ RCVD_API void rcvd_problem_destroy(rcvd_problem* p) {
 }
 RCVD_API int32_t rcvd_problem_set_frames(rcvd_problem* p, const uint8_t* in_range, const double* median, const double* adaptive) {
   if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  const bool grid = adaptive && p->cfg.depth_type == RCVD_DEPTH_GRID;
+  if (p->cfg.adaptive_deform > 0.0 && !grid) return set_err(RCVD_ERR_INVALID, "adaptive deformation cost requires node weights");
+  if (int rc = drop_structure(p)) return rc;
   if (in_range) p->in_range.assign(in_range, in_range + p->N); else p->in_range.assign(p->N, 1);
   if (median) p->median.assign(median, median + p->N); else p->median.assign(p->N, 1.0);
-  if (adaptive && p->cfg.depth_type == RCVD_DEPTH_GRID) p->adaptive.assign(adaptive, adaptive + (size_t)p->N * p->cfg.depth_grid_x * p->cfg.depth_grid_y); else p->adaptive.clear();
-  if (p->cfg.adaptive_deform > 0.0 && p->adaptive.empty()) return set_err(RCVD_ERR_INVALID, "adaptive deformation cost requires node weights");
-  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
-  p->structure_ready = false;
+  if (grid) p->adaptive.assign(adaptive, adaptive + (size_t)p->N * p->cfg.depth_grid_x * p->cfg.depth_grid_y); else p->adaptive.clear();
   return RCVD_OK;
 }
 // The setter of every family.  Everything is checked before anything is kept, so a refused call leaves the problem as it was:
@@ -1145,11 +1149,10 @@ static int32_t set_records(rcvd_problem* p, RecordSet rcvd_problem::*family, con
   }
   const int64_t count = n > 0 ? off[n] : 0;
   if (count > 0 && !rec) return set_err(RCVD_ERR_INVALID, "null %s records", what);
-  if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; }
+  if (int rc = drop_structure(p)) return rc;
   s.frames.assign(frames, frames + (size_t)n * s.nframes);
   if (n > 0) s.offsets.assign(off, off + n + 1); else s.offsets.assign(1, 0);
   s.records.assign(rec, rec + (size_t)count * s.width);
-  p->structure_ready = false;
   return RCVD_OK;
 }
 RCVD_API int32_t rcvd_problem_set_constraints(rcvd_problem* p, int32_t np, const int32_t* pf, const int64_t* off, const float* rec) {
@@ -1165,8 +1168,8 @@ RCVD_API int32_t rcvd_problem_set_depth_pairs(rcvd_problem* p, int32_t np, const
 // Global frame-pair graph for multi-GPU runs (every rank must build the same block structure).
 RCVD_API int32_t rcvd_problem_set_structure(rcvd_problem* p, int32_t np, const int32_t* pf) {
   if (!p || np < 0 || (np > 0 && !pf)) return set_err(RCVD_ERR_INVALID, "bad structure arrays");
+  if (int rc = drop_structure(p)) return rc;
   p->struct_pairs.assign(pf, pf + 2 * (size_t)np);
-  p->structure_ready = false;
   return RCVD_OK;
 }
 RCVD_API int32_t rcvd_nccl_unique_id(uint8_t out[128]) {
@@ -1177,26 +1180,27 @@ RCVD_API int32_t rcvd_nccl_unique_id(uint8_t out[128]) {
 }
 RCVD_API int32_t rcvd_problem_init_comm(rcvd_problem* p, int32_t nranks, int32_t rank, const uint8_t uid[128]) {
   if (!p || nranks < 1 || rank < 0 || rank >= nranks) return set_err(RCVD_ERR_INVALID, "bad rank/nranks");
-  if (nranks == 1) { p->nranks = 1; p->rank = 0; return RCVD_OK; }
-  if (!nccl::load()) return set_err(RCVD_ERR_NCCL, "libnccl.so.2 not found");
-  SET_DEVICE(p->device);
-  nccl::UniqueId id; memcpy(id.internal, uid, 128);
-  const int r = nccl::CommInitRank(&p->comm, nranks, id, rank);
-  if (r != 0) return set_err(RCVD_ERR_NCCL, "ncclCommInitRank failed: %s", nccl::GetErrorString ? nccl::GetErrorString(r) : "?");
-  p->nranks = nranks; p->rank = rank; p->structure_ready = false;
+  if (nranks > 1) {
+    if (!nccl::load()) return set_err(RCVD_ERR_NCCL, "libnccl.so.2 not found");
+    SET_DEVICE(p->device);
+    nccl::UniqueId id; memcpy(id.internal, uid, 128);
+    const int r = nccl::CommInitRank(&p->comm, nranks, id, rank);
+    if (r != 0) return set_err(RCVD_ERR_NCCL, "ncclCommInitRank failed: %s", nccl::GetErrorString ? nccl::GetErrorString(r) : "?");
+  }
+  if (int rc = drop_structure(p)) return rc;
+  p->nranks = nranks; p->rank = rank;
   return RCVD_OK;
 }
 RCVD_API int32_t rcvd_problem_set_state(rcvd_problem* p, const double* x) {
   if (!p || !x) return set_err(RCVD_ERR_INVALID, "null argument");
-  p->h_state.assign(x, x + (size_t)p->N * p->L.nf); p->state_dirty = true;
+  p->h_state.assign(x, x + p->h_state.size()); p->state_dirty = true;
   return RCVD_OK;
 }
 RCVD_API int32_t rcvd_problem_get_state(rcvd_problem* p, double* x) {
   if (!p || !x) return set_err(RCVD_ERR_INVALID, "null argument");
-  const size_t U = (size_t)p->N * p->L.nf;
-  if (!p->structure_ready || p->state_dirty) { if (p->h_state.size() != U) p->h_state.assign(U, 0.0); memcpy(x, p->h_state.data(), U * sizeof(double)); return RCVD_OK; }
+  if (!p->structure_ready || p->state_dirty) { std::copy(p->h_state.begin(), p->h_state.end(), x); return RCVD_OK; }
   SET_DEVICE(p->device);
-  return download_frames(p, x, p->d_x, p->L.nf, p->L.nf, p->L.nf);
+  return download_frames(p, x, p->d_x, p->L.nf);
 }
 RCVD_API int32_t rcvd_evaluate(rcvd_problem* p, double* cost, double* gradient) {
   if (!p || !cost) return set_err(RCVD_ERR_INVALID, "null argument");
@@ -1206,10 +1210,7 @@ RCVD_API int32_t rcvd_evaluate(rcvd_problem* p, double* cost, double* gradient) 
   rc = enqueue_evaluate(p, p->d_x, gradient != nullptr, false, p->d_g, SC_COST); if (rc) return rc;
   rc = read_scalars(p); if (rc) return rc;
   *cost = p->h_scal[SC_COST];
-  if (gradient) {
-    if ((rc = download_frames(p, gradient, p->d_g, p->L.nf, p->L.npad, p->L.nf))) return rc;
-  }
-  return RCVD_OK;
+  return gradient ? download_frames(p, gradient, p->d_g, p->L.npad) : RCVD_OK;
 }
 RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
   if (!p || !Hout) return set_err(RCVD_ERR_INVALID, "null argument");
@@ -1232,9 +1233,9 @@ RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
 }
 // factorisation + solve of (S H S + diag(D2)) y = b with the H blocks already on the device; S == nullptr: S = 1
 static int solve_loaded(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y) {
-  const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t Upad = (size_t)N * npad;
-  std::vector<double> hs(Upad, 1.0), hd(Upad, 1.0), hb(Upad, 0.0);
-  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) { const size_t u = (size_t)p->plan.uperm[f] * nf + l; hs[(size_t)f * npad + l] = S ? S[u] : 1.0; hd[(size_t)f * npad + l] = D2[u]; hb[(size_t)f * npad + l] = b[u]; }
+  const std::vector<int>& uperm = p->plan.uperm; const int nf = p->L.nf, npad = p->L.npad; const size_t Upad = (size_t)p->N * npad;
+  const std::vector<double> hs = S ? frames_to_internal(uperm, S, nf, npad, nf, 1.0) : std::vector<double>(Upad, 1.0);
+  const std::vector<double> hd = frames_to_internal(uperm, D2, nf, npad, nf, 1.0), hb = frames_to_internal(uperm, b, nf, npad, nf, 0.0);
   CK(cudaMemcpyAsync(p->d_S, hs.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
   CK(cudaMemcpyAsync(p->d_D2, hd.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
   CK(cudaMemcpyAsync(p->d_gs, hb.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
@@ -1243,7 +1244,7 @@ static int solve_loaded(rcvd_problem* p, const double* S, const double* D2, cons
   std::vector<double> hy(Upad);
   CK(cudaMemcpyAsync(hy.data(), p->d_y, Upad * 8, cudaMemcpyDeviceToHost, p->stream));
   rc = read_scalars(p); if (rc) return rc;
-  for (int f = 0; f < N; ++f) for (int l = 0; l < nf; ++l) y[(size_t)p->plan.uperm[f] * nf + l] = hy[(size_t)f * npad + l];
+  frames_to_caller(uperm, hy.data(), npad, y, nf, nf);
   if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, "factorisation hit a non-positive pivot");
   return RCVD_OK;
 }
@@ -1361,8 +1362,8 @@ RCVD_API int32_t rcvd_debug_last_iteration(rcvd_problem* p, double* g, double* x
   SET_DEVICE(p->device);
   int rc = read_scalars(p); if (rc) return rc;
   out[0] = p->h_scal[SC_COST]; out[1] = p->h_scal[SC_CAND];
-  if ((rc = download_frames(p, g, p->d_g, p->L.nf, p->L.npad, p->L.nf))) return rc;
-  return download_frames(p, xc, p->d_xc, p->L.nf, p->L.nf, p->L.nf);
+  if ((rc = download_frames(p, g, p->d_g, p->L.npad))) return rc;
+  return download_frames(p, xc, p->d_xc, p->L.nf);
 }
 // Bench hook: one factorisation + solve, un-captured on a single stream with one CUDA event per launch; returns the
 // summed device time per kernel class: out_ms[0..5] = load, potrf, trinv, trsm, update GEMM (k_update_tma), substitution;
@@ -1496,23 +1497,21 @@ RCVD_API int32_t rcvd_debug_level_profile(rcvd_problem* p, double* out, int32_t 
 }
 RCVD_API int64_t rcvd_launch_count(rcvd_problem* p) { return p ? p->launches : 0; }
 // Test / bench hook: elimination-order variant (-1 greedy minimum degree, >= 0 multiple elimination with that degree slack).
-RCVD_API int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack) { if (!p) return RCVD_ERR_INVALID; p->order_slack = slack; p->structure_ready = false; return RCVD_OK; }
+RCVD_API int32_t rcvd_debug_set_order_slack(rcvd_problem* p, int32_t slack) { if (!p) return set_err(RCVD_ERR_INVALID, "null problem"); if (int rc = drop_structure(p)) return rc; p->order_slack = slack; return RCVD_OK; }
 // Test / bench hook: 0 = single-stream factorisation graph, 1 (default) = overlap non-critical updates on a second stream.
-RCVD_API int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->overlap = on != 0; if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; } return RCVD_OK; }
+RCVD_API int32_t rcvd_debug_set_overlap(rcvd_problem* p, int32_t on) { if (!p) return set_err(RCVD_ERR_INVALID, "null problem"); p->overlap = on != 0; drop_graph(p); return RCVD_OK; }
 // Test / bench hook: side_items_per_cta > 0 caps the items per CTA of the one-team update launches (a larger grid); 0 (default) = no cap.
 // tma must be 1: the persistent TMA-fed kernel (k_update_tma) is the only update kernel.
 RCVD_API int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta) {
-  if (!p) return RCVD_ERR_INVALID;
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
   if (!tma) return set_err(RCVD_ERR_INVALID, "the cp.async update path was removed: k_update_tma is the only update kernel");
-  p->upd_ipc = side_items_per_cta;
-  if (p->solve_graph) { cudaGraphExecDestroy(p->solve_graph); p->solve_graph = nullptr; }
-  return RCVD_OK;
+  p->upd_ipc = side_items_per_cta; drop_graph(p); return RCVD_OK;
 }
-// Test / bench hook (nranks > 1): 1 (default) = distributed factorisation (owner-computes phase A, reduce-to-owner of H), 0 = replicated scheme
-// (all-reduce of H, factorisation replicated on every rank).  out (optional): {distributed active, first replicated level, levels}.
 // Test / bench hook: 1 = the handle will only evaluate cost / gradient (rcvd_evaluate): no normal matrix, no factor storage is allocated
-RCVD_API int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->eval_only = on != 0; p->structure_ready = false; return RCVD_OK; }
-RCVD_API int32_t rcvd_debug_set_distributed(rcvd_problem* p, int32_t on) { if (!p) return RCVD_ERR_INVALID; p->dist_enabled = on != 0; if (p->structure_ready) { int rc_ = save_state(p); if (rc_) return rc_; p->state_dirty = true; } p->structure_ready = false; return RCVD_OK; }
+RCVD_API int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on) { if (!p) return set_err(RCVD_ERR_INVALID, "null problem"); if (int rc = drop_structure(p)) return rc; p->eval_only = on != 0; return RCVD_OK; }
+// Test / bench hook (nranks > 1): 1 (default) = distributed factorisation (owner-computes phase A, reduce-to-owner of H), 0 = replicated scheme
+// (all-reduce of H, factorisation replicated on every rank).
+RCVD_API int32_t rcvd_debug_set_distributed(rcvd_problem* p, int32_t on) { if (!p) return set_err(RCVD_ERR_INVALID, "null problem"); if (int rc = drop_structure(p)) return rc; p->dist_enabled = on != 0; return RCVD_OK; }
 RCVD_API int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]) {
   if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
   SET_DEVICE(p->device);
@@ -1524,7 +1523,7 @@ RCVD_API int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]) {
 // 2 = k_accumulate_fast even where the run path applies (sorted records are valid input for it): the only way to run its Grid branch
 // below 65535 grid nodes.
 RCVD_API int32_t rcvd_debug_set_fast_path(rcvd_problem* p, int32_t on) {
-  if (!p) return RCVD_ERR_INVALID;
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
   if (on < 0 || on > 2) return set_err(RCVD_ERR_INVALID, "fast path switch must be 0, 1 or 2 (got %d)", on);
   p->fast_path = on; return RCVD_OK;
 }
@@ -1552,10 +1551,8 @@ RCVD_API int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, cons
   FactorPlan pl;
   if (int32_t rc = debug_plan(pl, cfg, np, pairs, nt, trip_centers, order_slack, nranks, rank, num_sms)) return rc;
   const int N = cfg->num_frames;
-  for (int i = 0; i < N; ++i) {
-    const int f = pl.uperm[i];
-    order[i] = pl.uperm[pl.elim_order[i]]; level[f] = pl.level[i]; owner[f] = pl.owner[i]; perm[i] = f;
-  }
+  frames_to_caller(pl.uperm, pl.level.data(), 1, level, 1, 1); frames_to_caller(pl.uperm, pl.owner.data(), 1, owner, 1, 1);
+  for (int i = 0; i < N; ++i) { order[i] = pl.uperm[pl.elim_order[i]]; perm[i] = pl.uperm[i]; }
   const int32_t v[13] = {(int32_t)pl.levels.size(), pl.nLoff, (int32_t)pl.hblocks.size(), pl.upd_targets, (int32_t)pl.upd_items.size(), (int32_t)pl.sub_tasks.size(),
                          pl.dist ? 1 : 0, pl.LB, pl.sub_first_level, (int32_t)pl.own_lblocks.size(), (int32_t)pl.own_hblocks.size(),
                          pl.dist ? pl.fa_cnt[rank] + pl.fb_cnt[rank] : N, (int32_t)pl.upd_tasks.size()};

@@ -95,3 +95,20 @@ def test_filter_and_builder_fail_loudly_without_a_device():
         solver._check(solver.lib().rcvd_trim_device_memory(0))
     with pytest.raises(RuntimeError, match=no_device):
         solver.fp64_tensor_peaks(0)
+
+
+# the A/B switches of include/rcvd_hooks.h with a valid argument list each
+DEBUG_SWITCHES = [("rcvd_debug_set_order_slack", 4), ("rcvd_debug_set_overlap", 1), ("rcvd_debug_set_update_kernel", 1, 0),
+                  ("rcvd_debug_set_eval_only", 0), ("rcvd_debug_set_distributed", 1), ("rcvd_debug_set_fast_path", 1)]
+
+
+def test_debug_switches_report_a_null_handle():
+    """Every A/B switch refuses a null handle with RCVD_ERR_INVALID and says so in rcvd_last_error(), in place of an earlier message."""
+    from robust_cvd_b200 import abi, solver
+    L = solver.lib()
+    cfg = abi.default_config(4, 1.5)
+    for name, *args in DEBUG_SWITCHES:
+        with pytest.raises(RuntimeError, match="bad rank/nranks/num_sms"):      # an unrelated error first (host only)
+            solver.factor_plan(cfg, [(0, 1)], num_sms=0)
+        assert getattr(L, name)(None, *(C.c_int32(a) for a in args)) == abi.ERR_INVALID, name
+        assert L.rcvd_last_error().decode() == "null problem", name

@@ -54,6 +54,10 @@ def test_linear_solve_and_single_stream_graph(name, overrides):
     G.set_overlap(False)
     y2 = G.debug_linear_solve(S, D2, b)
     assert np.linalg.norm(y2 - y) / np.linalg.norm(y) < 1e-9
+    # switching back captures the two-stream graph again
+    G.set_overlap(True)
+    y3 = G.debug_linear_solve(S, D2, b)
+    assert np.linalg.norm(y3 - y) / np.linalg.norm(y) < 1e-9
 
 
 @pytest.mark.parametrize("name,overrides", helpers.VARIANTS, ids=[v[0] for v in helpers.VARIANTS])
