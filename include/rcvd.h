@@ -358,8 +358,11 @@ int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t device, const 
  * masks [F][h][w] u8 (dynamic-mask frames: < 127 = dynamic); a constraint is static when
  * cv::distanceTransform(mask >= 127, DIST_L2, 5) > distance at every end, the end's pixel being
  * (int(loc.x * w), int(loc.y * w)) -- y scaled by the WIDTH, as the reference does.
- * pair_locs [n][4] / trip_locs [n][6] float32 in the builder's output layout; *_static one byte per constraint (out);
- * dist_out optional [F][h][w] float32 distance images. */
+ * pair_frames[P][2] with both frames in [0, num_frames), trip_frames[T] the centre frames t of the triplets t-1, t, t+1, each in
+ * [1, num_frames-2].  For each family, group i owns the constraints offsets[i] .. offsets[i+1]-1, offsets[0] must be 0, the offsets
+ * must not decrease, and the locations and flags may be null only if offsets[n] is 0.  pair_locs [n][4] / trip_locs [n][6] float32
+ * in the builder's output layout; *_static one byte per constraint (out); dist_out optional [F][h][w] float32 distance images.
+ * A call that fails with RCVD_ERR_INVALID changes no flag, and is refused before any device is needed. */
 int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t num_frames, int32_t height, int32_t width, float distance,
                           int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
                           int32_t num_triplets, const int32_t* trip_frames, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static,
@@ -370,8 +373,9 @@ int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t num_fram
  * its end in each of its frames (end 0 only when both frames are equal); then every pair or triplet constraint with an end on a
  * stamped pixel of its frame becomes non-static.  An end's pixel is (int(loc.x * w), int(loc.y * w)), y scaled by the WIDTH as the
  * reference does; the disc centre is used as is, the lookup pixel is clamped to the image (the reference reads past the frame there).
- * Arrays as in rcvd_static_flags (trip_centres: centre frame t of the triplet t-1, t, t+1); pair_static / trip_static in/out, one
- * byte per constraint, flags only go from static to non-static.  No pair constraint non-static, or distance < 0: nothing changes. */
+ * Arrays, list rules and refusals as in rcvd_static_flags (trip_centres: centre frame t of the triplet t-1, t, t+1); pair_static /
+ * trip_static in/out, one byte per constraint, flags only go from static to non-static.  No pair constraint non-static, or
+ * distance < 0: nothing changes. */
 int32_t rcvd_prune_static_flags(int32_t device, int32_t num_frames, int32_t height, int32_t width, int32_t distance,
                                 int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
                                 int32_t num_triplets, const int32_t* trip_centres, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static);

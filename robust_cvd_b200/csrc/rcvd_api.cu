@@ -225,15 +225,10 @@ struct rcvd_problem {
   rcvd_problem() {}
 };
 
-// Every kernel this file runs for a handle is launched here: the launch is checked and counted in p->launches (rcvd_launch_count).
-// pdl: a programmatic dependent launch, which may start before its predecessor on the stream ends (it waits with griddepcontrol.wait).
+// Every kernel this file runs for a handle is launched here, and counted in p->launches (rcvd_launch_count).
 template <class... Params, class... Args>
 static int launch(rcvd_problem* p, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
-  cudaLaunchAttribute attr = {};
-  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization; attr.val.programmaticStreamSerializationAllowed = 1;
-  cudaLaunchConfig_t lc = {};
-  lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = s; lc.attrs = &attr; lc.numAttrs = pdl ? 1 : 0;
-  CK(cudaLaunchKernelEx(&lc, kernel, args...));
+  if (int rc = launch_kernel(kernel, grid, block, smem, s, pdl, args...)) return rc;
   p->launches += 1;
   return RCVD_OK;
 }
@@ -1437,21 +1432,19 @@ RCVD_API int32_t rcvd_debug_fp64_tensor_peak(int32_t device, int32_t shape, doub
   const double flops_per_mma = 512.0 * (1 << shape);      // 2*m*n*k: 512, 1024, 2048, 4096
   double* out = nullptr; CK(cudaMalloc((void**)&out, (size_t)blocks * threads * sizeof(double)));
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
+  void (*const kernel)(double*, int) = shape == 0 ? k_dmma_peak<0> : shape == 1 ? k_dmma_peak<1> : shape == 2 ? k_dmma_peak<2> : k_dmma_peak<3>;
   double best = 0;
+  int rc = RCVD_OK;
   for (int rep = 0; rep < 4; ++rep) {
     cudaEventRecord(e0);
-    switch (shape) {
-      case 0: k_dmma_peak<0><<<blocks, threads>>>(out, iters); break;
-      case 1: k_dmma_peak<1><<<blocks, threads>>>(out, iters); break;
-      case 2: k_dmma_peak<2><<<blocks, threads>>>(out, iters); break;
-      default: k_dmma_peak<3><<<blocks, threads>>>(out, iters); break;
-    }
+    if ((rc = launch_kernel(kernel, blocks, threads, 0, nullptr, false, out, iters))) break;
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
     const double tf = flops_per_mma * 8 * iters * (double)blocks * (threads / 32) / (ms * 1e-3) / 1e12;
     if (rep > 0 && tf > best) best = tf;
   }
   cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(out);
+  if (rc) return rc;
   CK(cudaGetLastError());
   *tflops = best; return RCVD_OK;
 }

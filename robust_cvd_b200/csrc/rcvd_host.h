@@ -21,6 +21,20 @@ struct DevGuard {
 
 static inline int nblk(size_t n, int b = 256) { return (int)((n + b - 1) / b); }
 
+// Every kernel of the library is launched here.  A refused launch is reported at once, and its error is cleared from the runtime's
+// last error, so that it is not reported a second time by a later check of the same thread.
+// pdl: a programmatic dependent launch, which may start before its predecessor on the stream ends (it waits with griddepcontrol.wait).
+template <class... Params, class... Args>
+static int launch_kernel(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
+  cudaLaunchAttribute attr = {};
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization; attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t lc = {};
+  lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = s; lc.attrs = &attr; lc.numAttrs = pdl ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(&lc, kernel, args...);
+  if (e != cudaSuccess) { cudaGetLastError(); return set_err(RCVD_ERR_CUDA, "launch failed: %s", cudaGetErrorString(e)); }
+  return RCVD_OK;
+}
+
 // RCVD_OK when `device` is a usable CUDA device, else RCVD_ERR_NO_DEVICE: there is no CPU fallback behind any entry point.
 static inline int check_device(int device) {
   int ndev = 0;

@@ -25,16 +25,24 @@ struct VideoCall {
   cudaStream_t st = nullptr;
   std::vector<void*> bufs;
   bool ok = true;
+  int64_t* launches = nullptr;
   VideoCall() = default;
   VideoCall(const VideoCall&) = delete;
   VideoCall& operator=(const VideoCall&) = delete;
-  int open(int device) {
+  int open(int device, int64_t& launch_count) {   // launch() adds to the entry point's rcvd_*_launch_count counter
     if (int rc = check_device(device)) return rc;
     guard.emplace(device);
     if (guard->err != cudaSuccess) return set_err(RCVD_ERR_CUDA, "cudaSetDevice(%d) failed: %s", device, cudaGetErrorString(guard->err));
     cudaStream_t s;
     CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
     st = s;
+    launches = &launch_count;
+    return RCVD_OK;
+  }
+  template <class... Params, class... Args>
+  int launch(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, Args... args) {
+    if (int rc = launch_kernel(kernel, grid, block, smem, st, false, args...)) return rc;
+    ++*launches;
     return RCVD_OK;
   }
   // at least 16 bytes; a failure is remembered for allocated() and cleared from the runtime's last error
@@ -52,11 +60,11 @@ struct VideoCall {
   // checked before the first launch: a kernel on a null buffer faults with an illegal address, a sticky error of the whole
   // context, and PyTorch shares this context
   bool allocated() const { return ok; }
-  // launch errors, then the stream's; both always run, so no copy into host memory is pending when this returns
+  // errors of the unchecked copies, memsets and sort, then the stream's; both always run, so no copy into host memory is pending after
   int sync(const char* what) {
-    const cudaError_t launch = cudaGetLastError();
+    const cudaError_t enq = cudaGetLastError();
     const cudaError_t e = cudaStreamSynchronize(st);
-    if (launch != cudaSuccess || e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(launch != cudaSuccess ? launch : e));
+    if (enq != cudaSuccess || e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(enq != cudaSuccess ? enq : e));
     return RCVD_OK;
   }
   ~VideoCall() {
@@ -89,9 +97,10 @@ static int dense_run(const rcvd_config* cfg, int device, const double* params_in
   CK(cudaMallocAsync((void**)&d_p, pv.size() * 8, st)); CK(cudaMallocAsync(&d_out, out_bytes, st));
   CK(cudaMemcpyAsync(d_p, pv.data(), pv.size() * 8, cudaMemcpyHostToDevice, st));
   if (src) { CK(cudaMallocAsync((void**)&d_src, n * 4, st)); CK(cudaMemcpyAsync(d_src, src, n * 4, cudaMemcpyHostToDevice, st)); }
-  k_dense<MODE><<<nblk(n), 256, 0, st>>>(*cfg, L, d_p, d_src, d_out, h, w);
-  cudaError_t e = cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st);
+  const int rc = launch_kernel(k_dense<MODE>, nblk(n), 256, 0, st, false, *cfg, L, d_p, d_src, d_out, h, w);
+  cudaError_t e = rc ? cudaSuccess : cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st);
   cudaFreeAsync(d_p, st); cudaFreeAsync(d_out, st); if (d_src) cudaFreeAsync(d_src, st);
+  if (rc) return rc;
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "dense kernel failed: %s", cudaGetErrorString(e));
   return RCVD_OK;
@@ -147,7 +156,7 @@ RCVD_API int32_t rcvd_flow_guided_filter(const rcvd_filter_params* prm, int32_t 
   if (q.frame_radius > 0 && q.num_frames > 1 && (!fwd_flow || !fwd_mask || !bwd_flow || !bwd_mask)) return set_err(RCVD_ERR_INVALID, "flow stacks missing");
   if (q.num_far > 0 && (!far_pairs || !far_flow || !far_mask)) return set_err(RCVD_ERR_INVALID, "far-connection arrays missing");
   VideoCall call;
-  if (int rc = call.open(device)) return rc;
+  if (int rc = call.open(device, g_filter_launches)) return rc;
   const int F = q.num_frames; const size_t plane = (size_t)q.width * q.height, dplane = (size_t)q.depth_width * q.depth_height;
   // cameras: tan(fov / 2) in float on the host, like DepthVideo::project (lib/DepthVideo.cpp:640-641)
   std::vector<float> hc((size_t)F * 12, 0.f);
@@ -199,8 +208,7 @@ RCVD_API int32_t rcvd_flow_guided_filter(const rcvd_filter_params* prm, int32_t 
   for (int c0 = 0; c0 < q.num_out; c0 += chunk) {
     a.first_out = q.first_out + c0; a.num_out = std::min(chunk, q.num_out - c0); a.out = out_dev + (size_t)c0 * plane;
     const dim3 grid((q.width + 31) / 32, (q.height + 3) / 4, a.num_out);
-    if (q.median) k_flow_guided_filter<true><<<grid, 128, 0, call.st>>>(a); else k_flow_guided_filter<false><<<grid, 128, 0, call.st>>>(a);
-    g_filter_launches++;
+    if (int rc = call.launch(q.median ? k_flow_guided_filter<true> : k_flow_guided_filter<false>, grid, 128, 0, a)) return rc;
   }
   cudaMemcpyAsync(out, out_dev, (size_t)q.num_out * plane * 4, cudaMemcpyDeviceToHost, call.st);
   return call.sync("flow-guided filter");
@@ -234,7 +242,7 @@ RCVD_API int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t
   if (q.median && max_samples > kBilateralMaxSamples)
     return set_err(RCVD_ERR_INVALID, "the weighted median supports at most %d samples per pixel; this window has %lld", kBilateralMaxSamples, max_samples);
   VideoCall call;
-  if (int rc = call.open(device)) return rc;
+  if (int rc = call.open(device, g_filter_launches)) return rc;
   const size_t plane = (size_t)q.width * q.height;
   // launch geometry and shared memory
   BilateralArgs a{};
@@ -250,23 +258,16 @@ RCVD_API int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t
     staged = bytes <= 200 * 1024;
     smem = staged ? bytes : 0;
   }
-  auto launch_filter = [&](cudaStream_t s, int base, int n) {
+  void (*const filter)(BilateralArgs) = q.median ? (color ? k_bilateral_median<true> : k_bilateral_median<false>)
+                                      : color    ? (staged ? k_bilateral_mean<true, true> : k_bilateral_mean<true, false>)
+                                                 : (staged ? k_bilateral_mean<false, true> : k_bilateral_mean<false, false>);
+  auto launch_filter = [&](int base, int n) {
     a.out_base = base;
-    if (q.median) {
-      const dim3 grid((unsigned)((plane + kBfMedianWarps - 1) / kBfMedianWarps), 1, n);
-      if (color) k_bilateral_median<true><<<grid, 32 * kBfMedianWarps, smem, s>>>(a); else k_bilateral_median<false><<<grid, 32 * kBfMedianWarps, smem, s>>>(a);
-    } else {
-      const dim3 grid((q.width + kBfTx - 1) / kBfTx, (q.height + kBfTy - 1) / kBfTy, n);
-      if (color) { if (staged) k_bilateral_mean<true, true><<<grid, kBfTx * kBfTy, smem, s>>>(a); else k_bilateral_mean<true, false><<<grid, kBfTx * kBfTy, 0, s>>>(a); }
-      else { if (staged) k_bilateral_mean<false, true><<<grid, kBfTx * kBfTy, smem, s>>>(a); else k_bilateral_mean<false, false><<<grid, kBfTx * kBfTy, 0, s>>>(a); }
-    }
-    g_filter_launches++;
+    const dim3 grid = q.median ? dim3((unsigned)((plane + kBfMedianWarps - 1) / kBfMedianWarps), 1, n)
+                               : dim3((q.width + kBfTx - 1) / kBfTx, (q.height + kBfTy - 1) / kBfTy, n);
+    return call.launch(filter, grid, q.median ? 32 * kBfMedianWarps : kBfTx * kBfTy, smem, a);
   };
-  if (smem > 48 * 1024) {
-    const void* fn = q.median ? (color ? (const void*)k_bilateral_median<true> : (const void*)k_bilateral_median<false>)
-                              : (color ? (const void*)k_bilateral_mean<true, true> : (const void*)k_bilateral_mean<false, true>);
-    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  }
+  if (smem > 48 * 1024) CK(cudaFuncSetAttribute((const void*)filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // per-frame transform vectors in the dense kernel's frame layout (depth parameters at offD)
   std::vector<double> pv;
   if (recur) {
@@ -284,14 +285,14 @@ RCVD_API int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t
     // frame-sequential: filter output o, then rewrite its slot of the depth stack with xform_o(filtered) for the frames after it
     for (int o = 0; o < q.num_out; ++o) {
       a.out = out_dev + (size_t)o * plane;
-      launch_filter(call.st, o, 1);
+      if (int rc = launch_filter(o, 1)) return rc;
       const int f = out_frames[o];
-      k_dense<0><<<nblk(plane), 256, 0, call.st>>>(*xform_cfg, L, d_pv + (size_t)f * L.nf, a.out, d_depth + (size_t)f * plane, q.height, q.width);
+      if (int rc = call.launch(k_dense<0>, nblk(plane), 256, 0, *xform_cfg, L, d_pv + (size_t)f * L.nf, a.out, d_depth + (size_t)f * plane, q.height, q.width)) return rc;
     }
   } else {
     for (int o = 0; o < q.num_out; o += 65535) {   // grid.z limit
       a.out = out_dev + (size_t)o * plane;
-      launch_filter(call.st, o, std::min(65535, q.num_out - o));
+      if (int rc = launch_filter(o, std::min(65535, q.num_out - o))) return rc;
     }
   }
   cudaMemcpyAsync(out, out_dev, (size_t)q.num_out * plane * 4, cudaMemcpyDeviceToHost, call.st);
@@ -301,19 +302,18 @@ RCVD_API int32_t rcvd_bilateral_filter(const rcvd_bilateral_params* prm, int32_t
 // ---------------------------------------------------------------------------
 // Corner scores, shared by the constraint builder and the tracks (rcvd_builder.cuh)
 // ---------------------------------------------------------------------------
-// cv::cornerMinEigenVal(cv::cvtColor(BGR2GRAY), 3) of F colour frames [F][H][W][3] f32 in one batched pass; returns the [F][H][W]
-// scores, or nullptr without launching anything once an allocation of the call has failed.
-static float* enqueue_corner_scores(VideoCall& call, const float* color_bgr, int F, int H, int W, int64_t& launches) {
+// cv::cornerMinEigenVal(cv::cvtColor(BGR2GRAY), 3) of F colour frames [F][H][W][3] f32 in one batched pass into the [F][H][W] scores
+// `corner`.  Nothing is launched once an allocation of the call has failed; the caller reports that through call.allocated().
+static int enqueue_corner_scores(VideoCall& call, const float* color_bgr, int F, int H, int W, const float*& corner) {
   const size_t FP = (size_t)F * H * W;
   float* d_bgr = (float*)call.upload(color_bgr, FP * 12);
   float* d_gray = (float*)call.alloc(FP * 4), *d_pl = (float*)call.alloc(FP * 12), *d_corner = (float*)call.alloc(FP * 4); double* d_tmp = (double*)call.alloc(FP * 24);
-  if (!call.allocated()) return nullptr;
-  k_gray<<<(unsigned)((FP + 255) / 256), 256, 0, call.st>>>(d_bgr, d_gray, FP);
-  k_sobel_products<<<(unsigned)((FP + 255) / 256), 256, 0, call.st>>>(d_gray, d_pl, F, H, W);
-  k_box_h<<<(unsigned)((FP * 3 + 255) / 256), 256, 0, call.st>>>(d_pl, d_tmp, (size_t)3 * F * H, W);
-  k_box_v_eig<<<(unsigned)(((size_t)F * W + 127) / 128), 128, 0, call.st>>>(d_tmp, d_corner, F, H, W);
-  launches += 4;
-  return d_corner;
+  corner = d_corner;
+  if (!call.allocated()) return RCVD_OK;
+  if (int rc = call.launch(k_gray, (unsigned)((FP + 255) / 256), 256, 0, d_bgr, d_gray, FP)) return rc;
+  if (int rc = call.launch(k_sobel_products, (unsigned)((FP + 255) / 256), 256, 0, d_gray, d_pl, F, H, W)) return rc;
+  if (int rc = call.launch(k_box_h, (unsigned)((FP * 3 + 255) / 256), 256, 0, d_pl, d_tmp, (size_t)3 * F * H, W)) return rc;
+  return call.launch(k_box_v_eig, (unsigned)(((size_t)F * W + 127) / 128), 128, 0, d_tmp, d_corner, F, H, W);
 }
 
 // ---------------------------------------------------------------------------
@@ -340,11 +340,11 @@ RCVD_API int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t 
   if (trip_offsets) trip_offsets[0] = 0;
   if (I == 0) return RCVD_OK;
   VideoCall call;
-  if (int rc = call.open(device)) return rc;
+  if (int rc = call.open(device, g_builder_launches)) return rc;
   const int W = q.width, H = q.height;
   const size_t plane = (size_t)W * H;
   BuilderArgs a{};
-  a.corner = enqueue_corner_scores(call, color_bgr, F, H, W, g_builder_launches);
+  if (int rc = enqueue_corner_scores(call, color_bgr, F, H, W, a.corner)) return rc;
   a.dyn = dyn_dist ? (const float*)call.upload(dyn_dist, (size_t)F * q.dyn_width * q.dyn_height * 4) : nullptr;
   a.pair_frames = (const int*)call.upload(pair_frames, (size_t)P * 8); a.pair_flow = (const float*)call.upload(pair_flow, (size_t)P * plane * 8); a.pair_mask = (const uint8_t*)call.upload(pair_mask, (size_t)P * plane);
   a.trip_frames = (const int*)call.upload(trip_frames, (size_t)T * 4); a.trip_flow = (const float*)call.upload(trip_flow, (size_t)T * 2 * plane * 8); a.trip_mask = (const uint8_t*)call.upload(trip_mask, (size_t)T * 2 * plane);
@@ -356,13 +356,14 @@ RCVD_API int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t 
   a.dsx = dyn_dist ? q.dyn_width / float(W) : 1.f; a.dsy = dyn_dist ? q.dyn_height / float(H) : 1.f;
   a.sx = 1.f / W; a.sy = q.inv_aspect / H;
   const unsigned gx = (unsigned)((plane + 255) / 256);
-  if (P > 0) { k_pair_candidates<<<dim3(gx, P), 256, 0, call.st>>>(a); g_builder_launches++; }
-  if (T > 0) { k_triplet_candidates<<<dim3(gx, T), 256, 0, call.st>>>(a); g_builder_launches++; }
+  if (P > 0) { if (int rc = call.launch(k_pair_candidates, dim3(gx, P), 256, 0, a)) return rc; }
+  if (T > 0) { if (int rc = call.launch(k_triplet_candidates, dim3(gx, T), 256, 0, a)) return rc; }
   // ---- selection rounds until nothing is undecided ----
   int rounds = 0;
   for (;;) {
     cudaMemsetAsync(d_cnt, 0, 8, call.st);
-    k_select_round<<<dim3(gx, I), 256, 0, call.st>>>(a, d_cnt); g_builder_launches++; ++rounds;
+    if (int rc = call.launch(k_select_round, dim3(gx, I), 256, 0, a, d_cnt)) return rc;
+    ++rounds;
     unsigned long long und = 0;
     cudaMemcpyAsync(&und, d_cnt, 8, cudaMemcpyDeviceToHost, call.st);
     if (int rc = call.sync("constraint selection")) return rc;
@@ -372,7 +373,7 @@ RCVD_API int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t 
   g_builder_rounds = rounds;
   // ---- counts, offsets, emission ----
   cudaMemsetAsync(d_cnt, 0, (size_t)(2 * I + 2) * 8, call.st);
-  k_count_accepted<<<dim3(gx, I), 256, 0, call.st>>>(a, d_cnt + 1); g_builder_launches++;
+  if (int rc = call.launch(k_count_accepted, dim3(gx, I), 256, 0, a, d_cnt + 1)) return rc;
   std::vector<unsigned long long> cnt(I), off(I + 1, 0);
   cudaMemcpyAsync(cnt.data(), d_cnt + 1, (size_t)I * 8, cudaMemcpyDeviceToHost, call.st);
   if (int rc = call.sync("constraint count read-back")) return rc;
@@ -387,7 +388,7 @@ RCVD_API int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t 
   int* d_idx = (int*)call.alloc(total * 4); float* d_score = (float*)call.alloc(total * 4);
   float* d_po = (float*)call.alloc(std::max<size_t>(pair_total, 1) * 16); float* d_to = (float*)call.alloc(std::max<size_t>(total - pair_total, 1) * 24);
   if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_build_constraints");
-  k_emit<<<dim3(gx, I), 256, 0, call.st>>>(a, d_off, d_cnt + 1 + I, d_idx, d_score, d_po, d_to, pair_total); g_builder_launches++;
+  if (int rc = call.launch(k_emit, dim3(gx, I), 256, 0, a, d_off, d_cnt + 1 + I, d_idx, d_score, d_po, d_to, pair_total)) return rc;
   std::vector<int> idx(total); std::vector<float> score(total), po(pair_total * 4), to((total - pair_total) * 6);
   cudaMemcpyAsync(idx.data(), d_idx, total * 4, cudaMemcpyDeviceToHost, call.st); cudaMemcpyAsync(score.data(), d_score, total * 4, cudaMemcpyDeviceToHost, call.st);
   if (pair_total) cudaMemcpyAsync(po.data(), d_po, pair_total * 16, cudaMemcpyDeviceToHost, call.st);
@@ -408,39 +409,64 @@ RCVD_API int32_t rcvd_build_constraints(const rcvd_builder_params* prm, int32_t 
 }
 
 // ---------------------------------------------------------------------------
-// Dynamic-mask distance transform + static flags on the device (rcvd_builder.cuh)
+// Dynamic-mask distance transform + static flags, and their pruning, on the device (rcvd_builder.cuh)
 // ---------------------------------------------------------------------------
+// One constraint family of rcvd_static_flags / rcvd_prune_static_flags as the caller gives it: n groups, each with its frames (a pair's
+// two, or the centre t of the triplet t-1, t, t+1), offsets [n+1], then per constraint the locations of its `ends` ends and a flag.
+struct FlagList {
+  const char* what; int ends; int32_t n; const int32_t* frames; const int64_t* offsets; const float* locs; uint8_t* flags;
+  int64_t total() const { return n > 0 ? offsets[n] : 0; }
+  // The list rules of include/rcvd.h, checked on the host before the call opens its device: a refused call needs no device and leaves
+  // the caller's flags as they were, and the kernels only index inside the lists.
+  int check(int F) const {
+    if (n < 0) return set_err(RCVD_ERR_INVALID, "negative %s count", what);
+    if (n > 0 && (!frames || !offsets)) return set_err(RCVD_ERR_INVALID, "null argument");
+    if (n > 0 && offsets[0] != 0) return set_err(RCVD_ERR_INVALID, "%s offsets must start at 0", what);
+    for (int i = 0; i < n; ++i) {
+      const bool ok = ends == 2 ? frames[2 * i] >= 0 && frames[2 * i] < F && frames[2 * i + 1] >= 0 && frames[2 * i + 1] < F : frames[i] >= 1 && frames[i] + 1 < F;
+      if (!ok || offsets[i + 1] < offsets[i]) return set_err(RCVD_ERR_INVALID, "bad %s %d", what, i);
+    }
+    if (total() > 0 && (!locs || !flags)) return set_err(RCVD_ERR_INVALID, "null argument");
+    return RCVD_OK;
+  }
+};
+// A family on the device as k_static_flags, k_prune_stamp and k_prune_lookup read it: the frame of each end [n][3] (-1 past a pair's
+// two ends), offsets, locations and flags (a copy of the caller's with `with_flags`, else unset for the kernel to write).
+struct DevFlagList { int n, ends; int64_t total; const int* frames; const long long* offsets; const float* locs; uint8_t* flags; };
+static DevFlagList upload_flag_list(VideoCall& call, const FlagList& l, bool with_flags) {
+  std::vector<int32_t> f3((size_t)l.n * 3, -1);
+  for (int i = 0; i < l.n; ++i)
+    for (int e = 0; e < l.ends; ++e) f3[3 * i + e] = l.ends == 2 ? l.frames[2 * i + e] : l.frames[i] - 1 + e;
+  const int64_t total = l.total();
+  return {l.n, l.ends, total, (const int*)call.upload(f3.data(), f3.size() * 4),
+          (const long long*)call.upload(l.offsets, l.n > 0 ? (size_t)(l.n + 1) * 8 : 0), (const float*)call.upload(l.locs, (size_t)total * 8 * l.ends),
+          (uint8_t*)(with_flags ? call.upload(l.flags, (size_t)total) : call.alloc((size_t)total))};
+}
+
 static int64_t g_flag_launches = 0;
 RCVD_API int64_t rcvd_static_flag_launch_count() { return g_flag_launches; }
 // dist_out (optional): [F][h][w] float32 = cv::distanceTransform(mask >= 127 ? 255 : 0, DIST_L2, 5) of every frame (fixed-point chamfer).
-// pair_static / trip_static (optional): one byte per constraint.
 RCVD_API int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t F, int32_t h, int32_t w, float distance,
                                    int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
                                    int32_t num_triplets, const int32_t* trip_frames, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static,
                                    float* dist_out) {
-  if (!masks || F <= 0 || h <= 0 || w <= 0 || num_pairs < 0 || num_triplets < 0) return set_err(RCVD_ERR_INVALID, "bad static-flag arguments");
-  if ((num_pairs > 0 && (!pair_frames || !pair_offsets || !pair_static)) || (num_triplets > 0 && (!trip_frames || !trip_offsets || !trip_static))) return set_err(RCVD_ERR_INVALID, "null argument");
-  for (int i = 0; i < num_pairs; ++i) if (pair_frames[2 * i] < 0 || pair_frames[2 * i] >= F || pair_frames[2 * i + 1] < 0 || pair_frames[2 * i + 1] >= F || pair_offsets[i + 1] < pair_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad pair %d", i);
-  for (int i = 0; i < num_triplets; ++i) if (trip_frames[i] < 1 || trip_frames[i] + 1 >= F || trip_offsets[i + 1] < trip_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad triplet %d", i);
+  if (!masks || F <= 0 || h <= 0 || w <= 0) return set_err(RCVD_ERR_INVALID, "bad static-flag arguments");
+  const FlagList pairs{"pair", 2, num_pairs, pair_frames, pair_offsets, pair_locs, pair_static}, trips{"triplet", 3, num_triplets, trip_frames, trip_offsets, trip_locs, trip_static};
+  if (int rc = pairs.check(F)) return rc;
+  if (int rc = trips.check(F)) return rc;
   VideoCall call;
-  if (int rc = call.open(device)) return rc;
+  if (int rc = call.open(device, g_flag_launches)) return rc;
   const size_t plane = (size_t)w * h;
   const uint8_t* d_masks = (const uint8_t*)call.upload(masks, (size_t)F * plane);
   unsigned* d_scratch = (unsigned*)call.alloc((size_t)F * plane * 4); float* d_dist = (float*)call.alloc((size_t)F * plane * 4);
-  const int64_t np_total = num_pairs ? pair_offsets[num_pairs] : 0, nt_total = num_triplets ? trip_offsets[num_triplets] : 0;
-  std::vector<int32_t> pf3((size_t)num_pairs * 3, -1), tf3((size_t)num_triplets * 3, -1);
-  for (int i = 0; i < num_pairs; ++i) { pf3[3 * i] = pair_frames[2 * i]; pf3[3 * i + 1] = pair_frames[2 * i + 1]; }
-  for (int i = 0; i < num_triplets; ++i) { tf3[3 * i] = trip_frames[i] - 1; tf3[3 * i + 1] = trip_frames[i]; tf3[3 * i + 2] = trip_frames[i] + 1; }
-  int* d_pf = (int*)call.upload(pf3.data(), pf3.size() * 4); int* d_tf = (int*)call.upload(tf3.data(), tf3.size() * 4);
-  long long* d_po = (long long*)call.upload(pair_offsets, (size_t)(num_pairs + 1) * 8 * (num_pairs > 0)); long long* d_to = (long long*)call.upload(trip_offsets, (size_t)(num_triplets + 1) * 8 * (num_triplets > 0));
-  float* d_pl = (float*)call.upload(pair_locs, (size_t)np_total * 16); float* d_tl = (float*)call.upload(trip_locs, (size_t)nt_total * 24);
-  uint8_t* d_ps = (uint8_t*)call.alloc((size_t)np_total); uint8_t* d_ts = (uint8_t*)call.alloc((size_t)nt_total);
+  const DevFlagList dp = upload_flag_list(call, pairs, false), dt = upload_flag_list(call, trips, false);
   if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_static_flags");
-  k_chamfer5<<<F, kChamThreads, 0, call.st>>>(d_masks, d_scratch, d_dist, h, w); g_flag_launches++;
-  if (np_total > 0) { k_static_flags<<<dim3(8, num_pairs), 256, 0, call.st>>>(d_dist, h, w, distance, 2, d_pf, d_po, num_pairs, d_pl, d_ps); g_flag_launches++; }
-  if (nt_total > 0) { k_static_flags<<<dim3(8, num_triplets), 256, 0, call.st>>>(d_dist, h, w, distance, 3, d_tf, d_to, num_triplets, d_tl, d_ts); g_flag_launches++; }
-  if (np_total > 0) cudaMemcpyAsync(pair_static, d_ps, (size_t)np_total, cudaMemcpyDeviceToHost, call.st);
-  if (nt_total > 0) cudaMemcpyAsync(trip_static, d_ts, (size_t)nt_total, cudaMemcpyDeviceToHost, call.st);
+  if (int rc = call.launch(k_chamfer5, F, kChamThreads, 0, d_masks, d_scratch, d_dist, h, w)) return rc;
+  for (const DevFlagList* d : {&dp, &dt})
+    if (d->total > 0)
+      if (int rc = call.launch(k_static_flags, dim3(8, d->n), 256, 0, d_dist, h, w, distance, d->ends, d->frames, d->offsets, d->n, d->locs, d->flags)) return rc;
+  if (dp.total > 0) cudaMemcpyAsync(pair_static, dp.flags, (size_t)dp.total, cudaMemcpyDeviceToHost, call.st);
+  if (dt.total > 0) cudaMemcpyAsync(trip_static, dt.flags, (size_t)dt.total, cudaMemcpyDeviceToHost, call.st);
   if (dist_out) cudaMemcpyAsync(dist_out, d_dist, (size_t)F * plane * 4, cudaMemcpyDeviceToHost, call.st);
   return call.sync("static-flag kernels");
 }
@@ -450,34 +476,27 @@ RCVD_API int32_t rcvd_static_flags(int32_t device, const uint8_t* masks, int32_t
 RCVD_API int32_t rcvd_prune_static_flags(int32_t device, int32_t F, int32_t h, int32_t w, int32_t distance,
                                          int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
                                          int32_t num_triplets, const int32_t* trip_centres, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static) {
-  if (F <= 0 || h <= 0 || w <= 0 || num_pairs < 0 || num_triplets < 0) return set_err(RCVD_ERR_INVALID, "bad static-flag pruning arguments");
-  if ((num_pairs > 0 && (!pair_frames || !pair_offsets)) || (num_triplets > 0 && (!trip_centres || !trip_offsets))) return set_err(RCVD_ERR_INVALID, "null argument");
-  for (int i = 0; i < num_pairs; ++i) if (pair_frames[2 * i] < 0 || pair_frames[2 * i] >= F || pair_frames[2 * i + 1] < 0 || pair_frames[2 * i + 1] >= F || pair_offsets[i + 1] < pair_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad pair %d", i);
-  for (int i = 0; i < num_triplets; ++i) if (trip_centres[i] < 1 || trip_centres[i] + 1 >= F || trip_offsets[i + 1] < trip_offsets[i]) return set_err(RCVD_ERR_INVALID, "bad triplet %d", i);
-  const int64_t np_total = num_pairs ? pair_offsets[num_pairs] : 0, nt_total = num_triplets ? trip_offsets[num_triplets] : 0;
-  if ((np_total > 0 && (!pair_locs || !pair_static)) || (nt_total > 0 && (!trip_locs || !trip_static))) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (F <= 0 || h <= 0 || w <= 0) return set_err(RCVD_ERR_INVALID, "bad static-flag pruning arguments");
+  const FlagList pairs{"pair", 2, num_pairs, pair_frames, pair_offsets, pair_locs, pair_static}, trips{"triplet", 3, num_triplets, trip_centres, trip_offsets, trip_locs, trip_static};
+  if (int rc = pairs.check(F)) return rc;
+  if (int rc = trips.check(F)) return rc;
   bool stamps = false;
-  for (int64_t i = 0; i < np_total && !stamps; ++i) stamps = pair_static[i] == 0;
+  for (int64_t i = 0; i < pairs.total() && !stamps; ++i) stamps = pair_static[i] == 0;
   if (!stamps || distance < 0) return RCVD_OK;
   VideoCall call;
-  if (int rc = call.open(device)) return rc;
+  if (int rc = call.open(device, g_flag_launches)) return rc;
   const int words = (w + 31) / 32;
   const size_t bits_bytes = (size_t)F * h * words * 4;
   unsigned* d_bits = (unsigned*)call.alloc(bits_bytes);
-  std::vector<int32_t> pf3((size_t)num_pairs * 3, -1), tf3((size_t)num_triplets * 3, -1);
-  for (int i = 0; i < num_pairs; ++i) { pf3[3 * i] = pair_frames[2 * i]; pf3[3 * i + 1] = pair_frames[2 * i + 1]; }
-  for (int i = 0; i < num_triplets; ++i) { tf3[3 * i] = trip_centres[i] - 1; tf3[3 * i + 1] = trip_centres[i]; tf3[3 * i + 2] = trip_centres[i] + 1; }
-  int* d_pf = (int*)call.upload(pf3.data(), pf3.size() * 4); int* d_tf = (int*)call.upload(tf3.data(), tf3.size() * 4);
-  long long* d_po = (long long*)call.upload(pair_offsets, (size_t)(num_pairs + 1) * 8); long long* d_to = (long long*)call.upload(trip_offsets, (size_t)(num_triplets + 1) * 8 * (num_triplets > 0));
-  float* d_pl = (float*)call.upload(pair_locs, (size_t)np_total * 16); float* d_tl = (float*)call.upload(trip_locs, (size_t)nt_total * 24);
-  uint8_t* d_ps = (uint8_t*)call.upload(pair_static, (size_t)np_total); uint8_t* d_ts = (uint8_t*)call.upload(trip_static, (size_t)nt_total);
+  const DevFlagList dp = upload_flag_list(call, pairs, true), dt = upload_flag_list(call, trips, true);
   if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_prune_static_flags");
   cudaMemsetAsync(d_bits, 0, bits_bytes, call.st);
-  k_prune_stamp<<<dim3(8, num_pairs), 256, 0, call.st>>>(d_bits, h, w, words, distance, d_pf, d_po, num_pairs, d_pl, d_ps); g_flag_launches++;
-  k_prune_lookup<<<dim3(8, num_pairs), 256, 0, call.st>>>(d_bits, h, w, words, 2, d_pf, d_po, num_pairs, d_pl, d_ps); g_flag_launches++;
-  if (nt_total > 0) { k_prune_lookup<<<dim3(8, num_triplets), 256, 0, call.st>>>(d_bits, h, w, words, 3, d_tf, d_to, num_triplets, d_tl, d_ts); g_flag_launches++; }
-  cudaMemcpyAsync(pair_static, d_ps, (size_t)np_total, cudaMemcpyDeviceToHost, call.st);
-  if (nt_total > 0) cudaMemcpyAsync(trip_static, d_ts, (size_t)nt_total, cudaMemcpyDeviceToHost, call.st);
+  if (int rc = call.launch(k_prune_stamp, dim3(8, dp.n), 256, 0, d_bits, h, w, words, distance, dp.frames, dp.offsets, dp.n, dp.locs, dp.flags)) return rc;
+  for (const DevFlagList* d : {&dp, &dt})
+    if (d->total > 0)
+      if (int rc = call.launch(k_prune_lookup, dim3(8, d->n), 256, 0, d_bits, h, w, words, d->ends, d->frames, d->offsets, d->n, d->locs, d->flags)) return rc;
+  cudaMemcpyAsync(pair_static, dp.flags, (size_t)dp.total, cudaMemcpyDeviceToHost, call.st);
+  if (dt.total > 0) cudaMemcpyAsync(trip_static, dt.flags, (size_t)dt.total, cudaMemcpyDeviceToHost, call.st);
   return call.sync("static-flag pruning kernels");
 }
 
@@ -501,7 +520,7 @@ RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t devic
   for (int f = 0; f <= F; ++f) frame_offsets[f] = 0;
   *num_tracks = 0;
   VideoCall call;
-  if (int rc = call.open(device)) return rc;
+  if (int rc = call.open(device, g_track_launches)) return rc;
   const int plane = W * H;
   const size_t FP = (size_t)F * plane, dplane = dyn_masks ? (size_t)q.dyn_width * q.dyn_height : 0;
   const int max_rounds = 4 * (W + H) + 16, max_live = 2 * plane;   // at most one continued and one spawned track per pixel
@@ -510,7 +529,8 @@ RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t devic
   for (int x = 0; x < W; ++x) { volatile float u = x / float(W); volatile float v = u * W; mxv[x] = (int)v; }
   for (int y = 0; y < H; ++y) { volatile float u = y / float(H); volatile float v = u * q.inv_aspect; volatile float t = v / q.inv_aspect; volatile float z = t * H; myv[y] = (int)z; }
   // ---- corner scores and distance images of every frame, batched ----
-  const float* d_corner = enqueue_corner_scores(call, color_bgr, F, H, W, g_track_launches);
+  const float* d_corner = nullptr;
+  if (int rc = enqueue_corner_scores(call, color_bgr, F, H, W, d_corner)) return rc;
   uint8_t* d_dmask = dyn_masks ? (uint8_t*)call.upload(dyn_masks, (size_t)F * dplane) : nullptr;
   unsigned* d_cscratch = dyn_masks ? (unsigned*)call.alloc((size_t)F * dplane * 4) : nullptr;
   float* d_dist = dyn_masks ? (float*)call.alloc((size_t)F * dplane * 4) : nullptr;
@@ -531,7 +551,7 @@ RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t devic
   cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, d_keys, d_sorted, plane, 0, 64, call.st);
   void* d_sort_tmp = call.alloc(sort_bytes);
   if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_compute_tracks");
-  if (dyn_masks) { k_chamfer5<<<F, kChamThreads, 0, call.st>>>(d_dmask, d_cscratch, d_dist, q.dyn_height, q.dyn_width); g_track_launches++; }
+  if (dyn_masks) { if (int rc = call.launch(k_chamfer5, F, kChamThreads, 0, d_dmask, d_cscratch, d_dist, q.dyn_height, q.dyn_width)) return rc; }
   TrackArgs a{};
   a.w = W; a.h = H; a.dw = dyn_masks ? q.dyn_width : W; a.dh = dyn_masks ? q.dyn_height : H;
   a.spawn_r = q.spawn_distance; a.prune_r = q.prune_distance; a.min_dyn = q.min_dynamic_distance; a.ia = q.inv_aspect;
@@ -563,7 +583,7 @@ RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t devic
     const bool spawn = f < F - 1;
     const float* score = d_corner + (size_t)f * plane;
     if (spawn) {
-      k_tr_sort_keys<<<nblk(plane), 256, 0, call.st>>>(score, plane, d_keys); g_track_launches++;
+      if (int rc = call.launch(k_tr_sort_keys, nblk(plane), 256, 0, score, plane, d_keys)) return rc;
       cub::DeviceRadixSort::SortKeys(d_sort_tmp, sort_bytes, d_keys, d_sorted, plane, 0, 64, call.st);
     }
     for (;;) {   // rounds enqueued blind (they stop early on the device); a frame whose rounds did not all finish is run again with more
@@ -571,21 +591,19 @@ RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t devic
       cudaMemsetAsync(d_smask, 0, plane, call.st);
       if (cont) {
         cudaMemsetAsync(d_acc, 0xff, (size_t)plane * 4, call.st); cudaMemsetAsync(d_und[0], 0xff, (size_t)plane * 4, call.st); cudaMemsetAsync(d_und[1], 0xff, (size_t)plane * 4, call.st);
-        k_tr_continue<<<nblk(n_prev), 256, 0, call.st>>>(a, n_prev, d_loc[prev], d_flow + (size_t)f * plane * 2, d_fmask + (size_t)f * plane, d_pix, d_cloc, d_cstate, d_und[0]);
-        g_track_launches++;
-        for (int k = 0; k < rp; ++k) {
-          k_tr_prune_round<<<nblk(std::max(n_prev, plane)), 256, 0, call.st>>>(a, n_prev, k, d_pix, d_cstate, d_acc, d_und[k % 3], d_und[(k + 1) % 3], d_und[(k + 2) % 3], d_cnt);
-          g_track_launches++;
-        }
-        k_tr_stamp<<<n_prev, 256, 0, call.st>>>(a, d_pix, d_cstate, d_smask); g_track_launches++;
+        if (int rc = call.launch(k_tr_continue, nblk(n_prev), 256, 0, a, n_prev, d_loc[prev], d_flow + (size_t)f * plane * 2, d_fmask + (size_t)f * plane, d_pix, d_cloc, d_cstate, d_und[0])) return rc;
+        for (int k = 0; k < rp; ++k)
+          if (int rc = call.launch(k_tr_prune_round, nblk(std::max(n_prev, plane)), 256, 0, a, n_prev, k, d_pix, d_cstate, d_acc, d_und[k % 3], d_und[(k + 1) % 3], d_und[(k + 2) % 3], d_cnt)) return rc;
+        if (int rc = call.launch(k_tr_stamp, n_prev, 256, 0, a, d_pix, d_cstate, d_smask)) return rc;
       }
       if (spawn) {
         const uint8_t* sm = (fl & RCVD_TRACK_MASK) ? d_fmask + (size_t)f * plane : nullptr;
-        k_tr_spawn_init<<<nblk(plane), 256, 0, call.st>>>(a, sm, d_smask, d_mx, d_my, d_sstate); g_track_launches++;
-        for (int k = 0; k < rs; ++k) { k_tr_spawn_round<<<nblk(plane), 256, 0, call.st>>>(a, k, score, d_mx, d_my, d_sstate, d_cnt + max_rounds); g_track_launches++; }
+        if (int rc = call.launch(k_tr_spawn_init, nblk(plane), 256, 0, a, sm, d_smask, d_mx, d_my, d_sstate)) return rc;
+        for (int k = 0; k < rs; ++k)
+          if (int rc = call.launch(k_tr_spawn_round, nblk(plane), 256, 0, a, k, score, d_mx, d_my, d_sstate, d_cnt + max_rounds)) return rc;
       }
-      k_tr_emit<<<1, kTrEmitThreads, 0, call.st>>>(a, cont ? n_prev : 0, d_id[prev], d_cstate, d_cloc, spawn ? 1 : 0, d_sorted, d_sstate, next_id, d_id[nxt], d_loc[nxt], d_counts);
-      g_track_launches++;
+      if (int rc = call.launch(k_tr_emit, 1, kTrEmitThreads, 0, a, cont ? n_prev : 0, d_id[prev], d_cstate, d_cloc, spawn ? 1 : 0, d_sorted, d_sstate, next_id, d_id[nxt], d_loc[nxt], d_counts))
+        return rc;
       if (f > 0) flush(f - 1, prev, n_prev);
       cudaMemcpyAsync(cnt_h.data(), d_cnt, (size_t)2 * max_rounds * 4, cudaMemcpyDeviceToHost, call.st);
       cudaMemcpyAsync(counts_h, d_counts, 8, cudaMemcpyDeviceToHost, call.st);

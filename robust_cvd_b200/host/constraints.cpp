@@ -448,6 +448,26 @@ void FlowConstraintsCollection::computeOnDevice() {
   rcvd_trim_device_memory(currentDevice());
 }
 
+// The pair and triplet lists as rcvd_static_flags and rcvd_prune_static_flags take them, in map order: pair frames / triplet centres,
+// offsets, locations and one flag byte per constraint (the current flag with `withFlags`, else 0 for the call to overwrite).
+struct FlagLists { std::vector<int32_t> pf, tc; std::vector<int64_t> po{0}, to{0}; std::vector<float> pl, tl; std::vector<uint8_t> ps, ts; };
+template <class Pairs, class Trips> static FlagLists packFlagLists(const Pairs& pairs, const Trips& trips, bool withFlags) {
+  FlagLists l;
+  for (auto& kv : pairs) {
+    l.pf.push_back(kv.first.first); l.pf.push_back(kv.first.second); l.po.push_back(l.po.back() + int64_t(kv.second.size()));
+    for (auto& c : kv.second) { l.pl.insert(l.pl.end(), &c.loc[0][0], &c.loc[0][0] + 4); l.ps.push_back(withFlags && c.isStatic); }
+  }
+  for (auto& kv : trips) {
+    l.tc.push_back(kv.first); l.to.push_back(l.to.back() + int64_t(kv.second.size()));
+    for (auto& c : kv.second) { l.tl.insert(l.tl.end(), &c.loc[0][0], &c.loc[0][0] + 6); l.ts.push_back(withFlags && c.isStatic); }
+  }
+  return l;
+}
+template <class Pairs, class Trips> static void unpackFlags(const FlagLists& l, Pairs& pairs, Trips& trips) {
+  size_t i = 0; for (auto& kv : pairs) for (auto& c : kv.second) c.isStatic = l.ps[i++] != 0;
+  i = 0; for (auto& kv : trips) for (auto& c : kv.second) c.isStatic = l.ts[i++] != 0;
+}
+
 void FlowConstraintsCollection::resetStaticFlag() {
   for (auto& kv : pairs_) for (auto& c : kv.second) c.isStatic = true;
   for (auto& kv : triplets_) for (auto& c : kv.second) c.isStatic = true;
@@ -473,15 +493,11 @@ void FlowConstraintsCollection::setStaticFlagFromDynamicMask(int distance) {   /
         if (m->cols != w || m->rows != h) throw std::runtime_error("Dynamic masks have inconsistent dimensions.");
         std::memcpy(masks.data() + size_t(f) * plane, m->data.data(), plane);
       }
-      std::vector<int32_t> pf, tf; std::vector<int64_t> po(1, 0), to(1, 0); std::vector<float> pl, tl;
-      for (auto& kv : pairs_) { pf.push_back(kv.first.first); pf.push_back(kv.first.second); for (auto& c : kv.second) pl.insert(pl.end(), &c.loc[0][0], &c.loc[0][0] + 4); po.push_back(po.back() + int64_t(kv.second.size())); }
-      for (auto& kv : triplets_) { tf.push_back(kv.first); for (auto& c : kv.second) tl.insert(tl.end(), &c.loc[0][0], &c.loc[0][0] + 6); to.push_back(to.back() + int64_t(kv.second.size())); }
-      std::vector<uint8_t> ps(size_t(po.back()) + 1), ts(size_t(to.back()) + 1);
-      const int rc = rcvd_static_flags(currentDevice(), masks.data(), F, h, w, float(distance), int(pf.size() / 2), pf.data(), po.data(), pl.data(), ps.data(),
-                                       int(tf.size()), tf.data(), to.data(), tl.data(), ts.data(), nullptr);
+      FlagLists l = packFlagLists(pairs_, triplets_, false);
+      const int rc = rcvd_static_flags(currentDevice(), masks.data(), F, h, w, float(distance), int(l.pf.size() / 2), l.pf.data(), l.po.data(), l.pl.data(),
+                                       l.ps.data(), int(l.tc.size()), l.tc.data(), l.to.data(), l.tl.data(), l.ts.data(), nullptr);
       if (rc != RCVD_OK) throw std::runtime_error(std::string("rcvd_static_flags failed: ") + rcvd_last_error());
-      size_t i = 0; for (auto& kv : pairs_) for (auto& c : kv.second) c.isStatic = ps[i++] != 0;
-      i = 0; for (auto& kv : triplets_) for (auto& c : kv.second) c.isStatic = ts[i++] != 0;
+      unpackFlags(l, pairs_, triplets_);
       return;
     }
   }
@@ -518,22 +534,11 @@ void FlowConstraintsCollection::pruneStaticFlag(int distance) {   // :662-748
   if (!host) {
     // default: disc stamps into per-frame bit planes + per-constraint lookups on the device (rcvd_prune_static_flags)
     const int F = video_->numFrames();
-    std::vector<int32_t> pf, tf; std::vector<int64_t> po(1, 0), to(1, 0); std::vector<float> pl, tl; std::vector<uint8_t> ps, ts;
-    for (auto& kv : pairs_) {
-      pf.push_back(kv.first.first); pf.push_back(kv.first.second);
-      for (auto& c : kv.second) { pl.insert(pl.end(), &c.loc[0][0], &c.loc[0][0] + 4); ps.push_back(c.isStatic ? 1 : 0); }
-      po.push_back(po.back() + int64_t(kv.second.size()));
-    }
-    for (auto& kv : triplets_) {
-      tf.push_back(kv.first);
-      for (auto& c : kv.second) { tl.insert(tl.end(), &c.loc[0][0], &c.loc[0][0] + 6); ts.push_back(c.isStatic ? 1 : 0); }
-      to.push_back(to.back() + int64_t(kv.second.size()));
-    }
-    const int rc = rcvd_prune_static_flags(currentDevice(), F, h, w, distance, int(pf.size() / 2), pf.data(), po.data(), pl.data(), ps.data(),
-                                           int(tf.size()), tf.data(), to.data(), tl.data(), ts.data());
+    FlagLists l = packFlagLists(pairs_, triplets_, true);
+    const int rc = rcvd_prune_static_flags(currentDevice(), F, h, w, distance, int(l.pf.size() / 2), l.pf.data(), l.po.data(), l.pl.data(), l.ps.data(),
+                                           int(l.tc.size()), l.tc.data(), l.to.data(), l.tl.data(), l.ts.data());
     if (rc != RCVD_OK) throw std::runtime_error(std::string("rcvd_prune_static_flags failed: ") + rcvd_last_error());
-    size_t i = 0; for (auto& kv : pairs_) for (auto& c : kv.second) c.isStatic = ps[i++] != 0;
-    i = 0; for (auto& kv : triplets_) for (auto& c : kv.second) c.isStatic = ts[i++] != 0;
+    unpackFlags(l, pairs_, triplets_);
     return;
   }
   const int size = 2 * distance + 1;

@@ -417,22 +417,28 @@ def compute_tracks(color_bgr, frame_flags, flow=None, flow_mask=None, dyn_masks=
     return off, ids[:off[F]], locs[:off[F]], int(n.value)
 
 
+def _flag_family(frames, offsets, locs, width, flags=None):
+    """One constraint family of static_flags / prune_static_flags as C arguments (count, frames, offsets, locs, flags), and the flag
+    array the call writes: a copy of `flags`, or zeros when it is None."""
+    n = 0 if frames is None else len(frames)
+    if n == 0:
+        return (C.c_int32(0), None, None, None, None), np.zeros(0, np.uint8)
+    fr = np.ascontiguousarray(frames, np.int32)
+    off = np.ascontiguousarray(offsets, np.int64)
+    loc = np.ascontiguousarray(locs, np.float32).reshape(-1, width)
+    fl = np.zeros(int(off[-1]), np.uint8) if flags is None else np.array(flags, np.uint8).reshape(-1)
+    return (C.c_int32(n), _p(fr, C.c_int32), _p(off, C.c_int64), _p(loc, C.c_float), _p(fl, C.c_uint8)), fl
+
+
 def static_flags(masks, distance, pair_frames=None, pair_offsets=None, pair_locs=None, trip_frames=None, trip_offsets=None, trip_locs=None, want_distance=False, device=0):
     """rcvd_static_flags (FlowConstraintsCollection::setStaticFlagFromDynamicMask + dynamicDistance, reference lib/FlowConstraints.cpp:573-660,
     :257-286) on the GPU.  masks [F,h,w] u8.  Returns (pair_static u8[n], trip_static u8[m], distance images [F,h,w] f32 or None)."""
     m = np.ascontiguousarray(masks, np.uint8); F, h, w = m.shape
-    P = 0 if pair_frames is None else len(pair_frames); T = 0 if trip_frames is None else len(trip_frames)
-    pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2) if P else None
-    po = np.ascontiguousarray(pair_offsets, np.int64) if P else None
-    pl = np.ascontiguousarray(pair_locs, np.float32).reshape(-1, 4) if P else None
-    tf = np.ascontiguousarray(trip_frames, np.int32) if T else None
-    to = np.ascontiguousarray(trip_offsets, np.int64) if T else None
-    tl = np.ascontiguousarray(trip_locs, np.float32).reshape(-1, 6) if T else None
-    ps = np.zeros(int(po[-1]) if P else 0, np.uint8); ts = np.zeros(int(to[-1]) if T else 0, np.uint8)
+    pairs, ps = _flag_family(pair_frames, pair_offsets, pair_locs, 4)
+    trips, ts = _flag_family(trip_frames, trip_offsets, trip_locs, 6)
     dist = np.zeros((F, h, w), np.float32) if want_distance else None
     _check(lib().rcvd_static_flags(C.c_int32(device), _p(m, C.c_uint8), C.c_int32(F), C.c_int32(h), C.c_int32(w), C.c_float(distance),
-                                   C.c_int32(P), _p(pf, C.c_int32), _p(po, C.c_int64), _p(pl, C.c_float), _p(ps if P else None, C.c_uint8),
-                                   C.c_int32(T), _p(tf, C.c_int32), _p(to, C.c_int64), _p(tl, C.c_float), _p(ts if T else None, C.c_uint8), _p(dist, C.c_float)))
+                                   *pairs, *trips, _p(dist, C.c_float)))
     return ps, ts, dist
 
 
@@ -441,18 +447,10 @@ def prune_static_flags(num_frames, height, width, distance, pair_frames, pair_of
     """rcvd_prune_static_flags (FlowConstraintsCollection::pruneStaticFlag, reference lib/FlowConstraints.cpp:662-748) on the GPU.
     height x width: the "down" stream's size.  Arrays as in static_flags; pair_static / trip_static are the input flags (not modified).
     Returns the pruned (pair_static u8[n], trip_static u8[m])."""
-    P = len(pair_frames); T = 0 if trip_centres is None else len(trip_centres)
-    pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2) if P else None
-    po = np.ascontiguousarray(pair_offsets, np.int64) if P else None
-    pl = np.ascontiguousarray(pair_locs, np.float32).reshape(-1, 4) if P else None
-    ps = np.array(pair_static, np.uint8).reshape(-1) if P else np.zeros(0, np.uint8)
-    tc = np.ascontiguousarray(trip_centres, np.int32) if T else None
-    to = np.ascontiguousarray(trip_offsets, np.int64) if T else None
-    tl = np.ascontiguousarray(trip_locs, np.float32).reshape(-1, 6) if T else None
-    ts = np.array(trip_static, np.uint8).reshape(-1) if T else np.zeros(0, np.uint8)
+    pairs, ps = _flag_family(pair_frames, pair_offsets, pair_locs, 4, pair_static)
+    trips, ts = _flag_family(trip_centres, trip_offsets, trip_locs, 6, trip_static)
     _check(lib().rcvd_prune_static_flags(C.c_int32(device), C.c_int32(num_frames), C.c_int32(height), C.c_int32(width), C.c_int32(distance),
-                                         C.c_int32(P), _p(pf, C.c_int32), _p(po, C.c_int64), _p(pl, C.c_float), _p(ps if P else None, C.c_uint8),
-                                         C.c_int32(T), _p(tc, C.c_int32), _p(to, C.c_int64), _p(tl, C.c_float), _p(ts if T else None, C.c_uint8)))
+                                         *pairs, *trips))
     return ps, ts
 
 
