@@ -44,7 +44,13 @@ PYBIND11_MODULE(lib_python, m) {
       .def_readwrite("orientation", &Extrinsics::orientation)
       .def("left", [](const Extrinsics& e) { return vec3ToNp(e.left()); }).def("right", [](const Extrinsics& e) { return vec3ToNp(e.right()); })
       .def("down", [](const Extrinsics& e) { return vec3ToNp(e.down()); }).def("up", [](const Extrinsics& e) { return vec3ToNp(e.up()); })
-      .def("forward", [](const Extrinsics& e) { return vec3ToNp(e.forward()); }).def("backward", [](const Extrinsics& e) { return vec3ToNp(e.backward()); });
+      .def("forward", [](const Extrinsics& e) { return vec3ToNp(e.forward()); }).def("backward", [](const Extrinsics& e) { return vec3ToNp(e.backward()); })
+      .def("worldToCamera", [](const Extrinsics& e) {
+        const std::array<float, 16> M = e.worldToCamera();
+        py::array_t<float> a({4, 4}); std::memcpy(a.mutable_data(), M.data(), sizeof(M)); return a; })
+      .def_static("fromWorldToCamera", [](py::array_t<float, py::array::c_style | py::array::forcecast> a) {
+        if (a.ndim() != 2 || a.shape(0) != 4 || a.shape(1) != 4) throw std::runtime_error("Expected a 4x4 matrix.");
+        std::array<float, 16> M; std::memcpy(M.data(), a.data(), sizeof(M)); return Extrinsics::fromWorldToCamera(M); });
   py::class_<Intrinsics>(m, "Intrinsics")
       .def(py::init<>())
       .def_readwrite("vFov", &Intrinsics::vFov).def_readwrite("hFov", &Intrinsics::hFov)
@@ -77,6 +83,10 @@ PYBIND11_MODULE(lib_python, m) {
       .def("warp", [](const Xform& x, int h, int w) { Image im = x.warp(h, w); return imageToNp(&im); });
   m.attr("DepthXform") = m.attr("Xform");
   m.attr("SpatialXform") = m.attr("Xform");
+  m.def("computeDepthRange", [](py::array_t<float, py::array::c_style | py::array::forcecast> a) {
+    if (a.ndim() != 2) throw std::runtime_error("Depth image must be a 2-D float32 array.");
+    const std::pair<float, float> r = computeDepthRange(a.data(), size_t(a.size()));
+    return py::make_tuple(r.first, r.second); });
 
   py::class_<ColorFrame>(m, "ColorFrame").def("image", [](ColorFrame& f) { return imageToNp(f.image()); });
   py::class_<ColorStream>(m, "ColorStream")
@@ -92,6 +102,7 @@ PYBIND11_MODULE(lib_python, m) {
         std::memcpy(img.ptr<float>(), a.data(), size_t(a.shape(0)) * a.shape(1) * sizeof(float));
         f.setDepth(img);
       })
+      .def("warp", [](DepthFrame& f) { return imageToNp(f.warp()); })
       .def("clear", &DepthFrame::clear)
       .def("clearCache", &DepthFrame::clearCache).def("clearXformedCache", &DepthFrame::clearXformedCache)
       .def("depthXform", [](DepthFrame& f) -> Xform& { return f.depthXform(); }, py::return_value_policy::reference)
@@ -107,11 +118,15 @@ PYBIND11_MODULE(lib_python, m) {
       .def("width", &DepthStream::width).def("height", &DepthStream::height).def("setDir", &DepthStream::setDir)
       .def("resetDepthXforms", &DepthStream::resetDepthXforms).def("resetSpatialXforms", &DepthStream::resetSpatialXforms).def("clearCache", &DepthStream::clearCache);
 
+  py::class_<MetaFrame>(m, "MetaFrame").def("pts", &MetaFrame::pts);
   py::class_<DepthVideo>(m, "DepthVideo")
       .def(py::init<>())
+      .def("reset", &DepthVideo::reset)
       .def("printInfo", &DepthVideo::printInfo).def("save", &DepthVideo::save).def("load", &DepthVideo::load).def("saveDepth", &DepthVideo::saveDepth)
       .def("width", &DepthVideo::width).def("height", &DepthVideo::height).def("aspect", &DepthVideo::aspect).def("invAspect", &DepthVideo::invAspect)
       .def("path", &DepthVideo::path).def("numFrames", &DepthVideo::numFrames)
+      .def("frame", &DepthVideo::frame).def("duration", &DepthVideo::duration).def("timeToFrame", &DepthVideo::timeToFrame).def("time", &DepthVideo::time)
+      .def("colorFrame", &DepthVideo::colorFrame, py::return_value_policy::reference)
       .def("numColorStreams", &DepthVideo::numColorStreams).def("hasColorStream", &DepthVideo::hasColorStream).def("colorStreamIndex", &DepthVideo::colorStreamIndex)
       .def("colorStream", [](DepthVideo& v, int i) -> ColorStream& { return v.colorStream(i); }, py::return_value_policy::reference)
       .def("colorStream", [](DepthVideo& v, const std::string& n) -> ColorStream& { return v.colorStream(n); }, py::return_value_policy::reference)
@@ -176,7 +191,8 @@ PYBIND11_MODULE(lib_python, m) {
   py::class_<DepthVideoImporter>(m, "DepthVideoImporter")
       .def_static("importVideo", [](DepthVideo& v, const std::string& path, bool discover) { importVideo(v, path, discover); })
       .def_static("importPoses", &importPoses).def_static("loadScale", &loadScale)
-      .def_static("importColmapDepth", &importColmapDepth).def_static("importColmapRecon", &importColmapRecon);
+      .def_static("importColmapDepth", &importColmapDepth).def_static("importColmapRecon", &importColmapRecon)
+      .def_static("importTracks", &importTracks);
 
   py::enum_<StaticLossType>(m, "StaticLossType").value("Euclidean", StaticLossType::Euclidean).value("ReproDisparity", StaticLossType::ReproDisparity)
       .value("ReproDepthRatio", StaticLossType::ReproDepthRatio).value("ReproLogDepth", StaticLossType::ReproLogDepth);

@@ -10,6 +10,7 @@
 #include <filesystem>
 #include <fstream>
 #include <iostream>
+#include <limits>
 #include <sstream>
 #include <stdexcept>
 #include <sys/stat.h>
@@ -284,6 +285,17 @@ Image Xform::apply(const Image& src) const {
   return out;
 }
 
+// The reference starts the maximum at numeric_limits<float>::min(), the smallest positive normal float, so a range without a valid
+// depth is (FLT_MAX, FLT_MIN) and a maximum below FLT_MIN (a subnormal depth) reads as FLT_MIN; both kept.
+std::pair<float, float> computeDepthRange(const float* depth, size_t count) {
+  float lo = std::numeric_limits<float>::max(), hi = std::numeric_limits<float>::min();
+  for (size_t i = 0; i < count; ++i) {
+    const float d = depth[i];
+    if (std::isfinite(d) && d > 0) { lo = std::min(d, lo); hi = std::max(d, hi); }
+  }
+  return {lo, hi};
+}
+
 // --- Intrinsics::resolveMissingFov (lib/DepthPhoto.cpp:114-158) ---
 void Intrinsics::resolveMissingFov(float aspect) {
   bool vSet = vFov > 0, hSet = hFov > 0;
@@ -294,6 +306,32 @@ void Intrinsics::resolveMissingFov(float aspect) {
   if (!vSet && !hSet) { if (aspect > defaultAspect) { vFov = kDefaultVFov; vSet = true; } else { hFov = kDefaultHFov; hSet = true; } }
   if (vSet) { const float hh = std::tan(vFov / 2.0f); hFov = std::atan(hh * aspect) * 2.0f; }
   else if (hSet) { const float hw = std::tan(hFov / 2.0f); vFov = std::atan(hw / aspect) * 2.0f; }
+}
+
+// --- Extrinsics::worldToCamera / fromWorldToCamera (lib/DepthPhoto.cpp:63-99), row-major 4x4 ---
+// rotate * translate: the rows of rotate are the camera's right, up and backward vectors (orientation times the unit axes), and
+// translate moves the position to the origin, so the last column is rotate times -position.
+std::array<float, 16> Extrinsics::worldToCamera() const {
+  const Vec3f rows[3] = {right(), up(), backward()};
+  std::array<float, 16> M{};
+  for (int i = 0; i < 3; ++i) {
+    const Vec3f& r = rows[i];
+    M[4 * i] = r.x; M[4 * i + 1] = r.y; M[4 * i + 2] = r.z;
+    M[4 * i + 3] = r.x * -position.x + r.y * -position.y + r.z * -position.z;
+  }
+  M[15] = 1.f;
+  return M;
+}
+// The upper 3x3 block R is taken as the rotation; the position is -(Rᵀ t) for the last column t, the orientation Quaternionf(Rᵀ).
+Extrinsics Extrinsics::fromWorldToCamera(const std::array<float, 16>& W) {
+  float Rt[3][3], q[4];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rt[i][j] = W[4 * j + i];
+  Extrinsics e;
+  e.position = {-(Rt[0][0] * W[3] + Rt[0][1] * W[7] + Rt[0][2] * W[11]), -(Rt[1][0] * W[3] + Rt[1][1] * W[7] + Rt[1][2] * W[11]),
+                -(Rt[2][0] * W[3] + Rt[2][1] * W[7] + Rt[2][2] * W[11])};
+  matrixToQuat(Rt, q);
+  e.orientation.x = q[0]; e.orientation.y = q[1]; e.orientation.z = q[2]; e.orientation.w = q[3];
+  return e;
 }
 
 // --- streams / frames ---
@@ -360,7 +398,16 @@ void DepthFrame::setDepth(const Image& depth) {
   if (depth.type != cvMakeType(CV_32F, 1)) throw std::runtime_error("Depth image has incorrect type.");
   if (stream_.width_ < 0) { stream_.width_ = depth.cols; stream_.height_ = depth.rows; }
   else if (stream_.width_ != depth.cols || stream_.height_ != depth.rows) throw std::runtime_error("Depth frame has inconsistent dimensions.");
-  source_ = std::make_unique<Image>(depth); sourceLoaded_ = true; xformed_.reset(); medianValid_ = false;
+  source_ = std::make_unique<Image>(depth); sourceLoaded_ = true; clearXformedCache(); medianValid_ = false;
+}
+const Image* DepthFrame::warp() {
+  if (!warp_ || spatialXform_->desc() != warpDesc_ || spatialXform_->params() != warpParams_) {
+    const int h = stream_.height(), w = stream_.width();
+    if (h <= 0 || w <= 0) throw std::runtime_error("Depth stream '" + stream_.name() + "' has no known size: it has neither depth files nor a size given at creation.");
+    warp_ = std::make_unique<Image>(spatialXform_->warp(h, w));
+    warpDesc_ = spatialXform_->desc(); warpParams_ = spatialXform_->params();
+  }
+  return warp_.get();
 }
 float DepthFrame::sourceDepthMedian() {
   if (!medianValid_) {
@@ -392,6 +439,17 @@ void DepthVideo::init(const std::string& path, int width, int height, const std:
   path_ = path; pts_ = pts; width_ = width; height_ = height;
   aspect_ = width / float(height); invAspect_ = 1.f / aspect_;
   duration_ = pts_.empty() ? 0.f : pts_.back() * pts_.size() / float(pts_.size() - 1);
+}
+void DepthVideo::reset() {   // the width and height stay, as in the reference
+  path_.clear(); pts_.clear(); colorStreams_.clear(); depthStreams_.clear();
+  duration_ = 0.f; aspect_ = 0.f; invAspect_ = 0.f;
+}
+int DepthVideo::timeToFrame(float time) const {
+  if (pts_.empty()) throw std::runtime_error("Video has no frames.");
+  if (time < pts_[0]) throw std::runtime_error("Query time before first frame's time.");
+  if (time > duration_) throw std::runtime_error("Query time after video duration.");
+  for (size_t i = 0; i + 1 < pts_.size(); ++i) if (time >= pts_[i] && time < pts_[i + 1]) return int(i);
+  return numFrames() - 1;
 }
 bool DepthVideo::hasColorStream(const std::string& n) const { for (auto& s : colorStreams_) if (s->name_ == n) return true; return false; }
 int DepthVideo::colorStreamIndex(const std::string& n) const { for (size_t i = 0; i < colorStreams_.size(); ++i) if (colorStreams_[i]->name_ == n) return int(i); throw std::runtime_error("Color stream '" + n + "' not found."); }
@@ -516,6 +574,13 @@ void DepthVideo::saveDepth(int stream) {
     }
   }
 }
+// Entries of a directory sorted by name: std::filesystem (like boost::filesystem in the reference) iterates in no specified order.
+static std::vector<fs::directory_entry> sortedEntries(const std::string& dir) {
+  std::vector<fs::directory_entry> v{fs::directory_iterator(dir), fs::directory_iterator()};
+  std::sort(v.begin(), v.end(), [](const fs::directory_entry& a, const fs::directory_entry& b) { return a.path().filename() < b.path().filename(); });
+  return v;
+}
+
 void importVideo(DepthVideo& video, const std::string& path, bool discoverStreams) {
   logInfo("Importing 3D video '" + path + "'...");
   std::ifstream is(path + "/frames.txt", std::ios::binary);
@@ -529,14 +594,70 @@ void importVideo(DepthVideo& video, const std::string& path, bool discoverStream
     pts[i] = p;
   }
   video.init(path, w, h, pts);
-  if (discoverStreams) throw std::runtime_error("Stream discovery is not supported in this build (pose_optimization.py passes discoverStreams=False).");
-}
+  if (!discoverStreams) return;
 
-// Entries of a directory sorted by name: std::filesystem (like boost::filesystem in the reference) iterates in no specified order.
-static std::vector<fs::directory_entry> sortedEntries(const std::string& dir) {
-  std::vector<fs::directory_entry> v{fs::directory_iterator(dir), fs::directory_iterator()};
-  std::sort(v.begin(), v.end(), [](const fs::directory_entry& a, const fs::directory_entry& b) { return a.path().filename() < b.path().filename(); });
-  return v;
+  // Stream discovery (:39-195), in the reference's order.  Fixed colour streams first: directory, stream name, extension, type.
+  logInfo("  Discovering color streams...");
+  struct FixedStream { const char *dir, *name, *ext; int type; };
+  static const FixedStream kFixed[] = {{"color_full", "full", ".png", cvMakeType(CV_32F, 3)}, {"color_down", "down", ".raw", cvMakeType(CV_32F, 3)},
+                                       {"color_down_png", "down_png", ".png", cvMakeType(CV_32F, 3)}, {"dynamic_mask", "dynamic_mask", ".png", cvMakeType(CV_8U, 1)}};
+  for (const FixedStream& c : kFixed)
+    if (fs::is_directory(path + "/" + c.dir)) { logInfo(std::string("    Found color stream '") + c.dir + "'."); video.createColorStream(c.name, c.dir, c.ext, c.type, {-1, -1}); }
+  // Then every other subdirectory with a stream_info.txt of type "color".  Like the reference, a directory is skipped when its name
+  // equals a fixed stream's name (not its directory).  Sorted by name, which is the reference's full-path order.
+  for (const fs::directory_entry& e : sortedEntries(path)) {
+    if (!e.is_directory()) continue;
+    const std::string rel = fs::relative(e.path(), path).string();
+    if (std::any_of(std::begin(kFixed), std::end(kFixed), [&](const FixedStream& c) { return rel == c.name; })) continue;
+    const std::string infoFile = e.path().string() + "/stream_info.txt";
+    if (!fs::exists(infoFile)) continue;
+    std::ifstream info(infoFile, std::ios::binary);
+    if (info.fail()) throw std::runtime_error("Could not open frame file.");   // the reference's message
+    std::string type, ext, format; info >> type;
+    if (type != "color") continue;
+    info >> ext >> format;
+    int cvType;
+    if (format == "32FC3") cvType = cvMakeType(CV_32F, 3);
+    else if (format == "8UC1") cvType = cvMakeType(CV_8U, 1);
+    else throw std::runtime_error("Invalid format string.");
+    logInfo("    Found color stream '" + rel + "' (" + ext + ", " + format + ").");
+    video.createColorStream(rel, rel, ext, cvType, {-1, -1});
+  }
+  // Depth streams: every directory below the video with a depth/ subdirectory (not descended into), in sorted relative-path order.
+  logInfo("  Discovering depth streams...");
+  std::vector<std::string> depthStreams;
+  std::function<void(const std::string&)> visit = [&](const std::string& dir) {
+    for (const fs::directory_entry& e : sortedEntries(dir)) {
+      if (!e.is_directory()) continue;
+      if (fs::is_directory(e.path() / "depth")) depthStreams.push_back(fs::relative(e.path(), path).string());
+      else visit(e.path().string());
+    }
+  };
+  visit(path);
+  std::sort(depthStreams.begin(), depthStreams.end());
+  for (const std::string& s : depthStreams) {
+    logInfo("    Found depth stream '" + s + "'.");
+    if (s == "depth_colmap_dense") {   // COLMAP's depth is scaled into depth_colmap_dense_imported, which the stream then reads
+      importColmapDepth(video);
+      video.createDepthStream(s, "depth_colmap_dense_imported", {-1, -1});
+    } else if (s != "depth_colmap_dense_imported") {
+      video.createDepthStream(s, s, {-1, -1});
+      const std::string posesFile = path + "/" + s + "/poses.txt";
+      if (fs::exists(posesFile)) importPoses(video, posesFile, video.numDepthStreams() - 1);
+    }
+  }
+  // The first COLMAP reconstruction found sets the cameras of every depth stream.
+  for (const std::string& npz : {path + "/metadata.npz", path + "/colmap_dense/metadata.npz"}) {
+    if (!fs::is_regular_file(npz)) continue;
+    logInfo("  Importing COLMAP reconstruction from '" + npz + "'...");
+    for (int s = 0; s < video.numDepthStreams(); ++s) importColmapRecon(video, npz, s, false);
+    break;
+  }
+  const std::string trackFile = path + "/track2d.csv";
+  if (fs::is_regular_file(trackFile)) {
+    logInfo("  Importing tracks from '" + trackFile + "'...");
+    importTracks(video, trackFile);
+  }
 }
 
 void importPoses(DepthVideo& video, const std::string& posesFile, int stream) {
@@ -656,6 +777,50 @@ void importColmapRecon(DepthVideo& video, const std::string& npzFile, int stream
     ds.frame(frames[i]).intrinsics = in;
     if (!silent) { char b[160]; snprintf(b, sizeof(b), "  Frame %d: fx %g fy %g -> hFov %g vFov %g", frames[i], fx, fy, in.hFov, in.vFov); logInfo(b); }
   }
+}
+
+// track2d.csv: one "frame, track, x, y" line per observation in pixels of the "full" stream, frames in non-decreasing order.  Both
+// coordinates are divided by the image width.  A line without four fields is reported and skipped; any other line parses with atoi /
+// atof as in the reference, so a header line is an observation of track 0 at frame 0 at (0, 0).  (The reference trims each field
+// first; atoi and atof skip leading white space and stop at trailing white space, so that changes nothing.)  Where the reference
+// asserts or indexes before its first frame -- an observation that is not on the frame after its track's last one, a negative frame --
+// a RuntimeError is raised and no file is written.
+void importTracks(DepthVideo& video, const std::string& trackFile) {
+  std::ifstream f(trackFile);
+  if (f.fail()) throw std::runtime_error("Cannot open track file.");
+  const Image* img = video.colorStream("full").frame(0).image();
+  if (!img) throw std::runtime_error("Color stream 'full' has no image for frame 0, whose width the track coordinates are divided by.");
+  const float w = float(img->cols);
+  DepthVideoTrackTable tt;
+  std::map<int, int> tableId;   // track id in the file -> id in the table
+  int lastFrame = -1;
+  for (std::string line; std::getline(f, line);) {
+    const std::vector<std::string> parts = explode(line, ',');
+    if (parts.size() != 4) { logInfo("ERROR: invalid line '" + line + "'."); continue; }
+    const int frame = std::atoi(parts[0].c_str()), track = std::atoi(parts[1].c_str());
+    const float x = float(std::atof(parts[2].c_str())), y = float(std::atof(parts[3].c_str()));
+    if (frame < lastFrame) throw std::runtime_error("ERROR: Frames not in consecutive order.");
+    if (frame < 0) throw std::runtime_error("Track file '" + trackFile + "' has an observation at frame " + std::to_string(frame) + ".");
+    for (; lastFrame < frame; ++lastFrame) tt.frames.emplace_back();
+    const std::array<float, 2> obs{{x / w, y / w}};
+    const auto it = tableId.find(track);
+    int id;
+    if (it == tableId.end()) {
+      id = tableId[track] = int(tt.tracks.size());
+      tt.tracks.emplace_back();
+      tt.tracks.back().valid = true; tt.tracks.back().firstFrame = frame;
+    } else {
+      id = it->second;
+      const DepthVideoTrack& t = tt.tracks[id];
+      const int next = t.firstFrame + int(t.obs.size());
+      if (frame != next)
+        throw std::runtime_error("Track " + std::to_string(track) + " in '" + trackFile + "' has an observation at frame " + std::to_string(frame) +
+                                 " after its last one at frame " + std::to_string(next - 1) + "; each must follow on the next frame.");
+    }
+    tt.tracks[id].obs.push_back(obs);
+    tt.frames[frame].insert(id);
+  }
+  tt.save(video.path() + "/long_tracks.tracktable");
 }
 
 // --- .npz archives: a zip file (PKWARE APPNOTE) of .npy members, stored (np.savez) or deflated (np.savez_compressed).  numpy writes
