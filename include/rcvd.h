@@ -208,6 +208,43 @@ int32_t rcvd_problem_get_state(rcvd_problem* p, double* params);
 /* Robustified cost 1/2 sum rho(|r|^2) at the current state (ceres cost), and
  * optionally the gradient J^T r (length N*stride, nullable). */
 int32_t rcvd_evaluate(rcvd_problem* p, double* cost, double* gradient);
+/* Per-block residuals and Jacobian rows at the current state: what ceres::Problem::Evaluate gives a
+ * Ceres caller, one residual family at a time.  A family is a list of residual blocks; block b has
+ * m residuals and at most K Jacobian columns:
+ *   RCVD_ROWS_PAIRS         m = 3, one block per static-scene record, in the order of the records of
+ *                           rcvd_problem_set_constraints.  r = the StaticSceneCost residual, static
+ *                           weights applied; rho = the robust loss of robust_type at |r|^2.
+ *   RCVD_ROWS_TRIPLETS      m = 3, one block per record of rcvd_problem_set_triplets, in their order.
+ *                           r = the smoothness residual without its ScaledLoss weight w (record[9]);
+ *                           rho = w |r|^2.
+ *   RCVD_ROWS_DEPTH_PAIRS   m = 1, one block per record of rcvd_problem_set_depth_pairs, in their order.
+ *                           r = 1 / max(D0, 1e-6) - 1 / max(D1, 1e-6); rho as for the pairs.
+ *   RCVD_ROWS_REGULARISERS  m = 1.  For every in-range frame in ascending order: its scale rows (scale
+ *                           lattice x + y*scale_grid_x), its deformation rows (for grid node x + y*gx in
+ *                           ascending order: the edge to node x-1, then the edge to node above, y-1;
+ *                           k components each), its spatial rows (parameter order) and its focal row.
+ *                           Then three position rows (x, y, z) per in-range frame triplet f, f+1, f+2
+ *                           with f ascending.  ScaledLoss weights are in r (x sqrt(w)); rho = |r|^2.
+ * The row layout of each family, in the order above: */
+enum { RCVD_ROWS_PAIRS = 0, RCVD_ROWS_TRIPLETS = 1, RCVD_ROWS_DEPTH_PAIRS = 2, RCVD_ROWS_REGULARISERS = 3, RCVD_ROW_FAMILIES = 4 };
+typedef struct rcvd_row_family {
+  int64_t blocks;       /* residual blocks */
+  int32_t residuals;    /* m: residuals per block */
+  int32_t max_cols;     /* K: column slots per residual */
+} rcvd_row_family;
+struct rcvd_row_layout { rcvd_row_family family[RCVD_ROW_FAMILIES]; };
+/* Fills out->family[RCVD_ROWS_*].  Host only: runs nothing on the device. */
+int32_t rcvd_row_layout(rcvd_problem* p, struct rcvd_row_layout* out);
+/* Evaluates one family's blocks.  Every output is nullable and has one slot per block:
+ *   residuals [blocks][m], rho [blocks],
+ *   cols [blocks][m][K] int32, jac [blocks][m][K]: for residual q of block b, each column slot holds a
+ *   global parameter index (the caller's frame * rcvd_frame_stride + parameter) and dr_q / dparameter,
+ *   without the robust loss; parameters held constant (fix_poses, fix_depth_xforms, fix_spatial_xforms,
+ *   Fixed intrinsics) are left out as in rcvd_evaluate's gradient, and unused slots hold -1 and 0.
+ * With cols and jac both null no Jacobian is formed.  Each block writes only its own slots: two calls at
+ * the same state return identical arrays.  Refused with RCVD_ERR_INVALID before anything runs: a null
+ * handle, an unknown family, cols without jac or jac without cols, a handle with nranks > 1. */
+int32_t rcvd_evaluate_rows(rcvd_problem* p, int32_t family, double* residuals, double* rho, int32_t* cols, double* jac);
 /* Dense copy of the Gauss-Newton normal matrix J^T J at the current state
  * (row-major (N*stride)^2 doubles) -- test/debug entry point for small problems. */
 int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* H);

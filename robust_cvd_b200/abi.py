@@ -97,6 +97,20 @@ class TrackParams(C.Structure):
 
 TRACK_IN_RANGE, TRACK_HAS_COLOR, TRACK_FLOW, TRACK_MASK = 1, 2, 4, 8   # rcvd_compute_tracks frame flags
 
+# residual families of rcvd_evaluate_rows, in the order of rcvd_row_layout::family
+ROWS_PAIRS, ROWS_TRIPLETS, ROWS_DEPTH_PAIRS, ROWS_REGULARISERS = range(4)
+ROW_FAMILIES = ("pairs", "triplets", "depth_pairs", "regularisers")
+
+
+class RowFamily(C.Structure):
+    """rcvd_row_family (include/rcvd.h)."""
+    _fields_ = [("blocks", C.c_int64), ("residuals", C.c_int32), ("max_cols", C.c_int32)]
+
+
+class RowLayout(C.Structure):
+    """struct rcvd_row_layout (include/rcvd.h)."""
+    _fields_ = [("family", RowFamily * len(ROW_FAMILIES))]
+
 
 def default_config(num_frames, aspect, **kw):
     """Config with the reference's Params defaults (lib/PoseOptimizer.h:55-103)."""

@@ -159,6 +159,7 @@ struct RecordSet {
   const int width, nframes;
   std::vector<int32_t> frames; std::vector<int64_t> offsets{0}; std::vector<float> records;
   RecordTiles dev = {}; int num_tiles = 0;
+  const float* caller_records = nullptr;   // the device records in the caller's order (dev.records may be the run path's sorted copy)
   RecordSet(int width_, int nframes_) : width(width_), nframes(nframes_) {}
   int groups() const { return (int)offsets.size() - 1; }
   int64_t count() const { return offsets.back(); }
@@ -312,13 +313,13 @@ static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
     const bool tc = MODE == EvalMode::CostGradH && p->fast_path != 0;   // a tensor-core kernel (rcvd_debug_set_fast_path)
     if (tc && p->fast_path == 1 && p->records_sorted) rc = launch(p, k_accumulate_runs, ntiles, kTile, kRunSmem, st, false, d, x, p->d_H, g, part);
     else if (tc && fast_path_ok(p->cfg, p->L)) rc = launch(p, k_accumulate_fast, ntiles, kTile, kFastSmem, st, false, d, x, p->d_H, g, part);
-    else rc = launch(p, k_pairs<MODE>, ntiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active);
+    else rc = launch(p, k_pairs<MODE>, ntiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active, NoRows{});
     if (rc) return rc;
   }
   if (regblocks > 0 && (rc = launch(p, k_regularisers<MODE>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, g, part + p->part_reg, p->d_active,
-                                    p->first_frame, p->last_frame))) return rc;
-  if (p->trips.num_tiles > 0 && (rc = launch(p, k_triplets<MODE>, p->trips.num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part + p->part_trip, p->d_active))) return rc;
-  if (p->dpairs.num_tiles > 0 && (rc = launch(p, k_depth_pairs<MODE>, p->dpairs.num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part + p->part_dp, p->d_active))) return rc;
+                                    p->first_frame, p->last_frame, NoRows{}))) return rc;
+  if (p->trips.num_tiles > 0 && (rc = launch(p, k_triplets<MODE>, p->trips.num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part + p->part_trip, p->d_active, NoRows{}))) return rc;
+  if (p->dpairs.num_tiles > 0 && (rc = launch(p, k_depth_pairs<MODE>, p->dpairs.num_tiles, kTile, 0, st, false, d, x, p->d_H, g, part + p->part_dp, p->d_active, NoRows{}))) return rc;
   return RCVD_OK;
 }
 
@@ -346,7 +347,7 @@ static int upload_record_set(rcvd_problem* p, RecordSet& s) {
   s.num_tiles = (int)tile_group.size();
   float* rec; int32_t *fr, *tg, *tn; int64_t* tb; int rc;
   UP(rec, s.records); UP(fr, frames); UP(tg, tile_group); UP(tb, tile_begin); UP(tn, tile_count);
-  s.dev = RecordTiles{rec, fr, tg, tb, tn};
+  s.dev = RecordTiles{rec, fr, tg, tb, tn}; s.caller_records = rec;
   return RCVD_OK;
 }
 
@@ -370,7 +371,7 @@ static int set_up_problem_data(rcvd_problem* p) {
     if ((rc = launch(p, k_gather_records, (unsigned)((n * 6 + 255) / 256), 256, 0, p->stream, false, p->pairs.dev.records, d_i1, n, d_sorted))) return rc;
     CK(cudaFreeAsync(d_tmp, p->stream));
     CK(cudaGetLastError());
-    p->pairs.dev.records = d_sorted; p->records_sorted = true;      // (the unsorted copy and the sort buffers go back to the pool with the handle's other allocations)
+    p->pairs.dev.records = d_sorted; p->records_sorted = true;      // (the unsorted copy stays for rcvd_evaluate_rows; it and the sort buffers go back to the pool with the handle's other allocations)
   }
   UP(p->d_in_range, frames_to_internal(uperm, p->in_range.data(), 1, 1, 1));
   UP(p->d_median, frames_to_internal(uperm, p->median.data(), 1, 1, 1));
@@ -1224,6 +1225,147 @@ RCVD_API int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* Hout) {
   cudaStreamSynchronize(p->stream); cudaFree(d_out);
   if (rc) return rc;
   if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "copy failed: %s", cudaGetErrorString(e));
+  return RCVD_OK;
+}
+
+// ---- per-block rows (rcvd_row_layout, rcvd_evaluate_rows) ----
+// Most nodes one gather returns (gather_depth, gather_spatial): a bicubic gather drops the taps beyond the grid's edge.
+static int depth_taps(const rcvd_config& c) {
+  if (c.depth_type == RCVD_DEPTH_IDENTITY) return 0;
+  if (c.depth_type == RCVD_DEPTH_GLOBAL) return 1;
+  return c.depth_cubic ? std::min(4, c.depth_grid_x) * std::min(4, c.depth_grid_y) : 4;
+}
+static int spatial_taps(const rcvd_config& c) {
+  switch (c.spatial_type) {
+    case RCVD_SPATIAL_VERTICAL_LINEAR: return 2;
+    case RCVD_SPATIAL_CORNERS_BILINEAR: case RCVD_SPATIAL_BILINEAR_GRID: return 4;
+    case RCVD_SPATIAL_BICUBIC_GRID: return std::min(4, c.spatial_grid_x) * std::min(4, c.spatial_grid_y);
+    default: return 0;
+  }
+}
+// The regulariser rows in the CPU oracle's order: every in-range frame in the caller's order with its scale rows, its deformation rows
+// (grid node x + y*gx after node: the edge to the node on its left, then to the node above, k components each), its spatial rows and
+// its focal row; then three position rows per frame triplet (f, f+1, f+2) that k_regularisers evaluates.  Returns the number of rows;
+// slot (optional) receives the row of every k_regularisers row id, -1 where the id has none.  uperm: internal -> the caller's frame.
+static int64_t regulariser_rows(const rcvd_problem* p, const std::vector<int>& uperm, std::vector<int32_t>* slot) {
+  const rcvd_config& c = p->cfg; const Layout& L = p->L; const int N = p->N;
+  const RegCounts rc = reg_counts(c, L, N, std::max(0, c.scale_grid_x) * std::max(0, c.scale_grid_y));
+  std::vector<int> deform(rc.deform);      // kernel order (the horizontal edges, then the vertical ones) -> the oracle's
+  if (rc.deform > 0) {
+    const int gx = c.depth_grid_x, gy = c.depth_grid_y, nh = (gx - 1) * gy; int q = 0;
+    for (int y = 0; y < gy; ++y) for (int x = 0; x < gx; ++x) {
+      if (x > 0) for (int j = 0; j < L.k; ++j) deform[(y * (gx - 1) + x - 1) * L.k + j] = q++;
+      if (y > 0) for (int j = 0; j < L.k; ++j) deform[(nh + (y - 1) * gx + x) * L.k + j] = q++;
+    }
+  }
+  std::vector<int> rank(N, -1); int nin = 0, first = -1, last = -1;
+  for (int u = 0; u < N; ++u) if (p->in_range[u]) { rank[u] = nin++; if (first < 0) first = u; last = u; }
+  if (slot) slot->assign(rc.total, -1);
+  for (int i = 0; i < N && slot; ++i) {
+    const int u = uperm[i];
+    if (rank[u] < 0) continue;
+    for (int k = 0; k < rc.per_frame; ++k) {
+      const int d = k - rc.scale;
+      (*slot)[(size_t)i * rc.per_frame + k] = rank[u] * rc.per_frame + ((d >= 0 && d < rc.deform) ? rc.scale + deform[d] : k);
+    }
+  }
+  int64_t n = (int64_t)nin * rc.per_frame;
+  // k_regularisers' test on internal frames f (position rows keep the caller's frame order: make_factor_plan at one rank)
+  auto in = [&](int f) { return p->in_range[uperm[f]] != 0; };
+  for (int f = 0; rc.position_rows > 0 && f < N - 2; ++f) {
+    if (f < first || f >= last - 1 || !in(f) || !in(f + 1) || !in(f + 2)) continue;
+    for (int i = 0; i < 3; ++i) { if (slot) (*slot)[(size_t)rc.per_frame * N + 3 * f + i] = (int32_t)n; ++n; }
+  }
+  return n;
+}
+static rcvd_row_family row_family(const rcvd_problem* p, int family) {
+  const rcvd_config& c = p->cfg; const Layout& L = p->L;
+  const int depth = c.fix_depth_xforms ? 0 : depth_taps(c) * L.k, spatial = c.fix_spatial_xforms ? 0 : spatial_taps(c) * 2;
+  const int frame = (c.fix_poses ? 0 : 6) + (c.intr_opt == RCVD_INTR_PER_FRAME ? 1 : 0) + depth + spatial;   // columns of one frame
+  const int shared = c.intr_opt == RCVD_INTR_SHARED ? 1 : 0;
+  switch (family) {
+    case RCVD_ROWS_PAIRS: return {p->pairs.count(), 3, 2 * frame + shared};
+    case RCVD_ROWS_TRIPLETS: return {p->trips.count(), 3, 3 * frame + shared};
+    case RCVD_ROWS_DEPTH_PAIRS: return {p->dpairs.count(), 1, 2 * depth};
+    default: {
+      std::vector<int> identity(p->N);
+      for (int i = 0; i < p->N; ++i) identity[i] = i;
+      const RegCounts rc = reg_counts(c, L, p->N, std::max(0, c.scale_grid_x) * std::max(0, c.scale_grid_y));
+      int K = 0;   // scale rows: the nodes of one depth gather; deformation: two nodes; spatial, focal: one parameter; position: three
+      if (rc.scale) K = std::max(K, depth);
+      if (rc.deform && !c.fix_depth_xforms) K = std::max(K, 2);
+      if (rc.spatial && !c.fix_spatial_xforms) K = std::max(K, 1);
+      if (rc.focal) K = std::max(K, 1);
+      if (rc.position_rows && !c.fix_poses) K = std::max(K, 3);
+      return {regulariser_rows(p, identity, nullptr), 1, K};
+    }
+  }
+}
+static int check_rows_handle(const rcvd_problem* p) {
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  if (p->nranks > 1) return set_err(RCVD_ERR_INVALID, "rows of a sharded problem (nranks > 1) are not available");
+  return RCVD_OK;
+}
+// Launches the family's kernel in the Rows mode: from the caller's record order (not the run path's sorted copy), at the current state.
+static int enqueue_rows(rcvd_problem* p, int family, bool jac, const RowOut& o) {
+  DevProblem d = dev_problem(p);
+  d.pairs.records = p->pairs.caller_records;
+  const double* x = p->d_x; cudaStream_t st = p->stream;
+  switch (family) {
+    case RCVD_ROWS_PAIRS:
+      return launch(p, jac ? k_pairs<EvalMode::Rows, true> : k_pairs<EvalMode::Rows, false>, p->pairs.num_tiles, kTile, 0, st, false,
+                    d, x, nullptr, nullptr, nullptr, nullptr, o);
+    case RCVD_ROWS_TRIPLETS:
+      return launch(p, jac ? k_triplets<EvalMode::Rows, true> : k_triplets<EvalMode::Rows, false>, p->trips.num_tiles, kTile, 0, st, false,
+                    d, x, nullptr, nullptr, nullptr, nullptr, o);
+    case RCVD_ROWS_DEPTH_PAIRS:
+      return launch(p, jac ? k_depth_pairs<EvalMode::Rows, true> : k_depth_pairs<EvalMode::Rows, false>, p->dpairs.num_tiles, kTile, 0, st, false,
+                    d, x, nullptr, nullptr, nullptr, nullptr, o);
+    default:
+      return launch(p, jac ? k_regularisers<EvalMode::Rows, true> : k_regularisers<EvalMode::Rows, false>, p->part_trip - p->part_reg, 128, 0, st,
+                    false, d, reg_counts(p->cfg, p->L, p->N, p->nscale), x, nullptr, nullptr, nullptr, nullptr, p->first_frame, p->last_frame, o);
+  }
+}
+RCVD_API int32_t rcvd_row_layout(rcvd_problem* p, struct rcvd_row_layout* out) {
+  if (int rc = check_rows_handle(p)) return rc;
+  if (!out) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int f = 0; f < RCVD_ROW_FAMILIES; ++f) out->family[f] = row_family(p, f);
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_evaluate_rows(rcvd_problem* p, int32_t family, double* residuals, double* rho, int32_t* cols, double* jac) {
+  if (int rc = check_rows_handle(p)) return rc;
+  if (family < 0 || family >= RCVD_ROW_FAMILIES) return set_err(RCVD_ERR_INVALID, "unknown row family %d", family);
+  if ((cols == nullptr) != (jac == nullptr)) return set_err(RCVD_ERR_INVALID, "cols and jac go together: pass both or neither");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  rcvd_row_family fam = row_family(p, family);
+  std::vector<int32_t> slot;
+  if (family == RCVD_ROWS_REGULARISERS) fam.blocks = regulariser_rows(p, p->plan.uperm, &slot);
+  if (fam.blocks == 0) return RCVD_OK;
+  const bool want_jac = jac != nullptr;
+  const size_t nb = (size_t)fam.blocks, nr = nb * fam.residuals, nj = want_jac ? nr * fam.max_cols : 0;
+  // one device buffer: r [nr] | rho [nb] | jac [nj] | cols [nj] | regulariser slots
+  char* buf = nullptr;
+  CK(cudaMallocAsync((void**)&buf, std::max<size_t>((nr + nb + nj) * sizeof(double) + (nj + slot.size()) * sizeof(int32_t), 8), p->stream));
+  RowOut o;
+  o.r = (double*)buf; o.rho = o.r + nr; o.jac = o.rho + nb; o.cols = (int32_t*)(o.jac + nj);
+  o.K = fam.max_cols; o.uperm = p->d_uperm; o.slot = o.cols + nj;
+  auto run = [&]() -> int {
+    if (!slot.empty()) CK(cudaMemcpyAsync((void*)o.slot, slot.data(), slot.size() * sizeof(int32_t), cudaMemcpyHostToDevice, p->stream));
+    if (int rc2 = enqueue_rows(p, family, want_jac, o)) return rc2;
+    if (residuals) CK(cudaMemcpyAsync(residuals, o.r, nr * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    if (rho) CK(cudaMemcpyAsync(rho, o.rho, nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    if (want_jac) {
+      CK(cudaMemcpyAsync(jac, o.jac, nj * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+      CK(cudaMemcpyAsync(cols, o.cols, nj * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
+    }
+    return RCVD_OK;
+  };
+  rc = run();
+  cudaFreeAsync(buf, p->stream);
+  const cudaError_t e = cudaStreamSynchronize(p->stream);
+  if (rc) return rc;
+  if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "rcvd_evaluate_rows: %s", cudaGetErrorString(e));
   return RCVD_OK;
 }
 // factorisation + solve of (S H S + diag(D2)) y = b with the H blocks already on the device; S == nullptr: S = 1

@@ -1,7 +1,8 @@
 // rcvd_eval.cuh -- residual / Jacobian / normal-equation evaluation kernels.
 //
 // Each residual family runs in one of the modes of EvalMode: the cost alone (LM step acceptance), cost + gradient (the bounded
-// line search), cost + gradient + normal matrix, or marking the parameters its rows reference (the active mask).
+// line search), cost + gradient + normal matrix, marking the parameters its rows reference (the active mask), or writing every
+// residual block's rows to its own slot of a RowOut (rcvd_evaluate_rows).
 //   k_pairs<MODE>        : flow constraints, StaticSceneCost residual + analytic Jacobian + Cauchy correction + scatter of J^T J
 //                          and J^T r (reference hot loop D, lib/PoseOptimizer.cpp:237-308 evaluated by Ceres autodiff at :1198);
 //                          every transform / intrinsics mode
@@ -11,6 +12,7 @@
 //   k_depth_pairs<MODE>  : pairwise depth normalisation, DisparityDissimilarityCost rows (:425-462, added at :1005-1095)
 // The partial costs of all families meet in one deterministic two-stage reduction (k_reduce_partials).
 #pragma once
+#include <type_traits>
 #include "rcvd_device.cuh"
 #include "rcvd_ptx.cuh"
 
@@ -18,7 +20,23 @@ namespace rcvd {
 
 constexpr int kTile = 128;          // constraints per CTA tile (all from one group: a directed pair or a triplet centre)
 
-enum class EvalMode { Cost, CostGrad, CostGradH, MarkActive };
+enum class EvalMode { Cost, CostGrad, CostGradH, MarkActive, Rows };
+
+// Output of the Rows mode.  Block b of a family (its slot: the caller's record order, or the regulariser row order of
+// rcvd_row_layout) owns r[b*m .. b*m+m) and rho[b]: the unrobustified residual and rho(|r|^2) of the block's loss.  With the
+// Jacobian (the kernels' JAC flag) row i = b*m + q also owns K column slots cols / jac[i*K .. i*K+K): the global column (the caller's
+// frame * nf + local parameter) and dr_q / dx of every non-constant parameter the block reaches, then index -1 and value 0.
+struct RowOut {
+  double* r; double* rho; int32_t* cols; double* jac;
+  int K;
+  const int32_t* uperm;   // internal frame -> the caller's frame
+  const int32_t* slot;    // k_regularisers: kernel row id -> block slot, -1 where the id has no row
+  __device__ __forceinline__ void col(size_t row, int e, int32_t c, double v) const { cols[row * K + e] = c; jac[row * K + e] = v; }
+  __device__ __forceinline__ void pad(size_t row, int e) const { for (; e < K; ++e) col(row, e, -1, 0.0); }
+};
+// The last kernel parameter: a RowOut in the Rows mode, an empty struct in the others.
+struct NoRows {};
+template <EvalMode MODE> using RowArg = typename std::conditional<MODE == EvalMode::Rows, RowOut, NoRows>::type;
 
 // One constraint family on the device: groups of consecutive records (a group is a directed frame pair, or a triplet's centre
 // frame), cut into tiles of <= kTile records of one group.  Tile t is CTA t of the family's kernel.
@@ -110,23 +128,15 @@ __device__ __forceinline__ void block_store_sum(double v, double* partial) {
   }
 }
 
-// Column expansion and scatter of one row block over NF frames fr[] (pair constraints NF = 2, smoothness triplets NF = 3).
-// Jl: the 3 x 10 NF local Jacobian (per frame: pose 6, focal, depth D, warp 2), r the residual, sc its scale.  Every column a
-// parameter sees becomes (frame, local column, 3-vector) -- pose, PerFrame focal, depth nodes (x src; the offset too when k = 2),
-// spatial nodes, then the shared focal -- and g += J^T r, with WANT_H also H += J^T J (lower triangle, add_h).
-template <int NF, bool WANT_H>
-__device__ __forceinline__ void scatter_columns(const DevProblem& p, const int* fr, const float* __restrict__ rec, const Gather* dg, const Gather* sg,
-                                                const double* Jl, const double* r, double sc, double* __restrict__ H, double* __restrict__ g) {
+// Column expansion of one row block over NF frames fr[] (pair constraints NF = 2, smoothness triplets NF = 3).  Jl: the 3 x 10 NF
+// local Jacobian (per frame: pose 6, focal, depth D, warp 2).  Every column a parameter sees goes to push(frame, local column,
+// 3-vector), constant parameters included -- pose, PerFrame focal, depth nodes (x src; the offset too when k = 2), spatial nodes,
+// then the shared focal.
+template <int NF, class Push>
+__device__ __forceinline__ void for_each_column(const DevProblem& p, const int* fr, const float* __restrict__ rec, const Gather* dg, const Gather* sg,
+                                                const double* Jl, Push&& push) {
   constexpr int ld = 10 * NF;           // Jacobian row stride
-  constexpr int kMaxCols = 72 * NF;     // NF (6 + 1 + 16*2 + 16*2) + the shared focal, with slack
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
-  const double r0 = r[0] * sc, r1 = r[1] * sc, r2 = r[2] * sc;
-  int ef[kMaxCols]; short el[kMaxCols]; double ej[kMaxCols][3];
-  int E = 0;
-  auto push = [&](int f, int l, double a0, double a1, double a2) {
-    if (is_const_local(c, L, l)) return;
-    ef[E] = f; el[E] = (short)l; ej[E][0] = a0 * sc; ej[E][1] = a1 * sc; ej[E][2] = a2 * sc; ++E;
-  };
   for (int side = 0; side < NF; ++side) {
     const int f = fr[side], o = side * 10;
     const double src = (double)rec[3 * side + 2];
@@ -148,11 +158,45 @@ __device__ __forceinline__ void scatter_columns(const DevProblem& p, const int* 
     for (int i = 0; i < 3; ++i) { s[i] = Jl[i * ld + 6]; for (int side = 1; side < NF; ++side) s[i] += Jl[i * ld + side * 10 + 6]; }
     push(0, 6, s[0], s[1], s[2]);
   }
+}
+
+// Scatter of one row block: r the residual, sc its scale; g += J^T r over the columns of for_each_column that are not held constant,
+// with WANT_H also H += J^T J (lower triangle, add_h).
+template <int NF, bool WANT_H>
+__device__ __forceinline__ void scatter_columns(const DevProblem& p, const int* fr, const float* __restrict__ rec, const Gather* dg, const Gather* sg,
+                                                const double* Jl, const double* r, double sc, double* __restrict__ H, double* __restrict__ g) {
+  constexpr int kMaxCols = 72 * NF;     // NF (6 + 1 + 16*2 + 16*2) + the shared focal, with slack
+  const rcvd_config& c = p.cfg; const Layout& L = p.L;
+  const double r0 = r[0] * sc, r1 = r[1] * sc, r2 = r[2] * sc;
+  int ef[kMaxCols]; short el[kMaxCols]; double ej[kMaxCols][3];
+  int E = 0;
+  for_each_column<NF>(p, fr, rec, dg, sg, Jl, [&](int f, int l, double a0, double a1, double a2) {
+    if (is_const_local(c, L, l)) return;
+    ef[E] = f; el[E] = (short)l; ej[E][0] = a0 * sc; ej[E][1] = a1 * sc; ej[E][2] = a2 * sc; ++E;
+  });
   const int np = L.npad;
   for (int a = 0; a < E; ++a) {
     const double a0 = ej[a][0], a1 = ej[a][1], a2 = ej[a][2];
     red_add(g + (size_t)ef[a] * np + el[a], a0 * r0 + a1 * r1 + a2 * r2);
     if (WANT_H) for (int b = 0; b <= a; ++b) add_h(p, H, ef[a], el[a], ef[b], el[b], a0 * ej[b][0] + a1 * ej[b][1] + a2 * ej[b][2]);
+  }
+}
+
+// Rows mode of k_pairs / k_triplets: block `slot`'s three residuals r, its rho and (JAC) its rows of for_each_column, unscaled.
+template <int NF, bool JAC>
+__device__ __forceinline__ void store_rows(const DevProblem& p, const RowOut& o, size_t slot, const int* fr, const float* __restrict__ rec,
+                                           const Gather* dg, const Gather* sg, const double* Jl, const double* r, double rho) {
+  for (int q = 0; q < 3; ++q) o.r[slot * 3 + q] = r[q];
+  o.rho[slot] = rho;
+  if constexpr (JAC) {
+    const rcvd_config& c = p.cfg; const Layout& L = p.L;
+    int E = 0;
+    for_each_column<NF>(p, fr, rec, dg, sg, Jl, [&](int f, int l, double a0, double a1, double a2) {
+      if (is_const_local(c, L, l)) return;
+      const int32_t col = o.uperm[f] * L.nf + l;
+      o.col(slot * 3, E, col, a0); o.col(slot * 3 + 1, E, col, a1); o.col(slot * 3 + 2, E, col, a2); ++E;
+    });
+    for (int q = 0; q < 3; ++q) o.pad(slot * 3 + q, E);
   }
 }
 
@@ -166,10 +210,11 @@ __device__ __forceinline__ void mark_frame(const rcvd_config& c, const Layout& L
 }
 
 // Pair constraints in every mode and every transform / intrinsics configuration; scatter with L2 reductions.  MarkActive marks
-// the parameters referenced by at least one residual block (the Ceres program's parameter set, used for |x| / |step| norms).
-template <EvalMode MODE>
+// the parameters referenced by at least one residual block (the Ceres program's parameter set, used for |x| / |step| norms).  Rows
+// writes record i's rows to slot i: the records must be in the caller's order (not the run path's sorted copy).
+template <EvalMode MODE, bool JAC = false>
 __global__ void __launch_bounds__(kTile) k_pairs(DevProblem p, const double* __restrict__ x, double* __restrict__ H, double* __restrict__ g,
-                                                 double* __restrict__ partial, uint8_t* __restrict__ mask) {
+                                                 double* __restrict__ partial, uint8_t* __restrict__ mask, RowArg<MODE> rows) {
   const rcvd_config& c = p.cfg;
   const int t = blockIdx.x;
   const int pr = p.pairs.tile_group[t];
@@ -189,6 +234,10 @@ __global__ void __launch_bounds__(kTile) k_pairs(DevProblem p, const double* __r
       if constexpr (MODE == EvalMode::Cost) {
         Gather dg0, sg0, dg1, sg1;   // (as four variables the frame is 8 B smaller than with the arrays below)
         eval_constraint<false>(p, x, f0, f1, rec, dg0, sg0, dg1, sg1, ev, nullptr);
+      } else if constexpr (MODE == EvalMode::Rows) {
+        const int fr[2] = {f0, f1}; Gather dg[2], sg[2]; double Jl[JAC ? 60 : 1];
+        eval_constraint<JAC>(p, x, f0, f1, rec, dg[0], sg[0], dg[1], sg[1], ev, JAC ? Jl : nullptr);
+        store_rows<2, JAC>(p, rows, (size_t)(p.pairs.tile_begin[t] + threadIdx.x), fr, rec, dg, sg, Jl, ev.r, ev.rho0);
       } else {
         const int fr[2] = {f0, f1}; Gather dg[2], sg[2]; double Jl[60];
         eval_constraint<true>(p, x, f0, f1, rec, dg[0], sg[0], dg[1], sg[1], ev, Jl);
@@ -197,7 +246,7 @@ __global__ void __launch_bounds__(kTile) k_pairs(DevProblem p, const double* __r
       cost = 0.5 * ev.rho0;
     }
   }
-  if (MODE != EvalMode::MarkActive) block_store_sum(cost, partial + t);
+  if (MODE != EvalMode::MarkActive && MODE != EvalMode::Rows) block_store_sum(cost, partial + t);
 }
 
 // ---------------------------------------------------------------------------
@@ -538,10 +587,11 @@ __host__ __device__ inline RegCounts reg_counts(const rcvd_config& c, const Layo
   return r;
 }
 
-template <EvalMode MODE>
+// Rows: row id -> slot through rows.slot; rho = r^2 (ScaledLoss weights are folded into r as sqrt(w), the other rows have no loss).
+template <EvalMode MODE, bool JAC = false>
 __global__ void __launch_bounds__(128) k_regularisers(DevProblem p, RegCounts rc, const double* __restrict__ x, double* __restrict__ H,
                                                       double* __restrict__ g, double* __restrict__ partial, uint8_t* __restrict__ mask,
-                                                      int first_frame, int last_frame) {
+                                                      int first_frame, int last_frame, RowArg<MODE> rows) {
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int np = L.npad;
   const int id = blockIdx.x * blockDim.x + threadIdx.x;
@@ -624,14 +674,25 @@ __global__ void __launch_bounds__(128) k_regularisers(DevProblem p, RegCounts rc
         if (MODE == EvalMode::CostGradH) for (int b = 0; b <= a; ++b) if (ed[b] != 0.0) add_h(p, H, efr[a], el[a], efr[b], el[b], ed[a] * ed[b]);
       }
     }
+    if constexpr (MODE == EvalMode::Rows) {
+      const int s = rows.slot[id];
+      rows.r[s] = r; rows.rho[s] = r * r;
+      if constexpr (JAC) {
+        int E = 0;
+        for (int a = 0; a < nent; ++a)
+          if (!is_const_local(c, L, el[a])) { rows.col(s, E, rows.uperm[efr[a]] * L.nf + el[a], ed[a]); ++E; }
+        rows.pad(s, E);
+      }
+    }
   }
-  if (MODE != EvalMode::MarkActive) block_store_sum(cost, partial + blockIdx.x);
+  if (MODE != EvalMode::MarkActive && MODE != EvalMode::Rows) block_store_sum(cost, partial + blockIdx.x);
 }
 
 // --- scene-flow smoothness residual blocks (reference addSceneFlowSmoothnessLoss, lib/PoseOptimizer.cpp:1242-1339) ---
-template <EvalMode MODE>
+// Rows: r and J without the ScaledLoss weight w, rho = w |r|^2.
+template <EvalMode MODE, bool JAC = false>
 __global__ void __launch_bounds__(kTile) k_triplets(DevProblem p, const double* __restrict__ x, double* __restrict__ H, double* __restrict__ g,
-                                                    double* __restrict__ partial, uint8_t* __restrict__ mask) {
+                                                    double* __restrict__ partial, uint8_t* __restrict__ mask, RowArg<MODE> rows) {
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int t = blockIdx.x;
   const int fc = p.trips.group_frames[p.trips.tile_group[t]];
@@ -661,6 +722,10 @@ __global__ void __launch_bounds__(kTile) k_triplets(DevProblem p, const double* 
     if constexpr (MODE == EvalMode::Cost) {
       smooth_scene<false>(c, pose, phi, D, u, o, r, nullptr);
       cost = 0.5 * w * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2]);
+    } else if constexpr (MODE == EvalMode::Rows) {
+      const int fr[3] = {fc - 1, fc, fc + 1}; double Jl[JAC ? 90 : 1];
+      smooth_scene<JAC>(c, pose, phi, D, u, o, r, JAC ? Jl : nullptr);
+      store_rows<3, JAC>(p, rows, (size_t)(p.trips.tile_begin[t] + threadIdx.x), fr, rec, dg, sg, Jl, r, w * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2]));
     } else {
       const int fr[3] = {fc - 1, fc, fc + 1}; double Jl[90];
       smooth_scene<true>(c, pose, phi, D, u, o, r, Jl);
@@ -668,7 +733,7 @@ __global__ void __launch_bounds__(kTile) k_triplets(DevProblem p, const double* 
       scatter_columns<3, MODE == EvalMode::CostGradH>(p, fr, rec, dg, sg, Jl, r, sw, H, g);
     }
   }
-  if (MODE != EvalMode::MarkActive) block_store_sum(cost, partial + t);
+  if (MODE != EvalMode::MarkActive && MODE != EvalMode::Rows) block_store_sum(cost, partial + t);
 }
 
 // --- pairwise depth normalisation (normalizeDepth with normalizeDepthFromFirstFrame = false, lib/PoseOptimizer.cpp:1005-1095) ---
@@ -677,9 +742,9 @@ __global__ void __launch_bounds__(kTile) k_triplets(DevProblem p, const double* 
 // max(D, eps) is Jet max, (D < eps) ? eps : D: a clamped end contributes no derivative.  With a Global transform every constraint of
 // the tile touches the same 2k gradient and k (2k + 1) H entries (one pair): they are summed over the tile (warp shuffle, then shared
 // memory) and leave the SM as one RED each.  Grid transforms scatter per constraint over the gathered nodes.
-template <EvalMode MODE>
+template <EvalMode MODE, bool JAC = false>
 __global__ void __launch_bounds__(kTile) k_depth_pairs(DevProblem p, const double* __restrict__ x, double* __restrict__ H, double* __restrict__ g,
-                                                       double* __restrict__ partial, uint8_t* __restrict__ mask) {
+                                                       double* __restrict__ partial, uint8_t* __restrict__ mask, RowArg<MODE> rows) {
   const rcvd_config& c = p.cfg; const Layout& L = p.L;
   const int t = blockIdx.x, np = L.npad;
   const int pr = p.dpairs.tile_group[t];
@@ -696,6 +761,30 @@ __global__ void __launch_bounds__(kTile) k_depth_pairs(DevProblem p, const doubl
       for (int q = 0; q < dg[s].n; ++q)
         for (int j = 0; j < L.k; ++j) mask[(size_t)fr[s] * np + L.offD + dg[s].idx[q] * L.k + j] = 1;
     return;
+  } else if constexpr (MODE == EvalMode::Rows) {
+    if (!active) return;
+    constexpr double eps = 1e-6;
+    const double D0 = depth_value(c, L, dg[0], rec[2], x + (size_t)fr[0] * L.nf), D1 = depth_value(c, L, dg[1], rec[5], x + (size_t)fr[1] * L.nf);
+    const bool c0 = D0 < eps, c1 = D1 < eps;
+    const double r = 1.0 / (c0 ? eps : D0) - 1.0 / (c1 ? eps : D1);
+    double rho0, rho1;
+    robust_loss(c, r * r, rho0, rho1);
+    const size_t slot = (size_t)(p.dpairs.tile_begin[t] + threadIdx.x);
+    rows.r[slot] = r; rows.rho[slot] = rho0;
+    if constexpr (JAC) {
+      const double dr[2] = {c0 ? 0.0 : -1.0 / (D0 * D0), c1 ? 0.0 : 1.0 / (D1 * D1)};   // dr/dD of each end
+      int E = 0;
+      if (!c.fix_depth_xforms)
+        for (int s = 0; s < 2; ++s) {
+          const double src = (double)rec[3 * s + 2]; const int32_t base = rows.uperm[fr[s]] * L.nf + L.offD;
+          for (int q = 0; q < dg[s].n; ++q) {
+            const double w = dg[s].w[q];
+            rows.col(slot, E++, base + dg[s].idx[q] * L.k, dr[s] * w * src);
+            if (L.k == 2) rows.col(slot, E++, base + dg[s].idx[q] * 2 + 1, dr[s] * w);
+          }
+        }
+      rows.pad(slot, E);
+    }
   } else {
     double cost = 0.0, rs = 0.0, dr[2] = {0.0, 0.0};   // scaled residual and scaled dr/dD of each end (zero on idle threads)
     if (active) {

@@ -174,6 +174,27 @@ class Problem:
         _check(self.L.rcvd_normal_matrix_dense(self.h, _p(H, C.c_double)))
         return H
 
+    def row_layout(self):
+        """Per residual family (abi.ROW_FAMILIES): {"blocks", "residuals" (m, per block), "max_cols" (k, column slots per residual)}."""
+        out = abi.RowLayout()
+        _check(self.L.rcvd_row_layout(self.h, C.byref(out)))
+        return {name: {"blocks": f.blocks, "residuals": f.residuals, "max_cols": f.max_cols} for name, f in zip(abi.ROW_FAMILIES, out.family)}
+
+    def rows(self, family, jacobian=False):
+        """rcvd_evaluate_rows at the current state.  family: a name of abi.ROW_FAMILIES or an abi.ROWS_* value.  Returns (r [n, m],
+        rho [n]) and with jacobian=True also (cols [n, m, k] int32, J [n, m, k]): one block per constraint record in the order it was
+        set, or per regulariser row (include/rcvd.h gives the orders).  cols are indices into the [N * stride] state, -1 in unused slots."""
+        fam = abi.ROW_FAMILIES.index(family) if isinstance(family, str) else int(family)
+        if not 0 <= fam < len(abi.ROW_FAMILIES):
+            raise ValueError(f"unknown row family {family!r}")
+        lay = self.row_layout()[abi.ROW_FAMILIES[fam]]
+        n, m, k = lay["blocks"], lay["residuals"], lay["max_cols"]
+        r = np.zeros((n, m), np.float64); rho = np.zeros(n, np.float64)
+        cols = np.zeros((n, m, k), np.int32) if jacobian else None
+        J = np.zeros((n, m, k), np.float64) if jacobian else None
+        _check(self.L.rcvd_evaluate_rows(self.h, C.c_int32(fam), _p(r, C.c_double), _p(rho, C.c_double), _p(cols, C.c_int32), _p(J, C.c_double)))
+        return (r, rho, cols, J) if jacobian else (r, rho)
+
     def debug_linear_solve(self, S, D2, b):
         S = np.ascontiguousarray(S, np.float64); D2 = np.ascontiguousarray(D2, np.float64)
         b = np.ascontiguousarray(b, np.float64); y = np.zeros_like(b)
