@@ -39,6 +39,15 @@ int32_t rcvd_debug_factor_plan(const rcvd_config* cfg, int32_t np, const int32_t
 int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
                                  int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms,
                                  int32_t* passes, int32_t* sources, int32_t* join, int32_t* flags, int32_t counts[5]);
+/* the k_update_tma work items of the same plan, in the order `order` (1: locality order, the default of a handle; 0: sorted by cost
+ * within each launch): items[I][8] = {target L block, first source pair, source pairs, tile row origin, tile column origin, rows,
+ * columns, flags (1: diagonal tile of a symmetric target, 2: first pass into a fill block)}; launches[levels][6] = per level
+ * {offset, items} of its late launch and of its two deferred launches; products[Q][2] = per source pair the T indices of X_rk and
+ * X_ck.  counts = {I, 3 * levels, Q, unknowns per block the tiles cover (neff), npad} on return; with items non-null, counts[0..2]
+ * are the capacities of items, launches (in pairs of ints) and products (in pairs of ints) on entry. */
+int32_t rcvd_debug_update_items(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms, int32_t order,
+                                int32_t* items, int32_t* launches, int32_t* products, int32_t counts[5]);
 
 /* y = (S H S + diag(D2))^-1 b with the current H (exercises factorisation + substitution alone) */
 int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* D2, const double* b, double* y);
@@ -86,6 +95,7 @@ int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on);        /* (0) cos
 int32_t rcvd_debug_set_distributed(rcvd_problem* p, int32_t on);      /* (1) nranks > 1: distributed factorisation; 0 = all-reduce H + replicated factorisation */
 int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]);       /* {distributed, first replicated level, levels, frames owned by this rank} */
 int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta); /* (1, 0) tma must be 1 (0: RCVD_ERR_INVALID, the cp.async update path was removed); items-per-CTA cap of the one-team launches (0: none) */
+int32_t rcvd_debug_set_update_order(rcvd_problem* p, int32_t order);  /* (1) k_update_tma items of a launch in locality order; 0 = sorted by cost (same items, same factor) */
 
 #ifdef __cplusplus
 }

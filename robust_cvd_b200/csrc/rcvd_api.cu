@@ -217,7 +217,8 @@ struct rcvd_problem {
   // internal -> caller's frame ids
   int *d_lvl_own = nullptr, *d_load_lblocks = nullptr, *d_own_hblocks = nullptr, *d_uperm = nullptr;
   // TMA-fed persistent update kernel (rcvd_update.cuh)
-  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; int num_sms = 0, upd_ipc = 0;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
+  // d_upd_items: FactorPlan::upd_items_cost, then upd_items; upd_order (rcvd_debug_set_update_order) picks the list the launches read
+  UpdItem* d_upd_items = nullptr; CUtensorMap tmapT; int num_sms = 0, upd_ipc = 0, upd_order = 1;   // upd_ipc: items-per-CTA cap of the one-team launches (0: none)
   std::vector<double> level_ms;   // last rcvd_debug_profile_linear: per level x kernel class
   // test hooks (rcvd_debug_factor_dense, rcvd_debug_linear_paths): whether a factorisation has run, per-kernel-path launch counters
   // (enqueue_factor_solve counts, graph replays add graph_paths)
@@ -332,7 +333,9 @@ static int upload_plan(rcvd_problem* p) {
   UP(p->d_load_lblocks, pl.load_lblocks); UP(p->d_own_hblocks, pl.own_hblocks); UP(p->d_uperm, pl.uperm);
   UP(p->d_trsm_tasks, pl.trsm_tasks); UP(p->d_upd_pairs, pl.upd_pairs);
   UP(p->d_sub_tasks, pl.sub_tasks); UP(p->d_sub_need, pl.sub_need); DA(p->d_sub_counters, (size_t)4 * p->N + 4);
-  UP(p->d_fwd_tasks, pl.fwd_tasks); UP(p->d_upd_items, pl.upd_items);
+  UP(p->d_fwd_tasks, pl.fwd_tasks);
+  { std::vector<UpdItem> both(pl.upd_items_cost); both.insert(both.end(), pl.upd_items.begin(), pl.upd_items.end());
+    UP(p->d_upd_items, both); }
   return RCVD_OK;
 }
 
@@ -600,16 +603,17 @@ struct FactorSolve {
     return RCVD_OK;
   }
 
-  // the persistent TMA-fed update kernel over the items [off, off + n)
+  // the persistent TMA-fed update kernel over the items [off, off + n) of the list upd_order selects
   int update(cudaStream_t s, int off, int n) {
+    const UpdItem* items = p->d_upd_items + (size_t)p->upd_order * pl.upd_items.size() + off;
     if (n <= p->num_sms)   // few items: two DMMA teams per tile, one CTA per SM
       return launch(LP_UPD_TMA2, k_update_tma<2>, dim3(n), dim3(UpdShape<2>::threads), upd_smem_bytes(pl.upd_rb, 2), s, false,
-                    p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, pl.upd_neff, pl.upd_rb, 0);
-    int grid = std::min(n, 2 * p->num_sms);
+                    p->tmapT, p->d_Lb, items, n, p->d_upd_pairs, npad, pl.upd_neff, pl.upd_rb, 0);
+    int grid = upd_ctas(n, p->num_sms);
     if (p->upd_ipc > 0) grid = std::max(grid, (n + p->upd_ipc - 1) / p->upd_ipc);
     if (grid < n) p->paths[LP_UPD_TMA1_MULTI]++;
     return launch(LP_UPD_TMA1, k_update_tma<1>, dim3(grid), dim3(UpdShape<1>::threads), upd_smem_bytes(pl.upd_rb, 1), s, false,
-                  p->tmapT, p->d_Lb, p->d_upd_items + off, n, p->d_upd_pairs, npad, pl.upd_neff, pl.upd_rb, 0);
+                  p->tmapT, p->d_Lb, items, n, p->d_upd_pairs, npad, pl.upd_neff, pl.upd_rb, 0);
   }
 
   // The update passes of level li: after the waits for the earlier levels' U2 launches it needs, U1 on the main stream, then the
@@ -1642,6 +1646,12 @@ RCVD_API int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int3
   if (!tma) return set_err(RCVD_ERR_INVALID, "the cp.async update path was removed: k_update_tma is the only update kernel");
   p->upd_ipc = side_items_per_cta; drop_graph(p); return RCVD_OK;
 }
+// Test / bench hook: the order of k_update_tma's items within each launch: 1 (default) = locality order, 0 = sorted by cost.
+RCVD_API int32_t rcvd_debug_set_update_order(rcvd_problem* p, int32_t order) {
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  if (order < 0 || order > 1) return set_err(RCVD_ERR_INVALID, "update order must be 0 or 1 (got %d)", order);
+  p->upd_order = order; drop_graph(p); return RCVD_OK;
+}
 // Test / bench hook: 1 = the handle will only evaluate cost / gradient (rcvd_evaluate): no normal matrix, no factor storage is allocated
 RCVD_API int32_t rcvd_debug_set_eval_only(rcvd_problem* p, int32_t on) { if (!p) return set_err(RCVD_ERR_INVALID, "null problem"); if (int rc = drop_structure(p)) return rc; p->eval_only = on != 0; return RCVD_OK; }
 // Test / bench hook (nranks > 1): 1 (default) = distributed factorisation (owner-computes phase A, reduce-to-owner of H), 0 = replicated scheme
@@ -1719,6 +1729,33 @@ RCVD_API int32_t rcvd_debug_update_passes(const rcvd_config* cfg, int32_t np, co
     }
   }
   std::copy(need, need + 3, counts); counts[3] = pl.TB; counts[4] = pl.upd_window;
+  return RCVD_OK;
+}
+// Test hook: the update items of the plan of a frame graph, launch by launch (see include/rcvd_hooks.h).
+RCVD_API int32_t rcvd_debug_update_items(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                         int32_t order_slack, int32_t nranks, int32_t rank, int32_t num_sms, int32_t order,
+                                         int32_t* items, int32_t* launches, int32_t* products, int32_t counts[5]) {
+  if (!counts) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (order < 0 || order > 1) return set_err(RCVD_ERR_INVALID, "update order must be 0 or 1 (got %d)", order);
+  FactorPlan pl;
+  if (int32_t rc = debug_plan(pl, cfg, np, pairs, nt, trip_centers, order_slack, nranks, rank, num_sms)) return rc;
+  const int32_t need[3] = {(int32_t)pl.upd_items.size(), 3 * (int32_t)pl.levels.size(), (int32_t)pl.upd_pairs.size()};
+  if (items) {
+    if (!launches || !products || counts[0] < need[0] || counts[1] < need[1] || counts[2] < need[2]) return set_err(RCVD_ERR_INVALID, "null or short output array");
+    const std::vector<UpdItem>& v = order ? pl.upd_items : pl.upd_items_cost;
+    for (size_t i = 0; i < v.size(); ++i) {
+      const int32_t o[8] = {v[i].dst, v[i].first, v[i].count, v[i].m0, v[i].n0, v[i].mrows, v[i].ncols, v[i].flags};
+      std::copy(o, o + 8, items + 8 * i);
+    }
+    for (size_t l = 0; l < pl.levels.size(); ++l) {
+      const Level& lv = pl.levels[l];
+      const int32_t o[6] = {lv.it_off, lv.nit, lv.it2_off[0], lv.nit2[0], lv.it2_off[1], lv.nit2[1]};
+      std::copy(o, o + 6, launches + 6 * l);
+    }
+    for (size_t q = 0; q < pl.upd_pairs.size(); ++q) { products[2 * q] = pl.upd_pairs[q].x; products[2 * q + 1] = pl.upd_pairs[q].y; }
+  }
+  Layout L; make_layout(*cfg, L);
+  std::copy(need, need + 3, counts); counts[3] = pl.upd_neff; counts[4] = L.npad;
   return RCVD_OK;
 }
 // Structure statistics (for DESIGN.md / bench): frames, off-diagonal factor blocks, levels, H blocks, npad.

@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <map>
 #include <set>
+#include <tuple>
 #include <vector>
 
 #include "rcvd_linalg.cuh"
@@ -26,6 +27,49 @@ struct Level { int frame_off, nframes; int trsm_off, ntrsm; int upd_off, nupd; i
 // levels delays the main stream, as it would in the tail, whose side work must finish within the next level's potrf (DESIGN.md section 4).
 constexpr int kUpdWindow = 2, kUpdWindowMaxNf = 256;
 
+// DMMA work of an update item (m8n8 units x 4 k4 steps per source pair; a symmetric diagonal tile skips its upper warp tile)
+inline long upd_item_cost(const UpdItem& a) { return (long)a.count * (a.mrows / 8) * (a.ncols / 8) * ((a.flags & kUpdSymDiag) ? 3 : 4); }
+
+// Locality order of one update launch of `ctas` resident CTAs.  `in`: the launch's items, pass after pass, each pass's tiles adjacent.
+// Every item streams an 80-row strip of X_rk and one of X_ck for each of its source pairs: ~10 flop per operand byte at K = 200, so the
+// strips have to come from L2, and the factor (hundreds of MB) is far larger than L2.  A strip is reused only by the items that run at
+// about the same time, i.e. in the same wave of `ctas` consecutive items.  So: the source frames k, heaviest first, each followed by the
+// not yet emitted passes that read X_.k (all the tiles of a target stay adjacent; the d (d + 1) / 2 targets of a column k of d blocks
+// share its d blocks).  Then, within each wave, the items go to the CTA slots so that the CTAs' summed work stays balanced (heaviest
+// item to the least loaded CTA, from the last, partial wave backwards): the persistent CTAs take their items statically, so a
+// cost-sorted list was what kept them even.  Returns false if two items of the launch write the same target tile (they run concurrently).
+inline bool order_update_items(const std::vector<UpdItem>& in, const std::vector<int2>& pairs, const std::vector<int>& lcol, int ctas,
+                               UpdItem* out) {
+  struct Pass { size_t b, e; long cost; };
+  std::vector<Pass> passes; std::set<std::tuple<int, int, int>> tiles;
+  for (size_t i = 0; i < in.size(); ++i) {
+    if (!tiles.insert(std::make_tuple(in[i].dst, (int)in[i].m0, (int)in[i].n0)).second) return false;
+    if (i == 0 || in[i].dst != in[i - 1].dst || in[i].first != in[i - 1].first) passes.push_back({i, i, 0});
+    passes.back().e = i + 1; passes.back().cost += upd_item_cost(in[i]);
+  }
+  std::map<int, std::vector<int>> readers; std::map<int, long> weight;   // source frame -> passes reading it (pass order), their work
+  for (size_t q = 0; q < passes.size(); ++q) {
+    const UpdItem& it = in[passes[q].b];
+    std::set<int> ks; for (int p = it.first; p < it.first + it.count; ++p) ks.insert(lcol[pairs[p].x]);
+    for (int k : ks) { readers[k].push_back((int)q); weight[k] += passes[q].cost; }
+  }
+  std::vector<int> ks; for (auto& kv : weight) ks.push_back(kv.first);
+  std::stable_sort(ks.begin(), ks.end(), [&](int a, int b) { return weight[a] > weight[b]; });
+  std::vector<UpdItem> seq; seq.reserve(in.size()); std::vector<uint8_t> done(passes.size(), 0);
+  for (int k : ks) for (int q : readers[k]) if (!done[q]) { done[q] = 1; seq.insert(seq.end(), in.begin() + passes[q].b, in.begin() + passes[q].e); }
+  const size_t n = seq.size(), G = (size_t)std::max(ctas, 1);
+  std::vector<long> load(G, 0); std::vector<int> slot(G), idx;
+  for (size_t w = (n + G - 1) / G; w-- > 0;) {
+    const size_t b = w * G, m = std::min(G, n - b);
+    idx.resize(m); for (size_t i = 0; i < m; ++i) idx[i] = (int)i;
+    std::stable_sort(idx.begin(), idx.end(), [&](int x, int y) { return upd_item_cost(seq[b + x]) > upd_item_cost(seq[b + y]); });
+    slot.resize(m); for (size_t s = 0; s < m; ++s) slot[s] = (int)s;
+    std::stable_sort(slot.begin(), slot.end(), [&](int x, int y) { return load[x] < load[y]; });
+    for (size_t i = 0; i < m; ++i) { out[b + slot[i]] = seq[b + idx[i]]; load[slot[i]] += upd_item_cost(seq[b + idx[i]]); }
+  }
+  return true;
+}
+
 // Every frame id below is internal: frames are numbered owner-major (uperm / iperm map to and from the caller's ids).
 struct FactorPlan {
   std::vector<int> elim_order;                 // frames in elimination order
@@ -44,7 +88,9 @@ struct FactorPlan {
   // task lists of the level schedule
   std::vector<int> lvl_frames, lvl_own;
   std::vector<TrsmTask> trsm_tasks; std::vector<UpdPass> upd_tasks; std::vector<int2> upd_pairs; std::vector<SolveTask> fwd_tasks;
-  std::vector<UpdItem> upd_items; int upd_rb = 0, upd_neff = 0;
+  // upd_items: k_update_tma's work items in locality order (order_update_items); upd_items_cost: the same items of every launch sorted
+  // by cost, heaviest first (the A/B reference, rcvd_debug_set_update_order).  Both have the launches at the same offsets.
+  std::vector<UpdItem> upd_items, upd_items_cost; int upd_rb = 0, upd_neff = 0;
   int upd_targets = 0;      // (source level, target block) pairs of the elimination structure this rank updates
   int upd_window = 1;       // source levels per window of the deferred update passes
   int TB = 0;               // tail boundary: levels >= TB are the trailing run of levels with fewer than 3 frames (= LB when distributed)
@@ -279,8 +325,9 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
     }
     lv.ntrsm = (int)P.trsm_tasks.size() - lv.trsm_off; lv.nupd = lv.upd2_off[0] - lv.upd_off; lv.nfwd = (int)P.fwd_tasks.size() - lv.fwd_off;
     lv.nupd2[0] = lv.upd2_off[1] - lv.upd2_off[0]; lv.nupd2[1] = (int)P.upd_tasks.size() - lv.upd2_off[1];
-    // work items of the persistent update kernel: one per (target tile, source-pair list), heaviest first within each launch
-    std::vector<UpdItem>& items = P.upd_items;
+    // work items of the persistent update kernel: one per (target tile, source-pair list), per launch in cost order and in locality
+    // order; a launch of the two-team shape is a single wave and keeps the cost order in both
+    std::vector<UpdItem>& items = P.upd_items_cost;
     for (int pass = 0; pass < 3; ++pass) {
       const int t0 = pass ? lv.upd2_off[pass - 1] : lv.upd_off, tn = pass ? lv.nupd2[pass - 1] : lv.nupd;
       const size_t i0 = items.size();
@@ -293,8 +340,13 @@ inline const char* make_factor_plan(FactorPlan& P, const rcvd_config& cfg, const
           items.push_back(it);
         }
       }
-      auto cost = [](const UpdItem& a) { return (long)a.count * (a.mrows / 8) * (a.ncols / 8) * ((a.flags & kUpdSymDiag) ? 3 : 4); };
-      std::stable_sort(items.begin() + i0, items.end(), [&](const UpdItem& a, const UpdItem& b) { return cost(a) > cost(b); });
+      P.upd_items.resize(items.size());
+      const std::vector<UpdItem> built(items.begin() + i0, items.end());
+      std::stable_sort(items.begin() + i0, items.end(), [](const UpdItem& a, const UpdItem& b) { return upd_item_cost(a) > upd_item_cost(b); });
+      const int n = (int)built.size();
+      if (!order_update_items(built, P.upd_pairs, lcol, upd_ctas(n, num_sms), P.upd_items.data() + i0))
+        return "internal error: two update items of one launch write the same target tile";
+      if (n <= num_sms) std::copy(items.begin() + i0, items.end(), P.upd_items.begin() + i0);
       if (pass) { lv.it2_off[pass - 1] = (int)i0; lv.nit2[pass - 1] = (int)(items.size() - i0); } else { lv.it_off = (int)i0; lv.nit = (int)(items.size() - i0); }
     }
     P.levels.push_back(lv);

@@ -20,9 +20,9 @@
 //     step at the target's magnitude, and on diagonal blocks, where the target dominates the products, the componentwise backward
 //     error of the factor measured 72-83 u against 64 u.  The first pass into a fill block neither prefetches nor reads the target
 //     (it has no value yet): it stores 0 - products;
-//   * persistent CTAs (one per SM) walk a cost-sorted list of (target tile, source-pair list) work items, so the producer
-//     prefetches the next item's first stages while the DMMA warps are in the epilogue of the previous one, and a
-//     launch never has a tail of under-filled waves;
+//   * persistent CTAs walk a list of (target tile, source-pair list) work items, so the producer prefetches the next item's first
+//     stages while the DMMA warps are in the epilogue of the previous one.  The plan orders a launch's items so that each wave reads
+//     few distinct operand strips (L2 reuse) and every CTA gets the same work (rcvd_plan.h, order_update_items);
 //   * a single warp issues DMMAs far below the SM's rate, so a lone 4-warp tile is latency-bound (1300 DMMAs per warp at
 //     K = 200 on the narrow-level launches of the factorisation): TWO teams of four DMMA warps take alternate K stages of the same
 //     tile, team 1 hands its partial accumulators to team 0 through shared memory (named barriers, no __syncthreads) and goes on
@@ -52,6 +52,9 @@ constexpr int kUpdFirstFill = 2;   // first pass into a fill block: the target h
 constexpr int kUpdMaxTile = 80;       // rows / columns of a CTA tile (<= 5 m8n8 units per warp and dimension)
 constexpr int kUpdPartial = 4 * 25 * 32 * 2;   // doubles: team 1's accumulators on their way to team 0
 template <int TEAMS> struct UpdShape { static constexpr int stages = TEAMS == 2 ? 8 : 5, threads = TEAMS * 128 + 32, ctas = TEAMS == 2 ? 1 : 2; };
+// CTAs of a launch of n items: the two-team shape (one CTA per item) up to one item per SM, else the one-team shape, two CTAs per SM.
+// CTA b walks the items b, b + ctas, b + 2 ctas, ...: a "wave" of `ctas` consecutive items runs at about the same time.
+inline int upd_ctas(int n, int num_sms) { return n <= num_sms ? n : (n < 2 * num_sms ? n : 2 * num_sms); }
 __host__ __device__ inline size_t upd_smem_bytes(int rb, int teams) {
   const int stages = teams == 2 ? 8 : 5;
   return (size_t)stages * 2 * rb * 16 * sizeof(double) + (teams == 2 ? (size_t)kUpdPartial * sizeof(double) : 0) + 2 * stages * sizeof(uint64_t) + 1024;

@@ -95,6 +95,24 @@ def update_passes(cfg, pairs, trip_centers=(), order_slack=4, nranks=1, rank=0, 
     return {"passes": passes, "sources": sources, "join": join.reshape(-1, 2), "flags": flags, "tail": counts[3], "window": counts[4]}
 
 
+UPDATE_ITEM_FIELDS = ("dst", "first", "count", "m0", "n0", "mrows", "ncols", "flags")
+
+
+def update_items(cfg, pairs, trip_centers=(), order_slack=4, nranks=1, rank=0, num_sms=132, order=1):
+    """Test hook: the update kernel's work items of factor_plan's plan (host only), in the order `order` (1 locality, 0 cost-sorted).
+    Returns items [I, 8] (UPDATE_ITEM_FIELDS), launches [levels, 3, 2] ((offset, items) of the late launch and the two deferred
+    launches of every level), products [Q, 2] (T indices of X_rk and X_ck of every source pair), neff and npad."""
+    pf = np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
+    tc = np.ascontiguousarray(np.asarray(trip_centers, np.int32).reshape(-1))
+    args = (C.byref(cfg), C.c_int32(pf.shape[0]), _p(pf, C.c_int32), C.c_int32(tc.size), _p(tc, C.c_int32),
+            C.c_int32(order_slack), C.c_int32(nranks), C.c_int32(rank), C.c_int32(num_sms), C.c_int32(order))
+    counts = (C.c_int32 * 5)()
+    _check(lib().rcvd_debug_update_items(*args, None, None, None, counts))
+    items, launches, products = np.zeros((counts[0], 8), np.int32), np.zeros((counts[1], 2), np.int32), np.zeros((counts[2], 2), np.int32)
+    _check(lib().rcvd_debug_update_items(*args, _p(items, C.c_int32), _p(launches, C.c_int32), _p(products, C.c_int32), counts))
+    return {"items": items, "launches": launches.reshape(-1, 3, 2), "products": products, "neff": counts[3], "npad": counts[4]}
+
+
 class Problem:
     def __init__(self, cfg, device=0):
         self.cfg = cfg
@@ -277,6 +295,11 @@ class Problem:
         """Test / bench hook: side_items_per_cta > 0 caps the work items per CTA of the one-team update launches.  tma must be True:
         the persistent TMA-fed kernel is the only update kernel (False raises)."""
         _check(self.L.rcvd_debug_set_update_kernel(self.h, C.c_int32(1 if tma else 0), C.c_int32(side_items_per_cta)))
+
+    def set_update_order(self, order=1):
+        """Test / bench hook: the order of the update kernel's work items within each launch, 1 (default) locality order, 0 sorted by
+        cost.  Both run the same items: the factor is the same bit for bit."""
+        _check(self.L.rcvd_debug_set_update_order(self.h, C.c_int32(order)))
 
     def set_eval_only(self, on=True):
         """Test / bench hook: the handle only evaluates cost / gradient; no matrix storage is allocated."""
