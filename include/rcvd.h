@@ -262,6 +262,29 @@ int32_t rcvd_time_iteration(rcvd_problem* p, int32_t iters, double radius, doubl
  * ceres::Solve at lib/PoseOptimizer.cpp:954-962 and :1117-1125. */
 int32_t rcvd_solve(rcvd_problem* p, const rcvd_solve_options* opt, rcvd_solve_summary* summary);
 
+/* The linear solver of the damped LM step.  A single-GPU handle picks it when it builds its structure (the first call that
+ * needs it after a setter): the exact block-sparse Cholesky while the storage it needs for the problem's frame graph (H, the
+ * factor with its fill, the off-diagonal factor blocks and the diagonal inverses) is at most 4/5 of the device's total memory,
+ * else conjugate gradients preconditioned by the frames' damped diagonal blocks, which stores H, those N blocks and their
+ * inverses (Ceres' CGNR-style iterative solver: restated Ceres ConjugateGradientsSolver semantics, eta = 0.1, at most 500
+ * iterations per step).  nranks > 1 always factors (distributed Cholesky).  The choice depends on the device's total memory, not
+ * on what is free, so it is the same on every run. */
+enum { RCVD_LINEAR_CHOLESKY = 0, RCVD_LINEAR_CG = 1 };
+typedef struct rcvd_linear_info {
+  int32_t solver;               /* RCVD_LINEAR_* */
+  int32_t factor_blocks;        /* npad x npad blocks of factor storage allocated: N + fill + off-diagonal (Cholesky), N (CG) */
+  int64_t device_bytes;         /* the chosen solver's device storage (matrices, and for CG its vectors) */
+  int64_t cholesky_bytes;       /* what the block Cholesky needs for this problem */
+  int64_t cg_bytes;             /* what conjugate gradients need */
+  int64_t budget_bytes;         /* the Cholesky's budget on this device */
+  int64_t cg_iterations;        /* CG iterations of the last rcvd_solve, over all its steps (0 with the Cholesky) */
+  int32_t cg_max_iterations;    /* the most in one step */
+  int32_t cg_capped_steps;      /* steps whose CG stopped at the iteration cap (their iterate is still used) */
+  int32_t cg_solves;            /* CG solves of the last rcvd_solve */
+} rcvd_linear_info;
+/* Builds the structure if needed (as rcvd_evaluate does) and fills *out. */
+int32_t rcvd_problem_linear_info(rcvd_problem* p, rcvd_linear_info* out);
+
 /* ---- next-row kernels (SURVEY.md section 8f-1): dense transform application ---- */
 /* DepthXform::apply (lib/DepthMapTransform.cpp:394-415): dst = xform(src) per pixel.
  * depth_params: the frame's depth-transform params (host). src/dst: h*w float32 host. */

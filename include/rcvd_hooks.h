@@ -57,6 +57,16 @@ int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const double* 
  * rcvd_problem_set_constraints (no evaluation).  A non-zero entry in a frame pair the graph does not couple: RCVD_ERR_INVALID;
  * a non-positive pivot: RCVD_ERR_NUMERIC. */
 int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y);
+/* rcvd_debug_solve_matrix through conjugate gradients, on a handle whose structure chose them (a factor budget of 0); iterations = the
+ * CG iterations run.  A handle on the Cholesky path: RCVD_ERR_INVALID; a CG breakdown or non-positive pivot: RCVD_ERR_NUMERIC. */
+int32_t rcvd_debug_cg_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y, int32_t* iterations);
+/* The storage of both linear solvers (rcvd_linear_info) for the frame graph of np pairs and nt triplet centres under cfg, on one GPU, and
+ * the solver (RCVD_LINEAR_*) a device of device_total_bytes selects.  Host only: no handle, no device. */
+int32_t rcvd_debug_linear_storage(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                  int32_t order_slack, uint64_t device_total_bytes, int64_t* cholesky_bytes, int64_t* cg_bytes, int32_t* solver);
+/* mean device ms of one CG matrix product (S H S + D2) p (the SpMV over the stored H blocks and the per-frame sum) over reps, with the
+ * S, D2 and direction of the handle's last CG solve: the number tools/bench_long.py turns into achieved bandwidth */
+int32_t rcvd_debug_time_cg_product(rcvd_problem* p, int32_t reps, double* ms);
 /* what the last factorisation left on the device: order[N] = caller's frame index of each eliminated frame, in elimination order;
  * L = dense U x U lower-triangular factor of P A P^T in that order (padding stripped, strict upper triangle zero); Linv (may be null)
  * = the N * stride * stride explicit inverses of the diagonal blocks (k_trinv), same order.  RCVD_ERR_INVALID before any factorisation. */
@@ -96,6 +106,9 @@ int32_t rcvd_debug_set_distributed(rcvd_problem* p, int32_t on);      /* (1) nra
 int32_t rcvd_distribution_info(rcvd_problem* p, int32_t out[4]);       /* {distributed, first replicated level, levels, frames owned by this rank} */
 int32_t rcvd_debug_set_update_kernel(rcvd_problem* p, int32_t tma, int32_t side_items_per_cta); /* (1, 0) tma must be 1 (0: RCVD_ERR_INVALID, the cp.async update path was removed); items-per-CTA cap of the one-team launches (0: none) */
 int32_t rcvd_debug_set_update_order(rcvd_problem* p, int32_t order);  /* (1) k_update_tma items of a launch in locality order; 0 = sorted by cost (same items, same factor) */
+int32_t rcvd_debug_set_factor_budget(rcvd_problem* p, int64_t bytes); /* (-1) storage budget of the block Cholesky: -1 = 4/5 of the device's total memory;
+                                                                          0 = conjugate gradients on any single-GPU problem */
+int32_t rcvd_debug_set_cg_tolerance(rcvd_problem* p, double eta);     /* (0.1) the CG's quadratic-model tolerance eta, in (0, 1) */
 
 #ifdef __cplusplus
 }

@@ -112,6 +112,17 @@ class RowLayout(C.Structure):
     _fields_ = [("family", RowFamily * len(ROW_FAMILIES))]
 
 
+# linear solvers of rcvd_linear_info::solver
+LINEAR_CHOLESKY, LINEAR_CG = 0, 1
+
+
+class LinearInfo(C.Structure):
+    """rcvd_linear_info (include/rcvd.h)."""
+    _fields_ = [("solver", C.c_int32), ("factor_blocks", C.c_int32), ("device_bytes", C.c_int64), ("cholesky_bytes", C.c_int64),
+                ("cg_bytes", C.c_int64), ("budget_bytes", C.c_int64), ("cg_iterations", C.c_int64), ("cg_max_iterations", C.c_int32),
+                ("cg_capped_steps", C.c_int32), ("cg_solves", C.c_int32)]
+
+
 def default_config(num_frames, aspect, **kw):
     """Config with the reference's Params defaults (lib/PoseOptimizer.h:55-103)."""
     focal_long = kw.pop("focal_long", 0.3461538376301239)

@@ -12,6 +12,8 @@
 #include <cstring>
 #include <dlfcn.h>
 #include <limits>
+#include <map>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -20,6 +22,7 @@
 #include "rcvd_linalg.cuh"
 #include "rcvd_update.cuh"
 #include "rcvd_plan.h"
+#include "rcvd_cg.cuh"
 #include "rcvd_host.h"
 
 using namespace rcvd;
@@ -224,6 +227,15 @@ struct rcvd_problem {
   // (enqueue_factor_solve counts, graph replays add graph_paths)
   bool factored = false;
   int64_t paths[LP_N] = {0}, graph_paths[LP_N] = {0};
+  // The linear solver build_structure picked for the plan (rcvd_cg.cuh): conjugate gradients when the block Cholesky's storage
+  // exceeds factor_budget (-1: cholesky_budget of the device's total memory; rcvd_debug_set_factor_budget), the block Cholesky otherwise
+  bool use_cg = false; int64_t factor_budget = -1; uint64_t total_mem = 0;
+  LinearStorage storage = {}; int64_t linear_bytes = 0;   // both paths' needs for the plan; what allocate_storage allocated for the chosen one
+  double cg_eta = kCgEta;                                  // rcvd_debug_set_cg_tolerance
+  double *d_cg_r = nullptr, *d_cg_z = nullptr, *d_cg_p = nullptr, *d_cg_q = nullptr, *d_cg_slots = nullptr, *d_cg_part = nullptr;
+  int *d_cg_frames = nullptr, *d_cg_off = nullptr, *d_cg_ids = nullptr; CgState* d_cg = nullptr;
+  // CG iterations of the solves since the last rcvd_solve began (rcvd_problem_linear_info), and of the last solve alone
+  int64_t cg_iterations = 0; int cg_max = 0, cg_capped = 0, cg_steps = 0, cg_last = 0;
   rcvd_problem() {}
 };
 
@@ -415,13 +427,29 @@ static int allocate_storage(rcvd_problem* p) {
   DA(p->d_ytmp, Upad); DA(p->d_y, Upad); DA(p->d_Sy, Upad); DA(p->d_Hy, Upad); DA(p->d_scal, SC_N); DA(p->d_active, Upad); DA(p->d_fail, 1);
   DA(p->d_potrf_progress, (size_t)N);
   DA(p->d_partial, (size_t)p->npartial);
+  // the linear solver's storage, counted in linear_bytes (linear_storage restates it from the plan)
+  p->linear_bytes = 0;
+#define LA(ptr, n) do { DA(ptr, n); p->linear_bytes += (int64_t)std::max<size_t>((n), 1) * sizeof(*(ptr)); } while (0)
   if (p->eval_only) { DA(p->d_H, 1); DA(p->d_Lb, 1); DA(p->d_T, 1); DA(p->d_invL, 1); DA(p->d_invT, 1); }   // cost / gradient evaluations only: no matrices
-  else {
-    DA(p->d_H, p->plan.hblocks.size() * bs); DA(p->d_Lb, (size_t)(N + nLoff) * bs); DA(p->d_T, (size_t)std::max(nLoff, 1) * bs);
-    DA(p->d_invL, (size_t)N * bs); DA(p->d_invT, (size_t)N * npad * 16);
+  else if (p->use_cg) {
+    // H, the N damped diagonal blocks and their inverses: no fill blocks, no off-diagonal factor blocks
+    const size_t nH = p->plan.hblocks.size();
+    LA(p->d_H, nH * bs); LA(p->d_Lb, (size_t)N * bs); LA(p->d_invL, (size_t)N * bs); LA(p->d_invT, (size_t)N * npad * 16);
+    p->d_T = nullptr;
+    LA(p->d_cg_slots, 2 * nH * npad); LA(p->d_cg_r, Upad); LA(p->d_cg_z, Upad); LA(p->d_cg_p, Upad); LA(p->d_cg_q, Upad);
+    LA(p->d_cg_part, (size_t)cg_partials(N)); LA(p->d_cg, 1);
+    std::vector<int> off, ids, frames(N);
+    cg_slot_lists(p->plan, N, off, ids);
+    for (int f = 0; f < N; ++f) frames[f] = f;
+    if ((rc = upload(p, &p->d_cg_off, off)) || (rc = upload(p, &p->d_cg_ids, ids)) || (rc = upload(p, &p->d_cg_frames, frames))) return rc;
+    p->linear_bytes += (int64_t)(off.size() + ids.size() + frames.size()) * sizeof(int);
+  } else {
+    LA(p->d_H, p->plan.hblocks.size() * bs); LA(p->d_Lb, (size_t)(N + nLoff) * bs); LA(p->d_T, (size_t)std::max(nLoff, 1) * bs);
+    LA(p->d_invL, (size_t)N * bs); LA(p->d_invT, (size_t)N * npad * 16);
   }
+#undef LA
 #undef DA
-  {
+  if (!p->use_cg) {
     // 2-D TMA view of the T buffer (off-diagonal factor blocks X_rk, row-major): inner = k, outer = block * npad + row, box [rb][16], 128-B swizzle
     bool encoded = false;
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
@@ -482,6 +510,10 @@ static int build_structure(rcvd_problem* p) {
   graph.insert(graph.end(), p->dpairs.frames.begin(), p->dpairs.frames.end());
   if (const char* e = make_factor_plan(p->plan, p->cfg, graph, p->trips.frames, p->order_slack, p->nranks, p->rank, p->dist_enabled, p->num_sms))
     return set_err(RCVD_ERR_INVALID, "%s", e);
+  // The solver: the block Cholesky while its storage fits the budget; conjugate gradients beyond it, on one GPU (the distributed
+  // factorisation of nranks > 1 spreads the factor over the ranks instead)
+  p->storage = linear_storage(p->plan, p->N, p->L.npad);
+  p->use_cg = p->nranks == 1 && !p->eval_only && p->storage.cholesky > (p->factor_budget >= 0 ? p->factor_budget : cholesky_budget(p->total_mem));
   while (p->ev_side.size() < 2 * p->plan.levels.size()) { cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); p->ev_side.push_back(e); }
   int rc;
   if ((rc = upload_plan(p)) || (rc = set_up_problem_data(p)) || (rc = allocate_storage(p))) return rc;
@@ -668,7 +700,7 @@ struct FactorSolve {
     for (int l = 0; l < LS; ++l) {
       const Level& lv = pl.levels[l];
       if ((rc = launch(LP_SUB_LEVEL, k_fwd_diag, dim3((npad + 7) / 8, lv.nframes), dim3(256), 0, st, false, p->d_invL, p->d_rhs, p->d_ytmp,
-                       p->d_lvl_frames + lv.frame_off, npad))) return rc;
+                       p->d_lvl_frames + lv.frame_off, npad, nullptr))) return rc;
       if (lv.nfwd > 0 && (rc = launch(LP_SUB_LEVEL, k_fwd_update, dim3((npad + 7) / 8, lv.nfwd), dim3(256), 0, st, false, p->d_T, p->d_ytmp, p->d_rhs,
                                       p->d_fwd_tasks + lv.fwd_off, npad))) return rc;
     }
@@ -685,7 +717,7 @@ struct FactorSolve {
       if (lv.nfwd > 0 && (rc = launch(LP_SUB_LEVEL, k_bwd_update, dim3((npad + 31) / 32, lv.nfwd), dim3(256), 0, st, false, p->d_T, p->d_y, p->d_ytmp,
                                       p->d_fwd_tasks + lv.fwd_off, npad))) return rc;
       if ((rc = launch(LP_SUB_LEVEL, k_bwd_diag, dim3((npad + 31) / 32, lv.nframes), dim3(256), 0, st, false, p->d_invL, p->d_ytmp, p->d_y,
-                       p->d_lvl_frames + lv.frame_off, npad))) return rc;
+                       p->d_lvl_frames + lv.frame_off, npad, nullptr))) return rc;
     }
     mark(P_SOLVE);
     return RCVD_OK;
@@ -751,6 +783,72 @@ static int factor_solve(rcvd_problem* p) {
   p->factored = true;
   return RCVD_OK;
 }
+
+// ---- block-Jacobi preconditioned conjugate gradients (rcvd_cg.cuh) ----
+// The preconditioner: the damped diagonal blocks of the frames, loaded, factored and inverted by the block Cholesky's per-frame kernels
+// over every frame at once -- the factorisation of the edgeless frame graph, which is exactly a block-diagonal factor.
+static int enqueue_cg_preconditioner(rcvd_problem* p) {
+  FactorSolve f(p);
+  const int N = p->N, npad = p->L.npad;
+  if (int rc = f.launch(LP_OTHER, k_load_factor, dim3((npad * npad + 255) / 256, N), dim3(256), 0, p->stream, false, p->d_H, p->d_Lb, p->d_lblocks,
+                        p->d_S, p->d_D2, npad, p->L.nf, p->plan.upd_neff, p->d_cg_frames, N, 0)) return rc;
+  if (int rc = f.factor_diagonal(p->d_cg_frames, N, false)) return rc;
+  return f.launch(LP_TRINV, k_trinv, dim3(npad / 16, N), dim3(256), p->fk.trinv_bytes, p->stream, false, p->d_Lb, p->d_invT, p->d_invL, p->d_cg_frames, npad);
+}
+
+// out = (S H S + D2) v and the per-frame partials of v.out; nothing once cg->stop is set (cg null: unconditionally)
+static int enqueue_cg_product(rcvd_problem* p, const double* v, double* out, const CgState* cg) {
+  const int N = p->N, npad = p->L.npad, nf = p->L.nf, nH = (int)p->plan.hblocks.size();
+  const size_t smem = (size_t)(3 * npad + 8 * 256) * sizeof(double);
+  if (int rc = launch(p, k_cg_spmv, nH, kCgThreads, smem, p->stream, false, p->d_H, p->d_hblocks, p->d_S, v, p->d_cg_slots, nH, npad, nf, cg)) return rc;
+  return launch(p, k_cg_gather, N, kCgThreads, 0, p->stream, false, p->d_cg_slots, p->d_cg_off, p->d_cg_ids, p->d_S, p->d_D2, v, out, p->d_cg_part, npad, nf, cg);
+}
+
+// Iteration i of the PCG on A = S H S + D2, b = gs, x = d_y (rcvd_cg.cuh gives the Ceres semantics it restates).
+static int enqueue_cg_iteration(rcvd_problem* p, int i) {
+  const int N = p->N, npad = p->L.npad, n = N * npad;
+  cudaStream_t st = p->stream; const int* stop = &p->d_cg->stop; double* x = p->d_y; int rc;
+  auto apply = [&](const double* v, double* out) { return enqueue_cg_product(p, v, out, p->d_cg); };
+  auto scalar = [&](int phase, int nparts) {
+    return launch(p, k_cg_scalar, 1, kCgThreads, 0, st, false, p->d_cg_part, nparts, p->d_cg, p->d_fail, phase, p->cg_eta, kCgMaxIterations);
+  };
+  auto step = [&](int mode) {
+    return launch(p, k_cg_step, kCgDotBlocks, kCgThreads, 0, st, false, x, p->d_cg_p, p->d_cg_r, p->d_cg_q, p->d_gs, p->d_cg_part, n, mode, p->d_cg);
+  };
+  // z = L^-T L^-1 r, rho = r.z, p = z + beta p
+  if ((rc = launch(p, k_fwd_diag, dim3((npad + 7) / 8, N), 256, 0, st, false, p->d_invL, p->d_cg_r, p->d_ytmp, p->d_cg_frames, npad, stop)) ||
+      (rc = launch(p, k_bwd_diag, dim3((npad + 31) / 32, N), 256, 0, st, false, p->d_invL, p->d_ytmp, p->d_cg_z, p->d_cg_frames, npad, stop)) ||
+      (rc = launch(p, k_cg_dot, kCgDotBlocks, kCgThreads, 0, st, false, p->d_cg_r, p->d_cg_z, p->d_cg_part, n, p->d_cg)) || (rc = scalar(CG_RHO, kCgDotBlocks)) ||
+      (rc = launch(p, k_cg_direction, kCgDotBlocks, kCgThreads, 0, st, false, p->d_cg_z, p->d_cg_p, n, p->d_cg)))
+    return rc;
+  // q = A p, alpha = rho / p.q, x += alpha p, r -= alpha q (or r = b - A x), the quadratic-model test
+  if ((rc = apply(p->d_cg_p, p->d_cg_q)) || (rc = scalar(CG_CURVATURE, N))) return rc;
+  if (i % kCgResetPeriod != 0) rc = step(0);
+  else if (!(rc = step(1)) && !(rc = apply(x, p->d_cg_q))) rc = step(2);
+  return rc ? rc : scalar(CG_MODEL, kCgDotBlocks);
+}
+
+// y = A^-1 gs by PCG: the preconditioner, then iterations in chunks of kCgChunk with one read of the stop flag after each chunk.
+static int cg_solve(rcvd_problem* p) {
+  cudaStream_t st = p->stream; int rc;
+  if ((rc = enqueue_cg_preconditioner(p)) ||
+      (rc = launch(p, k_cg_init, kCgDotBlocks, kCgThreads, 0, st, false, p->d_gs, p->d_y, p->d_cg_r, p->d_cg_part, p->N * p->L.npad)) ||
+      (rc = launch(p, k_cg_scalar, 1, kCgThreads, 0, st, false, p->d_cg_part, kCgDotBlocks, p->d_cg, p->d_fail, (int)CG_INIT, p->cg_eta, kCgMaxIterations)))
+    return rc;
+  CgState h;
+  for (int i = 1;; ) {
+    for (int k = 0; k < kCgChunk && i <= kCgMaxIterations; ++k, ++i) if ((rc = enqueue_cg_iteration(p, i))) return rc;
+    CK(cudaMemcpyAsync(&h, p->d_cg, sizeof(h), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h.stop || i > kCgMaxIterations) break;
+  }
+  p->cg_last = h.iterations; p->cg_iterations += h.iterations; p->cg_max = std::max(p->cg_max, h.iterations);
+  p->cg_capped += h.capped; p->cg_steps += 1;
+  return RCVD_OK;
+}
+
+// The damped solve y = (S H S + D2)^-1 gs of the path build_structure chose.
+static int linear_solve(rcvd_problem* p) { return p->use_cg ? cg_solve(p) : factor_solve(p); }
 
 // ---------------------------------------------------------------------------
 // Evaluation
@@ -918,7 +1016,7 @@ static int enqueue_damped_step(rcvd_problem* p, const rcvd_solve_options& o, dou
   const int npad = p->L.npad; const size_t Upad = (size_t)p->N * npad; cudaStream_t st = p->stream;
   int rc;
   if ((rc = launch(p, k_lm_prepare, nblk(Upad), 256, 0, st, false, p->d_diagH, p->d_S, p->d_g, p->d_lmdiag, p->d_D2, p->d_gs, (int)Upad, reuse ? 1 : 0, radius, o.min_lm_diagonal, o.max_lm_diagonal))) return rc;
-  if ((rc = factor_solve(p))) return rc;
+  if ((rc = linear_solve(p))) return rc;
   if ((rc = launch(p, k_mul, nblk(Upad), 256, 0, st, false, p->d_S, p->d_y, p->d_Sy, (int)Upad))) return rc;
   CK(cudaMemsetAsync(p->d_Hy, 0, Upad * sizeof(double), st));
   if ((rc = launch(p, k_spmv_sym, dim3((npad + 7) / 8, p->plan.dist ? (int)p->plan.own_hblocks.size() : (int)p->plan.hblocks.size()), 256, 0, st, false, p->d_H, p->d_hblocks, p->d_Sy, p->d_Hy, npad, p->plan.dist ? p->d_own_hblocks : nullptr))) return rc;
@@ -949,6 +1047,7 @@ static int lm_solve(rcvd_problem* p, const rcvd_solve_options& o, rcvd_solve_sum
   int rc = ensure_ready(p); if (rc) return rc;
   const Layout& L = p->L; const int N = p->N, npad = L.npad; const size_t Upad = (size_t)N * npad, U = (size_t)N * L.nf; cudaStream_t st = p->stream;
   const int64_t launches0 = p->launches;
+  p->cg_iterations = 0; p->cg_max = 0; p->cg_capped = 0; p->cg_steps = 0;
   sum.num_constraints = p->pairs.count();
   const bool constrained = p->cfg.depth_lower_bound && L.nd > 0;
   if (constrained && (rc = launch(p, k_project_state, nblk(U), 256, 0, st, false, p->cfg, L, p->d_in_range, p->d_x, N))) return rc;
@@ -1080,6 +1179,20 @@ RCVD_API void rcvd_default_solve_options(rcvd_solve_options* o) {
   o->max_lm_diagonal = 1e32; o->max_consecutive_invalid_steps = 5; o->jacobi_scaling = 1;
 }
 
+// cudaDeviceProp::totalGlobalMem of `device`, queried once per process: cudaGetDeviceProperties reads every property of the device, a
+// cost a handle created per solve should not pay each time
+static cudaError_t device_total_mem(int device, uint64_t* out) {
+  static std::mutex m; static std::map<int, uint64_t> cache;
+  std::lock_guard<std::mutex> lock(m);
+  auto it = cache.find(device);
+  if (it == cache.end()) {
+    cudaDeviceProp prop;
+    if (cudaError_t e = cudaGetDeviceProperties(&prop, device)) return e;
+    it = cache.emplace(device, (uint64_t)prop.totalGlobalMem).first;
+  }
+  *out = it->second;
+  return cudaSuccess;
+}
 RCVD_API int32_t rcvd_problem_create(const rcvd_config* cfg, int32_t device, rcvd_problem** out) {
   if (!cfg || !out) return set_err(RCVD_ERR_INVALID, "null argument");
   Layout L;
@@ -1094,7 +1207,8 @@ RCVD_API int32_t rcvd_problem_create(const rcvd_config* cfg, int32_t device, rcv
   p->cfg = *cfg; p->L = L; p->N = cfg->num_frames; p->device = device;
   p->in_range.assign(p->N, 1); p->median.assign(p->N, 1.0); p->h_state.assign((size_t)p->N * L.nf, 0.0);
   cudaError_t e = cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, device);   // read once: the plan and the launch shapes use it
-  if (e != cudaSuccess) { delete p; return set_err(RCVD_ERR_CUDA, "cudaDeviceGetAttribute(multiprocessor count): %s", cudaGetErrorString(e)); }
+  if (e == cudaSuccess) e = device_total_mem(device, &p->total_mem);                             // the solver choice (build_structure)
+  if (e != cudaSuccess) { delete p; return set_err(RCVD_ERR_CUDA, "cudaDeviceGetAttribute / cudaGetDeviceProperties: %s", cudaGetErrorString(e)); }
   // the critical chain (potrf -> trsm -> next-level updates) runs at the highest priority, the overlapped updates at the lowest,
   // so that a freed SM goes to the chain first
   int prio_lo = 0, prio_hi = 0; cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
@@ -1381,12 +1495,13 @@ static int solve_loaded(rcvd_problem* p, const double* S, const double* D2, cons
   CK(cudaMemcpyAsync(p->d_D2, hd.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
   CK(cudaMemcpyAsync(p->d_gs, hb.data(), Upad * 8, cudaMemcpyHostToDevice, p->stream));
   CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), p->stream));
-  int rc = factor_solve(p); if (rc) return rc;
+  int rc = linear_solve(p); if (rc) return rc;
   std::vector<double> hy(Upad);
   CK(cudaMemcpyAsync(hy.data(), p->d_y, Upad * 8, cudaMemcpyDeviceToHost, p->stream));
   rc = read_scalars(p); if (rc) return rc;
   frames_to_caller(uperm, hy.data(), npad, y, nf, nf);
-  if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, "factorisation hit a non-positive pivot");
+  if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, p->use_cg ? "conjugate gradients broke down, or a diagonal block hit a non-positive pivot"
+                                                          : "factorisation hit a non-positive pivot");
   return RCVD_OK;
 }
 // Debug/test: solve (S H S + diag(D2)) y = b with H = J^T J at the current state.
@@ -1401,7 +1516,7 @@ RCVD_API int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const
 // Test hook: (H + diag(D2)) y = b for a caller-supplied dense symmetric H (U x U, U = N * stride, caller's frame order) through the
 // production factorisation graph with S = 1.  H is scattered into the H blocks of the problem's frame graph (no evaluation); an entry
 // in a frame pair the graph does not couple is an error.
-RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
+static int debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
   if (!p || !H || !D2 || !b || !y) return set_err(RCVD_ERR_INVALID, "null argument");
   if (p->nranks > 1) return set_err(RCVD_ERR_INVALID, "rcvd_debug_solve_matrix works on single-GPU handles only");
   if (p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no factor storage");
@@ -1424,9 +1539,24 @@ RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const
   CK(cudaMemcpyAsync(p->d_H, hH.data(), hH.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
   return solve_loaded(p, nullptr, D2, b, y);
 }
+RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
+  return debug_solve_matrix(p, H, D2, b, y);
+}
+// Test hook: the same system through the conjugate-gradient path (a handle whose structure chose it); iterations = the CG iterations run.
+RCVD_API int32_t rcvd_debug_cg_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y, int32_t* iterations) {
+  if (!p || !iterations) return set_err(RCVD_ERR_INVALID, "null argument");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  if (!p->use_cg) return set_err(RCVD_ERR_INVALID, "this handle solves with the block Cholesky: a factor budget of 0 (rcvd_debug_set_factor_budget) selects conjugate gradients");
+  p->cg_last = 0;
+  rc = debug_solve_matrix(p, H, D2, b, y);
+  *iterations = p->cg_last;
+  return rc;
+}
 // Test hook: the factor the last factorisation left on the device (see include/rcvd_hooks.h).
 RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, double* Linv) {
   if (!p || !order || !L) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (p->structure_ready && p->use_cg) return set_err(RCVD_ERR_INVALID, "this handle solves with conjugate gradients: there is no factor");
   if (!p->structure_ready || !p->factored) return set_err(RCVD_ERR_INVALID, "no factorisation has run on this handle");
   if (p->plan.dist) return set_err(RCVD_ERR_INVALID, "the distributed factorisation keeps its blocks on their owners");
   SET_DEVICE(p->device);
@@ -1516,6 +1646,7 @@ RCVD_API int32_t rcvd_debug_profile_linear(rcvd_problem* p, int32_t reps, double
   if (!p || !out_ms || reps == 0) return set_err(RCVD_ERR_INVALID, "bad argument");
   SET_DEVICE(p->device);
   int rc = ensure_ready(p); if (rc) return rc;
+  if (p->use_cg) return set_err(RCVD_ERR_INVALID, "this handle solves with conjugate gradients: there is no factorisation to profile");
   const bool ov = p->overlap; if (!keep_overlap) p->overlap = false;
   for (int i = 0; i < 8; ++i) out_ms[i] = 0.0;
   std::vector<std::pair<int, cudaEvent_t>> evs;
@@ -1756,6 +1887,61 @@ RCVD_API int32_t rcvd_debug_update_items(const rcvd_config* cfg, int32_t np, con
   }
   Layout L; make_layout(*cfg, L);
   std::copy(need, need + 3, counts); counts[3] = pl.upd_neff; counts[4] = L.npad;
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_problem_linear_info(rcvd_problem* p, rcvd_linear_info* out) {
+  if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  *out = rcvd_linear_info{};
+  out->solver = p->use_cg ? RCVD_LINEAR_CG : RCVD_LINEAR_CHOLESKY;
+  out->factor_blocks = p->eval_only ? 0 : p->use_cg ? p->N : p->N + p->plan.nLoff + std::max(p->plan.nLoff, 1);
+  out->device_bytes = p->eval_only ? 0 : p->linear_bytes;
+  out->cholesky_bytes = p->storage.cholesky; out->cg_bytes = p->storage.cg;
+  out->budget_bytes = p->factor_budget >= 0 ? p->factor_budget : cholesky_budget(p->total_mem);
+  out->cg_iterations = p->cg_iterations; out->cg_max_iterations = p->cg_max; out->cg_capped_steps = p->cg_capped; out->cg_solves = p->cg_steps;
+  return RCVD_OK;
+}
+// Bench hook: mean device time (CUDA events, after one warm-up) of one CG matrix product (S H S + D2) p -- k_cg_spmv + k_cg_gather --
+// with the S, D2 and direction of the handle's last CG solve.
+RCVD_API int32_t rcvd_debug_time_cg_product(rcvd_problem* p, int32_t reps, double* ms) {
+  if (!p || !ms || reps <= 0) return set_err(RCVD_ERR_INVALID, "bad argument");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  if (!p->use_cg) return set_err(RCVD_ERR_INVALID, "this handle solves with the block Cholesky");
+  if ((rc = enqueue_cg_product(p, p->d_cg_p, p->d_cg_q, nullptr))) return rc;
+  CK(cudaEventRecord(p->ev[0], p->stream));
+  for (int i = 0; i < reps; ++i) if ((rc = enqueue_cg_product(p, p->d_cg_p, p->d_cg_q, nullptr))) return rc;
+  CK(cudaEventRecord(p->ev[1], p->stream));
+  CK(cudaStreamSynchronize(p->stream));
+  *ms = ev_ms(p->ev[0], p->ev[1]) / reps;
+  return RCVD_OK;
+}
+// Test hook: the storage budget of the block Cholesky (bytes; -1: the default, cholesky_budget of the device's memory).  The solver
+// is chosen again when the structure is next built.
+RCVD_API int32_t rcvd_debug_set_factor_budget(rcvd_problem* p, int64_t bytes) {
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  if (bytes < -1) return set_err(RCVD_ERR_INVALID, "factor budget must be >= 0, or -1 for the default (got %lld)", (long long)bytes);
+  if (int rc = drop_structure(p)) return rc;
+  p->factor_budget = bytes; return RCVD_OK;
+}
+// Test hook: the CG's q_tolerance eta (default kCgEta = 0.1, Ceres' Solver::Options::eta).
+RCVD_API int32_t rcvd_debug_set_cg_tolerance(rcvd_problem* p, double eta) {
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  if (!(eta > 0.0 && eta < 1.0)) return set_err(RCVD_ERR_INVALID, "CG tolerance must be in (0, 1) (got %g)", eta);
+  p->cg_eta = eta; return RCVD_OK;
+}
+// Test hook: both linear solvers' device storage for the plan of a frame graph, and the one a device of device_total_bytes selects --
+// host only, no handle, no device.
+RCVD_API int32_t rcvd_debug_linear_storage(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,
+                                           int32_t order_slack, uint64_t device_total_bytes, int64_t* cholesky_bytes, int64_t* cg_bytes, int32_t* solver) {
+  if (!cholesky_bytes || !cg_bytes || !solver) return set_err(RCVD_ERR_INVALID, "null argument");
+  FactorPlan pl;
+  if (int32_t rc = debug_plan(pl, cfg, np, pairs, nt, trip_centers, order_slack, 1, 0, 132)) return rc;
+  Layout L; make_layout(*cfg, L);
+  const LinearStorage ls = linear_storage(pl, cfg->num_frames, L.npad);
+  *cholesky_bytes = ls.cholesky; *cg_bytes = ls.cg;
+  *solver = ls.cholesky > cholesky_budget(device_total_bytes) ? RCVD_LINEAR_CG : RCVD_LINEAR_CHOLESKY;
   return RCVD_OK;
 }
 // Structure statistics (for DESIGN.md / bench): frames, off-diagonal factor blocks, levels, H blocks, npad.

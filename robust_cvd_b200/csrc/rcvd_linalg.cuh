@@ -717,9 +717,11 @@ __global__ void __launch_bounds__(128) k_trsm_ll(double* __restrict__ T, const d
 // ---------------------------------------------------------------------------
 // Triangular solves as GEMVs with inv(L_kk); vectors have npad stride per frame.
 // ---------------------------------------------------------------------------
-// y_k = inv(L_kk) rhs_k   (grid: (ceil(npad/8), frames in level), 256 threads = 8 warps, one row per warp)
+// y_k = inv(L_kk) rhs_k   (grid: (ceil(npad/8), frames in level), 256 threads = 8 warps, one row per warp).  k_fwd_diag and
+// k_bwd_diag do nothing when `stop` (nullable) points to a non-zero flag: the stop flag of the CG solve (rcvd_cg.cuh) they precondition.
 __global__ void __launch_bounds__(256) k_fwd_diag(const double* __restrict__ invL, const double* __restrict__ rhs, double* __restrict__ y,
-                                                   const int* __restrict__ frames, int npad) {
+                                                   const int* __restrict__ frames, int npad, const int* __restrict__ stop) {
+  if (stop && *stop) return;
   const int frame = frames[blockIdx.y];
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -772,7 +774,8 @@ __global__ void __launch_bounds__(256) k_bwd_update(const double* __restrict__ T
 }
 // x_k = inv(L_kk)^T y_k    (grid: (ceil(npad/32), frames in level)); same thread layout
 __global__ void __launch_bounds__(256) k_bwd_diag(const double* __restrict__ invL, const double* __restrict__ y, double* __restrict__ x,
-                                                   const int* __restrict__ frames, int npad) {
+                                                   const int* __restrict__ frames, int npad, const int* __restrict__ stop) {
+  if (stop && *stop) return;
   __shared__ double red[8][33];
   const int frame = frames[blockIdx.y];
   const int cl = threadIdx.x & 31, rg = threadIdx.x >> 5;

@@ -228,6 +228,15 @@ void DepthVideoPoseOptimizer::solveAndWriteBack(ProblemArrays& pa, const Params&
              sum.iterations, sum.initial_cost, sum.final_cost, sum.termination == RCVD_TERM_CONVERGENCE ? "CONVERGENCE" : sum.termination == RCVD_TERM_NO_CONVERGENCE ? "NO_CONVERGENCE" : "FAILURE",
              sum.message, sum.total_ms, (long long)sum.gpu_launches);
     logInfo(b);
+    rcvd_linear_info li;
+    checkStatus(rcvd_problem_linear_info(p, &li));
+    if (li.solver == RCVD_LINEAR_CG)
+      snprintf(b, sizeof(b), "rcvd linear solver: block-Jacobi preconditioned conjugate gradients (the block Cholesky needs %.1f GB, over its %.1f GB "
+               "budget): %lld iterations in %d steps, at most %d, %d steps at the cap of 500", li.cholesky_bytes / 1e9, li.budget_bytes / 1e9,
+               (long long)li.cg_iterations, li.cg_solves, li.cg_max_iterations, li.cg_capped_steps);
+    else
+      snprintf(b, sizeof(b), "rcvd linear solver: block Cholesky (%.1f GB)", li.device_bytes / 1e9);
+    logInfo(b);
     checkStatus(rcvd_problem_get_state(p, pa.state.data()));
   } catch (...) { rcvd_problem_destroy(p); throw; }
   rcvd_problem_destroy(p);

@@ -113,6 +113,18 @@ def update_items(cfg, pairs, trip_centers=(), order_slack=4, nranks=1, rank=0, n
     return {"items": items, "launches": launches.reshape(-1, 3, 2), "products": products, "neff": counts[3], "npad": counts[4]}
 
 
+def linear_storage(cfg, pairs, trip_centers=(), order_slack=4, device_total_bytes=0):
+    """Test hook: the device storage of both linear solvers for the frame graph of `pairs` and `trip_centers` under cfg on one GPU, and
+    the solver a device of device_total_bytes selects (host only, no device).  Returns {"cholesky_bytes", "cg_bytes", "solver"}
+    (abi.LINEAR_*)."""
+    pf = np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
+    tc = np.ascontiguousarray(np.asarray(trip_centers, np.int32).reshape(-1))
+    chol, cg, which = C.c_int64(), C.c_int64(), C.c_int32()
+    _check(lib().rcvd_debug_linear_storage(C.byref(cfg), C.c_int32(pf.shape[0]), _p(pf, C.c_int32), C.c_int32(tc.size), _p(tc, C.c_int32),
+                                           C.c_int32(order_slack), C.c_uint64(device_total_bytes), C.byref(chol), C.byref(cg), C.byref(which)))
+    return {"cholesky_bytes": chol.value, "cg_bytes": cg.value, "solver": which.value}
+
+
 class Problem:
     def __init__(self, cfg, device=0):
         self.cfg = cfg
@@ -227,6 +239,37 @@ class Problem:
         y = np.zeros(self.U, np.float64)
         _check(self.L.rcvd_debug_solve_matrix(self.h, _p(H, C.c_double), _p(D2, C.c_double), _p(b, C.c_double), _p(y, C.c_double)))
         return y
+
+    def cg_solve_matrix(self, H, D2, b):
+        """Test hook: solve_matrix through conjugate gradients, on a handle whose structure chose them (set_factor_budget(0)).
+        Returns (y, CG iterations)."""
+        H = np.ascontiguousarray(H, np.float64); D2 = np.ascontiguousarray(D2, np.float64); b = np.ascontiguousarray(b, np.float64)
+        assert H.shape == (self.U, self.U) and D2.size == self.U and b.size == self.U
+        y = np.zeros(self.U, np.float64); it = C.c_int32()
+        _check(self.L.rcvd_debug_cg_solve_matrix(self.h, _p(H, C.c_double), _p(D2, C.c_double), _p(b, C.c_double), _p(y, C.c_double), C.byref(it)))
+        return y, it.value
+
+    def linear_info(self):
+        """The linear solver the handle chose and its storage, and the CG iterations of the last solve (rcvd_linear_info; builds the
+        structure if needed).  Returns a dict of abi.LinearInfo's fields."""
+        out = abi.LinearInfo()
+        _check(self.L.rcvd_problem_linear_info(self.h, C.byref(out)))
+        return {name: getattr(out, name) for name, _ in abi.LinearInfo._fields_}
+
+    def time_cg_product(self, reps=20):
+        """Bench hook: mean device ms of one CG matrix product (S H S + D2) p, with the last CG solve's S, D2 and direction."""
+        ms = C.c_double()
+        _check(self.L.rcvd_debug_time_cg_product(self.h, C.c_int32(reps), C.byref(ms)))
+        return ms.value
+
+    def set_factor_budget(self, nbytes=-1):
+        """Test hook: the block Cholesky's storage budget in bytes (-1: the default, 4/5 of the device's memory; 0: conjugate gradients
+        on any single-GPU problem).  Takes effect when the structure is next built."""
+        _check(self.L.rcvd_debug_set_factor_budget(self.h, C.c_int64(nbytes)))
+
+    def set_cg_tolerance(self, eta=0.1):
+        """Test hook: the CG's quadratic-model tolerance eta (default 0.1)."""
+        _check(self.L.rcvd_debug_set_cg_tolerance(self.h, C.c_double(eta)))
 
     def factor_dense(self, inverses=False):
         """Test hook: (order, L, Linv) of the last factorisation -- caller's frame index of each eliminated frame, the dense lower factor
