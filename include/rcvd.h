@@ -248,6 +248,31 @@ int32_t rcvd_evaluate_rows(rcvd_problem* p, int32_t family, double* residuals, d
 /* Dense copy of the Gauss-Newton normal matrix J^T J at the current state
  * (row-major (N*stride)^2 doubles) -- test/debug entry point for small problems. */
 int32_t rcvd_normal_matrix_dense(rcvd_problem* p, double* H);
+/* Marginal covariance blocks of the parameters at the current state: restated Ceres semantics of ceres::Covariance
+ * (apply_loss_function = true, no sigma^2 scaling).  H = J^T J as rcvd_normal_matrix_dense returns it (every residual family,
+ * regularisers included, robust-loss corrector applied, no damping).  Rows and columns are exactly zero for parameters held constant
+ * by the configuration (fix_poses, fix_depth_xforms, fix_spatial_xforms, Fixed intrinsics), of out-of-range frames, that no residual
+ * touches, and that the caller holds for this call: hold[N * stride] (nullable; non-zero = held).  The problem has no gauge fixing
+ * of its own, so holding is how the caller removes the gauge (holding one frame's six pose parameters does, for the static-scene
+ * problem).  The call factors S H S (S = diag(H)^-1/2 over the free parameters, 1 on the diagonal of every zeroed one) with the
+ * block Cholesky and returns Cov = S (S H S)^-1 S on the requested blocks, by selected inversion of the factor.
+ *   frame_pairs [num_blocks][2]  caller's frames (a, b): any diagonal block (a, a), or a pair that shares a residual (a static pair,
+ *                                a depth pair, a triplet, the position regulariser, shared intrinsics)
+ *   out [num_blocks][stride][stride]  row-major Cov(x_a, x_b); the (b, a) block is exactly the transpose of the (a, b) block, a
+ *                                diagonal block is exactly symmetric
+ *   min_pivot_seen (nullable)    the smallest pivot of a free parameter up to the first one that fails the rank test
+ * Rank test: a pivot of S H S <= min_pivot (finite, >= 0; suggested 1e-10) fails with RCVD_ERR_NUMERIC, naming the caller's frame
+ * and parameter of the first such pivot in elimination order; nothing is written to out, and no pseudo-inverse is returned.  Ceres'
+ * min_reciprocal_condition_number = 1e-14 is too close to the noise of the pivots of a null direction of this problem (measured at
+ * -3e-14 .. -7e-16 on the scaled matrix) to separate them; with the gauge held the smallest pivots measured are ~1e-3 (8 frames) to
+ * ~9e-4 (100 frames), so 1e-10 sits between the two with margin.
+ * Refused with RCVD_ERR_INVALID, leaving the handle as it was: a null handle or out, num_blocks < 0, a frame out of range, a pair
+ * without a block of H, a handle with nranks > 1, and a handle that solves with conjugate gradients (no factor; rcvd_linear_info).
+ * The call builds the structure if needed, as rcvd_evaluate does; it leaves the state alone, and the next rcvd_solve runs as if
+ * the call had not happened.  Device memory beyond the block Cholesky's storage: the task lists of the selected inversion (kept
+ * with the structure), and per call at most 64 MB of output staging plus N * stride doubles of pivots. */
+int32_t rcvd_covariance(rcvd_problem* p, const uint8_t* hold, double min_pivot, int32_t num_blocks, const int32_t* frame_pairs,
+                        double* out, double* min_pivot_seen);
 /* Runs `iters` residual+Jacobian+accumulate passes (no solve) and returns the
  * mean device time per pass in ms -- the hot kernel in isolation (bench). */
 int32_t rcvd_time_accumulate(rcvd_problem* p, int32_t iters, double* ms_per_pass);

@@ -60,6 +60,17 @@ int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* 
 /* rcvd_debug_solve_matrix through conjugate gradients, on a handle whose structure chose them (a factor budget of 0); iterations = the
  * CG iterations run.  A handle on the Cholesky path: RCVD_ERR_INVALID; a CG breakdown or non-positive pivot: RCVD_ERR_NUMERIC. */
 int32_t rcvd_debug_cg_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y, int32_t* iterations);
+/* rcvd_covariance for a dense symmetric U x U matrix H (caller's frame order), scattered into the H blocks of the handle's frame graph
+ * as rcvd_debug_solve_matrix does (no evaluation), min_pivot 1e-10.  Only the parameters in hold (nullable) are zeroed: no active
+ * mask, configuration constants or frame range apply.  Refusals and the rank test as in rcvd_covariance. */
+int32_t rcvd_debug_covariance_matrix(rcvd_problem* p, const double* H, const uint8_t* hold, int32_t num_blocks, const int32_t* frame_pairs,
+                                     double* out);
+/* launches of the covariance kernels since the handle was created: {k_selinv_product, k_selinv_trmm, k_selinv_pivots, k_selinv_gather,
+ * k_selinv_scale} */
+int32_t rcvd_debug_covariance_launches(rcvd_problem* p, int64_t out[5]);
+/* the last rcvd_covariance call: out = {device ms of the factorisation with its rank test, of the selected inversion, of the gather and
+ * copy-out; algorithmic flops of the selected inversion (2 nf^3 per block product, nf^3 per triangular multiply); its block products} */
+int32_t rcvd_debug_covariance_profile(rcvd_problem* p, double out[5]);
 /* The storage of both linear solvers (rcvd_linear_info) for the frame graph of np pairs and nt triplet centres under cfg, on one GPU, and
  * the solver (RCVD_LINEAR_*) a device of device_total_bytes selects.  Host only: no handle, no device. */
 int32_t rcvd_debug_linear_storage(const rcvd_config* cfg, int32_t np, const int32_t* pairs, int32_t nt, const int32_t* trip_centers,

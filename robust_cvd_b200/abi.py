@@ -123,6 +123,12 @@ class LinearInfo(C.Structure):
                 ("cg_capped_steps", C.c_int32), ("cg_solves", C.c_int32)]
 
 
+# rcvd_covariance: the suggested rank-test threshold on the pivots of the Jacobi-scaled normal matrix (include/rcvd.h says why it is
+# not Ceres' min_reciprocal_condition_number), and the kernels rcvd_debug_covariance_launches counts
+COVARIANCE_MIN_PIVOT = 1e-10
+COVARIANCE_KERNELS = ("product", "trmm", "pivots", "gather", "scale")
+
+
 def default_config(num_frames, aspect, **kw):
     """Config with the reference's Params defaults (lib/PoseOptimizer.h:55-103)."""
     focal_long = kw.pop("focal_long", 0.3461538376301239)

@@ -23,6 +23,7 @@
 #include "rcvd_update.cuh"
 #include "rcvd_plan.h"
 #include "rcvd_cg.cuh"
+#include "rcvd_selinv.cuh"
 #include "rcvd_host.h"
 
 using namespace rcvd;
@@ -236,6 +237,12 @@ struct rcvd_problem {
   int *d_cg_frames = nullptr, *d_cg_off = nullptr, *d_cg_ids = nullptr; CgState* d_cg = nullptr;
   // CG iterations of the solves since the last rcvd_solve began (rcvd_problem_linear_info), and of the last solve alone
   int64_t cg_iterations = 0; int cg_max = 0, cg_capped = 0, cg_steps = 0, cg_last = 0;
+  // rcvd_covariance (rcvd_selinv.cuh): the selected inversion's task lists, built at the first call on a structure and dropped with it;
+  // launches of its kernels (product, trmm, pivots, gather, scale) and the last call's phase times (factorisation, selected inversion,
+  // gather, ms)
+  bool sel_ready = false; SelPlan sel;
+  SelTile* d_sel_tiles = nullptr; SelOp* d_sel_ops = nullptr; SelTrmm* d_sel_trmm = nullptr; int *d_sel_row_off = nullptr, *d_sel_row_blk = nullptr;
+  int64_t sel_launches[5] = {0}; double sel_ms[3] = {0.0, 0.0, 0.0};
   rcvd_problem() {}
 };
 
@@ -301,7 +308,7 @@ static void free_all(rcvd_problem* p) {
   p->allocs.clear();
   if (p->stream) cudaStreamSynchronize(p->stream);
   if (p->h_scal) { cudaFreeHost(p->h_scal); p->h_scal = nullptr; }
-  p->structure_ready = false; p->factored = false;
+  p->structure_ready = false; p->factored = false; p->sel_ready = false;
 }
 
 static DevProblem dev_problem(const rcvd_problem* p) {
@@ -1516,12 +1523,9 @@ RCVD_API int32_t rcvd_debug_linear_solve(rcvd_problem* p, const double* S, const
 // Test hook: (H + diag(D2)) y = b for a caller-supplied dense symmetric H (U x U, U = N * stride, caller's frame order) through the
 // production factorisation graph with S = 1.  H is scattered into the H blocks of the problem's frame graph (no evaluation); an entry
 // in a frame pair the graph does not couple is an error.
-static int debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
-  if (!p || !H || !D2 || !b || !y) return set_err(RCVD_ERR_INVALID, "null argument");
-  if (p->nranks > 1) return set_err(RCVD_ERR_INVALID, "rcvd_debug_solve_matrix works on single-GPU handles only");
-  if (p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no factor storage");
-  SET_DEVICE(p->device);
-  int rc = ensure_ready(p); if (rc) return rc;
+// H (dense U x U, caller's frame order) into the H blocks of the handle's frame graph; an entry in a frame pair the graph does not couple
+// is an error
+static int scatter_matrix(rcvd_problem* p, const double* H) {
   const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t U = (size_t)N * nf, bs = (size_t)npad * npad;
   std::vector<uint8_t> coupled((size_t)N * N, 0);
   for (const HBlock& hb : p->plan.hblocks) { const int a = p->plan.uperm[hb.r], c = p->plan.uperm[hb.c]; coupled[(size_t)a * N + c] = coupled[(size_t)c * N + a] = 1; }
@@ -1537,6 +1541,15 @@ static int debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2
     for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) hH[h * bs + (size_t)i * npad + j] = H[((size_t)a * nf + i) * U + (size_t)c * nf + j];
   }
   CK(cudaMemcpyAsync(p->d_H, hH.data(), hH.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+  return RCVD_OK;
+}
+static int debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
+  if (!p || !H || !D2 || !b || !y) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (p->nranks > 1) return set_err(RCVD_ERR_INVALID, "rcvd_debug_solve_matrix works on single-GPU handles only");
+  if (p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no factor storage");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  if ((rc = scatter_matrix(p, H))) return rc;
   return solve_loaded(p, nullptr, D2, b, y);
 }
 RCVD_API int32_t rcvd_debug_solve_matrix(rcvd_problem* p, const double* H, const double* D2, const double* b, double* y) {
@@ -1552,6 +1565,160 @@ RCVD_API int32_t rcvd_debug_cg_solve_matrix(rcvd_problem* p, const double* H, co
   rc = debug_solve_matrix(p, H, D2, b, y);
   *iterations = p->cg_last;
   return rc;
+}
+// ---- marginal covariance blocks (rcvd_covariance; rcvd_selinv.cuh) ----
+enum { SEL_PRODUCT = 0, SEL_TRMM, SEL_PIVOTS, SEL_GATHER, SEL_SCALE, SEL_N };   // rcvd_debug_covariance_launches
+template <class... Params, class... Args>
+static int sel_launch(rcvd_problem* p, int counter, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, Args... args) {
+  if (int rc = launch(p, kernel, grid, block, smem, p->stream, false, args...)) return rc;
+  p->sel_launches[counter]++;
+  return RCVD_OK;
+}
+// The task lists of the selected inversion, once per structure
+static int sel_prepare(rcvd_problem* p) {
+  if (p->sel_ready) return RCVD_OK;
+  make_sel_plan(p->sel, p->plan, p->N, p->L.npad, p->L.nf);
+  int rc;
+  if ((rc = upload(p, &p->d_sel_tiles, p->sel.tiles)) || (rc = upload(p, &p->d_sel_ops, p->sel.ops)) || (rc = upload(p, &p->d_sel_trmm, p->sel.trmm)) ||
+      (rc = upload(p, &p->d_sel_row_off, p->sel.row_off)) || (rc = upload(p, &p->d_sel_row_blk, p->sel.row_blk))) return rc;
+  CK(cudaFuncSetAttribute(k_selinv_trmm, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_trmm_smem_bytes(p->L.npad)));
+  p->sel_ready = true;
+  return RCVD_OK;
+}
+// The refusals that need no device
+static int covariance_args(rcvd_problem* p, int32_t n, const int32_t* pairs, const double* out, double min_pivot) {
+  if (!p) return set_err(RCVD_ERR_INVALID, "null problem");
+  if (!out || n < 0 || (n > 0 && !pairs)) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (!(min_pivot >= 0.0) || !std::isfinite(min_pivot)) return set_err(RCVD_ERR_INVALID, "min_pivot must be finite and >= 0 (got %g)", min_pivot);
+  if (p->nranks > 1) return set_err(RCVD_ERR_INVALID, "covariance of a sharded problem (nranks > 1) is not available");
+  if (p->eval_only) return set_err(RCVD_ERR_INVALID, "this handle was set to evaluation-only (rcvd_debug_set_eval_only): no factor storage");
+  for (int q = 0; q < 2 * n; ++q)
+    if (pairs[q] < 0 || pairs[q] >= p->N) return set_err(RCVD_ERR_INVALID, "covariance block %d: frame %d is out of range [0, %d)", q / 2, pairs[q], p->N);
+  return RCVD_OK;
+}
+// The refusals that need the structure, and the output blocks: a diagonal block, or the L block of an H block in either orientation
+static int covariance_blocks(rcvd_problem* p, int32_t n, const int32_t* pairs, std::vector<SelGather>& gl) {
+  if (p->use_cg) return set_err(RCVD_ERR_INVALID, "this handle solves with conjugate gradients (the block-Cholesky storage exceeds its budget): there is no factor to invert");
+  const FactorPlan& pl = p->plan; const int N = p->N;
+  gl.resize(n);
+  for (int q = 0; q < n; ++q) {
+    const int ia = pl.iperm[pairs[2 * q]], ib = pl.iperm[pairs[2 * q + 1]];
+    if (ia == ib) { gl[q] = {ia, 0, ia, ia}; continue; }
+    const int v = pl.blk_of[(size_t)ia * N + ib];
+    if (v < 0) return set_err(RCVD_ERR_INVALID, "covariance block %d: frames %d and %d share no residual, so the normal matrix has no block (%d, %d)", q,
+                              pairs[2 * q], pairs[2 * q + 1], pairs[2 * q], pairs[2 * q + 1]);
+    const HBlock& hb = pl.hblocks[v >> 1];
+    gl[q] = {hb.lblk, (v & 1) ? 0 : 1, hb.r, hb.c};
+  }
+  return RCVD_OK;
+}
+// Factorisation of S H S + D2 with the H already in d_H, the rank test, the selected inversion and the gather (see rcvd_covariance).
+// problem_masks: also zero the parameters no residual touches and the frames out of range.
+static int covariance_core(rcvd_problem* p, const uint8_t* hold, bool problem_masks, double min_pivot, const std::vector<SelGather>& gl, double* out,
+                           double* min_pivot_seen) {
+  const int N = p->N, nf = p->L.nf, npad = p->L.npad; const size_t Upad = (size_t)N * npad, nb = (size_t)nf * nf; cudaStream_t st = p->stream;
+  int rc;
+  if ((rc = sel_prepare(p))) return rc;
+  const std::vector<uint8_t> hh = hold ? frames_to_internal<uint8_t>(p->plan.uperm, hold, nf, npad, nf, 0) : std::vector<uint8_t>(Upad, 0);
+  // scratch: pivots [Upad] | output chunk | gather list | held mask
+  const size_t chunk = std::max<size_t>(1, std::min<size_t>(gl.size(), ((size_t)64 << 20) / (nb * sizeof(double))));
+  char* buf = nullptr;
+  CK(cudaMallocAsync((void**)&buf, (Upad + chunk * nb) * sizeof(double) + std::max<size_t>(gl.size(), 1) * sizeof(SelGather) + Upad, st));
+  double* d_piv = (double*)buf; double* d_out = d_piv + Upad; SelGather* d_gl = (SelGather*)(d_out + chunk * nb); uint8_t* d_hold = (uint8_t*)(d_gl + std::max<size_t>(gl.size(), 1));
+  std::vector<double> piv(Upad), D2(Upad);
+  const int* elim = p->plan.elim_order.data();
+  int fail_frame = -1, fail_param = -1; double seen = std::numeric_limits<double>::infinity(), fail_value = 0.0;
+  auto run = [&]() -> int {
+    int r2;
+    CK(cudaMemcpyAsync(d_hold, hh.data(), Upad, cudaMemcpyHostToDevice, st));
+    if (!gl.empty()) CK(cudaMemcpyAsync(d_gl, gl.data(), gl.size() * sizeof(SelGather), cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(p->ev[0], st));
+    if ((r2 = sel_launch(p, SEL_SCALE, k_selinv_scale, nblk(Upad), 256, 0, p->d_H, (const uint8_t*)d_hold, problem_masks ? (const uint8_t*)p->d_active : nullptr,
+                         problem_masks ? (const uint8_t*)p->d_in_range : nullptr, p->d_S, p->d_D2, N, npad, nf))) return r2;
+    CK(cudaMemsetAsync(p->d_gs, 0, Upad * sizeof(double), st));   // the factorisation graph's substitution solves for a zero right-hand side
+    CK(cudaMemsetAsync(p->d_fail, 0, sizeof(int), st));
+    if ((r2 = factor_solve(p))) return r2;
+    if ((r2 = sel_launch(p, SEL_PIVOTS, k_selinv_pivots, dim3((nf + 7) / 8, N), 256, 0, (const double*)p->d_H, (const double*)p->d_Lb, (const double*)p->d_T,
+                         (const double*)p->d_S, (const double*)p->d_D2, (const int*)p->d_sel_row_off, (const int*)p->d_sel_row_blk, npad, nf, d_piv))) return r2;
+    CK(cudaEventRecord(p->ev[1], st));
+    CK(cudaMemcpyAsync(piv.data(), d_piv, Upad * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(D2.data(), p->d_D2, Upad * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if ((r2 = read_scalars(p))) return r2;
+    // the rank test: the first free parameter in elimination order whose pivot is <= min_pivot
+    for (int q = 0; q < N && fail_frame < 0; ++q)
+      for (int i = 0; i < nf; ++i) {
+        const size_t v = (size_t)elim[q] * npad + i;
+        if (D2[v] != 0.0) continue;                     // zeroed: a unit pivot of its own
+        seen = std::min(seen, piv[v]);
+        if (!(piv[v] > min_pivot)) { fail_frame = p->plan.uperm[elim[q]]; fail_param = i; fail_value = piv[v]; break; }
+      }
+    if (min_pivot_seen) *min_pivot_seen = fail_frame >= 0 ? fail_value : seen;
+    if (fail_frame >= 0)
+      return set_err(RCVD_ERR_NUMERIC, "covariance: the Jacobi-scaled normal matrix is rank-deficient: pivot %.3e <= min_pivot %.3e at frame %d, parameter %d "
+                     "(hold the parameters of the gauge, e.g. one frame's pose)", fail_value, min_pivot, fail_frame, fail_param);
+    if (*p->h_fail) return set_err(RCVD_ERR_NUMERIC, "covariance: the factorisation hit a non-positive pivot");
+    // the selected inversion, levels in reverse
+    CK(cudaEventRecord(p->ev[2], st));
+    for (const SelLevel& sl : p->sel.levels) {
+      if (sl.n[0] > 0 && (r2 = sel_launch(p, SEL_PRODUCT, k_selinv_product, sl.n[0], kSelThreads, 0, p->d_Lb, (const double*)p->d_T, (const double*)p->d_invL,
+                                          (const SelTile*)p->d_sel_tiles + sl.off[0], (const SelOp*)p->d_sel_ops, npad, 1.0))) return r2;
+      if (sl.n[1] > 0 && (r2 = sel_launch(p, SEL_TRMM, k_selinv_trmm, dim3(npad / kSelStrip, sl.n[1]), kSelThreads, sel_trmm_smem_bytes(npad), p->d_Lb,
+                                          (const double*)p->d_invL, (const SelTrmm*)p->d_sel_trmm + sl.off[1], npad, -1.0, 0))) return r2;
+      if (sl.n[2] > 0 && (r2 = sel_launch(p, SEL_PRODUCT, k_selinv_product, sl.n[2], kSelThreads, 0, p->d_Lb, (const double*)p->d_T, (const double*)p->d_invL,
+                                          (const SelTile*)p->d_sel_tiles + sl.off[2], (const SelOp*)p->d_sel_ops, npad, -1.0))) return r2;
+      if (sl.n[3] > 0 && (r2 = sel_launch(p, SEL_TRMM, k_selinv_trmm, dim3(npad / kSelStrip, sl.n[3]), kSelThreads, sel_trmm_smem_bytes(npad), p->d_Lb,
+                                          (const double*)p->d_invL, (const SelTrmm*)p->d_sel_trmm + sl.off[3], npad, 1.0, 1))) return r2;
+    }
+    CK(cudaEventRecord(p->ev[3], st));
+    for (size_t c0 = 0; c0 < gl.size(); c0 += chunk) {
+      const size_t cnt = std::min(chunk, gl.size() - c0);
+      if ((r2 = sel_launch(p, SEL_GATHER, k_selinv_gather, dim3(nblk(nb), (unsigned)cnt), 256, 0, (const double*)p->d_Lb, (const double*)p->d_S,
+                           (const SelGather*)d_gl + c0, npad, nf, d_out))) return r2;
+      CK(cudaMemcpyAsync(out + c0 * nb, d_out, cnt * nb * sizeof(double), cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaEventRecord(p->ev[4], st));
+    CK(cudaStreamSynchronize(st));
+    p->sel_ms[0] = ev_ms(p->ev[0], p->ev[1]); p->sel_ms[1] = ev_ms(p->ev[2], p->ev[3]); p->sel_ms[2] = ev_ms(p->ev[3], p->ev[4]);
+    return RCVD_OK;
+  };
+  rc = run();
+  p->factored = false;                // Lb holds Z now, not the factor
+  cudaFreeAsync(buf, st);
+  const cudaError_t e = cudaStreamSynchronize(st);
+  if (rc) return rc;
+  if (e != cudaSuccess) return set_err(RCVD_ERR_CUDA, "rcvd_covariance: %s", cudaGetErrorString(e));
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_covariance(rcvd_problem* p, const uint8_t* hold, double min_pivot, int32_t num_blocks, const int32_t* frame_pairs, double* out,
+                                 double* min_pivot_seen) {
+  if (int rc = covariance_args(p, num_blocks, frame_pairs, out, min_pivot)) return rc;
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  std::vector<SelGather> gl;
+  if ((rc = covariance_blocks(p, num_blocks, frame_pairs, gl))) return rc;
+  if ((rc = enqueue_evaluate(p, p->d_x, true, true, p->d_g, SC_COST))) return rc;
+  return covariance_core(p, hold, true, min_pivot, gl, out, min_pivot_seen);
+}
+RCVD_API int32_t rcvd_debug_covariance_matrix(rcvd_problem* p, const double* H, const uint8_t* hold, int32_t num_blocks, const int32_t* frame_pairs,
+                                              double* out) {
+  if (int rc = covariance_args(p, num_blocks, frame_pairs, out, 1e-10)) return rc;
+  if (!H) return set_err(RCVD_ERR_INVALID, "null argument");
+  SET_DEVICE(p->device);
+  int rc = ensure_ready(p); if (rc) return rc;
+  std::vector<SelGather> gl;
+  if ((rc = covariance_blocks(p, num_blocks, frame_pairs, gl)) || (rc = scatter_matrix(p, H))) return rc;
+  return covariance_core(p, hold, false, 1e-10, gl, out, nullptr);
+}
+RCVD_API int32_t rcvd_debug_covariance_launches(rcvd_problem* p, int64_t out[5]) {
+  if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  std::copy(p->sel_launches, p->sel_launches + SEL_N, out);
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_debug_covariance_profile(rcvd_problem* p, double out[5]) {
+  if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  std::copy(p->sel_ms, p->sel_ms + 3, out);
+  out[3] = p->sel_ready ? p->sel.flops : 0.0; out[4] = p->sel_ready ? (double)p->sel.products : 0.0;
+  return RCVD_OK;
 }
 // Test hook: the factor the last factorisation left on the device (see include/rcvd_hooks.h).
 RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, double* Linv) {

@@ -225,6 +225,48 @@ class Problem:
         _check(self.L.rcvd_evaluate_rows(self.h, C.c_int32(fam), _p(r, C.c_double), _p(rho, C.c_double), _p(cols, C.c_int32), _p(J, C.c_double)))
         return (r, rho, cols, J) if jacobian else (r, rho)
 
+    def _covariance_args(self, pairs, hold):
+        pf = np.repeat(np.arange(self.N, dtype=np.int32)[:, None], 2, 1) if pairs is None else np.asarray(pairs, np.int32).reshape(-1, 2)
+        pf = np.ascontiguousarray(pf)
+        hd = None if hold is None else np.ascontiguousarray(np.asarray(hold).reshape(-1) != 0, np.uint8)
+        assert hd is None or hd.size == self.U
+        return pf, hd, np.zeros((pf.shape[0], self.stride, self.stride), np.float64)
+
+    def covariance(self, pairs=None, hold=None, min_pivot=abi.COVARIANCE_MIN_PIVOT):
+        """rcvd_covariance (ceres::Covariance, restated): the covariance blocks Cov(x_a, x_b) at the current state for `pairs` ([n, 2]
+        caller's frames; default every diagonal block (a, a)), with the parameters of `hold` ([N * stride] or [N, stride], non-zero =
+        held) and the configuration's constant parameters zeroed.  Returns [n, stride, stride]; the smallest free pivot of the rank test
+        is left in self.last_min_pivot.  A rank-deficient matrix (a pivot <= min_pivot) raises RuntimeError naming frame and parameter."""
+        pf, hd, out = self._covariance_args(pairs, hold)
+        seen = C.c_double()
+        _check(self.L.rcvd_covariance(self.h, _p(hd, C.c_uint8), C.c_double(min_pivot), C.c_int32(pf.shape[0]), _p(pf, C.c_int32), _p(out, C.c_double),
+                                      C.byref(seen)))
+        self.last_min_pivot = seen.value
+        return out
+
+    def covariance_matrix(self, H, pairs=None, hold=None):
+        """Test hook: covariance() of a dense symmetric H [U, U] (caller's frame order) scattered into the handle's H blocks; only the
+        parameters of `hold` are zeroed."""
+        H = np.ascontiguousarray(H, np.float64)
+        assert H.shape == (self.U, self.U)
+        pf, hd, out = self._covariance_args(pairs, hold)
+        _check(self.L.rcvd_debug_covariance_matrix(self.h, _p(H, C.c_double), _p(hd, C.c_uint8), C.c_int32(pf.shape[0]), _p(pf, C.c_int32),
+                                                   _p(out, C.c_double)))
+        return out
+
+    def covariance_launches(self):
+        """Test hook: launches of each covariance kernel since the handle was created (abi.COVARIANCE_KERNELS)."""
+        out = (C.c_int64 * len(abi.COVARIANCE_KERNELS))()
+        _check(self.L.rcvd_debug_covariance_launches(self.h, out))
+        return dict(zip(abi.COVARIANCE_KERNELS, list(out)))
+
+    def covariance_profile(self):
+        """Bench hook: the last covariance() call's device ms of the factorisation (with the rank test), the selected inversion and the
+        gather, and the selected inversion's algorithmic flops and block products."""
+        out = (C.c_double * 5)()
+        _check(self.L.rcvd_debug_covariance_profile(self.h, out))
+        return dict(zip(("factor_ms", "selinv_ms", "gather_ms", "selinv_flops", "selinv_products"), list(out)))
+
     def debug_linear_solve(self, S, D2, b):
         S = np.ascontiguousarray(S, np.float64); D2 = np.ascontiguousarray(D2, np.float64)
         b = np.ascontiguousarray(b, np.float64); y = np.zeros_like(b)
