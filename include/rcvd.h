@@ -465,6 +465,31 @@ int32_t rcvd_prune_static_flags(int32_t device, int32_t num_frames, int32_t heig
                                 int32_t num_pairs, const int32_t* pair_frames, const int64_t* pair_offsets, const float* pair_locs, uint8_t* pair_static,
                                 int32_t num_triplets, const int32_t* trip_centres, const int64_t* trip_offsets, const float* trip_locs, uint8_t* trip_static);
 
+/* ---- flow-consistency masks (DESIGN.md section 1 row 8f-8) ----
+ * Replaces consistent_flow_masks (reference utils/consistency.py, called by Flow.compute_flow_masks, flow.py:180-209) for a batch of
+ * frame pairs (i, j).  For direction i -> j at pixel (x, y) with flow (u, v) = flow_ij: the target position (x + u, y + v) in float64
+ * must lie in [0, width-1] x [0, height-1]; grid_sample(bilinear, border, align_corners=False) of -flow_ji and of colour j at that
+ * position, with the grid coordinate 2 X / W - 1 rounded from float64 to float32 and the sampling in float32 as torch's vectorised CPU
+ * kernel computes it (fused multiply-adds); then sse(flow_ij, sample) < flow_thresh_sq and sse(colour i, sample) < color_thresh_sq,
+ * sse = d0^2 + d1^2 (+ d2^2) in float32 in that order.  The mask is the AND of the three tests; a NaN fails.  Direction j -> i likewise.
+ *   pair_frames [num_pairs][2]  local colour ids (i, j) in [0, num_frames): a frame shared by several pairs is passed once
+ *   flow_ij / flow_ji [num_pairs][height][width][2] f32, colors [num_frames][height][width][3] f32 (BGR; any channel order works)
+ *   mask_ij / mask_ji [num_pairs][height][width] u8 0 / 255 (out)
+ *   counts      [num_pairs][2] (nullable) non-zero pixels of mask_ij, mask_ji
+ *   sse_flow / sse_color [num_pairs][2][height][width] f32 (nullable) the two sse values per direction (0: i -> j, 1: j -> i); NaN
+ *               where the target position is NaN (torch samples something unspecified there; the mask is 0 either way)
+ * Thresholds are float32, as the reference's comparison of a float32 array with a Python number is: flow_thresh^2 and
+ * 3 * color_thresh^2.  num_pairs = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null
+ * parameter block or array, a non-positive size or frame count, width * height >= 2^31, a negative pair count, a NaN threshold, a
+ * pair frame out of range. */
+typedef struct rcvd_flow_mask_params {
+  int32_t width, height, num_pairs, num_frames;
+  float flow_thresh_sq;            /* float32(flow_thresh^2) */
+  float color_thresh_sq;           /* float32(3 * color_thresh^2) */
+} rcvd_flow_mask_params;
+int32_t rcvd_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij, const float* flow_ji,
+                        const float* colors, uint8_t* mask_ij, uint8_t* mask_ji, int64_t* counts, float* sse_flow, float* sse_color);
+
 #ifdef __cplusplus
 }
 #endif

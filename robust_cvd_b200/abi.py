@@ -97,6 +97,12 @@ class TrackParams(C.Structure):
 
 TRACK_IN_RANGE, TRACK_HAS_COLOR, TRACK_FLOW, TRACK_MASK = 1, 2, 4, 8   # rcvd_compute_tracks frame flags
 
+
+class FlowMaskParams(C.Structure):
+    """rcvd_flow_mask_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_pairs", "num_frames")] + \
+               [("flow_thresh_sq", C.c_float), ("color_thresh_sq", C.c_float)]
+
 # residual families of rcvd_evaluate_rows, in the order of rcvd_row_layout::family
 ROWS_PAIRS, ROWS_TRIPLETS, ROWS_DEPTH_PAIRS, ROWS_REGULARISERS = range(4)
 ROW_FAMILIES = ("pairs", "triplets", "depth_pairs", "regularisers")

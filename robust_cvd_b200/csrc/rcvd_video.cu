@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, and long point tracks.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks and the flow-consistency masks.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -15,6 +15,7 @@
 #include "rcvd_bilateral.cuh"
 #include "rcvd_builder.cuh"
 #include "rcvd_tracks.cuh"
+#include "rcvd_flowmask.cuh"
 
 using namespace rcvd;
 
@@ -631,4 +632,88 @@ RCVD_API int32_t rcvd_compute_tracks(const rcvd_track_params* prm, int32_t devic
   if (total > capacity || (total > 0 && (!obs_track || !obs_loc))) return set_err(RCVD_ERR_INVALID, "output capacity too small: %lld observations", (long long)total);
   if (total > 0) { std::memcpy(obs_track, ids.data(), (size_t)total * 4); std::memcpy(obs_loc, locs.data(), (size_t)total * 8); }
   return RCVD_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Flow-consistency masks (rcvd_flowmask.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_flowmask_launches = 0;
+RCVD_API int64_t rcvd_flow_mask_launch_count() { return g_flowmask_launches; }
+// The argument rules of rcvd_flow_masks, checked on the host before any device is needed.
+static int check_flow_mask_args(const rcvd_flow_mask_params* prm, const int32_t* pair_frames, const float* flow_ij, const float* flow_ji, const float* colors) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_flow_mask_params& q = *prm;
+  if (q.width <= 0 || q.height <= 0 || q.num_frames <= 0 || q.num_pairs < 0 || (int64_t)q.width * q.height >= (int64_t(1) << 31) ||
+      std::isnan(q.flow_thresh_sq) || std::isnan(q.color_thresh_sq))
+    return set_err(RCVD_ERR_INVALID, "bad flow-mask parameters");
+  if (q.num_pairs > 0 && (!pair_frames || !flow_ij || !flow_ji || !colors)) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int i = 0; i < 2 * q.num_pairs; ++i)
+    if (pair_frames[i] < 0 || pair_frames[i] >= q.num_frames) return set_err(RCVD_ERR_INVALID, "pair %d out of range", i / 2);
+  return RCVD_OK;
+}
+// Uploads the inputs of rcvd_flow_masks and allocates its outputs on the call's device; a.pair0 is left for the launches.
+static FlowMaskArgs upload_flow_mask_inputs(VideoCall& call, const rcvd_flow_mask_params& q, const int32_t* pair_frames, const float* flow_ij,
+                                            const float* flow_ji, const float* colors, bool counts, bool sse_flow, bool sse_color) {
+  const size_t P = q.num_pairs, plane = (size_t)q.width * q.height;
+  FlowMaskArgs a{};
+  a.w = q.width; a.h = q.height; a.flow_thresh_sq = q.flow_thresh_sq; a.color_thresh_sq = q.color_thresh_sq;
+  a.pair_frames = (const int*)call.upload(pair_frames, P * 8);
+  a.flow_ij = (const float*)call.upload(flow_ij, P * plane * 8); a.flow_ji = (const float*)call.upload(flow_ji, P * plane * 8);
+  a.colors = (const float*)call.upload(colors, (size_t)q.num_frames * plane * 12);
+  a.mask_ij = (uint8_t*)call.alloc(P * plane); a.mask_ji = (uint8_t*)call.alloc(P * plane);
+  a.counts = counts ? (unsigned long long*)call.alloc(P * 16) : nullptr;
+  a.sse_flow = sse_flow ? (float*)call.alloc(P * plane * 8) : nullptr;
+  a.sse_color = sse_color ? (float*)call.alloc(P * plane * 8) : nullptr;
+  return a;
+}
+// every pair in launches of at most 65535 (grid.y) pairs
+static int launch_flow_masks(VideoCall& call, FlowMaskArgs a, int P) {
+  if (a.counts) cudaMemsetAsync(a.counts, 0, (size_t)P * 16, call.st);
+  const unsigned gx = (unsigned)nblk((size_t)a.w * a.h, kFmThreads);
+  for (int p0 = 0; p0 < P; p0 += 65535) {
+    a.pair0 = p0;
+    if (int rc = call.launch(k_flow_masks, dim3(gx, std::min(65535, P - p0), 2), kFmThreads, 0, a)) return rc;
+  }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij, const float* flow_ji,
+                                 const float* colors, uint8_t* mask_ij, uint8_t* mask_ji, int64_t* counts, float* sse_flow, float* sse_color) {
+  if (int rc = check_flow_mask_args(prm, pair_frames, flow_ij, flow_ji, colors)) return rc;
+  const rcvd_flow_mask_params& q = *prm;
+  if (q.num_pairs > 0 && (!mask_ij || !mask_ji)) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (q.num_pairs == 0) return RCVD_OK;
+  VideoCall call;
+  if (int rc = call.open(device, g_flowmask_launches)) return rc;
+  const size_t P = q.num_pairs, plane = (size_t)q.width * q.height;
+  const FlowMaskArgs a = upload_flow_mask_inputs(call, q, pair_frames, flow_ij, flow_ji, colors, counts != nullptr, sse_flow != nullptr, sse_color != nullptr);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_flow_masks");
+  if (int rc = launch_flow_masks(call, a, q.num_pairs)) return rc;
+  cudaMemcpyAsync(mask_ij, a.mask_ij, P * plane, cudaMemcpyDeviceToHost, call.st);
+  cudaMemcpyAsync(mask_ji, a.mask_ji, P * plane, cudaMemcpyDeviceToHost, call.st);
+  if (counts) cudaMemcpyAsync(counts, a.counts, P * 16, cudaMemcpyDeviceToHost, call.st);   // unsigned long long -> int64_t: counts < 2^31
+  if (sse_flow) cudaMemcpyAsync(sse_flow, a.sse_flow, P * plane * 8, cudaMemcpyDeviceToHost, call.st);
+  if (sse_color) cudaMemcpyAsync(sse_color, a.sse_color, P * plane * 8, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("flow-mask kernel");
+}
+RCVD_API int32_t rcvd_debug_time_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij,
+                                            const float* flow_ji, const float* colors, int32_t reps, double* ms) {
+  if (int rc = check_flow_mask_args(prm, pair_frames, flow_ij, flow_ji, colors)) return rc;
+  if (reps < 1 || !ms || prm->num_pairs == 0) return set_err(RCVD_ERR_INVALID, "bad timing arguments");
+  VideoCall call;
+  if (int rc = call.open(device, g_flowmask_launches)) return rc;
+  const FlowMaskArgs a = upload_flow_mask_inputs(call, *prm, pair_frames, flow_ij, flow_ji, colors, true, false, false);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_flow_masks");
+  if (int rc = launch_flow_masks(call, a, prm->num_pairs)) return rc;   // warm-up
+  cudaEvent_t e0, e1;
+  CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+  cudaEventRecord(e0, call.st);
+  int rc = RCVD_OK;
+  for (int r = 0; r < reps && rc == RCVD_OK; ++r) rc = launch_flow_masks(call, a, prm->num_pairs);
+  cudaEventRecord(e1, call.st);
+  if (rc == RCVD_OK) rc = call.sync("flow-mask timing");
+  float t = 0.f;
+  if (rc == RCVD_OK) cudaEventElapsedTime(&t, e0, e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  *ms = (double)t / reps;
+  return rc;
 }

@@ -583,6 +583,39 @@ def prune_static_flags(num_frames, height, width, distance, pair_frames, pair_of
     return ps, ts
 
 
+def _flow_mask_args(colors, pair_frames, flow_ij, flow_ji, flow_thresh_sq, color_thresh_sq):
+    col = np.ascontiguousarray(colors, np.float32)
+    pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
+    fij = np.ascontiguousarray(flow_ij, np.float32); fji = np.ascontiguousarray(flow_ji, np.float32)
+    F, h, w = col.shape[:3]
+    if col.shape != (F, h, w, 3) or fij.shape != (len(pf), h, w, 2) or fji.shape != fij.shape:
+        raise ValueError(f"flow-mask inputs of shapes colours {col.shape}, flows {fij.shape} / {fji.shape} for {len(pf)} pairs")
+    prm = abi.FlowMaskParams(width=w, height=h, num_pairs=len(pf), num_frames=F, flow_thresh_sq=flow_thresh_sq, color_thresh_sq=color_thresh_sq)
+    return prm, (_p(pf, C.c_int32), _p(fij, C.c_float), _p(fji, C.c_float), _p(col, C.c_float)), (pf, fij, fji, col)
+
+
+def flow_masks(colors, pair_frames, flow_ij, flow_ji, flow_thresh_sq=1.0, color_thresh_sq=3.0, want_sse=False, device=0):
+    """rcvd_flow_masks (consistent_flow_masks, reference utils/consistency.py) on the GPU.  colors [F,h,w,3] f32, pair_frames [P,2] local
+    colour ids, flow_ij / flow_ji [P,h,w,2] f32; thresholds as float32 (flow_thresh^2, 3 color_thresh^2).  Returns (mask_ij [P,h,w] u8
+    0/255, mask_ji, counts [P,2] i64) and with want_sse also (sse_flow, sse_color) [P,2,h,w] f32 (direction 0: i -> j)."""
+    prm, args, keep = _flow_mask_args(colors, pair_frames, flow_ij, flow_ji, flow_thresh_sq, color_thresh_sq)
+    P, h, w = prm.num_pairs, prm.height, prm.width
+    mij = np.zeros((P, h, w), np.uint8); mji = np.zeros((P, h, w), np.uint8); cnt = np.zeros((P, 2), np.int64)
+    sf = np.zeros((P, 2, h, w), np.float32) if want_sse else None
+    sc = np.zeros((P, 2, h, w), np.float32) if want_sse else None
+    _check(lib().rcvd_flow_masks(C.byref(prm), C.c_int32(device), *args, _p(mij, C.c_uint8), _p(mji, C.c_uint8), _p(cnt, C.c_int64),
+                                 _p(sf, C.c_float), _p(sc, C.c_float)))
+    return (mij, mji, cnt, sf, sc) if want_sse else (mij, mji, cnt)
+
+
+def time_flow_masks(colors, pair_frames, flow_ij, flow_ji, reps=50, flow_thresh_sq=1.0, color_thresh_sq=3.0, device=0):
+    """Bench hook: mean device ms of one rcvd_flow_masks kernel pass over all the pairs (inputs uploaded once, CUDA events)."""
+    prm, args, keep = _flow_mask_args(colors, pair_frames, flow_ij, flow_ji, flow_thresh_sq, color_thresh_sq)
+    ms = C.c_double()
+    _check(lib().rcvd_debug_time_flow_masks(C.byref(prm), C.c_int32(device), *args, C.c_int32(reps), C.byref(ms)))
+    return ms.value
+
+
 FP64_MMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
 
 
