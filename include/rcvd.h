@@ -490,6 +490,33 @@ typedef struct rcvd_flow_mask_params {
 int32_t rcvd_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij, const float* flow_ji,
                         const float* colors, uint8_t* mask_ij, uint8_t* mask_ji, int64_t* counts, float* sse_flow, float* sse_color);
 
+/* ---- flow visualisations (DESIGN.md section 1 row 8f-9) ----
+ * Replaces the per-pair work of Flow.visualize_flow (reference flow.py:128-178) for a batch of frame pairs (i, j):
+ *   vis      the composite vis_flow/frame_i_j.png, [2 height][4 width] pixels: the top row [255 colour i, 255 colour j, flow_to_image(flow_ij),
+ *            flow_to_image(flow_ji)], the bottom row the same tiles through apply_mask (mask_ij on the i tiles, mask_ji on the j tiles);
+ *   warp_ij  vis_flow_warped/frame_i_j_warped.png, colour j sampled at pixel + flow_ij; warp_ji: colour i sampled at pixel + flow_ji.
+ * Arithmetic as the reference's under numpy 2 (DESIGN.md row 8f-9): the flow colouring in float64 after a float32 max-rad reduction
+ * (max(-1, nan) = -1 negates a flow holding a NaN), the colour tiles in float32, the conversion to 8 bits as cv2.imwrite's (round half
+ * to even, saturate); the warp as torch's CUDA grid_sample(bilinear, border, align_corners=False) of the grid 2 uv / (W-1, H-1) - 1.
+ *   pair_frames [num_pairs][2]  local colour ids (i, j) in [0, num_frames): a frame shared by several pairs is passed once
+ *   flow_ij / flow_ji [num_pairs][height][width][2] f32; mask_ij / mask_ji [num_pairs][height][width] u8 (a pixel is masked in when > 0)
+ *   colors      [num_frames][height][width][3] f32, the colour files' values in [0, 1] and channel order (BGR)
+ *   vis         [num_pairs][2 height][4 width][3] u8 (out), PNG (RGB) byte order
+ *   warp_ij / warp_ji [num_pairs][height][width][3] u8 (out, PNG byte order): written when prm->warp != 0, and then not null
+ *   warp_values [num_pairs][2][height][width][3] f32 (nullable, with warp) the warp values before rounding, array channel order
+ *   maxrad      [num_pairs][2] f32 (nullable) each flow's max of sqrt(u^2 + v^2) over its non-NaN pixels, unknown ones (|u| or |v| > 1e7)
+ *               zeroed; has_nan [num_pairs][2] u8 (nullable) 1 where a rad is NaN (the flow is then divided by -1 + eps)
+ * num_pairs = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null parameter block or array,
+ * width or height < 2 (the reference's grid divides by width - 1 and height - 1), num_frames <= 0, 8 * width * height >= 2^31, a negative
+ * pair count, a pair frame out of range. */
+typedef struct rcvd_flow_vis_params {
+  int32_t width, height, num_pairs, num_frames;
+  int32_t warp;                    /* nonzero: also the two warps */
+} rcvd_flow_vis_params;
+int32_t rcvd_flow_visualize(const rcvd_flow_vis_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij, const float* flow_ji,
+                            const uint8_t* mask_ij, const uint8_t* mask_ji, const float* colors, uint8_t* vis, uint8_t* warp_ij, uint8_t* warp_ji,
+                            float* warp_values, float* maxrad, uint8_t* has_nan);
+
 #ifdef __cplusplus
 }
 #endif

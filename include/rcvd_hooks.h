@@ -15,6 +15,7 @@ int64_t rcvd_builder_launch_count(void);
 int64_t rcvd_static_flag_launch_count(void);
 int64_t rcvd_tracks_launch_count(void);
 int64_t rcvd_flow_mask_launch_count(void);
+int64_t rcvd_flow_vis_launch_count(void);
 /* rcvd_flow_masks' kernel alone: the inputs are uploaded once, the kernel (with counts) runs reps times between two CUDA events, and
  * *ms is the mean device time of one launch over all the pairs.  Arguments and refusals as rcvd_flow_masks; reps >= 1. */
 int32_t rcvd_debug_time_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij,

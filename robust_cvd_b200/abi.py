@@ -103,6 +103,11 @@ class FlowMaskParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_pairs", "num_frames")] + \
                [("flow_thresh_sq", C.c_float), ("color_thresh_sq", C.c_float)]
 
+
+class FlowVisParams(C.Structure):
+    """rcvd_flow_vis_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_pairs", "num_frames", "warp")]
+
 # residual families of rcvd_evaluate_rows, in the order of rcvd_row_layout::family
 ROWS_PAIRS, ROWS_TRIPLETS, ROWS_DEPTH_PAIRS, ROWS_REGULARISERS = range(4)
 ROW_FAMILIES = ("pairs", "triplets", "depth_pairs", "regularisers")

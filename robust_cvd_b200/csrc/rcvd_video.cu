@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks and the flow-consistency masks.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks and the flow visualisations.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -16,6 +16,7 @@
 #include "rcvd_builder.cuh"
 #include "rcvd_tracks.cuh"
 #include "rcvd_flowmask.cuh"
+#include "rcvd_flowvis.cuh"
 
 using namespace rcvd;
 
@@ -716,4 +717,64 @@ RCVD_API int32_t rcvd_debug_time_flow_masks(const rcvd_flow_mask_params* prm, in
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   *ms = (double)t / reps;
   return rc;
+}
+
+// ---------------------------------------------------------------------------
+// Flow visualisations (rcvd_flowvis.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_flowvis_launches = 0;
+RCVD_API int64_t rcvd_flow_vis_launch_count() { return g_flowvis_launches; }
+RCVD_API int32_t rcvd_flow_visualize(const rcvd_flow_vis_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij,
+                                     const float* flow_ji, const uint8_t* mask_ij, const uint8_t* mask_ji, const float* colors, uint8_t* vis,
+                                     uint8_t* warp_ij, uint8_t* warp_ji, float* warp_values, float* maxrad, uint8_t* has_nan) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_flow_vis_params& q = *prm;
+  if (q.width < 2 || q.height < 2 || q.num_frames <= 0 || q.num_pairs < 0 || 8 * (int64_t)q.width * q.height >= (int64_t(1) << 31))
+    return set_err(RCVD_ERR_INVALID, "bad flow-visualisation parameters");
+  if (q.num_pairs == 0) return RCVD_OK;
+  if (!pair_frames || !flow_ij || !flow_ji || !mask_ij || !mask_ji || !colors || !vis || (q.warp && (!warp_ij || !warp_ji)))
+    return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int i = 0; i < 2 * q.num_pairs; ++i)
+    if (pair_frames[i] < 0 || pair_frames[i] >= q.num_frames) return set_err(RCVD_ERR_INVALID, "pair %d out of range", i / 2);
+  VideoCall call;
+  if (int rc = call.open(device, g_flowvis_launches)) return rc;
+  const size_t P = q.num_pairs, plane = (size_t)q.width * q.height;
+  FlowVisArgs a{};
+  a.w = q.width; a.h = q.height;
+  a.pair_frames = (const int*)call.upload(pair_frames, P * 8);
+  a.flow_ij = (const float*)call.upload(flow_ij, P * plane * 8); a.flow_ji = (const float*)call.upload(flow_ji, P * plane * 8);
+  a.mask_ij = (const uint8_t*)call.upload(mask_ij, P * plane); a.mask_ji = (const uint8_t*)call.upload(mask_ji, P * plane);
+  a.colors = (const float*)call.upload(colors, (size_t)q.num_frames * plane * 12);
+  a.stats = (unsigned*)call.alloc(P * 16);
+  a.vis = (uint8_t*)call.alloc(P * plane * 24);
+  if (q.warp) {
+    a.warp_ij = (uint8_t*)call.alloc(P * plane * 3); a.warp_ji = (uint8_t*)call.alloc(P * plane * 3);
+    if (warp_values) a.warp_values = (float*)call.alloc(P * plane * 24);
+  }
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_flow_visualize");
+  cudaMemsetAsync(a.stats, 0, P * 16, call.st);
+  const unsigned gx = (unsigned)nblk(plane, kFvThreads);
+  for (int p0 = 0; p0 < q.num_pairs; p0 += 65535) {     // grid.y <= 65535 pairs per launch
+    a.pair0 = p0;
+    const unsigned np = (unsigned)std::min(65535, q.num_pairs - p0);
+    if (int rc = call.launch(k_flow_vis_stats, dim3(gx, np, 2), kFvThreads, 0, a)) return rc;
+    if (int rc = call.launch(k_flow_vis, dim3(gx, np), kFvThreads, 0, a)) return rc;
+  }
+  cudaMemcpyAsync(vis, a.vis, P * plane * 24, cudaMemcpyDeviceToHost, call.st);
+  if (q.warp) {
+    cudaMemcpyAsync(warp_ij, a.warp_ij, P * plane * 3, cudaMemcpyDeviceToHost, call.st);
+    cudaMemcpyAsync(warp_ji, a.warp_ji, P * plane * 3, cudaMemcpyDeviceToHost, call.st);
+    if (warp_values) cudaMemcpyAsync(warp_values, a.warp_values, P * plane * 24, cudaMemcpyDeviceToHost, call.st);
+  }
+  std::vector<unsigned> st;
+  if (maxrad || has_nan) {
+    st.resize(P * 4);
+    cudaMemcpyAsync(st.data(), a.stats, P * 16, cudaMemcpyDeviceToHost, call.st);
+  }
+  if (int rc = call.sync("flow-visualisation kernels")) return rc;
+  for (size_t k = 0; k < 2 * P && !st.empty(); ++k) {
+    if (maxrad) std::memcpy(maxrad + k, &st[2 * k], 4);
+    if (has_nan) has_nan[k] = st[2 * k + 1] ? 1 : 0;
+  }
+  return RCVD_OK;
 }

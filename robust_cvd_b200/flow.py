@@ -1,11 +1,13 @@
-"""Flow-consistency masks and pair mask ratios of a robust_cvd working directory, with the mask arithmetic on the GPU.
+"""Flow-consistency masks, pair mask ratios and flow visualisations of a robust_cvd working directory, with the per-pixel work on the GPU.
 
-Drop-in for the reference's Flow.compute_flow_masks and Flow.compute_flow_pair_stats (flow.py:44-74, :180-209), which process.py runs
-after RAFT: it reads flow/flow_%06d_%06d.raw and color_down/frame_%06d.raw and writes flow_mask/mask_%06d_%06d.png (8-bit, 0 / 255)
-and flow_list.json, the files the constraint builder, static flags, tracks and filters read.  The per-pixel test is rcvd_flow_masks
-(include/rcvd.h); the files are read with numpy, and the PNGs are encoded on a thread pool while the next chunk of pairs computes.
+Drop-in for the reference's Flow.compute_flow_masks, Flow.compute_flow_pair_stats and Flow.visualize_flow (flow.py:44-74, :128-209),
+which process.py runs after RAFT: it reads flow/flow_%06d_%06d.raw and color_down/frame_%06d.raw and writes flow_mask/mask_%06d_%06d.png
+(8-bit, 0 / 255) and flow_list.json, the files the constraint builder, static flags, tracks and filters read; with --vis_flow it also
+writes vis_flow/frame_%06d_%06d.png and vis_flow_warped/frame_%06d_%06d_warped.png.  The per-pixel work is rcvd_flow_masks and
+rcvd_flow_visualize (include/rcvd.h); the files are read with numpy, and the PNGs are encoded on a thread pool while the next chunk of
+pairs computes.
 
-There is no CPU fallback: without librcvd_b200.so or a usable CUDA device compute_flow_masks raises RuntimeError.
+There is no CPU fallback: without librcvd_b200.so or a usable CUDA device compute_flow_masks and visualize_flow raise RuntimeError.
 """
 import json
 import os
@@ -24,6 +26,8 @@ from .synthetic_files import read_raw
 FLOW_FMT = os.path.join("flow", "flow_{:06d}_{:06d}.raw")
 MASK_FMT = os.path.join("flow_mask", "mask_{:06d}_{:06d}.png")
 COLOR_FMT = os.path.join("color_down", "frame_{:06d}.raw")
+VIS_FMT = os.path.join("vis_flow", "frame_{:06d}_{:06d}.png")
+WARP_FMT = os.path.join("vis_flow_warped", "frame_{:06d}_{:06d}_warped.png")
 _FLOW_NAME = re.compile(r"^flow_(\d+)_(\d+)\.raw$")
 
 
@@ -74,33 +78,49 @@ def _check_inputs(path, pairs):
             raise ValueError(f"pair ({i}, {j}): flow and colour images differ in size or channels: {shapes}")
 
 
-def png_gray_bytes(img, level=1):
-    """An 8-bit grayscale PNG of img [h, w] u8 (filter type 0 on every row, one zlib IDAT)."""
-    img = np.ascontiguousarray(img, np.uint8)
-    h, w = img.shape
-    raw = np.zeros((h, w + 1), np.uint8)
-    raw[:, 1:] = img
+def _png_bytes(img, color_type, level):
+    """An 8-bit PNG of img [h, w] or [h, w, 3] u8 (filter type 0 on every row, one zlib IDAT)."""
+    h, w = img.shape[:2]
+    raw = np.zeros((h, img[0].size + 1), np.uint8)
+    raw[:, 1:] = img.reshape(h, -1)
 
     def chunk(t, d):
         return struct.pack(">I", len(d)) + t + d + struct.pack(">I", zlib.crc32(t + d) & 0xffffffff)
-    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 0, 0, 0, 0)) +
+    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, color_type, 0, 0, 0)) +
             chunk(b"IDAT", zlib.compress(raw.tobytes(), level)) + chunk(b"IEND", b""))
+
+
+def png_gray_bytes(img, level=1):
+    """An 8-bit grayscale PNG of img [h, w] u8 (filter type 0 on every row, one zlib IDAT)."""
+    img = np.ascontiguousarray(img, np.uint8)
+    if img.ndim != 2:
+        raise ValueError(f"a grayscale PNG needs an [h, w] image, not {img.shape}")
+    return _png_bytes(img, 0, level)
+
+
+def png_rgb_bytes(img, level=1):
+    """An 8-bit RGB PNG (colour type 2) of img [h, w, 3] u8, whose channels are in PNG (R, G, B) order."""
+    img = np.ascontiguousarray(img, np.uint8)
+    if img.ndim != 3 or img.shape[2] != 3:
+        raise ValueError(f"an RGB PNG needs an [h, w, 3] image, not {img.shape}")
+    return _png_bytes(img, 2, level)
 
 
 def _write_png(fn, img):
     t = time.perf_counter()
-    data = png_gray_bytes(img)
+    data = png_gray_bytes(img) if img.ndim == 2 else png_rgb_bytes(img)
     with open(fn, "wb") as f:
         f.write(data)
     return time.perf_counter() - t
 
 
-def _chunks(pairs, plane_bytes, chunk_bytes):
-    """Consecutive groups of pairs whose flows and colours take at most chunk_bytes of host memory (at least one pair each)."""
+def _chunks(pairs, plane_bytes, chunk_bytes, pair_bytes=16):
+    """Consecutive groups of pairs whose per-pair arrays (pair_bytes per pixel: both flows, and whatever else a pair reads or writes)
+    and colours take at most chunk_bytes of host memory (at least one pair each)."""
     out, cur, frames = [], [], set()
     for p in pairs:
         new = frames | set(p)
-        if cur and (len(cur) + 1) * 16 * plane_bytes + len(new) * 12 * plane_bytes > chunk_bytes:
+        if cur and (len(cur) + 1) * pair_bytes * plane_bytes + len(new) * 12 * plane_bytes > chunk_bytes:
             out.append(cur)
             cur, new = [], set(p)
         cur.append(p)
@@ -177,6 +197,120 @@ def compute_flow_masks(path, flow_thresh=1, color_thresh=1, device=None, chunk_b
     return stats
 
 
+def _flow_name_pair(name):
+    """The reference's get_indices for visualize_flow: the integers after the first '_' of the name without its extension, sorted.  A
+    name that does not give exactly two integers is refused (the reference crashes on it part-way)."""
+    parts = os.path.splitext(name)[0].split("_")[1:]
+    try:
+        idx = sorted(int(s) for s in parts)
+    except ValueError:
+        idx = []
+    if len(idx) != 2:
+        raise ValueError(f"flow/{name}: not a flow_<i>_<j> file name")
+    return tuple(idx)
+
+
+def vis_pairs_to_compute(path, warp=False):
+    """The sorted pairs (i, j), i <= j, that visualize_flow writes: every entry of flow/ parsed as the reference does, a pair skipped when
+    its vis_flow PNG exists and, with warp, its vis_flow_warped/frame_i_j_warped.png (sorted indices) too."""
+    pairs = sorted({_flow_name_pair(n) for n in os.listdir(os.path.join(path, "flow"))})
+    return [(i, j) for i, j in pairs if not (os.path.isfile(os.path.join(path, VIS_FMT.format(i, j))) and
+                                             (not warp or os.path.isfile(os.path.join(path, WARP_FMT.format(i, j)))))]
+
+
+def _png_size(fn):
+    """(rows, cols) from a PNG's IHDR."""
+    with open(fn, "rb") as f:
+        head = f.read(24)
+    if len(head) < 24 or head[:8] != b"\x89PNG\r\n\x1a\n" or head[12:16] != b"IHDR":
+        raise ValueError(f"{fn}: not a PNG file")
+    w, h = struct.unpack(">II", head[16:24])
+    return h, w
+
+
+def _check_vis_inputs(path, pairs):
+    """Both flows and masks and both colours of every pair exist and have one size of at least 2 x 2: refused before anything is
+    written."""
+    for i, j in pairs:
+        shapes = {}
+        for fn, size in ((FLOW_FMT.format(i, j), _raw_shape), (FLOW_FMT.format(j, i), _raw_shape), (MASK_FMT.format(i, j), _png_size),
+                         (MASK_FMT.format(j, i), _png_size), (COLOR_FMT.format(i), _raw_shape), (COLOR_FMT.format(j), _raw_shape)):
+            full = os.path.join(path, fn)
+            if not os.path.isfile(full):
+                raise FileNotFoundError(f"{full} is missing: the visualisation of pair ({i}, {j}) needs both flows, both masks and both colours")
+            shapes[fn] = size(full)
+        sizes = {s[:2] for s in shapes.values()}
+        chans = [s[2] for s in shapes.values() if len(s) == 3]
+        if len(sizes) != 1 or chans != [2, 2, 3, 3]:
+            raise ValueError(f"pair ({i}, {j}): flows, masks and colours differ in size or channels: {shapes}")
+        h, w = sizes.pop()
+        if h < 2 or w < 2:
+            raise ValueError(f"pair ({i}, {j}): images of {h} x {w} pixels; the warp's grid divides by width - 1 and height - 1")
+
+
+def _read_vis_chunk(path, chunk, files):
+    """_read_chunk plus both masks of every pair, decoded by the `files` pool."""
+    colors, pf, fij, fji, rs = _read_chunk(path, chunk, files)
+    t = time.perf_counter()
+    masks = list(files.map(lambda k: _read_mask(os.path.join(path, MASK_FMT.format(*k))), [p for i, j in chunk for p in ((i, j), (j, i))]))
+    mij, mji = np.stack(masks[0::2]), np.stack(masks[1::2])
+    return colors, pf, fij, fji, mij, mji, rs + time.perf_counter() - t
+
+
+def visualize_flow(path, warp=False, device=None, chunk_bytes=256 << 20, workers=None):
+    """Flow.visualize_flow on the GPU: for every pair of vis_pairs_to_compute(path, warp) writes vis_flow/frame_i_j.png (the flow
+    colours and masks composite) and, with warp, vis_flow_warped/frame_i_j_warped.png (colour j warped by flow i -> j) and
+    frame_j_i_warped.png, both rewritten when the pair runs.  Both output directories are always created.  Pairs are processed in chunks
+    of at most chunk_bytes of inputs and outputs; PNGs are encoded by `workers` threads while the next chunk reads and computes.  A name
+    in flow/ that does not parse, a missing flow, mask or colour of a pair, or a size mismatch raises before anything is written.
+    Returns timings as compute_flow_masks does."""
+    t0 = time.perf_counter()
+    L = solver.lib()
+    dev = L.rcvd_current_device() if device is None else int(device)
+    if dev < 0:
+        raise RuntimeError("rcvd error 5: no usable CUDA device for the flow visualisation; this library has no CPU fallback")
+    pairs = vis_pairs_to_compute(path, warp)
+    _check_vis_inputs(path, pairs)
+    for d in (VIS_FMT, WARP_FMT):
+        os.makedirs(os.path.join(path, os.path.dirname(d)), exist_ok=True)
+    stats = {"pairs": len(pairs), "read_s": 0.0, "compute_s": 0.0, "png_s": 0.0, "wait_s": 0.0, "total_s": 0.0}
+    if not pairs:
+        stats["total_s"] = time.perf_counter() - t0
+        return stats
+    rows, cols, _ = _raw_shape(os.path.join(path, COLOR_FMT.format(pairs[0][0])))
+    # per pair and pixel: flows 16 B, masks 2 B, composite 24 B, warps 6 B
+    chunks = _chunks(pairs, rows * cols, chunk_bytes, pair_bytes=48)
+    workers = workers or min(8, os.cpu_count() or 1)
+    with ThreadPoolExecutor(1) as reader, ThreadPoolExecutor(4) as files, ThreadPoolExecutor(workers) as writers:
+        pending = []
+        nxt = reader.submit(_read_vis_chunk, path, chunks[0], files)
+        for k, chunk in enumerate(chunks):
+            t = time.perf_counter()
+            colors, pf, fij, fji, mij, mji, rs = nxt.result()
+            stats["wait_s"] += time.perf_counter() - t
+            stats["read_s"] += rs
+            if k + 1 < len(chunks):
+                nxt = reader.submit(_read_vis_chunk, path, chunks[k + 1], files)
+            t = time.perf_counter()
+            vis, wij, wji = solver.flow_visualize(colors, pf, fij, fji, mij, mji, warp=warp, device=dev)
+            stats["compute_s"] += time.perf_counter() - t
+            del colors, fij, fji, mij, mji
+            t = time.perf_counter()
+            stats["png_s"] += sum(f.result() for f in pending)   # at most one chunk of images waits for its PNGs
+            stats["wait_s"] += time.perf_counter() - t
+            pending = []
+            for n, (i, j) in enumerate(chunk):
+                pending.append(writers.submit(_write_png, os.path.join(path, VIS_FMT.format(i, j)), vis[n]))
+                if warp:
+                    pending.append(writers.submit(_write_png, os.path.join(path, WARP_FMT.format(i, j)), wij[n]))
+                    pending.append(writers.submit(_write_png, os.path.join(path, WARP_FMT.format(j, i)), wji[n]))
+        t = time.perf_counter()
+        stats["png_s"] += sum(f.result() for f in pending)
+        stats["wait_s"] += time.perf_counter() - t
+    stats["total_s"] = time.perf_counter() - t0
+    return stats
+
+
 def _read_mask(fn):
     """A mask PNG through the project's PNG decoder (lib_python._imreadPng, the cv::imread subset the C++ readers use)."""
     host = os.path.join(os.path.dirname(os.path.abspath(__file__)), "host")
@@ -216,9 +350,9 @@ def compute_flow_pair_stats(path, frame_pairs):
 
 
 class Flow:
-    """The mask and pair-statistics stages of the reference's Flow class (flow.py), on the GPU: a caller of
-    Flow(path, out_path).compute_flow_masks() / .compute_flow_pair_stats(frame_pairs) switches by importing this class instead.  RAFT
-    (compute_flow) and the visualisation are not part of it."""
+    """The reference's Flow class (flow.py) on the GPU, every method but compute_flow (RAFT, which needs network weights): a caller of
+    Flow(path, out_path).compute_flow_masks() / .compute_flow_pair_stats(frame_pairs) / .visualize_flow(warp) switches by importing
+    this class instead."""
 
     def __init__(self, path, out_path):
         self.path = path
@@ -233,3 +367,6 @@ class Flow:
 
     def compute_flow_pair_stats(self, frame_pairs):
         return compute_flow_pair_stats(self.path, frame_pairs)
+
+    def visualize_flow(self, warp=False):
+        visualize_flow(self.path, warp)

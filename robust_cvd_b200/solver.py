@@ -608,6 +608,33 @@ def flow_masks(colors, pair_frames, flow_ij, flow_ji, flow_thresh_sq=1.0, color_
     return (mij, mji, cnt, sf, sc) if want_sse else (mij, mji, cnt)
 
 
+def flow_visualize(colors, pair_frames, flow_ij, flow_ji, mask_ij, mask_ji, warp=False, want_values=False, device=0):
+    """rcvd_flow_visualize (Flow.visualize_flow, reference flow.py:128-178) on the GPU.  colors [F,h,w,3] f32 in [0, 1], pair_frames
+    [P,2] local colour ids, flow_ij / flow_ji [P,h,w,2] f32, mask_ij / mask_ji [P,h,w] u8.  Returns vis [P,2h,4w,3] u8 and, with warp,
+    warp_ij / warp_ji [P,h,w,3] u8 (else None), all in PNG (RGB) byte order.  want_values adds (warp_values [P,2,h,w,3] f32 or None,
+    maxrad [P,2] f32, has_nan [P,2] bool)."""
+    col = np.ascontiguousarray(colors, np.float32)
+    pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1, 2)
+    fij = np.ascontiguousarray(flow_ij, np.float32); fji = np.ascontiguousarray(flow_ji, np.float32)
+    mij = np.ascontiguousarray(mask_ij, np.uint8); mji = np.ascontiguousarray(mask_ji, np.uint8)
+    F, h, w = col.shape[:3]
+    P = len(pf)
+    if col.shape != (F, h, w, 3) or fij.shape != (P, h, w, 2) or fji.shape != fij.shape or mij.shape != (P, h, w) or mji.shape != mij.shape:
+        raise ValueError(f"flow-visualisation inputs of shapes colours {col.shape}, flows {fij.shape} / {fji.shape}, masks {mij.shape} / "
+                         f"{mji.shape} for {P} pairs")
+    prm = abi.FlowVisParams(width=w, height=h, num_pairs=P, num_frames=F, warp=int(bool(warp)))
+    vis = np.zeros((P, 2 * h, 4 * w, 3), np.uint8)
+    wij = np.zeros((P, h, w, 3), np.uint8) if warp else None
+    wji = np.zeros((P, h, w, 3), np.uint8) if warp else None
+    wv = np.zeros((P, 2, h, w, 3), np.float32) if warp and want_values else None
+    mr = np.zeros((P, 2), np.float32); nan = np.zeros((P, 2), np.uint8)
+    _check(lib().rcvd_flow_visualize(C.byref(prm), C.c_int32(device), _p(pf, C.c_int32), _p(fij, C.c_float), _p(fji, C.c_float),
+                                     _p(mij, C.c_uint8), _p(mji, C.c_uint8), _p(col, C.c_float), _p(vis, C.c_uint8), _p(wij, C.c_uint8),
+                                     _p(wji, C.c_uint8), _p(wv, C.c_float), _p(mr if want_values else None, C.c_float),
+                                     _p(nan if want_values else None, C.c_uint8)))
+    return (vis, wij, wji, wv, mr, nan.astype(bool)) if want_values else (vis, wij, wji)
+
+
 def time_flow_masks(colors, pair_frames, flow_ij, flow_ji, reps=50, flow_thresh_sq=1.0, color_thresh_sq=3.0, device=0):
     """Bench hook: mean device ms of one rcvd_flow_masks kernel pass over all the pairs (inputs uploaded once, CUDA events)."""
     prm, args, keep = _flow_mask_args(colors, pair_frames, flow_ij, flow_ji, flow_thresh_sq, color_thresh_sq)
