@@ -517,6 +517,30 @@ int32_t rcvd_flow_visualize(const rcvd_flow_vis_params* prm, int32_t device, con
                             const uint8_t* mask_ij, const uint8_t* mask_ji, const float* colors, uint8_t* vis, uint8_t* warp_ij, uint8_t* warp_ji,
                             float* warp_values, float* maxrad, uint8_t* has_nan);
 
+/* ---- downscaled colour frames (DESIGN.md section 1 row 8f-10) ----
+ * Replaces the per-frame work of Video.downscale_frames (reference video.py:154-182): np.float32(img) / 255.0 of each 8-bit frame,
+ * then cv2.resize(img, (width, height), interpolation=cv2.INTER_AREA), bit for bit (OpenCV 4.13's integer-factor, area-table and
+ * upscale paths, all in float32).  One call resizes a batch of frames to up to RCVD_RESIZE_MAX_OUTPUTS sizes, so a frame is uploaded
+ * once for all of them.
+ *   frames      [num_frames][height][width][3] u8, in the decoder's channel order (B, G, R as cv::imread gives)
+ *   outputs[k]  [num_frames][outputs[k].height][outputs[k].width][3]: RCVD_RESIZE_RAW float32 in the frames' channel order (the
+ *               .raw files' values); RCVD_RESIZE_PNG u8 in reversed channel order (R, G, B, the pixels of cv2.imwrite(fn, img * 255):
+ *               x * 255 in float32, rounded half to even, saturated)
+ * num_frames = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null parameter block, a
+ * non-positive source or output size, a size of 2^31 pixels or more, num_frames < 0, num_outputs outside 1 .. RCVD_RESIZE_MAX_OUTPUTS,
+ * an unknown kind, a null frames or output buffer. */
+enum { RCVD_RESIZE_RAW = 0, RCVD_RESIZE_PNG = 1, RCVD_RESIZE_MAX_OUTPUTS = 3 };
+typedef struct rcvd_resize_output {
+  int32_t width, height;
+  int32_t kind;                    /* RCVD_RESIZE_RAW or RCVD_RESIZE_PNG */
+} rcvd_resize_output;
+typedef struct rcvd_resize_params {
+  int32_t width, height, num_frames;   /* the source frames */
+  int32_t num_outputs;
+  rcvd_resize_output outputs[RCVD_RESIZE_MAX_OUTPUTS];
+} rcvd_resize_params;
+int32_t rcvd_resize_area(const rcvd_resize_params* prm, int32_t device, const uint8_t* frames, void* const* outputs);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,6 +16,11 @@ int64_t rcvd_static_flag_launch_count(void);
 int64_t rcvd_tracks_launch_count(void);
 int64_t rcvd_flow_mask_launch_count(void);
 int64_t rcvd_flow_vis_launch_count(void);
+int64_t rcvd_resize_launch_count(void);
+/* rcvd_resize_area's kernels alone: the frames are uploaded once, the kernels of every output run reps times between two CUDA events,
+ * and *ms is the mean device time of one pass over all the frames and outputs.  Arguments and refusals as rcvd_resize_area (the output
+ * buffers are not needed); num_frames >= 1, reps >= 1. */
+int32_t rcvd_debug_time_resize_area(const rcvd_resize_params* prm, int32_t device, const uint8_t* frames, int32_t reps, double* ms);
 /* rcvd_flow_masks' kernel alone: the inputs are uploaded once, the kernel (with counts) runs reps times between two CUDA events, and
  * *ms is the mean device time of one launch over all the pairs.  Arguments and refusals as rcvd_flow_masks; reps >= 1. */
 int32_t rcvd_debug_time_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij,

@@ -108,6 +108,20 @@ class FlowVisParams(C.Structure):
     """rcvd_flow_vis_params (include/rcvd.h)."""
     _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_pairs", "num_frames", "warp")]
 
+
+RESIZE_RAW, RESIZE_PNG, RESIZE_MAX_OUTPUTS = 0, 1, 3
+
+
+class ResizeOutput(C.Structure):
+    """rcvd_resize_output (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "kind")]
+
+
+class ResizeParams(C.Structure):
+    """rcvd_resize_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_frames", "num_outputs")] + \
+               [("outputs", ResizeOutput * RESIZE_MAX_OUTPUTS)]
+
 # residual families of rcvd_evaluate_rows, in the order of rcvd_row_layout::family
 ROWS_PAIRS, ROWS_TRIPLETS, ROWS_DEPTH_PAIRS, ROWS_REGULARISERS = range(4)
 ROW_FAMILIES = ("pairs", "triplets", "depth_pairs", "regularisers")

@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks and the flow visualisations.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations and the downscaled colour frames.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -17,6 +17,7 @@
 #include "rcvd_tracks.cuh"
 #include "rcvd_flowmask.cuh"
 #include "rcvd_flowvis.cuh"
+#include "rcvd_resize.cuh"
 
 using namespace rcvd;
 
@@ -777,4 +778,100 @@ RCVD_API int32_t rcvd_flow_visualize(const rcvd_flow_vis_params* prm, int32_t de
     if (has_nan) has_nan[k] = st[2 * k + 1] ? 1 : 0;
   }
   return RCVD_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Downscaled colour frames (rcvd_resize.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_resize_launches = 0;
+RCVD_API int64_t rcvd_resize_launch_count() { return g_resize_launches; }
+// The argument rules of rcvd_resize_area, checked on the host before any device is needed (outputs: checked when non-null).
+static int check_resize_args(const rcvd_resize_params* prm, const uint8_t* frames, void* const* outputs, bool need_outputs) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_resize_params& q = *prm;
+  auto bad_size = [](int w, int h) { return w <= 0 || h <= 0 || (int64_t)w * h >= (int64_t(1) << 31); };
+  if (bad_size(q.width, q.height) || q.num_frames < 0) return set_err(RCVD_ERR_INVALID, "bad resize source: %d x %d, %d frames", q.width, q.height, q.num_frames);
+  if (q.num_outputs < 1 || q.num_outputs > RCVD_RESIZE_MAX_OUTPUTS) return set_err(RCVD_ERR_INVALID, "%d resize outputs (1 .. %d)", q.num_outputs, RCVD_RESIZE_MAX_OUTPUTS);
+  for (int k = 0; k < q.num_outputs; ++k) {
+    const rcvd_resize_output& o = q.outputs[k];
+    if (bad_size(o.width, o.height) || (o.kind != RCVD_RESIZE_RAW && o.kind != RCVD_RESIZE_PNG))
+      return set_err(RCVD_ERR_INVALID, "bad resize output %d: %d x %d, kind %d", k, o.width, o.height, o.kind);
+  }
+  if (q.num_frames > 0 && !frames) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (need_outputs && q.num_frames > 0) {
+    if (!outputs) return set_err(RCVD_ERR_INVALID, "null argument");
+    for (int k = 0; k < q.num_outputs; ++k)
+      if (!outputs[k]) return set_err(RCVD_ERR_INVALID, "null buffer for resize output %d", k);
+  }
+  return RCVD_OK;
+}
+// Uploads the frames once and every output's tables; allocates the outputs (a.frame0 is left for the launches).
+static std::vector<ResizeArgs> upload_resize_inputs(VideoCall& call, const rcvd_resize_params& q, const uint8_t* frames) {
+  const size_t F = q.num_frames;
+  const uint8_t* d_src = (const uint8_t*)call.upload(frames, F * q.width * q.height * 3);
+  std::vector<ResizeArgs> out;
+  for (int k = 0; k < q.num_outputs; ++k) {
+    const rcvd_resize_output& o = q.outputs[k];
+    ResizeArgs a{};
+    a.W = q.width; a.H = q.height; a.w = o.width; a.h = o.height; a.src = d_src; a.png = o.kind == RCVD_RESIZE_PNG;
+    const double sx = 1.0 / ((double)o.width / q.width), sy = 1.0 / ((double)o.height / q.height);
+    const int isx = (int)std::nearbyint(sx), isy = (int)std::nearbyint(sy);
+    if (sx >= 1 && sy >= 1 && std::abs(sx - isx) < DBL_EPSILON && std::abs(sy - isy) < DBL_EPSILON) {
+      a.ix = isx; a.iy = isy; a.inv_area = 1.f / (float)(isx * isy);
+    } else {
+      const bool linear = sx < 1 || sy < 1;
+      // reused for the y tables: a copy from pageable memory has read its source when cudaMemcpyAsync returns
+      std::vector<int> off, src; std::vector<float> wt;
+      resize_axis_taps(q.width, o.width, linear, off, src, wt);
+      a.x = {(const int*)call.upload(off.data(), off.size() * 4), (const int*)call.upload(src.data(), src.size() * 4), (const float*)call.upload(wt.data(), wt.size() * 4)};
+      resize_axis_taps(q.height, o.height, linear, off, src, wt);
+      a.y = {(const int*)call.upload(off.data(), off.size() * 4), (const int*)call.upload(src.data(), src.size() * 4), (const float*)call.upload(wt.data(), wt.size() * 4)};
+    }
+    a.out = call.alloc(F * o.width * o.height * 3 * (a.png ? 1 : 4));
+    out.push_back(a);
+  }
+  return out;
+}
+// every output, every frame in launches of at most 65535 (grid.y) frames
+static int launch_resize(VideoCall& call, std::vector<ResizeArgs> outs, int F) {
+  for (ResizeArgs& a : outs)
+    for (int f0 = 0; f0 < F; f0 += 65535) {
+      a.frame0 = f0;
+      if (int rc = call.launch(k_resize_area, dim3(nblk((size_t)a.w * a.h, kRsThreads), std::min(65535, F - f0)), kRsThreads, 0, a)) return rc;
+    }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_resize_area(const rcvd_resize_params* prm, int32_t device, const uint8_t* frames, void* const* outputs) {
+  if (int rc = check_resize_args(prm, frames, outputs, true)) return rc;
+  const rcvd_resize_params& q = *prm;
+  if (q.num_frames == 0) return RCVD_OK;
+  VideoCall call;
+  if (int rc = call.open(device, g_resize_launches)) return rc;
+  const std::vector<ResizeArgs> outs = upload_resize_inputs(call, q, frames);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_resize_area");
+  if (int rc = launch_resize(call, outs, q.num_frames)) return rc;
+  for (int k = 0; k < q.num_outputs; ++k)
+    cudaMemcpyAsync(outputs[k], outs[k].out, (size_t)q.num_frames * outs[k].w * outs[k].h * 3 * (outs[k].png ? 1 : 4), cudaMemcpyDeviceToHost, call.st);
+  return call.sync("resize kernel");
+}
+RCVD_API int32_t rcvd_debug_time_resize_area(const rcvd_resize_params* prm, int32_t device, const uint8_t* frames, int32_t reps, double* ms) {
+  if (int rc = check_resize_args(prm, frames, nullptr, false)) return rc;
+  if (reps < 1 || !ms || prm->num_frames == 0) return set_err(RCVD_ERR_INVALID, "bad timing arguments");
+  VideoCall call;
+  if (int rc = call.open(device, g_resize_launches)) return rc;
+  const std::vector<ResizeArgs> outs = upload_resize_inputs(call, *prm, frames);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_resize_area");
+  if (int rc = launch_resize(call, outs, prm->num_frames)) return rc;   // warm-up
+  cudaEvent_t e0, e1;
+  CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+  cudaEventRecord(e0, call.st);
+  int rc = RCVD_OK;
+  for (int r = 0; r < reps && rc == RCVD_OK; ++r) rc = launch_resize(call, outs, prm->num_frames);
+  cudaEventRecord(e1, call.st);
+  if (rc == RCVD_OK) rc = call.sync("resize timing");
+  float t = 0.f;
+  if (rc == RCVD_OK) cudaEventElapsedTime(&t, e0, e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  *ms = (double)t / reps;
+  return rc;
 }

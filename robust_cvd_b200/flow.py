@@ -15,12 +15,12 @@ import re
 import struct
 import sys
 import time
-import zlib
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 from . import solver
+from .png import png_gray_bytes, png_rgb_bytes, write_png  # noqa: F401  (png_*_bytes: part of this module's interface)
 from .synthetic_files import read_raw
 
 FLOW_FMT = os.path.join("flow", "flow_{:06d}_{:06d}.raw")
@@ -76,42 +76,6 @@ def _check_inputs(path, pairs):
         chans = [s[2] for s in shapes.values()]
         if len(sizes) != 1 or chans != [2, 2, 3, 3]:
             raise ValueError(f"pair ({i}, {j}): flow and colour images differ in size or channels: {shapes}")
-
-
-def _png_bytes(img, color_type, level):
-    """An 8-bit PNG of img [h, w] or [h, w, 3] u8 (filter type 0 on every row, one zlib IDAT)."""
-    h, w = img.shape[:2]
-    raw = np.zeros((h, img[0].size + 1), np.uint8)
-    raw[:, 1:] = img.reshape(h, -1)
-
-    def chunk(t, d):
-        return struct.pack(">I", len(d)) + t + d + struct.pack(">I", zlib.crc32(t + d) & 0xffffffff)
-    return (b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, color_type, 0, 0, 0)) +
-            chunk(b"IDAT", zlib.compress(raw.tobytes(), level)) + chunk(b"IEND", b""))
-
-
-def png_gray_bytes(img, level=1):
-    """An 8-bit grayscale PNG of img [h, w] u8 (filter type 0 on every row, one zlib IDAT)."""
-    img = np.ascontiguousarray(img, np.uint8)
-    if img.ndim != 2:
-        raise ValueError(f"a grayscale PNG needs an [h, w] image, not {img.shape}")
-    return _png_bytes(img, 0, level)
-
-
-def png_rgb_bytes(img, level=1):
-    """An 8-bit RGB PNG (colour type 2) of img [h, w, 3] u8, whose channels are in PNG (R, G, B) order."""
-    img = np.ascontiguousarray(img, np.uint8)
-    if img.ndim != 3 or img.shape[2] != 3:
-        raise ValueError(f"an RGB PNG needs an [h, w, 3] image, not {img.shape}")
-    return _png_bytes(img, 2, level)
-
-
-def _write_png(fn, img):
-    t = time.perf_counter()
-    data = png_gray_bytes(img) if img.ndim == 2 else png_rgb_bytes(img)
-    with open(fn, "wb") as f:
-        f.write(data)
-    return time.perf_counter() - t
 
 
 def _chunks(pairs, plane_bytes, chunk_bytes, pair_bytes=16):
@@ -188,8 +152,8 @@ def compute_flow_masks(path, flow_thresh=1, color_thresh=1, device=None, chunk_b
             stats["wait_s"] += time.perf_counter() - t
             pending = []
             for n, (i, j) in enumerate(chunk):
-                pending.append(writers.submit(_write_png, os.path.join(path, MASK_FMT.format(i, j)), mij[n]))
-                pending.append(writers.submit(_write_png, os.path.join(path, MASK_FMT.format(j, i)), mji[n]))
+                pending.append(writers.submit(write_png, os.path.join(path, MASK_FMT.format(i, j)), mij[n]))
+                pending.append(writers.submit(write_png, os.path.join(path, MASK_FMT.format(j, i)), mji[n]))
         t = time.perf_counter()
         stats["png_s"] += sum(f.result() for f in pending)
         stats["wait_s"] += time.perf_counter() - t
@@ -300,10 +264,10 @@ def visualize_flow(path, warp=False, device=None, chunk_bytes=256 << 20, workers
             stats["wait_s"] += time.perf_counter() - t
             pending = []
             for n, (i, j) in enumerate(chunk):
-                pending.append(writers.submit(_write_png, os.path.join(path, VIS_FMT.format(i, j)), vis[n]))
+                pending.append(writers.submit(write_png, os.path.join(path, VIS_FMT.format(i, j)), vis[n]))
                 if warp:
-                    pending.append(writers.submit(_write_png, os.path.join(path, WARP_FMT.format(i, j)), wij[n]))
-                    pending.append(writers.submit(_write_png, os.path.join(path, WARP_FMT.format(j, i)), wji[n]))
+                    pending.append(writers.submit(write_png, os.path.join(path, WARP_FMT.format(i, j)), wij[n]))
+                    pending.append(writers.submit(write_png, os.path.join(path, WARP_FMT.format(j, i)), wji[n]))
         t = time.perf_counter()
         stats["png_s"] += sum(f.result() for f in pending)
         stats["wait_s"] += time.perf_counter() - t

@@ -275,7 +275,10 @@ PYBIND11_MODULE(lib_python, m) {
   m.def("_distanceTransformL2_5", [](py::array_t<uint8_t, py::array::c_style | py::array::forcecast> b) {
     Image im; im.create((int)b.shape(0), (int)b.shape(1), cvMakeType(CV_8U, 1)); std::memcpy(im.data.data(), b.data(), im.data.size());
     Image r = distanceTransformL2_5(im); return imageToNp(&r); });
-  m.def("_imreadPng", [](const std::string& f, bool gray) { Image im = imreadPng(f, gray); return imageToNp(im.empty() ? nullptr : &im); });
+  m.def("_imreadPng", [](const std::string& f, bool gray) {   // the decode runs without the GIL, so a thread pool decodes in parallel
+    Image im;
+    { py::gil_scoped_release nogil; im = imreadPng(f, gray); }
+    return imageToNp(im.empty() ? nullptr : &im); });
   m.def("_makeQuat", [](float x, float y, float z, float w) { Quatf q; q.x = x; q.y = y; q.z = z; q.w = w; return q; });   // tests: the reference binds no quaternion constructor
   m.def("_quatToAngleAxis", [](float x, float y, float z, float w) { Quatf q; q.x = x; q.y = y; q.z = z; q.w = w; double aa[3]; quatToAngleAxis(q, aa); return py::make_tuple(aa[0], aa[1], aa[2]); });
   m.def("_angleAxisToQuat", [](double a, double b, double c) { const double aa[3] = {a, b, c}; Quatf q = angleAxisToQuat(aa); return py::make_tuple(q.x, q.y, q.z, q.w); });

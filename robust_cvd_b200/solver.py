@@ -643,6 +643,41 @@ def time_flow_masks(colors, pair_frames, flow_ij, flow_ji, reps=50, flow_thresh_
     return ms.value
 
 
+def _resize_params(frames, outputs):
+    """The frames as a contiguous [F, H, W, 3] u8 array and the rcvd_resize_params of `outputs`: (height, width, "raw" | "png") each."""
+    fr = np.ascontiguousarray(frames, np.uint8)
+    if fr.ndim != 4 or fr.shape[3] != 3:
+        raise ValueError(f"frames of shape {fr.shape}: need [frames, height, width, 3] u8")
+    if not 1 <= len(outputs) <= abi.RESIZE_MAX_OUTPUTS:
+        raise ValueError(f"{len(outputs)} outputs: need 1 .. {abi.RESIZE_MAX_OUTPUTS}")
+    kinds = {"raw": abi.RESIZE_RAW, "png": abi.RESIZE_PNG}
+    prm = abi.ResizeParams(width=fr.shape[2], height=fr.shape[1], num_frames=fr.shape[0], num_outputs=len(outputs))
+    for k, (h, w, kind) in enumerate(outputs):
+        prm.outputs[k] = abi.ResizeOutput(width=int(w), height=int(h), kind=kinds[kind])
+    return fr, prm
+
+
+def resize_area(frames, outputs, device=0):
+    """rcvd_resize_area (np.float32(img) / 255.0 then cv2.resize(..., INTER_AREA), as Video.downscale_frames, reference
+    video.py:154-182) on the GPU.  frames [F, H, W, 3] u8 in B, G, R order; outputs: up to three (height, width, kind) with kind "raw"
+    (float32 [F, h, w, 3], B, G, R: the .raw files' values) or "png" (u8 [F, h, w, 3], R, G, B: the pixels of cv2.imwrite(fn, img * 255)).
+    Returns one array per output."""
+    fr, prm = _resize_params(frames, outputs)
+    outs = [np.empty((fr.shape[0], int(h), int(w), 3), np.float32 if kind == "raw" else np.uint8) for h, w, kind in outputs]
+    ptrs = (C.c_void_p * len(outs))(*(o.ctypes.data for o in outs))
+    _check(lib().rcvd_resize_area(C.byref(prm), C.c_int32(device), _p(fr, C.c_uint8), ptrs))
+    return outs
+
+
+def time_resize_area(frames, outputs, reps=20, device=0):
+    """Bench hook: mean device ms of one rcvd_resize_area kernel pass over all the frames and outputs (frames uploaded once, CUDA
+    events)."""
+    fr, prm = _resize_params(frames, outputs)
+    ms = C.c_double()
+    _check(lib().rcvd_debug_time_resize_area(C.byref(prm), C.c_int32(device), _p(fr, C.c_uint8), C.c_int32(reps), C.byref(ms)))
+    return ms.value
+
+
 FP64_MMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
 
 
