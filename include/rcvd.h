@@ -541,6 +541,30 @@ typedef struct rcvd_resize_params {
 } rcvd_resize_params;
 int32_t rcvd_resize_area(const rcvd_resize_params* prm, int32_t device, const uint8_t* frames, void* const* outputs);
 
+/* ---- depth visualisations (DESIGN.md section 1 row 8f-11) ----
+ * Replaces the per-frame work of visualization.visualize_depth_dir / visualize_depth (reference utils/visualization.py:53-134) for a
+ * batch of frames of one size.  Two passes; a null output skips its pass.
+ *   range   counts[f]: the finite values of frame f; stats[f][4]: the order statistics (0-based ranks among the finite values, as
+ *           doubles) at floor(v) and floor(v) + 1 of v = (n - 1) q for q = q[0], then q = q[1], both n - 1 when v >= n - 1 (numpy's
+ *           linear-method neighbours).  For RCVD_DEPTH_VIS_F32, v is float32(n - 1) * float32(q) rounded to float32 and compared with
+ *           float32(n - 1); for RCVD_DEPTH_VIS_U8C3 it is double.  Not written when counts[f] is 0.
+ *   colour  index[f][y][x] = np.uint8(((d - offset) / scale) ** 0.5 * 255), in float32 with float32(offset) and float32(scale) for
+ *           F32 and in double per channel for U8C3, whose three indices are then converted to gray as cv::cvtColor(BGR2GRAY) does;
+ *           rgb[f][y][x][0..2] = colormap[index][0..2].  colormap (256 x 3 u8) is needed when rgb is non-null.
+ *   frames  [num_frames][height][width] float32 (RCVD_DEPTH_VIS_F32) or [num_frames][height][width][3] u8, B, G, R (RCVD_DEPTH_VIS_U8C3)
+ * num_frames = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null parameter block, a
+ * non-positive size, 3 * width * height >= 2^31, num_frames < 0, an unknown kind, a quantile outside [0, 1] while range outputs are
+ * given, only one of counts and stats, a null frames buffer, rgb without a colormap. */
+enum { RCVD_DEPTH_VIS_F32 = 0, RCVD_DEPTH_VIS_U8C3 = 1 };
+typedef struct rcvd_depth_vis_params {
+  int32_t width, height, num_frames;
+  int32_t kind;                    /* RCVD_DEPTH_VIS_F32 or RCVD_DEPTH_VIS_U8C3 */
+  double q[2];                     /* range pass: quantiles in [0, 1] (for F32, float32 values: np.float32(p) / np.float32(100)) */
+  double offset, scale;            /* colour pass: the bounds d_min and d_max - d_min */
+} rcvd_depth_vis_params;
+int32_t rcvd_depth_visualize(const rcvd_depth_vis_params* prm, int32_t device, const void* frames, const uint8_t* colormap,
+                             int64_t* counts, double* stats, uint8_t* index, uint8_t* rgb);
+
 #ifdef __cplusplus
 }
 #endif

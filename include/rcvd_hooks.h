@@ -21,6 +21,12 @@ int64_t rcvd_resize_launch_count(void);
  * and *ms is the mean device time of one pass over all the frames and outputs.  Arguments and refusals as rcvd_resize_area (the output
  * buffers are not needed); num_frames >= 1, reps >= 1. */
 int32_t rcvd_debug_time_resize_area(const rcvd_resize_params* prm, int32_t device, const uint8_t* frames, int32_t reps, double* ms);
+int64_t rcvd_depth_vis_launch_count(void);
+/* rcvd_depth_visualize's kernels alone: the frames are uploaded once, then each pass runs reps times between two CUDA events; *ms_range
+ * and *ms_color are the mean device times of one pass over all the frames (the colour pass writes rgb).  Arguments and refusals as
+ * rcvd_depth_visualize with both passes; num_frames >= 1, reps >= 1. */
+int32_t rcvd_debug_time_depth_visualize(const rcvd_depth_vis_params* prm, int32_t device, const void* frames, const uint8_t* colormap,
+                                        int32_t reps, double* ms_range, double* ms_color);
 /* rcvd_flow_masks' kernel alone: the inputs are uploaded once, the kernel (with counts) runs reps times between two CUDA events, and
  * *ms is the mean device time of one launch over all the pairs.  Arguments and refusals as rcvd_flow_masks; reps >= 1. */
 int32_t rcvd_debug_time_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij,

@@ -122,6 +122,15 @@ class ResizeParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_frames", "num_outputs")] + \
                [("outputs", ResizeOutput * RESIZE_MAX_OUTPUTS)]
 
+
+DEPTH_VIS_F32, DEPTH_VIS_U8C3 = 0, 1
+
+
+class DepthVisParams(C.Structure):
+    """rcvd_depth_vis_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_frames", "kind")] + \
+               [("q", C.c_double * 2), ("offset", C.c_double), ("scale", C.c_double)]
+
 # residual families of rcvd_evaluate_rows, in the order of rcvd_row_layout::family
 ROWS_PAIRS, ROWS_TRIPLETS, ROWS_DEPTH_PAIRS, ROWS_REGULARISERS = range(4)
 ROW_FAMILIES = ("pairs", "triplets", "depth_pairs", "regularisers")

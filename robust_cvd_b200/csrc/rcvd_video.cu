@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations and the downscaled colour frames.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations, the downscaled colour frames and the depth visualisations.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -18,6 +18,7 @@
 #include "rcvd_flowmask.cuh"
 #include "rcvd_flowvis.cuh"
 #include "rcvd_resize.cuh"
+#include "rcvd_depthvis.cuh"
 
 using namespace rcvd;
 
@@ -873,5 +874,96 @@ RCVD_API int32_t rcvd_debug_time_resize_area(const rcvd_resize_params* prm, int3
   if (rc == RCVD_OK) cudaEventElapsedTime(&t, e0, e1);
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   *ms = (double)t / reps;
+  return rc;
+}
+
+// ---------------------------------------------------------------------------
+// Depth visualisations (rcvd_depthvis.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_depth_vis_launches = 0;
+RCVD_API int64_t rcvd_depth_vis_launch_count() { return g_depth_vis_launches; }
+// The argument rules of rcvd_depth_visualize, checked on the host before any device is needed.
+static int check_depth_vis_args(const rcvd_depth_vis_params* prm, const void* frames, const uint8_t* colormap, bool range, const int64_t* counts,
+                                const double* stats, const uint8_t* rgb) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_depth_vis_params& q = *prm;
+  if (q.width <= 0 || q.height <= 0 || (int64_t)q.width * q.height * 3 >= (int64_t(1) << 31) || q.num_frames < 0)
+    return set_err(RCVD_ERR_INVALID, "bad depth visualisation frames: %d x %d, %d frames", q.width, q.height, q.num_frames);
+  if (q.kind != RCVD_DEPTH_VIS_F32 && q.kind != RCVD_DEPTH_VIS_U8C3) return set_err(RCVD_ERR_INVALID, "unknown depth visualisation kind %d", q.kind);
+  if (!counts != !stats) return set_err(RCVD_ERR_INVALID, "the range pass needs both counts and stats");
+  if (range && !(q.q[0] >= 0 && q.q[0] <= 1 && q.q[1] >= 0 && q.q[1] <= 1)) return set_err(RCVD_ERR_INVALID, "quantiles %g, %g outside [0, 1]", q.q[0], q.q[1]);
+  if (q.num_frames > 0 && !frames) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (rgb && !colormap) return set_err(RCVD_ERR_INVALID, "rgb output without a colormap");
+  return RCVD_OK;
+}
+static DepthVisArgs depth_vis_args(VideoCall& call, const rcvd_depth_vis_params& q, const void* frames, const uint8_t* colormap) {
+  DepthVisArgs a{};
+  a.w = q.width; a.h = q.height; a.u8 = q.kind == RCVD_DEPTH_VIS_U8C3;
+  a.src = call.upload(frames, (size_t)q.num_frames * q.width * q.height * (a.u8 ? 3 : 4));
+  a.q[0] = q.q[0]; a.q[1] = q.q[1]; a.offset = q.offset; a.scale = q.scale;
+  a.lut = colormap ? (const uint8_t*)call.upload(colormap, 256 * 3) : nullptr;
+  return a;
+}
+static int launch_depth_range(VideoCall& call, const DepthVisArgs& a, int F) {
+  return call.launch(k_depth_range, dim3(F), kDvSelThreads, 0, a);
+}
+// every frame in launches of at most 65535 (grid.y) frames
+static int launch_depth_color(VideoCall& call, DepthVisArgs a, int F) {
+  for (int f0 = 0; f0 < F; f0 += 65535) {
+    a.frame0 = f0;
+    if (int rc = call.launch(k_depth_color, dim3(nblk((size_t)a.w * a.h, kDvThreads), std::min(65535, F - f0)), kDvThreads, 0, a)) return rc;
+  }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_depth_visualize(const rcvd_depth_vis_params* prm, int32_t device, const void* frames, const uint8_t* colormap,
+                                      int64_t* counts, double* stats, uint8_t* index, uint8_t* rgb) {
+  if (int rc = check_depth_vis_args(prm, frames, colormap, counts != nullptr, counts, stats, rgb)) return rc;
+  const rcvd_depth_vis_params& q = *prm;
+  const size_t F = q.num_frames, px = F * q.width * q.height;
+  if (F == 0) return RCVD_OK;
+  VideoCall call;
+  if (int rc = call.open(device, g_depth_vis_launches)) return rc;
+  DepthVisArgs a = depth_vis_args(call, q, frames, colormap);
+  if (counts) { a.counts = (long long*)call.alloc(F * 8); a.stats = (double*)call.alloc(F * kDvRanks * 8); }
+  if (index) a.index = (uint8_t*)call.alloc(px);
+  if (rgb) a.rgb = (uint8_t*)call.alloc(px * 3);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_depth_visualize");
+  if (counts) {
+    if (int rc = launch_depth_range(call, a, q.num_frames)) return rc;
+    cudaMemcpyAsync(counts, a.counts, F * 8, cudaMemcpyDeviceToHost, call.st);
+    cudaMemcpyAsync(stats, a.stats, F * kDvRanks * 8, cudaMemcpyDeviceToHost, call.st);
+  }
+  if (index || rgb) {
+    if (int rc = launch_depth_color(call, a, q.num_frames)) return rc;
+    if (index) cudaMemcpyAsync(index, a.index, px, cudaMemcpyDeviceToHost, call.st);
+    if (rgb) cudaMemcpyAsync(rgb, a.rgb, px * 3, cudaMemcpyDeviceToHost, call.st);
+  }
+  return call.sync("depth visualisation kernels");
+}
+RCVD_API int32_t rcvd_debug_time_depth_visualize(const rcvd_depth_vis_params* prm, int32_t device, const void* frames, const uint8_t* colormap,
+                                                 int32_t reps, double* ms_range, double* ms_color) {
+  if (int rc = check_depth_vis_args(prm, frames, colormap, true, nullptr, nullptr, nullptr)) return rc;
+  if (reps < 1 || !ms_range || !ms_color || !colormap || prm->num_frames == 0) return set_err(RCVD_ERR_INVALID, "bad timing arguments");
+  const size_t F = prm->num_frames;
+  VideoCall call;
+  if (int rc = call.open(device, g_depth_vis_launches)) return rc;
+  DepthVisArgs a = depth_vis_args(call, *prm, frames, colormap);
+  a.counts = (long long*)call.alloc(F * 8); a.stats = (double*)call.alloc(F * kDvRanks * 8);
+  a.rgb = (uint8_t*)call.alloc(F * prm->width * prm->height * 3);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_depth_visualize");
+  cudaEvent_t e[3];
+  for (cudaEvent_t& ev : e) CK(cudaEventCreate(&ev));
+  int rc = launch_depth_range(call, a, prm->num_frames);   // warm-up
+  if (rc == RCVD_OK) rc = launch_depth_color(call, a, prm->num_frames);
+  cudaEventRecord(e[0], call.st);
+  for (int r = 0; r < reps && rc == RCVD_OK; ++r) rc = launch_depth_range(call, a, prm->num_frames);
+  cudaEventRecord(e[1], call.st);
+  for (int r = 0; r < reps && rc == RCVD_OK; ++r) rc = launch_depth_color(call, a, prm->num_frames);
+  cudaEventRecord(e[2], call.st);
+  if (rc == RCVD_OK) rc = call.sync("depth visualisation timing");
+  float t0 = 0.f, t1 = 0.f;
+  if (rc == RCVD_OK) { cudaEventElapsedTime(&t0, e[0], e[1]); cudaEventElapsedTime(&t1, e[1], e[2]); }
+  for (cudaEvent_t ev : e) cudaEventDestroy(ev);
+  *ms_range = (double)t0 / reps; *ms_color = (double)t1 / reps;
   return rc;
 }

@@ -678,6 +678,64 @@ def time_resize_area(frames, outputs, reps=20, device=0):
     return ms.value
 
 
+def _depth_vis_params(frames, q=(0.0, 1.0), offset=0.0, scale=1.0):
+    """The frames as a contiguous array and their rcvd_depth_vis_params: [F, H, W] float32 (RCVD_DEPTH_VIS_F32) or [F, H, W, 3] u8
+    (RCVD_DEPTH_VIS_U8C3)."""
+    fr = np.ascontiguousarray(frames)
+    if fr.dtype == np.float32 and fr.ndim == 3:
+        kind = abi.DEPTH_VIS_F32
+    elif fr.dtype == np.uint8 and fr.ndim == 4 and fr.shape[3] == 3:
+        kind = abi.DEPTH_VIS_U8C3
+    else:
+        raise ValueError(f"frames of shape {fr.shape} and type {fr.dtype}: need [frames, height, width] float32 or "
+                         "[frames, height, width, 3] u8")
+    prm = abi.DepthVisParams(width=fr.shape[2], height=fr.shape[1], num_frames=fr.shape[0], kind=kind, offset=float(offset),
+                             scale=float(scale))
+    prm.q[0], prm.q[1] = float(q[0]), float(q[1])
+    return fr, prm
+
+
+def depth_range(frames, q, device=0):
+    """The range pass of rcvd_depth_visualize: per frame the count of finite values (int64 [F]) and the order statistics at numpy's
+    linear-method neighbours of (n - 1) q for both quantiles q (float64 [F, 4]: floor and next for q[0], then for q[1]; rows of
+    frames without a finite value are undefined).  q: quantiles in [0, 1] as np.percentile holds them (for float32 frames,
+    np.float32(p) / np.float32(100))."""
+    fr, prm = _depth_vis_params(frames, q)
+    counts = np.empty(fr.shape[0], np.int64)
+    stats = np.empty((fr.shape[0], 4), np.float64)
+    _check(lib().rcvd_depth_visualize(C.byref(prm), C.c_int32(device), C.c_void_p(fr.ctypes.data), None, _p(counts, C.c_int64),
+                                      _p(stats, C.c_double), None, None))
+    return counts, stats
+
+
+def depth_colorize(frames, offset, scale, colormap=None, index=False, device=0):
+    """The colour pass of rcvd_depth_visualize (visualization.visualize_depth, reference utils/visualization.py:53-68): per pixel
+    np.uint8(((d - offset) / scale) ** 0.5 * 255), float32 for [F, H, W] float32 frames (offset and scale rounded to float32), float64
+    per channel then cv2's BGR-to-gray conversion for [F, H, W, 3] u8 frames.  colormap [256, 3] u8: the returned [F, H, W, 3] u8 image
+    is colormap[index].  index=True also returns the [F, H, W] u8 indices: (rgb, index), rgb None without a colormap."""
+    fr, prm = _depth_vis_params(frames, offset=offset, scale=scale)
+    shape = fr.shape[:3]
+    lut = None if colormap is None else np.ascontiguousarray(colormap, np.uint8).reshape(256, 3)
+    rgb = None if lut is None else np.empty(shape + (3,), np.uint8)
+    idx = np.empty(shape, np.uint8) if index else None
+    if rgb is None and idx is None:
+        raise ValueError("depth_colorize needs a colormap or index=True")
+    _check(lib().rcvd_depth_visualize(C.byref(prm), C.c_int32(device), C.c_void_p(fr.ctypes.data), _p(lut, C.c_uint8), None, None,
+                                      _p(idx, C.c_uint8), _p(rgb, C.c_uint8)))
+    return (rgb, idx) if index else rgb
+
+
+def time_depth_visualize(frames, q, offset, scale, colormap, reps=20, device=0):
+    """Bench hook: mean device ms of one range pass and of one colour pass of rcvd_depth_visualize over all the frames (frames uploaded
+    once, CUDA events): (ms_range, ms_color)."""
+    fr, prm = _depth_vis_params(frames, q, offset, scale)
+    lut = np.ascontiguousarray(colormap, np.uint8).reshape(256, 3)
+    a, b = C.c_double(), C.c_double()
+    _check(lib().rcvd_debug_time_depth_visualize(C.byref(prm), C.c_int32(device), C.c_void_p(fr.ctypes.data), _p(lut, C.c_uint8),
+                                                 C.c_int32(reps), C.byref(a), C.byref(b)))
+    return a.value, b.value
+
+
 FP64_MMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
 
 
