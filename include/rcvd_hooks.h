@@ -104,6 +104,9 @@ int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double* L, doub
  * (k_fwd_* / k_bwd_*), k_substitution, k_trinv, the rest (k_load_factor, k_potrf_trail), k_update_tma<1> launches with fewer CTAs
  * than items (CTAs that walk several items), k_trsm_ll launches (either shape) streamed beside their level's k_potrf_smem} */
 int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]);
+/* launches of each pair kernel that assembles the normal matrix (cost + gradient + H) since the handle was created: {k_pairs,
+ * k_accumulate_runs, k_accumulate_fast}.  rcvd_debug_set_fast_path and the configuration choose among them. */
+int32_t rcvd_debug_pair_kernel_launches(rcvd_problem* p, int64_t out[3]);
 
 /* one damped LM step at the current state with trust-region `radius`; out = {|(S H S + D2) y - S g| / |S g| (device SpMV over the
  * assembled H), |S g|, cost, |g|_2, |y|_2, non-positive-pivot flag}: the parity evidence bench.py prints at the size it times */

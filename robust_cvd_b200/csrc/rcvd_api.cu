@@ -202,6 +202,7 @@ struct rcvd_problem {
   // multi GPU
   int nranks = 1, rank = 0; nccl::Comm comm = nullptr;
   int64_t launches = 0, graph_launches = 0;
+  int64_t pair_launches[3] = {0, 0, 0};   // rcvd_debug_pair_kernel_launches: CostGradH launches of k_pairs, k_accumulate_runs, k_accumulate_fast
   // The caller-visible state (N x nf, caller's frame order) is h_state whenever !structure_ready || state_dirty, and d_x otherwise:
   // drop_structure saves d_x to h_state before it invalidates the structure, ensure_ready uploads h_state when state_dirty.
   std::vector<double> h_state; bool state_dirty = true; bool overlap = true; int order_slack = 4;   // multiple elimination with degree slack 4 (measured at config 2: slack 1..5 -> 13.65 13.11 12.74 12.66 13.09 ms per iteration); -1: greedy minimum degree
@@ -331,10 +332,12 @@ static int enqueue_residuals(rcvd_problem* p, const double* x, double* g) {
   cudaStream_t st = p->stream; double* part = p->d_partial; int rc;
   if (ntiles > 0) {
     const bool tc = MODE == EvalMode::CostGradH && p->fast_path != 0;   // a tensor-core kernel (rcvd_debug_set_fast_path)
-    if (tc && p->fast_path == 1 && p->records_sorted) rc = launch(p, k_accumulate_runs, ntiles, kTile, kRunSmem, st, false, d, x, p->d_H, g, part);
-    else if (tc && fast_path_ok(p->cfg, p->L)) rc = launch(p, k_accumulate_fast, ntiles, kTile, kFastSmem, st, false, d, x, p->d_H, g, part);
+    int which = 0;
+    if (tc && p->fast_path == 1 && p->records_sorted) { which = 1; rc = launch(p, k_accumulate_runs, ntiles, kTile, kRunSmem, st, false, d, x, p->d_H, g, part); }
+    else if (tc && fast_path_ok(p->cfg, p->L)) { which = 2; rc = launch(p, k_accumulate_fast, ntiles, kTile, kFastSmem, st, false, d, x, p->d_H, g, part); }
     else rc = launch(p, k_pairs<MODE>, ntiles, kTile, 0, st, false, d, x, p->d_H, g, part, p->d_active, NoRows{});
     if (rc) return rc;
+    if (MODE == EvalMode::CostGradH) p->pair_launches[which] += 1;
   }
   if (regblocks > 0 && (rc = launch(p, k_regularisers<MODE>, regblocks, 128, 0, st, false, d, rcn, x, p->d_H, g, part + p->part_reg, p->d_active,
                                     p->first_frame, p->last_frame, NoRows{}))) return rc;
@@ -1748,6 +1751,11 @@ RCVD_API int32_t rcvd_debug_factor_dense(rcvd_problem* p, int32_t* order, double
       for (int i = 0; i < nf; ++i) for (int j = 0; j < nf; ++j) out[(size_t)i * nf + j] = j <= i ? hL[f * bs + (size_t)i * npad + j] : 0.0;
     }
   }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_debug_pair_kernel_launches(rcvd_problem* p, int64_t out[3]) {
+  if (!p || !out) return set_err(RCVD_ERR_INVALID, "null argument");
+  std::copy(p->pair_launches, p->pair_launches + 3, out);
   return RCVD_OK;
 }
 RCVD_API int32_t rcvd_debug_linear_paths(rcvd_problem* p, int64_t out[13]) {

@@ -376,6 +376,14 @@ class Problem:
         2 selects k_accumulate_fast even on bilinear grids, where the run path would serve."""
         _check(self.L.rcvd_debug_set_fast_path(self.h, C.c_int32(int(on))))
 
+    PAIR_KERNELS = ("k_pairs", "k_accumulate_runs", "k_accumulate_fast")
+
+    def pair_kernel_launches(self):
+        """Test hook: launches of each pair kernel that assembled the normal matrix since the handle was created (PAIR_KERNELS)."""
+        out = (C.c_int64 * len(self.PAIR_KERNELS))()
+        _check(self.L.rcvd_debug_pair_kernel_launches(self.h, out))
+        return dict(zip(self.PAIR_KERNELS, list(out)))
+
     def set_update_kernel(self, tma=True, side_items_per_cta=0):
         """Test / bench hook: side_items_per_cta > 0 caps the work items per CTA of the one-team update launches.  tma must be True:
         the persistent TMA-fed kernel is the only update kernel (False raises)."""
