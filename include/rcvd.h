@@ -565,6 +565,39 @@ typedef struct rcvd_depth_vis_params {
 int32_t rcvd_depth_visualize(const rcvd_depth_vis_params* prm, int32_t device, const void* frames, const uint8_t* colormap,
                              int64_t* counts, double* stats, uint8_t* index, uint8_t* rgb);
 
+/* ---- homography-registered optical flows (DESIGN.md section 1 row 8f-12) ----
+ * Replace the per-pixel work of optical_flow_homography.getimage / infer / resize_flow (reference optical_flow_homography.py:139-242,
+ * run by Flow.compute_flow, flow.py:84-126) for a batch of frame pairs; the model runs between them.  Arithmetic as OpenCV 4.13 and
+ * numpy compute it on x86-64, bit for bit (robust_cvd_b200/csrc/rcvd_flowreg.cuh names every quirk).
+ * rcvd_homography_warp: registered[p] = cv2.warpPerspective(frames[pair_frames[p]], H_BA, (width, height)), INTER_LINEAR,
+ * BORDER_CONSTANT 0, through OpenCV's fixed-point path.
+ *   frames      [num_frames][height][width][3] u8 (B, G, R as cv::imread gives; any channel order works): a frame is passed once
+ *   pair_frames [num_pairs] local id of the frame each pair warps (frame j of pair (i, j))
+ *   inverse     [num_pairs][9] the map cv2 applies: cv::invert(H_BA) (closed form, row-major)
+ *   registered  [num_pairs][height][width][3] u8 (out)
+ * num_pairs = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null parameter block or
+ * array, a non-positive size, 3 * width * height >= 2^31, a negative count, no frames for a pair, a pair frame out of range. */
+typedef struct rcvd_homography_warp_params {
+  int32_t width, height, num_pairs, num_frames;
+} rcvd_homography_warp_params;
+int32_t rcvd_homography_warp(const rcvd_homography_warp_params* prm, int32_t device, const uint8_t* frames, const int32_t* pair_frames,
+                             const double* inverse, uint8_t* registered);
+/* rcvd_flow_unregister: out[p] = float32(resize_flow(un-registered flow, (out_width, out_height))), the values of flow/flow_i_j.raw:
+ * per pixel fxx = x + u, fyy = y + v in float32, h_inv.dot([fxx; fyy; 1]) in double as OpenBLAS' dgemm (fma(h2, 1, fma(h1, fyy,
+ * h0 fxx))), x / z - x, y / z - y; then cv2.resize(INTER_CUBIC) of that float64 field and times (out_width / width, out_height /
+ * height).  The full-size float64 flow is never stored: each output pixel recomputes its 4 x 4 source taps.
+ *   flow  [num_pairs][height][width][2] f32, the model's flow_up[0] (u, v)
+ *   h_inv [num_pairs][9] np.linalg.inv(H_BA), row-major
+ *   out   [num_pairs][out_height][out_width][2] f32 (out)
+ * num_pairs = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null parameter block or
+ * array, a non-positive size, 2 * width * height >= 2^31 for either size, a negative pair count. */
+typedef struct rcvd_flow_unregister_params {
+  int32_t width, height;           /* the model's flow: the color_flow frames */
+  int32_t out_width, out_height;   /* the .raw files: the color_down frames */
+  int32_t num_pairs;
+} rcvd_flow_unregister_params;
+int32_t rcvd_flow_unregister(const rcvd_flow_unregister_params* prm, int32_t device, const float* flow, const double* h_inv, float* out);
+
 #ifdef __cplusplus
 }
 #endif

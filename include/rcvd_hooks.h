@@ -31,6 +31,14 @@ int32_t rcvd_debug_time_depth_visualize(const rcvd_depth_vis_params* prm, int32_
  * *ms is the mean device time of one launch over all the pairs.  Arguments and refusals as rcvd_flow_masks; reps >= 1. */
 int32_t rcvd_debug_time_flow_masks(const rcvd_flow_mask_params* prm, int32_t device, const int32_t* pair_frames, const float* flow_ij,
                                    const float* flow_ji, const float* colors, int32_t reps, double* ms);
+int64_t rcvd_flow_register_launch_count(void);
+/* rcvd_homography_warp's / rcvd_flow_unregister's kernel alone: the inputs are uploaded once, the kernel runs reps times between two
+ * CUDA events, and *ms is the mean device time of one pass over all the pairs.  Arguments and refusals as the entry point (the output
+ * buffer is not needed); num_pairs >= 1, reps >= 1. */
+int32_t rcvd_debug_time_homography_warp(const rcvd_homography_warp_params* prm, int32_t device, const uint8_t* frames, const int32_t* pair_frames,
+                                        const double* inverse, int32_t reps, double* ms);
+int32_t rcvd_debug_time_flow_unregister(const rcvd_flow_unregister_params* prm, int32_t device, const float* flow, const double* h_inv,
+                                        int32_t reps, double* ms);
 int64_t rcvd_builder_last_rounds(void);          /* selection rounds of the last rcvd_build_constraints call */
 
 /* {frames, off-diagonal factor blocks, levels, H blocks, npad, stride, tiles, update targets ((source level, target block) pairs)} */

@@ -123,6 +123,16 @@ class ResizeParams(C.Structure):
                [("outputs", ResizeOutput * RESIZE_MAX_OUTPUTS)]
 
 
+class HomographyWarpParams(C.Structure):
+    """rcvd_homography_warp_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_pairs", "num_frames")]
+
+
+class FlowUnregisterParams(C.Structure):
+    """rcvd_flow_unregister_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "out_width", "out_height", "num_pairs")]
+
+
 DEPTH_VIS_F32, DEPTH_VIS_U8C3 = 0, 1
 
 

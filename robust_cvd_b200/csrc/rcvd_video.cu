@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations, the downscaled colour frames and the depth visualisations.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations, the downscaled colour frames, the depth visualisations and the homography-registered flows.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -19,6 +19,7 @@
 #include "rcvd_flowvis.cuh"
 #include "rcvd_resize.cuh"
 #include "rcvd_depthvis.cuh"
+#include "rcvd_flowreg.cuh"
 
 using namespace rcvd;
 
@@ -966,4 +967,150 @@ RCVD_API int32_t rcvd_debug_time_depth_visualize(const rcvd_depth_vis_params* pr
   for (cudaEvent_t ev : e) cudaEventDestroy(ev);
   *ms_range = (double)t0 / reps; *ms_color = (double)t1 / reps;
   return rc;
+}
+
+// ---------------------------------------------------------------------------
+// Homography-registered optical flows (rcvd_flowreg.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_flowreg_launches = 0;
+RCVD_API int64_t rcvd_flow_register_launch_count() { return g_flowreg_launches; }
+// mean device ms of one launch(call) over reps runs after a warm-up run, between two CUDA events
+template <class Launch>
+static int time_launches(VideoCall& call, int reps, double* ms, const char* what, Launch launch) {
+  if (int rc = launch()) return rc;   // warm-up
+  cudaEvent_t e0, e1;
+  CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+  cudaEventRecord(e0, call.st);
+  int rc = RCVD_OK;
+  for (int r = 0; r < reps && rc == RCVD_OK; ++r) rc = launch();
+  cudaEventRecord(e1, call.st);
+  if (rc == RCVD_OK) rc = call.sync(what);
+  float t = 0.f;
+  if (rc == RCVD_OK) cudaEventElapsedTime(&t, e0, e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  *ms = (double)t / reps;
+  return rc;
+}
+
+// The argument rules of rcvd_homography_warp, checked on the host before any device is needed.
+static int check_homography_warp_args(const rcvd_homography_warp_params* prm, const uint8_t* frames, const int32_t* pair_frames, const double* inverse) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_homography_warp_params& q = *prm;
+  if (q.width <= 0 || q.height <= 0 || 3 * (int64_t)q.width * q.height >= (int64_t(1) << 31) || q.num_pairs < 0 || q.num_frames < 0 ||
+      (q.num_pairs > 0 && q.num_frames == 0))
+    return set_err(RCVD_ERR_INVALID, "bad homography-warp parameters: %d x %d, %d pairs, %d frames", q.width, q.height, q.num_pairs, q.num_frames);
+  if (q.num_pairs > 0 && (!frames || !pair_frames || !inverse)) return set_err(RCVD_ERR_INVALID, "null argument");
+  for (int i = 0; i < q.num_pairs; ++i)
+    if (pair_frames[i] < 0 || pair_frames[i] >= q.num_frames) return set_err(RCVD_ERR_INVALID, "pair %d: frame %d out of range", i, pair_frames[i]);
+  return RCVD_OK;
+}
+static HomographyWarpArgs upload_homography_warp_inputs(VideoCall& call, const rcvd_homography_warp_params& q, const uint8_t* frames,
+                                                        const int32_t* pair_frames, const double* inverse) {
+  const size_t P = q.num_pairs, img = (size_t)q.width * q.height * 3;
+  HomographyWarpArgs a{};
+  a.W = q.width; a.H = q.height;
+  a.bw = std::min(1024 / std::min(16, q.height), q.width);
+  a.frames = (const uint8_t*)call.upload(frames, (size_t)q.num_frames * img);
+  a.pair_frame = (const int*)call.upload(pair_frames, P * 4);
+  a.minv = (const double*)call.upload(inverse, P * 72);
+  const std::vector<int> tab = warp_weight_table();   // read by the copy before cudaMemcpyAsync returns (pageable source)
+  a.wtab = (const int*)call.upload(tab.data(), tab.size() * 4);
+  a.out = (uint8_t*)call.alloc(P * img);
+  return a;
+}
+// every pair in launches of at most 65535 (grid.y) pairs
+static int launch_homography_warp(VideoCall& call, HomographyWarpArgs a, int P) {
+  const unsigned gx = (unsigned)nblk((size_t)a.W * a.H, kFrThreads);
+  for (int p0 = 0; p0 < P; p0 += 65535) {
+    a.pair0 = p0;
+    if (int rc = call.launch(k_homography_warp, dim3(gx, std::min(65535, P - p0)), kFrThreads, 0, a)) return rc;
+  }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_homography_warp(const rcvd_homography_warp_params* prm, int32_t device, const uint8_t* frames, const int32_t* pair_frames,
+                                      const double* inverse, uint8_t* registered) {
+  if (int rc = check_homography_warp_args(prm, frames, pair_frames, inverse)) return rc;
+  const rcvd_homography_warp_params& q = *prm;
+  if (q.num_pairs == 0) return RCVD_OK;
+  if (!registered) return set_err(RCVD_ERR_INVALID, "null argument");
+  VideoCall call;
+  if (int rc = call.open(device, g_flowreg_launches)) return rc;
+  const HomographyWarpArgs a = upload_homography_warp_inputs(call, q, frames, pair_frames, inverse);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_homography_warp");
+  if (int rc = launch_homography_warp(call, a, q.num_pairs)) return rc;
+  cudaMemcpyAsync(registered, a.out, (size_t)q.num_pairs * q.width * q.height * 3, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("homography-warp kernel");
+}
+RCVD_API int32_t rcvd_debug_time_homography_warp(const rcvd_homography_warp_params* prm, int32_t device, const uint8_t* frames,
+                                                 const int32_t* pair_frames, const double* inverse, int32_t reps, double* ms) {
+  if (int rc = check_homography_warp_args(prm, frames, pair_frames, inverse)) return rc;
+  if (reps < 1 || !ms || prm->num_pairs == 0) return set_err(RCVD_ERR_INVALID, "bad timing arguments");
+  VideoCall call;
+  if (int rc = call.open(device, g_flowreg_launches)) return rc;
+  const HomographyWarpArgs a = upload_homography_warp_inputs(call, *prm, frames, pair_frames, inverse);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_homography_warp");
+  return time_launches(call, reps, ms, "homography-warp timing", [&] { return launch_homography_warp(call, a, prm->num_pairs); });
+}
+
+// The argument rules of rcvd_flow_unregister, checked on the host before any device is needed.
+static int check_flow_unregister_args(const rcvd_flow_unregister_params* prm, const float* flow, const double* h_inv) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_flow_unregister_params& q = *prm;
+  auto bad_size = [](int w, int h) { return w <= 0 || h <= 0 || 2 * (int64_t)w * h >= (int64_t(1) << 31); };
+  if (bad_size(q.width, q.height) || bad_size(q.out_width, q.out_height) || q.num_pairs < 0)
+    return set_err(RCVD_ERR_INVALID, "bad flow-unregister parameters: %d x %d -> %d x %d, %d pairs", q.width, q.height, q.out_width, q.out_height, q.num_pairs);
+  if (q.num_pairs > 0 && (!flow || !h_inv)) return set_err(RCVD_ERR_INVALID, "null argument");
+  return RCVD_OK;
+}
+// Uploads the flows, the inverses and the cubic tables, and allocates the output (a.pair0 is left for the launches).
+static FlowUnregisterArgs upload_flow_unregister_inputs(VideoCall& call, const rcvd_flow_unregister_params& q, const float* flow, const double* h_inv) {
+  const size_t P = q.num_pairs;
+  FlowUnregisterArgs a{};
+  a.W = q.width; a.H = q.height; a.w = q.out_width; a.h = q.out_height;
+  a.copy = q.out_width == q.width && q.out_height == q.height;
+  a.sx = q.out_width / (double)q.width; a.sy = q.out_height / (double)q.height;
+  a.flow = (const float*)call.upload(flow, P * q.width * q.height * 8);
+  a.hinv = (const double*)call.upload(h_inv, P * 72);
+  // reused for the y tables: a copy from pageable memory has read its source when cudaMemcpyAsync returns
+  std::vector<int> first; std::vector<float> coef; std::vector<uint8_t> inside;
+  resize_cubic_taps(q.width, q.out_width, first, coef, inside);
+  a.xs = (const int*)call.upload(first.data(), first.size() * 4);
+  a.xc = (const float*)call.upload(coef.data(), coef.size() * 4);
+  a.xin = (const uint8_t*)call.upload(inside.data(), inside.size());
+  resize_cubic_taps(q.height, q.out_height, first, coef, inside);
+  a.ys = (const int*)call.upload(first.data(), first.size() * 4);
+  a.yc = (const float*)call.upload(coef.data(), coef.size() * 4);
+  a.out = (float*)call.alloc(P * q.out_width * q.out_height * 8);
+  return a;
+}
+static int launch_flow_unregister(VideoCall& call, FlowUnregisterArgs a, int P) {
+  const unsigned gx = (unsigned)nblk((size_t)a.w * a.h, kFrThreads);
+  for (int p0 = 0; p0 < P; p0 += 65535) {
+    a.pair0 = p0;
+    if (int rc = call.launch(k_flow_unregister, dim3(gx, std::min(65535, P - p0)), kFrThreads, 0, a)) return rc;
+  }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_flow_unregister(const rcvd_flow_unregister_params* prm, int32_t device, const float* flow, const double* h_inv, float* out) {
+  if (int rc = check_flow_unregister_args(prm, flow, h_inv)) return rc;
+  const rcvd_flow_unregister_params& q = *prm;
+  if (q.num_pairs == 0) return RCVD_OK;
+  if (!out) return set_err(RCVD_ERR_INVALID, "null argument");
+  VideoCall call;
+  if (int rc = call.open(device, g_flowreg_launches)) return rc;
+  const FlowUnregisterArgs a = upload_flow_unregister_inputs(call, q, flow, h_inv);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_flow_unregister");
+  if (int rc = launch_flow_unregister(call, a, q.num_pairs)) return rc;
+  cudaMemcpyAsync(out, a.out, (size_t)q.num_pairs * q.out_width * q.out_height * 8, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("flow-unregister kernel");
+}
+RCVD_API int32_t rcvd_debug_time_flow_unregister(const rcvd_flow_unregister_params* prm, int32_t device, const float* flow, const double* h_inv,
+                                                 int32_t reps, double* ms) {
+  if (int rc = check_flow_unregister_args(prm, flow, h_inv)) return rc;
+  if (reps < 1 || !ms || prm->num_pairs == 0) return set_err(RCVD_ERR_INVALID, "bad timing arguments");
+  VideoCall call;
+  if (int rc = call.open(device, g_flowreg_launches)) return rc;
+  const FlowUnregisterArgs a = upload_flow_unregister_inputs(call, *prm, flow, h_inv);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_flow_unregister");
+  return time_launches(call, reps, ms, "flow-unregister timing", [&] { return launch_flow_unregister(call, a, prm->num_pairs); });
 }

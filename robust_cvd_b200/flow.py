@@ -1,33 +1,38 @@
-"""Flow-consistency masks, pair mask ratios and flow visualisations of a robust_cvd working directory, with the per-pixel work on the GPU.
+"""Homography-registered optical flows, flow-consistency masks, pair mask ratios and flow visualisations of a robust_cvd working
+directory, with the per-pixel work on the GPU.
 
-Drop-in for the reference's Flow.compute_flow_masks, Flow.compute_flow_pair_stats and Flow.visualize_flow (flow.py:44-74, :128-209),
-which process.py runs after RAFT: it reads flow/flow_%06d_%06d.raw and color_down/frame_%06d.raw and writes flow_mask/mask_%06d_%06d.png
-(8-bit, 0 / 255) and flow_list.json, the files the constraint builder, static flags, tracks and filters read; with --vis_flow it also
-writes vis_flow/frame_%06d_%06d.png and vis_flow_warped/frame_%06d_%06d_warped.png.  The per-pixel work is rcvd_flow_masks and
-rcvd_flow_visualize (include/rcvd.h); the files are read with numpy, and the PNGs are encoded on a thread pool while the next chunk of
-pairs computes.
+Drop-in for the reference's Flow class (flow.py): compute_flow (flow.py:84-126, optical_flow_homography.py) reads color_flow/frame_%06d.png
+and writes flow/flow_%06d_%06d.raw; compute_flow_masks, compute_flow_pair_stats and visualize_flow (flow.py:44-74, :128-209), which
+process.py runs after it, read flow/flow_%06d_%06d.raw and color_down/frame_%06d.raw and write flow_mask/mask_%06d_%06d.png (8-bit,
+0 / 255) and flow_list.json, the files the constraint builder, static flags, tracks and filters read; with --vis_flow they also write
+vis_flow/frame_%06d_%06d.png and vis_flow_warped/frame_%06d_%06d_warped.png.  The per-pixel work is rcvd_homography_warp,
+rcvd_flow_unregister, rcvd_flow_masks and rcvd_flow_visualize (include/rcvd.h); the files are read with numpy, and the outputs are
+written on a thread pool while the next pairs compute.  The optical-flow model (RAFT) and the feature detector (SURF) are the caller's.
 
-There is no CPU fallback: without librcvd_b200.so or a usable CUDA device compute_flow_masks and visualize_flow raise RuntimeError.
+There is no CPU fallback: without librcvd_b200.so or a usable CUDA device these functions raise RuntimeError.
 """
 import json
 import os
 import re
 import struct
 import sys
+import threading
 import time
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 from . import solver
-from .png import png_gray_bytes, png_rgb_bytes, write_png  # noqa: F401  (png_*_bytes: part of this module's interface)
-from .synthetic_files import read_raw
+from .png import png_gray_bytes, png_header, png_rgb_bytes, write_png  # noqa: F401  (png_*_bytes: part of this module's interface)
+from .synthetic_files import read_raw, write_raw
 
 FLOW_FMT = os.path.join("flow", "flow_{:06d}_{:06d}.raw")
 MASK_FMT = os.path.join("flow_mask", "mask_{:06d}_{:06d}.png")
 COLOR_FMT = os.path.join("color_down", "frame_{:06d}.raw")
 VIS_FMT = os.path.join("vis_flow", "frame_{:06d}_{:06d}.png")
 WARP_FMT = os.path.join("vis_flow_warped", "frame_{:06d}_{:06d}_warped.png")
+FRAME_FMT = os.path.join("color_flow", "frame_{:06d}.png")
+RAFT_MODEL_PATH = os.path.join("models", "raft-things.pth")
 _FLOW_NAME = re.compile(r"^flow_(\d+)_(\d+)\.raw$")
 
 
@@ -157,6 +162,201 @@ def compute_flow_masks(path, flow_thresh=1, color_thresh=1, device=None, chunk_b
         t = time.perf_counter()
         stats["png_s"] += sum(f.result() for f in pending)
         stats["wait_s"] += time.perf_counter() - t
+    stats["total_s"] = time.perf_counter() - t0
+    return stats
+
+
+IDENTITY = np.array([1.0, 0, 0, 0, 1.0, 0, 0, 0, 1.0]).reshape(3, 3)
+
+
+def cv_invert3(H):
+    """cv::invert(H, DECOMP_LU) of a 3 x 3 double matrix, the map cv2.warpPerspective applies: its closed form (cofactors times 1 / det,
+    det expanded along row 0, every product rounded); a zero det gives the zero matrix, as cv::invert leaves it."""
+    m = np.asarray(H, np.float64).reshape(3, 3).tolist()
+    (a, b, c), (d, e, f), (g, h, i) = m
+    det = a * (e * i - f * h) - b * (d * i - f * g) + c * (d * h - e * g)
+    if det == 0:
+        return np.zeros((3, 3))
+    r = 1.0 / det
+    return np.array([[(e * i - f * h) * r, (c * h - b * i) * r, (b * f - c * e) * r],
+                     [(f * g - d * i) * r, (a * i - c * g) * r, (c * d - a * f) * r],
+                     [(d * h - e * g) * r, (b * g - a * h) * r, (a * e - b * d) * r]])
+
+
+def frame_features(img, detector):
+    """detectAndDescribe: the keypoint positions float32 [n, 2] and the descriptors (None without keypoints) of detector.detectAndCompute."""
+    kps, des = detector.detectAndCompute(img, None)
+    return np.float32([kp.pt for kp in kps]), des
+
+
+def homography(feat1, feat2, ratio=0.75, reproj_thresh=4.0):
+    """getimage's H_BA, which maps frame 2 onto frame 1, from the frame_features of both frames: frame 2's descriptors matched to frame
+    1's (BruteForce knnMatch, k = 2), the matches that pass Lowe's ratio test, and findHomography(RANSAC, reproj_thresh) of more than 4
+    of them.  The identity when anything fails, as the reference's fallbacks give: no descriptors (knnMatch raises), at most 4 matches,
+    findHomography raising or returning None, or a matrix np.linalg.inv refuses."""
+    import cv2
+    (kps1, des1), (kps2, des2) = feat1, feat2
+    try:
+        knn = cv2.DescriptorMatcher_create("BruteForce").knnMatch(des2, des1, 2)
+        good = [(m[0].queryIdx, m[0].trainIdx) for m in knn if len(m) == 2 and m[0].distance < m[1].distance * ratio]
+        if len(good) <= 4:
+            return IDENTITY.copy()
+        H, _ = cv2.findHomography(np.float32([kps2[q] for q, _ in good]), np.float32([kps1[t] for _, t in good]), cv2.RANSAC,
+                                  reproj_thresh)
+    except Exception:
+        return IDENTITY.copy()
+    if H is None:
+        return IDENTITY.copy()
+    try:
+        np.linalg.inv(H)
+    except np.linalg.LinAlgError:
+        return IDENTITY.copy()
+    return H
+
+
+class _Args(dict):
+    """The reference's argument record (a dict read by attribute, None when absent), which RAFT's constructor reads."""
+    __getattr__ = dict.get
+
+
+def _default_model(path_pairs, size, device):
+    """The reference's RAFT, imported from the caller's path and built as optical_flow_homography.process builds it."""
+    try:
+        import torch
+        from raft.core.raft import RAFT
+        im1, im2, out = path_pairs
+        args = _Args(model="raft", pretrained_weights=RAFT_MODEL_PATH, im1=im1, im2=im2, out=out, size=size, fp16=False, homography=True,
+                     rgb_max=255.0, visualize=False)
+        model = torch.nn.DataParallel(RAFT(args))
+        model.load_state_dict(torch.load(args.pretrained_weights, map_location=device))
+        model = model.module
+        model.to(device)
+        model.eval()
+        return model
+    except Exception as e:
+        raise RuntimeError(f"the default flow model is the reference's RAFT (raft.core.raft, weights {RAFT_MODEL_PATH}), which could not be "
+                           f"loaded ({type(e).__name__}: {e}); pass model= (a module called as model(img1, img2, iters=20, "
+                           "test_mode=True))") from e
+
+
+def _default_features():
+    import cv2
+    try:
+        return cv2.xfeatures2d.SURF_create
+    except AttributeError as e:
+        raise RuntimeError("the default feature detector is SURF (cv2.xfeatures2d.SURF_create), which this cv2 lacks (it is in the "
+                           "opencv-contrib build); pass features= (a callable returning a detector with detectAndCompute)") from e
+
+
+def flow_pairs_to_compute(path, index_pairs):
+    """The pairs (i, j) of index_pairs, first occurrence first, whose flow/flow_i_j.raw is missing: none when every file exists."""
+    out, seen = [], set()
+    for i, j in index_pairs:
+        p = (int(i), int(j))
+        if p not in seen and not os.path.isfile(os.path.join(path, FLOW_FMT.format(*p))):
+            out.append(p)
+        seen.add(p)
+    return out
+
+
+def _check_flow_inputs(path, pairs):
+    """Every frame of the pairs is an 8-bit RGB PNG of color_flow/frame_000000.png's size, and color_down/frame_000000.raw exists: refused
+    before anything is written.  Returns ((H, W) of the frames, (w, h) of color_down)."""
+    frames = sorted({0} | {f for p in pairs for f in p})
+    size = None
+    for f in frames:
+        fn = os.path.join(path, FRAME_FMT.format(f))
+        if not os.path.isfile(fn):
+            raise FileNotFoundError(f"{fn} is missing")
+        hd = png_header(fn)
+        if hd["bit_depth"] != 8 or hd["color_type"] != 2 or hd["interlace"]:
+            raise ValueError(f"{fn}: a {hd['bit_depth']}-bit PNG of colour type {hd['color_type']} (interlace {hd['interlace']}); the frames "
+                             "must be 8-bit RGB, not interlaced")
+        size = size or (hd["height"], hd["width"])
+        if (hd["height"], hd["width"]) != size:
+            raise ValueError(f"{fn}: {hd['width']} x {hd['height']} pixels, but frame 0 has {size[1]} x {size[0]}")
+    down = os.path.join(path, COLOR_FMT.format(0))
+    if not os.path.isfile(down):
+        raise FileNotFoundError(f"{down} is missing: the flows are resized to the color_down frames' size")
+    rows, cols, _ = _raw_shape(down)
+    return size, (cols, rows)
+
+
+def compute_flow(path, index_pairs, flow_model="raft", model=None, features=None, device=None, workers=None, batch=16):
+    """Flow.compute_flow with the per-pixel work on the GPU: writes flow/flow_i_j.raw for every pair of index_pairs whose file is
+    missing (nothing runs when all exist), as optical_flow_homography.process computes it: H_BA from the features of both color_flow
+    frames, frame j registered by cv2.warpPerspective (rcvd_homography_warp), the model's flow_up[0] of (frame i, registered frame j),
+    un-registered through np.linalg.inv(H_BA) and resized to color_down's size by resize_flow (rcvd_flow_unregister).
+
+    model: the flow network, called once per pair as model(img1, img2, iters=20, test_mode=True) on float32 [1, 3, H, W] BGR tensors
+    under no_grad; None builds the reference's RAFT from the caller's path.  features: a callable returning a detector with
+    detectAndCompute (one per worker thread); None is cv2.xfeatures2d.SURF_create.  Each frame is decoded and its features computed once,
+    on `workers` threads, which also match the pairs and write the files while the model runs.  A flow_model other than "raft" raises
+    ValueError; a missing model or detector raises RuntimeError, and a missing or odd frame or a missing color_down/frame_000000.raw
+    raises, all before anything is written.  Returns timings: {"pairs", "model_s", "kernel_s", "wait_s" (the caller's thread blocked on
+    decoding, features and matching), "total_s"}."""
+    import torch
+    from .video import _decode_png   # video imports this module
+    t0 = time.perf_counter()
+    if flow_model != "raft":
+        raise ValueError(f"flow model {flow_model!r}: only 'raft' is supported")
+    pairs = flow_pairs_to_compute(path, index_pairs)
+    stats = {"pairs": len(pairs), "model_s": 0.0, "kernel_s": 0.0, "wait_s": 0.0, "total_s": 0.0}
+    if not pairs:
+        os.makedirs(os.path.join(path, "flow"), exist_ok=True)
+        stats["total_s"] = time.perf_counter() - t0
+        return stats
+    factory = features or _default_features()
+    (H, W), size = _check_flow_inputs(path, pairs)
+    tdev = torch.device("cuda") if device is None else torch.device("cuda", int(device))
+    if model is None:
+        model = _default_model(([os.path.join(path, FRAME_FMT.format(i)) for i, _ in pairs],
+                                [os.path.join(path, FRAME_FMT.format(j)) for _, j in pairs],
+                                [os.path.join(path, FLOW_FMT.format(i, j)) for i, j in pairs]), size, tdev)
+    dev = solver.lib().rcvd_current_device() if device is None else int(device)
+    if dev < 0:
+        raise RuntimeError("rcvd error 5: no usable CUDA device for the flows; this library has no CPU fallback")
+    os.makedirs(os.path.join(path, "flow"), exist_ok=True)
+    print("Resizing flow to", size)
+    local = threading.local()
+
+    def load(f):
+        img = _decode_png(os.path.join(path, FRAME_FMT.format(f)))
+        if not hasattr(local, "detector"):
+            local.detector = factory()
+        return img, frame_features(img, local.detector)
+
+    workers = workers or min(8, os.cpu_count() or 1)
+    with ThreadPoolExecutor(workers) as pool:
+        frames = {f: pool.submit(load, f) for f in sorted({f for p in pairs for f in p})}
+        # every frame's job is queued before any pair's, so a pair's job never waits on a job queued behind it
+        hs = [pool.submit(lambda i, j: homography(frames[i].result()[1], frames[j].result()[1]), i, j) for i, j in pairs]
+        pending = []
+        for b0 in range(0, len(pairs), batch):
+            chunk = pairs[b0:b0 + batch]
+            t = time.perf_counter()
+            H_BA = [h.result() for h in hs[b0:b0 + batch]]
+            js = sorted({j for _, j in chunk})
+            src = np.stack([frames[j].result()[0] for j in js])
+            stats["wait_s"] += time.perf_counter() - t
+            t = time.perf_counter()
+            reg = solver.homography_warp(src, [js.index(j) for _, j in chunk], [cv_invert3(h) for h in H_BA], device=dev)
+            stats["kernel_s"] += time.perf_counter() - t
+            t = time.perf_counter()
+            flows = []
+            with torch.no_grad():
+                for n, (i, _) in enumerate(chunk):
+                    img1 = torch.from_numpy(frames[i].result()[0]).to(tdev).permute(2, 0, 1).contiguous().float()[None]
+                    img2 = torch.from_numpy(reg[n]).to(tdev).permute(2, 0, 1).contiguous().float()[None]
+                    _, flow_up = model(img1, img2, iters=20, test_mode=True)
+                    flows.append(flow_up[0].permute(1, 2, 0).cpu().numpy())
+            stats["model_s"] += time.perf_counter() - t
+            t = time.perf_counter()
+            out = solver.flow_unregister(np.stack(flows), [np.linalg.inv(h) for h in H_BA], size, device=dev)
+            stats["kernel_s"] += time.perf_counter() - t
+            pending += [pool.submit(write_raw, os.path.join(path, FLOW_FMT.format(i, j)), out[n]) for n, (i, j) in enumerate(chunk)]
+        for f in pending:
+            f.result()
     stats["total_s"] = time.perf_counter() - t0
     return stats
 
@@ -314,9 +514,9 @@ def compute_flow_pair_stats(path, frame_pairs):
 
 
 class Flow:
-    """The reference's Flow class (flow.py) on the GPU, every method but compute_flow (RAFT, which needs network weights): a caller of
-    Flow(path, out_path).compute_flow_masks() / .compute_flow_pair_stats(frame_pairs) / .visualize_flow(warp) switches by importing
-    this class instead."""
+    """The reference's Flow class (flow.py) on the GPU: a caller of Flow(path, out_path).compute_flow(index_pairs, flow_model) /
+    .compute_flow_masks() / .compute_flow_pair_stats(frame_pairs) / .visualize_flow(warp) switches by importing this class instead.
+    compute_flow builds the reference's RAFT and SURF, as the reference does; compute_flow(path, ..., model=, features=) takes others."""
 
     def __init__(self, path, out_path):
         self.path = path
@@ -325,6 +525,12 @@ class Flow:
     @staticmethod
     def max_size():
         return 1024
+
+    def check_flow_files(self, index_pairs):
+        return all(os.path.exists(os.path.join(self.path, FLOW_FMT.format(i, j))) for i, j in index_pairs)
+
+    def compute_flow(self, index_pairs, flow_model):
+        compute_flow(self.path, index_pairs, flow_model)
 
     def compute_flow_masks(self, flow_thresh=1, color_thresh=1):
         compute_flow_masks(self.path, flow_thresh, color_thresh)

@@ -686,6 +686,64 @@ def time_resize_area(frames, outputs, reps=20, device=0):
     return ms.value
 
 
+def _homography_warp_args(frames, pair_frames, inverse):
+    fr = np.ascontiguousarray(frames, np.uint8)
+    pf = np.ascontiguousarray(pair_frames, np.int32).reshape(-1)
+    inv = np.ascontiguousarray(inverse, np.float64).reshape(-1, 9)
+    if fr.ndim != 4 or fr.shape[3] != 3 or len(inv) != len(pf):
+        raise ValueError(f"homography-warp inputs of shapes frames {fr.shape}, pair frames {pf.shape}, inverses {inv.shape}: need "
+                         "[frames, height, width, 3] u8, [pairs] and [pairs, 3, 3]")
+    prm = abi.HomographyWarpParams(width=fr.shape[2], height=fr.shape[1], num_pairs=len(pf), num_frames=fr.shape[0])
+    return prm, (_p(fr, C.c_uint8), _p(pf, C.c_int32), _p(inv, C.c_double)), (fr, pf, inv)
+
+
+def homography_warp(frames, pair_frames, inverse, device=0):
+    """rcvd_homography_warp (cv2.warpPerspective(frame, H_BA, (W, H)) of optical_flow_homography.getimage, INTER_LINEAR, BORDER_CONSTANT
+    0) on the GPU.  frames [F, H, W, 3] u8, pair_frames [P] local id of the frame each pair warps, inverse [P, 3, 3] cv::invert(H_BA)
+    (flow.cv_invert3).  Returns the registered frames [P, H, W, 3] u8."""
+    prm, args, keep = _homography_warp_args(frames, pair_frames, inverse)
+    out = np.empty((prm.num_pairs, prm.height, prm.width, 3), np.uint8)
+    _check(lib().rcvd_homography_warp(C.byref(prm), C.c_int32(device), *args, _p(out, C.c_uint8)))
+    return out
+
+
+def time_homography_warp(frames, pair_frames, inverse, reps=20, device=0):
+    """Bench hook: mean device ms of one rcvd_homography_warp kernel pass over all the pairs (inputs uploaded once, CUDA events)."""
+    prm, args, keep = _homography_warp_args(frames, pair_frames, inverse)
+    ms = C.c_double()
+    _check(lib().rcvd_debug_time_homography_warp(C.byref(prm), C.c_int32(device), *args, C.c_int32(reps), C.byref(ms)))
+    return ms.value
+
+
+def _flow_unregister_args(flow, h_inv, size):
+    fl = np.ascontiguousarray(flow, np.float32)
+    hi = np.ascontiguousarray(h_inv, np.float64).reshape(-1, 9)
+    if fl.ndim != 4 or fl.shape[3] != 2 or len(hi) != len(fl):
+        raise ValueError(f"flow-unregister inputs of shapes flows {fl.shape}, inverses {hi.shape}: need [pairs, height, width, 2] float32 "
+                         "and [pairs, 3, 3]")
+    w, h = (int(v) for v in size)
+    prm = abi.FlowUnregisterParams(width=fl.shape[2], height=fl.shape[1], out_width=w, out_height=h, num_pairs=len(fl))
+    return prm, (_p(fl, C.c_float), _p(hi, C.c_double)), (fl, hi)
+
+
+def flow_unregister(flow, h_inv, size, device=0):
+    """rcvd_flow_unregister (infer's un-registration and resize_flow, optical_flow_homography.py:204-242) on the GPU.  flow [P, H, W, 2]
+    float32 (the model's flow_up[0] as H x W x 2), h_inv [P, 3, 3] np.linalg.inv(H_BA), size (w, h) of color_down.  Returns the float32
+    values of flow/flow_i_j.raw, [P, h, w, 2]."""
+    prm, args, keep = _flow_unregister_args(flow, h_inv, size)
+    out = np.empty((prm.num_pairs, prm.out_height, prm.out_width, 2), np.float32)
+    _check(lib().rcvd_flow_unregister(C.byref(prm), C.c_int32(device), *args, _p(out, C.c_float)))
+    return out
+
+
+def time_flow_unregister(flow, h_inv, size, reps=20, device=0):
+    """Bench hook: mean device ms of one rcvd_flow_unregister kernel pass over all the pairs (inputs uploaded once, CUDA events)."""
+    prm, args, keep = _flow_unregister_args(flow, h_inv, size)
+    ms = C.c_double()
+    _check(lib().rcvd_debug_time_flow_unregister(C.byref(prm), C.c_int32(device), *args, C.c_int32(reps), C.byref(ms)))
+    return ms.value
+
+
 def _depth_vis_params(frames, q=(0.0, 1.0), offset=0.0, scale=1.0):
     """The frames as a contiguous array and their rcvd_depth_vis_params: [F, H, W] float32 (RCVD_DEPTH_VIS_F32) or [F, H, W, 3] u8
     (RCVD_DEPTH_VIS_U8C3)."""
