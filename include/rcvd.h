@@ -598,6 +598,29 @@ typedef struct rcvd_flow_unregister_params {
 } rcvd_flow_unregister_params;
 int32_t rcvd_flow_unregister(const rcvd_flow_unregister_params* prm, int32_t device, const float* flow, const double* h_inv, float* out);
 
+/* ---- dynamic-object masks (DESIGN.md section 1 row 8f-13) ----
+ * Replaces the per-pixel work of dynamic_mask_generation (reference dynamic_mask_generation.py:107-182, run by
+ * DatasetProcessor.compute_dynamic_mask, process.py:147-165) around the caller's instance-segmentation model, for a batch of frames of
+ * one size:
+ *   masks[f] = cv2.bitwise_not(cv2.dilate(union, np.ones((d, d), np.uint8))) with union = 255 where any of frame f's instances is
+ *              inside, 0 elsewhere: 0 where dynamic, 255 elsewhere.  d = dilation, 0 meaning 3 (OpenCV's empty kernel); the window at
+ *              (y, x) is rows y - d / 2 .. y - d / 2 + d - 1 by the same columns, clipped to the image.
+ *   anon[f]  = the frame with every pixel of the undilated union set to 255 in all three channels, in R, G, B order (the pixels
+ *              cv2.imwrite stores for the reference's B, G, R copy; write_png stores them as they are).
+ *   instance_offsets [num_frames + 1] int64: frame f's instances are instances[instance_offsets[f] .. instance_offsets[f + 1])
+ *   instances        [instance_offsets[num_frames]][height][width] u8, non-zero = inside (the caller selects the dynamic classes)
+ *   frames           [num_frames][height][width][3] u8, B, G, R; nullable, needed by anon
+ *   masks            [num_frames][height][width] u8 (out);  anon [num_frames][height][width][3] u8 (out, nullable)
+ * num_frames = 0 returns RCVD_OK without a device.  Refused with RCVD_ERR_INVALID before any device work: a null parameter block, a
+ * non-positive size, 3 * width * height >= 2^31, num_frames < 0, dilation < 0, anon without frames, null offsets or masks, offsets
+ * that do not start at 0 or decrease, null instances while there are some. */
+typedef struct rcvd_dynamic_mask_params {
+  int32_t width, height, num_frames;
+  int32_t dilation;                /* the reference's --dilation_factor, >= 0 */
+} rcvd_dynamic_mask_params;
+int32_t rcvd_dynamic_masks(const rcvd_dynamic_mask_params* prm, int32_t device, const int64_t* instance_offsets, const uint8_t* instances,
+                           const uint8_t* frames, uint8_t* masks, uint8_t* anon);
+
 #ifdef __cplusplus
 }
 #endif

@@ -39,6 +39,12 @@ int32_t rcvd_debug_time_homography_warp(const rcvd_homography_warp_params* prm, 
                                         const double* inverse, int32_t reps, double* ms);
 int32_t rcvd_debug_time_flow_unregister(const rcvd_flow_unregister_params* prm, int32_t device, const float* flow, const double* h_inv,
                                         int32_t reps, double* ms);
+int64_t rcvd_dynamic_mask_launch_count(void);
+/* rcvd_dynamic_masks' kernels alone: the inputs are uploaded once, the kernels (with the anonymised frames when frames is non-null)
+ * run reps times between two CUDA events, and *ms is the mean device time of one pass over all the frames.  Arguments and refusals as
+ * rcvd_dynamic_masks (the outputs are not needed); num_frames >= 1, reps >= 1. */
+int32_t rcvd_debug_time_dynamic_masks(const rcvd_dynamic_mask_params* prm, int32_t device, const int64_t* instance_offsets,
+                                      const uint8_t* instances, const uint8_t* frames, int32_t reps, double* ms);
 int64_t rcvd_builder_last_rounds(void);          /* selection rounds of the last rcvd_build_constraints call */
 
 /* {frames, off-diagonal factor blocks, levels, H blocks, npad, stride, tiles, update targets ((source level, target block) pairs)} */

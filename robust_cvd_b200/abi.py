@@ -141,6 +141,11 @@ class DepthVisParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_frames", "kind")] + \
                [("q", C.c_double * 2), ("offset", C.c_double), ("scale", C.c_double)]
 
+
+class DynamicMaskParams(C.Structure):
+    """rcvd_dynamic_mask_params (include/rcvd.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("width", "height", "num_frames", "dilation")]
+
 # residual families of rcvd_evaluate_rows, in the order of rcvd_row_layout::family
 ROWS_PAIRS, ROWS_TRIPLETS, ROWS_DEPTH_PAIRS, ROWS_REGULARISERS = range(4)
 ROW_FAMILIES = ("pairs", "triplets", "depth_pairs", "regularisers")

@@ -1,5 +1,5 @@
 // rcvd_video.cu -- C ABI (include/rcvd.h) of the video-processing entry points: dense depth / spatial transforms, the flow-guided
-// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations, the downscaled colour frames, the depth visualisations and the homography-registered flows.  Like the solver (rcvd_api.cu) they
+// and bilateral depth filters, the flow-constraint builder, static flags and their pruning, long point tracks, the flow-consistency masks, the flow visualisations, the downscaled colour frames, the depth visualisations, the homography-registered flows and the dynamic-object masks.  Like the solver (rcvd_api.cu) they
 // have NO CPU fallback: without a usable CUDA device every one of them fails with RCVD_ERR_NO_DEVICE.
 #include <algorithm>
 #include <cmath>
@@ -20,6 +20,7 @@
 #include "rcvd_resize.cuh"
 #include "rcvd_depthvis.cuh"
 #include "rcvd_flowreg.cuh"
+#include "rcvd_dynmask.cuh"
 
 using namespace rcvd;
 
@@ -1113,4 +1114,90 @@ RCVD_API int32_t rcvd_debug_time_flow_unregister(const rcvd_flow_unregister_para
   const FlowUnregisterArgs a = upload_flow_unregister_inputs(call, *prm, flow, h_inv);
   if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_flow_unregister");
   return time_launches(call, reps, ms, "flow-unregister timing", [&] { return launch_flow_unregister(call, a, prm->num_pairs); });
+}
+
+// ---------------------------------------------------------------------------
+// Dynamic-object masks (rcvd_dynmask.cuh)
+// ---------------------------------------------------------------------------
+static int64_t g_dynmask_launches = 0;
+RCVD_API int64_t rcvd_dynamic_mask_launch_count() { return g_dynmask_launches; }
+// The argument rules of rcvd_dynamic_masks, checked on the host before any device is needed.
+static int check_dynamic_mask_args(const rcvd_dynamic_mask_params* prm, const int64_t* offsets, const uint8_t* instances, const uint8_t* frames,
+                                   bool anon) {
+  if (!prm) return set_err(RCVD_ERR_INVALID, "null argument");
+  const rcvd_dynamic_mask_params& q = *prm;
+  if (q.width <= 0 || q.height <= 0 || 3 * (int64_t)q.width * q.height >= (int64_t(1) << 31) || q.num_frames < 0 || q.dilation < 0)
+    return set_err(RCVD_ERR_INVALID, "bad dynamic-mask parameters: %d x %d, %d frames, dilation %d", q.width, q.height, q.num_frames, q.dilation);
+  if (anon && !frames) return set_err(RCVD_ERR_INVALID, "the anonymised frames need the frames");
+  if (q.num_frames == 0) return RCVD_OK;
+  if (!offsets) return set_err(RCVD_ERR_INVALID, "null argument");
+  if (offsets[0] != 0) return set_err(RCVD_ERR_INVALID, "instance offsets must start at 0");
+  for (int f = 0; f < q.num_frames; ++f)
+    if (offsets[f + 1] < offsets[f]) return set_err(RCVD_ERR_INVALID, "instance offsets decrease at frame %d", f);
+  if (offsets[q.num_frames] > 0 && !instances) return set_err(RCVD_ERR_INVALID, "null argument");
+  return RCVD_OK;
+}
+static DynMaskArgs upload_dynamic_mask_inputs(VideoCall& call, const rcvd_dynamic_mask_params& q, const int64_t* offsets, const uint8_t* instances,
+                                              const uint8_t* frames, bool anon) {
+  const size_t F = q.num_frames, plane = (size_t)q.width * q.height;
+  DynMaskArgs a{};
+  a.w = q.width; a.h = q.height; a.F = q.num_frames;
+  const int d = q.dilation == 0 ? 3 : q.dilation;   // cv::dilate replaces an empty kernel by 3 x 3
+  const int reach = std::max(q.width, q.height);     // a longer reach covers the same pixels
+  a.a = std::min(d / 2, reach); a.b = std::min(d - 1 - d / 2, reach);   // its default anchor (d / 2, d / 2)
+  a.seg = std::max(64, (q.height + 65534) / 65535);  // at most 65535 (grid.y) segments per column
+  a.offsets = (const long long*)call.upload(offsets, (F + 1) * 8);
+  a.instances = (const uint8_t*)call.upload(instances, (size_t)offsets[F] * plane);
+  a.frames = anon ? (const uint8_t*)call.upload(frames, F * plane * 3) : nullptr;
+  a.u = (uint8_t*)call.alloc(F * plane);
+  a.mask = (uint8_t*)call.alloc(F * plane);
+  a.ends = (int2*)call.alloc(F * ((q.height + a.seg - 1) / a.seg) * q.width * sizeof(int2));
+  a.anon = anon ? (uint8_t*)call.alloc(F * plane * 3) : nullptr;
+  return a;
+}
+// the three kernels over every frame, in launches of at most 65535 (grid.y) frames
+static int launch_dynamic_masks(VideoCall& call, DynMaskArgs a) {
+  const size_t plane = (size_t)a.w * a.h;
+  const bool vec = plane % 16 == 0;   // every frame's and instance's plane then starts 16-byte aligned
+  for (int f0 = 0; f0 < a.F; f0 += 65535) {
+    a.frame0 = f0;
+    const unsigned n = (unsigned)std::min(65535, a.F - f0);
+    if (int rc = vec ? call.launch(k_dm_union<16>, dim3(nblk(plane, kDmThreads * 16), n), kDmThreads, 0, a)
+                     : call.launch(k_dm_union<1>, dim3(nblk(plane, kDmThreads), n), kDmThreads, 0, a)) return rc;
+  }
+  if (int rc = call.launch(k_dm_rows, dim3(nblk((size_t)a.F * a.h * 32, kDmThreads)), kDmThreads, 0, a)) return rc;
+  const unsigned nseg = (unsigned)((a.h + a.seg - 1) / a.seg);
+  for (int f0 = 0; f0 < a.F; f0 += 65535) {
+    a.frame0 = f0;
+    const dim3 grid(nblk(a.w, kDmThreads), nseg, std::min(65535, a.F - f0));
+    if (int rc = call.launch(k_dm_col_ends, grid, kDmThreads, 0, a)) return rc;
+    if (int rc = call.launch(k_dm_cols, grid, kDmThreads, 0, a)) return rc;
+  }
+  return RCVD_OK;
+}
+RCVD_API int32_t rcvd_dynamic_masks(const rcvd_dynamic_mask_params* prm, int32_t device, const int64_t* instance_offsets, const uint8_t* instances,
+                                    const uint8_t* frames, uint8_t* masks, uint8_t* anon) {
+  if (int rc = check_dynamic_mask_args(prm, instance_offsets, instances, frames, anon != nullptr)) return rc;
+  const rcvd_dynamic_mask_params& q = *prm;
+  if (q.num_frames == 0) return RCVD_OK;
+  if (!masks) return set_err(RCVD_ERR_INVALID, "null argument");
+  VideoCall call;
+  if (int rc = call.open(device, g_dynmask_launches)) return rc;
+  const DynMaskArgs a = upload_dynamic_mask_inputs(call, q, instance_offsets, instances, frames, anon != nullptr);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_dynamic_masks");
+  if (int rc = launch_dynamic_masks(call, a)) return rc;
+  const size_t px = (size_t)q.num_frames * q.width * q.height;
+  cudaMemcpyAsync(masks, a.mask, px, cudaMemcpyDeviceToHost, call.st);
+  if (anon) cudaMemcpyAsync(anon, a.anon, px * 3, cudaMemcpyDeviceToHost, call.st);
+  return call.sync("dynamic-mask kernels");
+}
+RCVD_API int32_t rcvd_debug_time_dynamic_masks(const rcvd_dynamic_mask_params* prm, int32_t device, const int64_t* instance_offsets,
+                                               const uint8_t* instances, const uint8_t* frames, int32_t reps, double* ms) {
+  if (int rc = check_dynamic_mask_args(prm, instance_offsets, instances, frames, false)) return rc;
+  if (reps < 1 || !ms || prm->num_frames == 0) return set_err(RCVD_ERR_INVALID, "bad timing arguments");
+  VideoCall call;
+  if (int rc = call.open(device, g_dynmask_launches)) return rc;
+  const DynMaskArgs a = upload_dynamic_mask_inputs(call, *prm, instance_offsets, instances, frames, frames != nullptr);
+  if (!call.allocated()) return set_err(RCVD_ERR_CUDA, "device allocation failed in rcvd_debug_time_dynamic_masks");
+  return time_launches(call, reps, ms, "dynamic-mask timing", [&] { return launch_dynamic_masks(call, a); });
 }

@@ -802,6 +802,48 @@ def time_depth_visualize(frames, q, offset, scale, colormap, reps=20, device=0):
     return a.value, b.value
 
 
+def _dynamic_mask_args(instances, offsets, shape, dilation, frames):
+    """The contiguous u8 inputs of rcvd_dynamic_masks and its parameter block.  instances [total, h, w] bool or u8 (non-zero = inside),
+    offsets [F + 1] int64, shape (h, w), frames [F, h, w, 3] u8 B, G, R or None."""
+    h, w = (int(v) for v in shape)
+    ins = np.ascontiguousarray(instances)
+    ins = ins.view(np.uint8) if ins.dtype == np.bool_ else ins
+    off = np.ascontiguousarray(offsets, np.int64).reshape(-1)
+    if ins.dtype != np.uint8 or ins.ndim != 3 or ins.shape[1:] != (h, w) or len(off) < 1:
+        raise ValueError(f"dynamic-mask inputs of shapes instances {ins.shape} ({ins.dtype}), offsets {off.shape}: need [total, {h}, {w}] "
+                         "bool or u8 and [frames + 1] offsets")
+    if off[-1] != len(ins):
+        raise ValueError(f"instance offsets end at {off[-1]}, but {len(ins)} instances are given")
+    fr = None
+    if frames is not None:
+        fr = np.ascontiguousarray(frames, np.uint8)
+        if fr.shape != (len(off) - 1, h, w, 3):
+            raise ValueError(f"frames of shape {fr.shape}: need [{len(off) - 1}, {h}, {w}, 3] u8")
+    prm = abi.DynamicMaskParams(width=w, height=h, num_frames=len(off) - 1, dilation=int(dilation))
+    return prm, (_p(off, C.c_int64), _p(ins, C.c_uint8), _p(fr, C.c_uint8)), (ins, off, fr)
+
+
+def dynamic_masks(instances, offsets, shape, dilation=5, frames=None, device=0):
+    """rcvd_dynamic_masks (the mask and --save_anno image of dynamic_mask_generation, reference dynamic_mask_generation.py:143-182)
+    on the GPU.  Frame f's instances are instances[offsets[f]:offsets[f + 1]] ([total, h, w] bool or u8, non-zero = inside); shape is
+    (h, w).  Returns (masks [F, h, w] u8: cv2.bitwise_not(cv2.dilate(union, np.ones((dilation, dilation)))), anon [F, h, w, 3] u8 R, G,
+    B: frames (B, G, R) with the undilated union set to 255, or None without frames)."""
+    prm, args, keep = _dynamic_mask_args(instances, offsets, shape, dilation, frames)
+    masks = np.empty((prm.num_frames, prm.height, prm.width), np.uint8)
+    anon = None if frames is None else np.empty((prm.num_frames, prm.height, prm.width, 3), np.uint8)
+    _check(lib().rcvd_dynamic_masks(C.byref(prm), C.c_int32(device), *args, _p(masks, C.c_uint8), _p(anon, C.c_uint8)))
+    return masks, anon
+
+
+def time_dynamic_masks(instances, offsets, shape, dilation=5, frames=None, reps=20, device=0):
+    """Bench hook: mean device ms of one rcvd_dynamic_masks kernel pass over all the frames, with the anonymised frames when frames are
+    given (inputs uploaded once, CUDA events)."""
+    prm, args, keep = _dynamic_mask_args(instances, offsets, shape, dilation, frames)
+    ms = C.c_double()
+    _check(lib().rcvd_debug_time_dynamic_masks(C.byref(prm), C.c_int32(device), *args, C.c_int32(reps), C.byref(ms)))
+    return ms.value
+
+
 FP64_MMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
 
 

@@ -56,6 +56,18 @@ def _decode_png(fn):
     return img
 
 
+def check_frame_header(fn, hd):
+    """Refuses a frame whose png_header `hd` the project's decoder does not read as ffmpeg's frames: not 8-bit RGB (colour type 2),
+    interlaced, or carrying an eXIf chunk."""
+    if hd["bit_depth"] != 8 or hd["color_type"] != 2:
+        raise ValueError(f"{fn}: a {hd['bit_depth']}-bit PNG of colour type {hd['color_type']}; the frames must be 8-bit RGB "
+                         "(colour type 2), as ffmpeg's rgb24 writes them")
+    if hd["interlace"]:
+        raise ValueError(f"{fn}: an interlaced PNG; the frames must not be interlaced")
+    if hd["exif"]:
+        raise ValueError(f"{fn}: carries an eXIf chunk; a frame's EXIF orientation is not applied, so such frames are refused")
+
+
 def _check_full_frames(full_dir, count, files):
     """(height, width) of the frames color_full/frame_%06d.png, 0 <= i < count, after checking each one's header on the `files` pool:
     present, 8-bit RGB (colour type 2), not interlaced, no eXIf chunk, frame 0's size."""
@@ -67,13 +79,7 @@ def _check_full_frames(full_dir, count, files):
     heads = list(files.map(header, range(count)))
     size = (heads[0][1]["height"], heads[0][1]["width"])
     for fn, hd in heads:
-        if hd["bit_depth"] != 8 or hd["color_type"] != 2:
-            raise ValueError(f"{fn}: a {hd['bit_depth']}-bit PNG of colour type {hd['color_type']}; the frames must be 8-bit RGB "
-                             "(colour type 2), as ffmpeg's rgb24 writes them")
-        if hd["interlace"]:
-            raise ValueError(f"{fn}: an interlaced PNG; the frames must not be interlaced")
-        if hd["exif"]:
-            raise ValueError(f"{fn}: carries an eXIf chunk; a frame's EXIF orientation is not applied, so such frames are refused")
+        check_frame_header(fn, hd)
         if (hd["height"], hd["width"]) != size:
             raise ValueError(f"{fn}: {hd['width']} x {hd['height']} pixels, but frame 0 has {size[1]} x {size[0]}")
     return size
